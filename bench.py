@@ -1,12 +1,17 @@
 #!/usr/bin/env python
-"""bench.py - benchmarks of the B200 Wave-U-Net engine (one JSON line on stdout).
+"""bench.py - benchmarks of the Wave-U-Net engine on H100 (one JSON line on stdout).
 
 Headline metric (BASELINE.json): audio samples/sec, fwd+bwd, M4 context model.
 Pinned definition (SURVEY 8(d)): OUTPUT FRAMES per second = B * T_out / step_time, a stereo frame counts once; one step =
 forward + MSE loss + backward (+ NCCL gradient all-reduce when N > 1) + Adam, i.e. one `sess.run([separator_solver, ...])` of
-/root/reference/Training.py:103-109, on synthetic windows (147443 in / 16389 out, stereo), batch 16 per GPU (weak scaling).
+the reference's Training.py:103-109, on synthetic windows (147443 in / 16389 out, stereo), batch 16 per GPU (weak scaling).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--no-extras] [--no-graph] [--no-overlap]
+                  [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the timed path computed in its last timed step - the loss, the gradient buffer and the
+parameters after Adam, float32, a fixed seeded sample of at most 4M elements each - as DIR/<name>.npy, so that two builds
+can be compared output for output (the inputs and the parameter initialisation are seeded: identical from run to run).
 
 The line also carries, under "extra_configs", short measurements of the other BASELINE.json configurations made in the same
 run: M5 `full` (learned upsampling) batch 16, M6 `full_multi_instrument` GLOBAL batch 32 (strong scaling: 32/N windows per
@@ -44,7 +49,8 @@ def load_peaks():
         p = json.load(open(path))
         return dict(source="measured (MEASURED_PEAKS.json)", hbm_gbs=p["hbm_gbs"], tf_burst=p["bf16_tflops"],
                     tf_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]))
-    return dict(source="fallback (B200_PROFILING.md)", hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0)
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 - a ceiling, not a measured rate
+    return dict(source="H100 SXM data sheet", hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0)
 
 
 def host_cores():
@@ -64,7 +70,7 @@ def host_cores():
 
 
 def kernel_source_hash():
-    """sha256 over the CUDA/C++ sources of libwun.so: ties an ncu capture under profiles/ to the build that ran."""
+    """sha256 over the CUDA/C++ sources of libwun.so: ties a measurement to the build that ran."""
     h = hashlib.sha256()
     d = os.path.join(PKG, "csrc")
     for name in sorted(os.listdir(d)):
@@ -75,7 +81,7 @@ def kernel_source_hash():
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -599,6 +605,23 @@ def predict_bench(rank, world, dev, dist, reps=2):
             "n_gpus": world}
 
 
+DUMP_MAX_ELEMS = 4 << 20      # per array: 16 MB of float32, 32 MB for the two big ones
+
+
+def dump_outputs(run, out_dir):
+    """The last timed step's results as a caller of the step receives them: loss, gradients, updated parameters."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": run.sep._loss.reshape(-1), "gradients": run.sep.grads.reshape(-1), "params": run.sep.params.reshape(-1)}
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.size > DUMP_MAX_ELEMS:                               # the same seeded sample of positions in every run
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+
+
 def run_ours(args, rank, world, local_rank):
     import torch
 
@@ -618,6 +641,8 @@ def run_ours(args, rank, world, local_rank):
     graphed = run.prepare(use_graph=not args.no_graph)
     ms_total, t_begin, t_end = run.time_steps(args.steps, args.warmup, prewarm_s=0.0 if args.no_prewarm else 1.5)
     clk = clocks.stop(t_begin, t_end) if rank == 0 else None
+    if getattr(args, "dump_outputs", None) and rank == 0:
+        dump_outputs(run, args.dump_outputs)
     e_steps = max(3, min(args.steps, 10))
     e2e = run.e2e(e_steps, args.warmup)
 
@@ -638,7 +663,7 @@ def run_ours(args, rank, world, local_rank):
         "config": {"workload": "M4 baseline_stereo L=12, 147443-in/16389-out stereo, batch %d per GPU, "
                                "fwd+loss+bwd+Adam%s" % (run.B, "+NCCL all-reduce" if world > 1 else ""),
                    "global_batch": run.B * world, "parallelism": "dp%d" % world,
-                   "l2_policy": "per-step working set (~1.2 GB activations + gradients) exceeds the 126 MB L2",
+                   "l2_policy": "per-step working set (~1.2 GB activations + gradients) exceeds the 50 MB L2",
                    "cuda_graph": graphed, "cuda_graph_error": run.graph_error,
                    "untimed_prewarm_steps": 0 if args.no_prewarm else int(1.5 / 0.006),
                    "allreduce": (("bucketed (%d buckets) on a comm stream, overlapped with backward" % len(run.ar.views))
@@ -720,12 +745,6 @@ def run_ours(args, rank, world, local_rank):
                                 "frac_of_burst": round(v["tflops"] / peaks["tf_burst"], 4)} for k, v in fam.items()}
         line["top_launch"] = {"layer": top["layer"], "pass": top["pass"], "us": round(top["us"], 1),
                               "gflop": round(top["gflop"], 2), "frac_of_burst": round(top["tflops"] / peaks["tf_burst"], 4)}
-        try:
-            os.makedirs(os.path.join(REPO, "gpurun_out"), exist_ok=True)
-            with open(os.path.join(REPO, "gpurun_out", "layer_table_n%d.json" % world), "w") as f:
-                json.dump({"source_hash": kernel_source_hash(), "ms_per_step": ms_step, "rows": rows, "families": fam}, f, indent=1)
-        except Exception:
-            pass
 
     # ---- the other BASELINE.json configurations, briefly, in the same run ----------------------------------------------
     if not args.no_extras:
@@ -802,6 +821,8 @@ def main():
     ap.add_argument("--no-extras", action="store_true", help="skip the M5 / M6 / Predict measurements")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-prewarm", action="store_true", help="skip the untimed pre-warm replays (profiler runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, gradients and updated parameters to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,10 +1,10 @@
 /*
- * wun.h - C ABI of the B200 Wave-U-Net forward/backward engine (libwun.so).
+ * wun.h - C ABI of the Wave-U-Net forward/backward engine for H100 (libwun.so).
  *
  * The reference has no FFI layer; its boundary for this path is the Python duck type
  *     UnetAudioSeparator(model_config).get_padding(shape) / .get_output(mix, training, ...)
- * (/root/reference/Models/UnetAudioSeparator.py:15-144) plus the loss / Adam lines of
- * /root/reference/Training.py:50-77.  Each entry point below names the reference lines it replaces.
+ * (the reference's Models/UnetAudioSeparator.py:15-144) plus the loss / Adam lines of
+ * its Training.py:50-77.  Each entry point below names the reference lines it replaces.
  * The Python facade in wave-u-net_b200/Models/UnetAudioSeparator.py binds these with ctypes
  * (see INTEGRATION.md).
  *

@@ -1,7 +1,7 @@
 """pytest wiring: marker registration and import paths.
 
 `-m "not gpu"` runs everywhere (oracle vs golden fixtures, host logic, C-ABI symbol checks, gloo
-multi-process); `-m gpu` needs a B200 and is the parity suite proper (CUDA path through the C-ABI
+multi-process); `-m gpu` needs an H100 and is the parity suite proper (CUDA path through the C-ABI
 vs oracle)."""
 import os
 import sys
@@ -16,7 +16,7 @@ for p in (REPO, PKG, os.path.join(REPO, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (B200); run with -m gpu")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100); run with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -7,7 +7,7 @@
 // kernels_umma.h), written from those contracts in double-precision accumulation: the tensor-core kernels' tiling, pipelines
 // and bf16 hi/lo arithmetic do not appear - only WHAT they must produce.  tests/test_cpu_device.py runs whole training steps of
 // the engine's real host code this way and compares loss, every gradient and the Adam update with the oracle: that checks the
-// parameter blocks the host builds for the tcgen05 kernels (plane / class / group / term tables, packed-weight jobs, pair-merged
+// parameter blocks the host builds for the tensor-core kernels (plane / class / group / term tables, packed-weight jobs, pair-merged
 // halves, split-pass jobs, fused output epilogue, scales, accumulate ranges) for configurations no GPU test has run.
 #include <cuda_runtime.h>
 #include <math.h>
@@ -119,7 +119,7 @@ static void run_pack(const UmmaPackLaunch& P) {
     }
 }
 
-// ---- tcgen05 plane convolution (all tilings) + the fused output epilogue -------------------------------------------------------
+// ---- tensor-core plane convolution + the fused output epilogue -------------------------------------------------------
 static bool run_umma_conv(const UmmaLaunch& L, const OutputFuse* F) {
     const int ncol_out = F ? F->O.nconv * F->O.C : 0;
     double lsum = 0.0;
@@ -475,6 +475,9 @@ bool execute(const std::string& name, void** args) {
         }
         return true;
     }
+    // the partial tiles / per-CTA column sums are an internal format of the device kernels: the wgrad and split references above
+    // and below produce the final dW and bias sums themselves, so what the reduction adds on the device is already there
+    if (has(name, "wgrad_reduce_kernel") || has(name, "first_wgrad_sum_kernel")) return true;
     if (has(name, "split_views_kernel")) {              // the split arrays themselves are an internal operand format of the device
         const SplitJobs& J = *static_cast<const SplitJobs*>(args[0]);      // kernels; what the rest of the step sees: the bias sums
         for (int j = 0; j < J.njobs; ++j) {
@@ -516,8 +519,10 @@ bool execute(const std::string& name, void** args) {
     }
     if (has(name, "output_fwd_kernel")) { run_output_fwd(*static_cast<const OutputLaunch*>(args[0])); return true; }
     if (has(name, "output_dgrad_kernel")) { run_output_dgrad(*static_cast<const OutputLaunch*>(args[0]), *static_cast<float* const*>(args[1])); return true; }
-    if (has(name, "output_wgrad_kernel")) {
-        run_output_wgrad(*static_cast<const OutputLaunch*>(args[0]), *static_cast<float* const*>(args[1]), *static_cast<const float*>(args[2]));
+    // output_wgrad_kernel leaves per-CTA sums; the reference of the whole gradient runs at the launch that adds them up
+    if (has(name, "output_wgrad_kernel")) return true;
+    if (has(name, "output_wgrad_sum_kernel")) {
+        run_output_wgrad(*static_cast<const OutputLaunch*>(args[0]), *static_cast<float* const*>(args[3]), *static_cast<const float*>(args[4]));
         return true;
     }
     if (has(name, "upsample_bwd_kernel")) { run_upsample_bwd(*static_cast<const UpsampleBwdLaunch*>(args[0])); return true; }

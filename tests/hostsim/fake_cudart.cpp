@@ -166,6 +166,17 @@ void dw_block(Acc& a, float* dW, long long woff, int Cp, int Cg, int w_sp, int w
     else a.flat('A', dW + woff, 4LL * ((long long)(Cp - 1) * w_sp + (long long)(Cg - 1) * w_sg + 1));
 }
 
+// the partial tiles a bulk-fed wgrad launch stores (kernels_umma.cu: one 128 x 256-float slot per CTA of the launch)
+long long wgrad_partial_bytes(const UmmaWgradLaunch& L) {
+    long long slots = 0;
+    for (int g = 0; g < L.ngroups; ++g) slots += (long long)L.grp[g].n_tapsets * L.grp[g].n_mtiles * L.grp[g].n_ntiles * L.grp[g].n_ctas_x;
+    return slots * 128 * 256 * 4;
+}
+// the per-CTA column sums of split job j: [batch][chunk][2048-row block][16]
+long long colsum_part_bytes(const SplitJobs& J, int j) {
+    return 4LL * J.batch * J.job[j].nchunk * ((J.job[j].rows + 2047) / 2048) * 16;
+}
+
 void decode_wgrad_groups(Acc& a, const UmmaWgradLaunch& L, const WgSplit* S) {
     for (int g = 0; g < L.ngroups; ++g) {
         const WgGroup& G = L.grp[g];
@@ -230,10 +241,25 @@ Acc decode(const std::string& name, void** args, bool* known) {
                 a.flat('A', F.grads + F.O.w_off[k], 4LL * F.O.ofs * (F.O.C + F.O.F) * F.O.C);
                 a.flat('A', F.grads + F.O.b_off[k], 4LL * F.O.C);
             }
-    } else if (has(name, "plane_conv_umma_")) {                // _kernel<>, _persistent<>, _persistent_dg2 / _fw2, _fold
+    } else if (has(name, "plane_conv_umma_")) {                // plane_conv_umma_kernel<NPAD, DG>
         decode_umma_conv(a, *static_cast<const UmmaLaunch*>(args[0]));
     } else if (has(name, "wgrad_umma_bulk_kernel")) {
-        decode_wgrad_groups(a, *static_cast<const UmmaWgradLaunch*>(args[0]), static_cast<const WgSplit*>(args[1]));
+        const UmmaWgradLaunch& L = *static_cast<const UmmaWgradLaunch*>(args[0]);
+        decode_wgrad_groups(a, L, static_cast<const WgSplit*>(args[1]));
+        if (L.partial) a.flat('W', L.partial, wgrad_partial_bytes(L));
+    } else if (has(name, "wgrad_reduce_kernel")) {
+        const UmmaWgradLaunch& L = *static_cast<const UmmaWgradLaunch*>(args[0]);
+        const SplitJobs& J = *static_cast<const SplitJobs*>(args[1]);
+        if (L.partial) {
+            a.flat('R', L.partial, wgrad_partial_bytes(L));
+            for (int g = 0; g < L.ngroups; ++g)
+                for (int t = 0; t < L.grp[g].ntaps; ++t) dw_block(a, L.dW, L.grp[g].woff[t], L.grp[g].P.C, L.grp[g].G.C, L.w_sp, L.w_sg);
+        }
+        for (int j = 0; j < J.njobs; ++j)
+            if (J.job[j].colsum) {
+                a.flat('R', J.job[j].colsum_part, colsum_part_bytes(J, j));
+                a.flat('A', J.job[j].colsum, 4LL * J.job[j].V.C);
+            }
     } else if (has(name, "wgrad_umma_kernel")) {
         decode_wgrad_groups(a, *static_cast<const UmmaWgradLaunch*>(args[0]), nullptr);
     } else if (has(name, "split_views_kernel")) {
@@ -242,7 +268,8 @@ Acc decode(const std::string& name, void** args, bool* known) {
             const SplitJob& S = J.job[j];
             a.plane(S.V, J.batch, S.row0, (long long)S.row0 + S.rows);
             a.flat('W', S.out, (long long)J.batch * S.nchunk * 4 * S.rows * 16);
-            if (S.colsum) a.flat('A', S.colsum, 4LL * S.V.C);
+            if (S.colsum) a.flat('A', S.colsum, 4LL * S.V.C);                  // (what the host reference of the launch adds)
+            if (S.colsum && S.colsum_part) a.flat('W', S.colsum_part, colsum_part_bytes(J, j));
         }
     } else if (has(name, "umma_pack_kernel")) {
         const UmmaPackLaunch& P = *static_cast<const UmmaPackLaunch*>(args[0]);
@@ -256,6 +283,12 @@ Acc decode(const std::string& name, void** args, bool* known) {
                     if (P.pairC > 0 && P.woff2[t] >= 0) weight_slice(a, P.W, P.woff2[t], J.g_C[g], half, P.w_sk, P.w_sn);
                 }
         }
+    } else if (has(name, "first_wgrad_sum_kernel")) {
+        const FirstWgrad& P = *static_cast<const FirstWgrad*>(args[0]);
+        const int C = *static_cast<const int*>(args[1]), N = *static_cast<const int*>(args[2]);
+        a.flat('R', P.part, 4LL * 2 * P.L.batch * P.grid_x * (P.L.k * C * N + N));
+        a.flat('A', P.dW, 4LL * P.L.k * C * N);
+        if (P.db) a.flat('A', P.db, 4LL * N);
     } else if (has(name, "first_fwd_kernel") || has(name, "first_wgrad_kernel")) {
         const bool wg = has(name, "first_wgrad_kernel");
         const FirstLayer& L = wg ? static_cast<const FirstWgrad*>(args[0])->L : *static_cast<const FirstLayer*>(args[0]);
@@ -265,8 +298,9 @@ Acc decode(const std::string& name, void** args, bool* known) {
         a.view(wg ? 'R' : 'W', L.odd, L.batch, L.odd_bstride, 0, L.mo_hi - L.mo_lo, N, N);
         if (wg) {
             const FirstWgrad& P = *static_cast<const FirstWgrad*>(args[0]);
-            a.flat('A', P.dW, 4LL * L.k * C * N);
+            a.flat('A', P.dW, 4LL * L.k * C * N);                       // (what the host reference of the launch adds)
             if (P.db) a.flat('A', P.db, 4LL * N);
+            a.flat('W', P.part, 4LL * 2 * L.batch * P.grid_x * (L.k * C * N + N));
         } else {
             a.flat('R', L.W, 4LL * L.k * C * N);
             a.flat('R', L.bias, 4LL * N);
@@ -291,10 +325,20 @@ Acc decode(const std::string& name, void** args, bool* known) {
         decode_output(a, O, true, false);
         a.flat('R', O.dpre, 4LL * O.batch * O.T_out * O.nconv * O.C);
         a.flat('W', *static_cast<float* const*>(args[1]), 4LL * O.batch * O.Tf * O.F);
-    } else if (has(name, "output_wgrad_kernel")) {
+    } else if (has(name, "output_wgrad_kernel")) {                  // per-CTA sums: [tap][row chunk][(C + F + 1) * nconv * C]
         const OutputLaunch& O = *static_cast<const OutputLaunch*>(args[0]);
-        float* grads = *static_cast<float* const*>(args[1]);
+        const float* part = *static_cast<float* const*>(args[1]);
+        const long long per = *static_cast<const int*>(args[2]), nx = ((long long)O.batch * O.T_out + per - 1) / per;
         decode_output(a, O, true, false);
+        a.flat('R', O.dpre, 4LL * O.batch * O.T_out * O.nconv * O.C);
+        a.flat('W', part, 4LL * O.ofs * nx * (O.C + O.F + 1) * O.nconv * O.C);
+    } else if (has(name, "output_wgrad_sum_kernel")) {
+        const OutputLaunch& O = *static_cast<const OutputLaunch*>(args[0]);
+        const float* part = *static_cast<float* const*>(args[1]);
+        const long long nx = *static_cast<const int*>(args[2]);
+        float* grads = *static_cast<float* const*>(args[3]);
+        a.flat('R', part, 4LL * O.ofs * nx * (O.C + O.F + 1) * O.nconv * O.C);
+        decode_output(a, O, true, false);                                  // (what the host reference of the launch reads)
         a.flat('R', O.dpre, 4LL * O.batch * O.T_out * O.nconv * O.C);
         for (int k = 0; k < O.nconv; ++k) {
             a.flat('A', grads + O.w_off[k], 4LL * O.ofs * (O.C + O.F) * O.C);
@@ -545,7 +589,7 @@ cudaError_t cudaStreamWaitEvent(cudaStream_t s, cudaEvent_t e, unsigned flags) {
 }
 cudaError_t cudaFuncSetAttribute(const void* func, cudaFuncAttribute attr, int value) {
     if (attr == cudaFuncAttributeMaxDynamicSharedMemorySize) {
-        if (value > 232448) return cudaErrorInvalidValue;          // 227 KB: the opt-in limit per CTA on sm_100
+        if (value > 232448) return cudaErrorInvalidValue;          // 227 KB: the opt-in limit per CTA on sm_90
         std::lock_guard<std::mutex> lk(g_mu);
         g_max_dyn_smem[func] = value;
     }

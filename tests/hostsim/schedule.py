@@ -58,7 +58,7 @@ def build():
     srcs = [os.path.join(csrc, s) for s in SOURCES]
     if _newer(sim, srcs + headers):                          # (the runtime is linked dynamically: no relink when only it changes)
         # the device code is never executed: lowest optimisation levels, the host code is what runs
-        subprocess.check_call([NVCC, "--cudart", "none", "-gencode", "arch=compute_100a,code=sm_100a", "-O1", "-Xptxas", "-O0",
+        subprocess.check_call([NVCC, "--cudart", "none", "-gencode", "arch=compute_90a,code=sm_90a", "-O1", "-Xptxas", "-O0",
                                "-std=c++17", "-diag-suppress", "177", "-Xcompiler", "-fPIC", "-shared", "-o", sim] + srcs +
                               ["-L" + BUILD, "-lfakecudart", "-Xlinker", "-rpath=$ORIGIN"], cwd=PKG)
     return sim
@@ -263,7 +263,7 @@ def check(meta, ops, max_reports=20, init_regions=("ws", "ws_infer", "grads", "l
 
 
 def launch_limit_violations(ops):
-    """Launch geometry against the sm_100 limits (the real values the engine passes to the runtime, not the planner's audit):
+    """Launch geometry against the sm_90 limits (the real values the engine passes to the runtime, not the planner's audit):
     <= 1024 threads per CTA, grid y / z <= 65535, dynamic shared memory <= 227 KB and - above the 48 KB default - within what the
     kernel opted in to with cudaFuncSetAttribute, cluster width <= 8 dividing grid.x, non-empty grids."""
     bad = []

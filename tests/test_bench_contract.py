@@ -108,7 +108,7 @@ def _lines(capsys):
 
 
 def test_single_gpu_line_has_the_contract_keys(stubbed, capsys, tmp_path, monkeypatch):
-    monkeypatch.setattr(bench, "REPO", str(tmp_path))           # the per-layer table is written under REPO/gpurun_out
+    monkeypatch.setattr(bench, "REPO", str(tmp_path))
     monkeypatch.setattr(bench, "kernel_source_hash", lambda: "0" * 16)
     bench.run_ours(_args(), 0, 1, 0)
     (line,) = _lines(capsys)
@@ -130,7 +130,7 @@ def test_single_gpu_line_has_the_contract_keys(stubbed, capsys, tmp_path, monkey
     assert set(line["extra_configs"]) == {"m6_full_multi_instrument_b32", "m5_full_learned_b16", "predict_3min_44k"}
     assert line["cpu_baseline"]["kind"] == "port" and line["cpu_baseline"]["cores"] == 16
     assert "aborted_in" not in line and "dp_check" not in line
-    assert os.path.exists(os.path.join(str(tmp_path), "gpurun_out", "layer_table_n1.json"))
+    assert os.listdir(str(tmp_path)) == []                      # the tree can be read-only: the benchmark writes nothing there
 
 
 def test_footprint_model_is_reported_only_for_the_sources_it_was_made_from(stubbed, capsys, tmp_path, monkeypatch):
@@ -143,7 +143,7 @@ def test_footprint_model_is_reported_only_for_the_sources_it_was_made_from(stubb
     bench.run_ours(_args(no_extras=True, no_cpu_baseline=True), 0, 1, 0)
     (line,) = _lines(capsys)
     fm = line["step_footprint_model"]
-    assert fm["distinct_bytes"] == 7.95e9 and abs(fm["frac_of_step"] - fm["hbm_floor_ms"] / 4.8) < 1e-12 and 0.2 < fm["frac_of_step"] < 0.3
+    assert fm["distinct_bytes"] == 7.95e9 and abs(fm["frac_of_step"] - fm["hbm_floor_ms"] / 4.8) < 1e-12 and 0.45 < fm["frac_of_step"] < 0.55
     monkeypatch.setattr(bench, "kernel_source_hash", lambda: "b" * 16)          # other kernel sources: stale, not reported
     bench.run_ours(_args(no_extras=True, no_cpu_baseline=True), 0, 1, 0)
     (line,) = _lines(capsys)
@@ -265,3 +265,24 @@ def test_stack_roofline_accounting_reproduces_the_survey_table(first_layer, monk
     assert abs(sr["bound_ms"] - total * 1e3) < 1e-9
     adam = sr["items"][-1]
     assert adam["layer"] == "adam" and abs(adam["mbytes"] - 7 * 4 * 10263390 * 1e-6) < 1e-6      # SURVEY a15: 10 263 390 parameters
+
+
+def test_dump_outputs_writes_the_last_step_as_a_fixed_sample_within_the_size_cap(tmp_path, monkeypatch):
+    """--dump-outputs: loss, gradients and parameters as float32 .npy; arrays above the cap are sampled at the SAME seeded
+    positions in every run, so that two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
+    monkeypatch.setattr(bench, "DUMP_MAX_ELEMS", 1000)
+    n = 5000
+    sep = types.SimpleNamespace(_loss=torch.tensor([0.25]), grads=torch.arange(n, dtype=torch.float32) * 2,
+                                params=torch.arange(n, dtype=torch.float64))
+    run = types.SimpleNamespace(sep=sep)
+    for d in ("a", "b"):
+        bench.dump_outputs(run, os.path.join(str(tmp_path), d))
+    a = {k: np.load(os.path.join(str(tmp_path), "a", k + ".npy")) for k in ("loss", "gradients", "params")}
+    b = {k: np.load(os.path.join(str(tmp_path), "b", k + ".npy")) for k in ("loss", "gradients", "params")}
+    assert a["loss"].tolist() == [0.25] and all(v.dtype == np.float32 for v in a.values())
+    assert a["gradients"].size == a["params"].size == 1000
+    assert np.array_equal(a["gradients"], 2 * a["params"])         # the same positions in both arrays
+    assert all(np.array_equal(a[k], b[k]) for k in a)              # and in every run

@@ -4,7 +4,7 @@ tests/hostsim/ builds the engine's sources a second time with `nvcc --cudart non
 mode that runtime carries every launch out on host memory with the reference routines of tests/hostsim/cpu_kernels.cpp - an
 independent statement, in plain double-precision loops, of what each kernel must compute from its by-value parameter block.
 What runs unmodified is everything the HOST does: the planner, the plane / class / group / term tables and packed-weight jobs
-built for the tcgen05 kernels (incl. pair-merged halves, output-channel splits, the fused output epilogue's frame mapping), the
+built for the tensor-core kernels (incl. pair-merged halves and output-channel splits), the
 split-pass jobs that carry the bias sums, the first-layer / upsampling-backward / output-layer blocks, gradient scales,
 accumulate ranges, memsets and the device-side Adam state.  Loss, every gradient, the source estimates and the parameters after
 two TF-form Adam steps must agree with the oracle to rounding (1e-5 / 1e-4: the reference routines accumulate in double).
@@ -44,7 +44,7 @@ def _need_simulation(_build_once):
         pytest.skip("host simulation of the engine not built (needs nvcc and g++)")
 
 
-FORCED = {"WUN_PERS_MIN": "0", "WUN_FOLD": "0", "WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}
+FORCED = {"WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}
 
 
 def run_steps(named, overrides, batch, nf, env=None, grad_scale=1.0):
@@ -106,25 +106,23 @@ def test_two_training_steps_and_inference_on_the_cpu_device_match_the_oracle(var
         try:
             assert_matches_oracle(res)
             ks = res["kernels"]
-            assert any(k.startswith("plane_conv_umma") for k in ks) and "wgrad_umma_bulk_kernel" in ks and "umma_pack_kernel" in ks
-            if forced:
-                assert "plane_conv_umma_persistent_dg2" in ks and any(k.startswith("plane_conv_umma_persistent_out<") for k in ks), sorted(ks)
-            else:
-                assert "plane_conv_umma_fold" in ks and "output_fwd_kernel" in ks
+            assert any(k.startswith("plane_conv_umma_kernel<") and k.endswith("false>") for k in ks), sorted(ks)   # forward
+            assert any(k.startswith("plane_conv_umma_kernel<") and k.endswith("true>") for k in ks), sorted(ks)    # dgrad
+            assert any(k.startswith("wgrad_umma_bulk_kernel<") for k in ks) and "umma_pack_kernel" in ks, sorted(ks)
+            assert "output_fwd_kernel" in ks, sorted(ks)
         except AssertionError as ex:
             raise AssertionError("%s: %s" % (name, ex))
 
 
 SWITCHES = [
-    {"WUN_OUT_FUSE": "2"},                       # the output convs' own weight gradient inside the fused epilogue
-    {"WUN_OUT_FUSE": "0"},                       # separate output kernels next to the persistent convs
-    {"WUN_BULK_WGRAD": "0"},                     # converter-fed tcgen05 wgrad, bias sums by colsum_kernel
+    {"WUN_OUT_FUSE": "2"},                       # output-layer switch in its other positions (the output layer runs in its own
+    {"WUN_OUT_FUSE": "0"},                       #   kernels either way: the step must not change)
+    {"WUN_BULK_WGRAD": "0"},                     # converter-fed tensor-core wgrad, bias sums by colsum_kernel
     {"WUN_SPLIT_COLSUM": "0"},
     {"WUN_FIRST_LAYER": "0"},                    # first layer through the generic plane kernels
     {"WUN_DISABLE_UMMA": "1"},                   # the exact-fp32 CUDA-core path for everything
     {"WUN_UMMA_DGRAD": "0"},
     {"WUN_PAIR_FWD": "0", "WUN_PAIR_DGRAD": "0"},
-    {"WUN_NSPLIT_MAX": "4", "WUN_TEAMS": "4", "WUN_PERSISTENT": "0"},      # output-channel splits of the non-persistent kernel
     {"WUN_SIDE_STREAM": "0"},
 ]
 

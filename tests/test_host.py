@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(wun.LIB_PATH)
     for s in declared:
         assert hasattr(lib, s), s
-    assert b"sm_100a" in wun.lib.wun_version()
+    assert b"sm_90a" in wun.lib.wun_version()
 
 
 def test_config_presets_and_cli():
@@ -135,7 +135,8 @@ def test_compute_entry_points_fail_loudly_without_gpu():
 # ------------------------------------------------------------------------------------------------
 # plan audit: every tensor-core launch the planner would issue, against the hardware limits (no GPU needed)
 # ------------------------------------------------------------------------------------------------
-SMEM_LIMIT = {"dense2": 200 * 1024, "sparse4": 220 * 1024, "persistent": 220 * 1024, "fold": 220 * 1024}   # cudaFuncSetAttribute values in kernels_umma.cu
+SMEM_LIMIT = 200 * 1024      # cudaFuncSetAttribute value of the conv and wgrad instantiations in kernels_umma.cu
+SMEM_PER_SM = 228 * 1024     # H100: shared memory of one SM (1 KB of it reserved per resident CTA)
 
 
 def _audit(preset, batch, overrides=None):
@@ -148,75 +149,57 @@ def _audit(preset, batch, overrides=None):
 @pytest.mark.parametrize("preset", ["baseline", "baseline_context", "baseline_stereo", "full", "full_multi_instrument", "full_44KHz"])
 @pytest.mark.parametrize("batch", [1, 2, 4, 8, 16, 32])
 def test_planned_tcgen05_launches_respect_hardware_limits(preset, batch):
+    """Every tensor-core (wgmma) launch the planner would issue, against the H100 limits."""
     lines = _audit(preset, batch)
     convs = [d for d in lines if d["op"] == "conv"]
     wgs = [d for d in lines if d["op"] == "wgrad"]
     assert convs and wgs
-    pow2 = lambda v: v >= 32 and (v & (v - 1)) == 0
     for d in convs:
-        assert d["NPAD"] % 16 == 0 and 16 <= d["NPAD"] <= 256 and d["NPAD"] * d["nsplit"] >= d["N"], d
-        assert d["MT"] in (1, 2) and d["rows_alloc"] % 8 == 0 and d["rows_alloc"] >= d["MT"] * 128 + d["span"], d
-        need = d["MT"] * d["NPAD"] * (2 if d["kernel"] == "persistent" else 1) * (2 if d["fuse"] else 1)
-        assert pow2(d["tmem"]) and need <= d["tmem"] <= 512, d
-        if d["kernel"] == "dense2":
-            assert d["tmem"] <= 256, d                     # two CTAs per SM share the 512 TMEM columns
+        assert d["kernel"] == "wgmma", d
+        # accumulators: 64 rows x NPAD fp32 registers per warpgroup
+        assert d["NPAD"] % 16 == 0 and 16 <= d["NPAD"] <= 128 and d["NPAD"] * d["nsplit"] >= d["N"] and d["nsplit"] <= 4, d
+        assert d["MT"] == 1 and d["rows_alloc"] % 8 == 0 and d["rows_alloc"] >= 128 + d["span"], d
         assert 1 <= d["TB"] <= 4 and 2 <= d["nbs"] <= 6, d
-        assert d["nteams"] == {"dense2": 2, "sparse4": 4}.get(d["kernel"], d["nteams"]) and d["nteams"] in (2, 3, 4), d
-        assert d["smem"] <= SMEM_LIMIT[d["kernel"]], d
+        assert d["smem"] <= SMEM_LIMIT and 2 * (d["smem"] + 1024) <= SMEM_PER_SM, d      # two CTAs per SM
         assert d["tiles"] >= 1 and d["span"] <= 24, d
-        if d["pair"]:                                      # pair-merged class: two halves of `pair` columns, never the folded kernel
-            assert d["N"] == 2 * d["pair"] and d["pair"] % 4 == 0 and d["N"] <= 256 and d["kernel"] != "fold", d
-        if d["epi2"]:                                      # two epilogue groups: the persistent dgrad with two converter teams
-            assert d["kernel"] == "persistent" and d["pass"] == 1 and d["nteams"] == 2, d
-        if d["outfuse"]:                                   # output layer in the epilogue: persistent forward conv, one column block
-            assert d["kernel"] == "persistent" and d["pass"] == 0 and d["nteams"] == 3 and d["NPAD"] <= 128 and d["nsplit"] == 1, d
-        if d["kernel"] == "fold":                          # cluster of ksplit CTAs per tile: portable size, one wave of clusters
-            assert 1 <= d["ksplit"] <= 8 and d["tiles"] <= [0, 148, 74, 45, 33, 26, 22, 15, 15][d["ksplit"]], d   # tools/cluster_probe on B200
-            assert d["nteams"] == 4 and not d["fuse"], d
-            assert d["MT"] * 128 * (d["NPAD"] + 4) * 4 <= d["smem"], d      # the partial-accumulator tile aliases the pipeline memory
-        else:
-            assert d["ksplit"] == 0, d
+        if d["pair"]:                                      # pair-merged class: two halves of `pair` columns
+            assert d["N"] == 2 * d["pair"] and d["pair"] % 4 == 0, d
+        assert not d["outfuse"], d                         # the output layer runs in its own kernels
     for d in wgs:
         assert d["NT"] % 16 == 0 and 16 <= d["NT"] <= 128 and d["NT"] * d["ntiles"] >= min(d["Cp"], d["Cg"]), d
         assert d["mtiles"] * 128 >= max(d["Cp"], d["Cg"]), d
         assert d["taps_per_cta"] * d["tapsets"] >= d["ntaps"] and 1 <= d["taps_per_cta"] <= 8, d
-        assert pow2(d["tmem"]) and d["taps_per_cta"] * d["NT"] <= d["tmem"] <= 512, d
-        assert d["nstages"] in (2, 3) and d["smem"] <= 200 * 1024, d
+        assert d["taps_per_cta"] * d["NT"] <= 256, d       # register accumulators: 128 fp32 per thread
+        assert d["nstages"] in (2, 3) and d["smem"] <= SMEM_LIMIT, d
         gx, gy, gz = [int(v) for v in d["grid"].split("x")]
         assert gx >= 1 and 1 <= gy <= 65535 and 1 <= gz <= 65535 and d["chunks_per_cta"] >= 1 and d["n_ctas_x"] <= gx, d
 
 
 def test_plan_audit_matches_the_measured_configuration():
-    """The tiling DESIGN.md / profiles/ describe for the benchmark (M4, batch 16): persistent 256-row tiles for down1-3,
-    two CTAs per SM in the middle, batch-folded cluster split-K launches for the deep layers."""
+    """The tiling of the benchmark (M4, batch 16): every conv but the first layer's on the tensor cores, the wide layers split
+    over output channels, one wgrad launch per layer."""
     lines = _audit("baseline_stereo", 16)
     fwd = {d["layer"]: d for d in lines if d["op"] == "conv" and d["pass"] == 0}
-    assert [fwd[i]["kernel"] for i in (1, 2, 3)] == ["persistent"] * 3
-    assert fwd[3]["NPAD"] == 96 and fwd[3]["MT"] == 2 and fwd[3]["tmem"] == 512 and fwd[3]["nteams"] == 3
-    assert fwd[4]["kernel"] == "dense2" and fwd[8]["kernel"] == "fold" and fwd[8]["ksplit"] == 3
-    assert fwd[12]["kernel"] == "fold" and fwd[12]["ksplit"] == 8 and fwd[12]["nsplit"] == 2     # bottleneck: 8 tiles x 8-CTA clusters
+    assert all(d["kernel"] == "wgmma" for d in fwd.values())
+    assert fwd[3]["NPAD"] == 96 and fwd[3]["nsplit"] == 1
+    assert fwd[12]["nsplit"] >= 3 and fwd[12]["NPAD"] <= 128                  # bottleneck: 312 output channels
     assert 0 not in fwd                                                       # the first layer (C_in = 2) is a CUDA-core kernel
-    assert len([d for d in lines if d["op"] == "conv"]) == 60                # the launch list of profiles/: 13 + 13 + 34
+    assert len([d for d in lines if d["op"] == "conv"]) == 60                # 13 forward + 13 dgrad + 34 (split classes)
     assert len({d["layer"] for d in lines if d["op"] == "wgrad"}) == 24
 
 
 def test_round2_planner_decisions_for_the_benchmark():
     """What bench.py times at M4 batch 16 (DESIGN.md 2 / 4.1): pair-merged forward classes for the up blocks that still fill the GPU,
-    the pair-merged dgrad only where the merged width keeps the fused-N MMAs (down1), the output layer riding in the last up
-    block's persistent forward conv - and no forward merge / fused output at batch 1, where those launches do not fill the GPU."""
+    the pair-merged dgrad only where the merged width stays narrow (down1) - and no forward merge at batch 1, where those
+    launches do not fill the GPU."""
     lines = [d for d in _audit("baseline_stereo", 16) if d["op"] == "conv"]
     fwd = {d["layer"]: d for d in lines if d["pass"] == 0}
     dg = [d for d in lines if d["pass"] == 1]
-    assert sorted(l for l, d in fwd.items() if d["pair"]) == [21, 22, 23, 24]            # up8 .. up11
-    assert all(fwd[l]["N"] == 2 * fwd[l]["pair"] for l in (21, 22, 23, 24))
-    assert [(d["layer"], d["N"]) for d in dg if d["pair"]] == [(1, 48)]                    # down1: 2 x 24 columns, fused-N
-    assert [d["layer"] for d in lines if d.get("outfuse")] == [24] and fwd[24]["kernel"] == "persistent"
-    assert sum(1 for d in dg if d["kernel"] == "persistent") >= 6
+    assert sorted(l for l, d in fwd.items() if d["pair"]) == [20, 21, 22, 23, 24]        # up7 .. up11
+    assert all(fwd[l]["N"] == 2 * fwd[l]["pair"] for l in (20, 21, 22, 23, 24))
+    assert [(d["layer"], d["N"]) for d in dg if d["pair"]] == [(1, 48)]                    # down1: 2 x 24 columns
     small = [d for d in _audit("baseline_stereo", 1) if d["op"] == "conv"]
-    assert not any((d["pair"] and d["pass"] == 0) or d.get("outfuse") for d in small)       # (down1's dgrad still has 144 tiles at batch 1)
-    # every model family of BASELINE.json gets the fused output layer at its benchmark batch
-    for preset, batch in (("full", 16), ("full_multi_instrument", 32), ("baseline", 16)):
-        assert any(d.get("outfuse") for d in _audit(preset, batch) if d["op"] == "conv"), preset
+    assert not any(d["pair"] and d["pass"] == 0 for d in small)
 
 
 def test_long_window_mode_plans_and_amortises_the_context():

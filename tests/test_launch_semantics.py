@@ -378,7 +378,7 @@ def run_wgrad_group(mem, G, dW):
 @pytest.mark.parametrize("name,named,ov,batch,nf", FWD_CASES, ids=[c[0] for c in FWD_CASES])
 def test_exported_wgrad_groups_reproduce_the_oracle(name, named, ov, batch, nf, monkeypatch):
     """The weight-gradient groups the engine builds per layer ((class, plane) pairs with up to 8 taps each - what the split pass
-    and the tcgen05 wgrad kernel consume), executed on the host on the activations and pre-activation gradients the exported
+    and the tensor-core wgrad kernel consume), executed on the host on the activations and pre-activation gradients the exported
     forward / dgrad launches produced, must give dL/dW of every convolution; the column sums of each class's gradient view give
     dL/db (fused into the split pass on the device).  Reference: torch autograd through the oracle (UnetAudioSeparator.py:97-125), float64."""
     cfg, eng, mem, _, param_grads, keys, t_in = _host_backward(named, ov, batch, nf, 1, monkeypatch)

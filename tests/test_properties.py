@@ -64,7 +64,7 @@ def test_plan_invariants_for_arbitrary_small_networks(L, f0, nf, learned, contex
     assert eng.workspace_bytes(batch, True) >= eng.workspace_bytes(batch, False) > 0
     assert eng.forward_backward_flops(batch) <= 3.0 * eng.forward_flops(batch) + 1
     for d in eng.plan_audit(batch):                             # whatever runs on tensor cores respects the hardware limits
-        assert d["smem"] <= 220 * 1024 and d["tmem"] <= 512
+        assert d["smem"] <= 200 * 1024
 
 
 names = st.text(alphabet=st.characters(min_codepoint=33, max_codepoint=126), min_size=1, max_size=40)

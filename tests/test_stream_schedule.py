@@ -8,8 +8,8 @@ exact words it reads, writes or atomically accumulates into; tests/hostsim/sched
 streams and events and a shadow memory at 4-byte granularity.  Any pair of conflicting accesses that the events do not order is
 a race the GPU parity tests could only catch by luck.
 
-Covered: the planner's default choices and the GPU-filling kernel variants forced onto mid-size nets (persistent / two-epilogue
-dgrad / pair-merged / fused output epilogue) for the five model families, every A/B switch of the stream structure in its other
+Covered: the planner's default choices and the GPU-filling kernel variants forced onto mid-size nets (pair-merged classes) for
+the five model families, every A/B switch of the stream structure in its other
 position, inference, the bucketed all-reduce on a communication stream (wun/parallel.py) followed by Adam and the NEXT step's
 weight packs - and the checker itself: dropping any single necessary stream wait from a trace must be reported."""
 import os
@@ -50,7 +50,7 @@ def test_the_simulation_library_builds_where_the_tool_chain_exists():
     assert _SIM is not None and os.path.exists(_SIM), _WHY
 
 
-FORCED = {"WUN_PERS_MIN": "0", "WUN_FOLD": "0", "WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}      # as tests/test_gpu_parity.py
+FORCED = {"WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}      # as tests/test_gpu_parity.py
 FAMILIES = [
     ("m4_like_L5", ["baseline_stereo"], dict(num_layers=5), 3, 2000),
     ("m5_like_L4", ["full"], dict(num_layers=4, num_initial_filters=16), 2, 1500),
@@ -76,8 +76,9 @@ def test_forced_gpu_filling_variants_are_race_free_incl_bucketed_allreduce(name,
     meta, ops = schedule.trace("train_dp", named, ov, batch, nf, FORCED)
     stats = assert_race_free(meta, ops)
     ks = kernels(ops)
-    assert "plane_conv_umma_persistent_dg2" in ks and any(k.startswith("plane_conv_umma_persistent_out<") for k in ks), sorted(ks)
-    assert {"split_views_kernel", "wgrad_umma_bulk_kernel", "umma_pack_kernel", "upsample_bwd_kernel"} <= ks
+    assert any(k.startswith("plane_conv_umma_kernel<") and k.endswith("true>") for k in ks), sorted(ks)
+    assert any(k.startswith("wgrad_umma_bulk_kernel<") for k in ks), sorted(ks)
+    assert {"split_views_kernel", "umma_pack_kernel", "upsample_bwd_kernel", "output_fwd_kernel"} <= ks
     assert len(stats["per_stream"]) == 5 and min(stats["per_stream"]) > 0      # caller, packs + wgrad, split passes, helper, comm
     assert stats["joined_into_caller"]          # every forked stream is joined back: the step is capturable as one CUDA graph
     # the launch count the library reports (bench.py's gpu_launches) is what was launched: 2 steps of (step + 2 memsets + 2 Adam)
@@ -89,12 +90,11 @@ def test_forced_gpu_filling_variants_are_race_free_incl_bucketed_allreduce(name,
 def test_default_planner_choices_are_race_free(name, named, ov, batch, nf):
     meta, ops = schedule.trace("train_dp", named, ov, batch, nf)
     assert_race_free(meta, ops)
-    assert "plane_conv_umma_fold" in kernels(ops)                 # what the planner picks for launches that do not fill the GPU
+    assert any(k.startswith("plane_conv_umma_kernel<") for k in kernels(ops))
 
 
 SWITCHES = ["WUN_SPLIT_AHEAD=0", "WUN_SIDE_STREAM=0", "WUN_DGRAD_PAR=0", "WUN_FIRST_TAIL=0", "WUN_BULK_WGRAD=0", "WUN_PACK_EVENTS=0",
-            "WUN_OUT_FUSE=0", "WUN_OUT_FUSE=2", "WUN_FIRST_LAYER=0", "WUN_SPLIT_COLSUM=0", "WUN_DISABLE_UMMA=1", "WUN_UMMA_WGRAD=0",
-            "WUN_EPI2=0", "WUN_PERSISTENT=0"]
+            "WUN_OUT_FUSE=0", "WUN_OUT_FUSE=2", "WUN_FIRST_LAYER=0", "WUN_SPLIT_COLSUM=0", "WUN_DISABLE_UMMA=1", "WUN_UMMA_WGRAD=0"]
 
 
 @pytest.mark.parametrize("switch", SWITCHES)
@@ -187,18 +187,17 @@ BENCHMARK_SIZES = [("baseline_stereo", 16, "train"), ("full", 16, "train"), ("fu
 @pytest.mark.parametrize("preset,batch,scenario", BENCHMARK_SIZES, ids=["%s_b%d" % (p, b) for p, b, _ in BENCHMARK_SIZES])
 def test_launch_geometry_at_the_benchmark_sizes_respects_the_hardware_limits(preset, batch, scenario):
     """The grid, block, dynamic shared memory and cluster width the engine REALLY passes to the runtime for every launch of the
-    configurations bench.py times (full windows; trace only, no shadow memory): within the sm_100 limits, and every launch above
+    configurations bench.py times (full windows; trace only, no shadow memory): within the sm_90 limits, and every launch above
     the 48 KB default opted in to its shared memory with cudaFuncSetAttribute first."""
     import Config
     cfg = Config.build_config([preset], experiment_id=0)["model_config"]
     meta, ops = schedule.trace(scenario, [preset], {}, batch, cfg["num_frames"])
     assert schedule.launch_limit_violations(ops) == []
     geos = [o[4] for o in ops if o[0] == "L" and o[4] is not None]
-    assert max(g[6] for g in geos) > 150 * 1024                       # the big tiles do use most of the 227 KB
-    assert any(g[8] > 1 for g in geos)                               # and the batch-folded kernel its thread-block clusters
-    if scenario == "train":                                          # one CTA per SM for the persistent tile loops
-        pers = [o[4] for o in ops if o[0] == "L" and "plane_conv_umma_persistent" in o[2]]
-        assert pers and all(g[0] <= 148 and g[1] == 1 and g[2] == 1 for g in pers), pers[:3]
+    convs = [o[4] for o in ops if o[0] == "L" and "plane_conv_umma_kernel" in o[2]]
+    assert convs and all(g[3] == 256 and 2 * (g[6] + 1024) <= 228 * 1024 for g in convs), convs[:3]   # two CTAs per SM
+    if scenario == "train":                                          # the wgrad stages use most of the 227 KB
+        assert max(o[4][6] for o in ops if o[0] == "L" and "wgrad_umma_bulk_kernel" in o[2]) > 100 * 1024
 
 
 def test_the_limit_check_notices_an_oversized_launch():

@@ -1,4 +1,4 @@
-"""Per-tensor gradient error of the engine (tcgen05 on / off) vs the fp64 and fp32 oracle on one M4 window."""
+"""Per-tensor gradient error of the engine (tensor cores on / off) vs the fp64 and fp32 oracle on one M4 window."""
 import os, sys, numpy as np, torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO); sys.path.insert(0, os.path.join(REPO, "wave-u-net_b200"))

@@ -1,4 +1,4 @@
-"""Experiment configuration for the B200 Wave-U-Net engine (sacred-free).
+"""Experiment configuration for the Wave-U-Net engine (sacred-free).
 
 Mirrors the *data* the reference's sacred ingredient produces
 (/root/reference/Config.py:6-161): one ``model_config`` dict plus an

@@ -1,4 +1,4 @@
-"""Windowed inference with the B200 engine: drop-in for the tiling half of the reference's Evaluate.py.
+"""Windowed inference with the H100 engine: drop-in for the tiling half of the reference's Evaluate.py.
 
 predict_track() keeps the semantics of /root/reference/Evaluate.py:82-145 exactly -
   mono-mix or channel duplication (:98-102), zero-extension of short inputs (:107-111), (T_in-T_out)//2 context

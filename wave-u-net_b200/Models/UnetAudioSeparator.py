@@ -1,4 +1,4 @@
-"""Drop-in for the reference's Wave-U-Net separator class, backed by the B200 CUDA engine (libwun.so).
+"""Drop-in for the reference's Wave-U-Net separator class, backed by the H100 CUDA engine (libwun.so).
 
 Same class name, constructor argument and method names/arguments as
 /root/reference/Models/UnetAudioSeparator.py:9-144:

@@ -1,4 +1,4 @@
-"""Training entry point of the B200 Wave-U-Net engine - stand-in for the reference's sacred experiment.
+"""Training entry point of the Wave-U-Net engine - stand-in for the reference's sacred experiment.
 
 Keeps the reference's functions and command line (/root/reference/Training.py:24-166, README.md:84-92):
 

@@ -1,4 +1,4 @@
-// engine.cu - C ABI (include/wun.h) of the B200 Wave-U-Net engine: turns the host plan into kernel launches.
+// engine.cu - C ABI (include/wun.h) of the Wave-U-Net engine (H100, sm_90a): turns the host plan into kernel launches.
 //
 // Forward  = get_output             /root/reference/Models/UnetAudioSeparator.py:85-144
 // Backward = what tf.gradients builds for AdamOptimizer.minimize, /root/reference/Training.py:77
@@ -55,7 +55,7 @@ struct WunHandle {
     Plan plan;
     std::vector<OpBackward> bwd_down, bwd_up;
     OpBackward bwd_bottleneck;
-    bool umma_enabled = true;            // tcgen05 path on (WUN_DISABLE_UMMA=1 turns it off, for A/B tests)
+    bool umma_enabled = true;            // tensor-core path on (WUN_DISABLE_UMMA=1 turns it off, for A/B tests)
     bool umma_pass[3] = {true, true, true};   // per pass (fwd, dgrad, wgrad): WUN_UMMA_FWD=0 / WUN_UMMA_DGRAD=0 / WUN_UMMA_WGRAD=0
     size_t arena_bytes = 0;              // scratch for packed bf16 weights (max over launches)
     std::vector<std::string> kernel_used;   // [layer*3 + pass] -> "simt" | "umma" (filled by dry runs)
@@ -75,7 +75,7 @@ struct WunHandle {
     int fork_used = 0;
     bool use_side = true;                // WUN_SIDE_STREAM=0 disables
     bool first_fast = true;              // dedicated first-layer kernels (kernels_first.cu); WUN_FIRST_LAYER=0 = generic path
-    bool bulk_wgrad = true;              // split pass + bulk-copy-fed tcgen05 wgrad; WUN_BULK_WGRAD=0 = converter-fed kernel
+    bool bulk_wgrad = true;              // split pass + bulk-copy-fed tensor-core wgrad; WUN_BULK_WGRAD=0 = converter-fed kernel
     // output layer in the last up block's conv epilogue (kernels_umma.h OutputFuse).  WUN_OUT_FUSE: 0 = separate kernels, 1 (default) =
     // estimates + loss + dL/dpre + the gradient w.r.t. the features fused, the output convs' weight gradient as its own launch on
     // the wgrad stream (off the critical path), 2 = the weight gradient in the epilogue too (measured slower: it serialises
@@ -90,6 +90,8 @@ struct WunHandle {
     int pair_dgrad = 4;                  // pair-merged dgrad classes (launch.h OutView::pairC); WUN_PAIR_DGRAD=0 off, 1 all, 2 down blocks only,
                                          // 3 up blocks only, 4 (default) down blocks whose merged width still takes the fused-N MMAs (2C <= 64)
     size_t split_item_bytes = 0;         // per batch item: largest split arena any layer's wgrad needs (dry run)
+    size_t wg_partial_bytes = 0;         // largest partial-tile scratch of a layer's wgrad (any batch; dry run)
+    size_t out_part_bytes = 0;           // the output layer's per-CTA weight-gradient sums (any batch; dry run)
     cudaStream_t wstream = nullptr;      // stream the wgrad-side launches go to (side or main)
     // split passes run one layer AHEAD of the wgrad kernels, on their own stream, into a double-buffered arena: the split pass is
     // DRAM-bound, the wgrad kernel L2 / tensor bound, so they overlap well (WUN_SPLIT_AHEAD=0: same stream, one arena half)
@@ -289,7 +291,7 @@ static void export_launch(WunHandle* h, const ConvLaunch& L) {
     }
 }
 
-// Every plane convolution goes through here: tcgen05 when the launch is eligible, CUDA cores otherwise.
+// Every plane convolution goes through here: tensor cores (wgmma) when the launch is eligible, CUDA cores otherwise.
 static int launch_conv(WunHandle* h, const ConvLaunch& L) {
     if (h->dry && h->export_launches) export_launch(h, L);
     UmmaChoice ch;
@@ -305,13 +307,7 @@ static int launch_conv(WunHandle* h, const ConvLaunch& L) {
                 long long tiles = 0, mmas = 0; int max_rows = 0, span = 0;
                 for (int q = 0; q < L.ncls; ++q) {
                     const int rows = L.cls[q].m_hi - L.cls[q].m_lo;
-                    int qspan = 0;                              // widest tap span of the class (folded tiling)
-                    for (int ta = L.cls[q].term_begin; ta < L.cls[q].term_end; ++ta)
-                        for (int tb = ta; tb < L.cls[q].term_end && L.terms[tb].plane == L.terms[ta].plane; ++tb)
-                            qspan = std::max(qspan, std::abs(L.terms[tb].d - L.terms[ta].d));
-                    const long long tq = ch.folded
-                        ? (rows > 0 ? ((long long)L.batch * (rows + qspan) + ch.MT * 128 - 1) / (ch.MT * 128) * ch.nsplit : 0)
-                        : (long long)((rows + ch.MT * 128 - 1) / (ch.MT * 128)) * ch.nsplit * L.batch;
+                    const long long tq = (long long)((rows + ch.MT * 128 - 1) / (ch.MT * 128)) * ch.nsplit * L.batch;
                     tiles += tq;
                     max_rows = std::max(max_rows, rows);
                     int t = L.cls[q].term_begin;
@@ -324,15 +320,14 @@ static int launch_conv(WunHandle* h, const ConvLaunch& L) {
                         ksteps += (long long)((L.planes[L.terms[t].plane].C + 15) / 16) * (t1 - t);
                         t = t1;
                     }
-                    mmas += tq * ch.MT * ksteps * (ch.fuse ? 2 : 3);
+                    mmas += tq * ch.MT * ksteps * 3;
                 }
                 char line[512];
-                snprintf(line, sizeof(line), "conv layer=%d pass=%d kernel=%s N=%d NPAD=%d nsplit=%d MT=%d rows_alloc=%d span=%d tmem=%d "
-                         "TB=%d nbs=%d nteams=%d fuse=%d ksplit=%d tiles=%lld mmas=%lld max_rows=%d smem=%zu pack_bytes=%zu pair=%d outfuse=%d epi2=%d",
-                         h->cur_layer, h->cur_pass, ch.folded ? "fold" : (ch.persistent ? "persistent" : (ch.nteams == 4 ? "sparse4" : "dense2")), L.N,
-                         ch.NPAD, ch.nsplit, ch.MT, ch.rows_alloc, span, ch.tmem_cols, ch.TB, ch.nbs, ch.nteams, ch.fuse, ch.ksplit, tiles, mmas,
+                snprintf(line, sizeof(line), "conv layer=%d pass=%d kernel=wgmma N=%d NPAD=%d nsplit=%d MT=%d rows_alloc=%d span=%d "
+                         "TB=%d nbs=%d tiles=%lld mmas=%lld max_rows=%d smem=%zu pack_bytes=%zu pair=%d outfuse=%d",
+                         h->cur_layer, h->cur_pass, L.N, ch.NPAD, ch.nsplit, ch.MT, ch.rows_alloc, span, ch.TB, ch.nbs, tiles, mmas,
                          max_rows, umma_choice_smem_bytes(ch), ch.pack_bytes, L.pairC,
-                         (h->fuse_out && umma_output_fusable(L, ch, h->fuse_out->O)) ? 1 : 0, ch.epi2);
+                         (h->fuse_out && umma_output_fusable(L, ch, h->fuse_out->O)) ? 1 : 0);
                 h->audit->push_back(line);
             }
             return WUN_OK;
@@ -363,7 +358,7 @@ static int launch_conv(WunHandle* h, const ConvLaunch& L) {
             if (fuse) h->out_fused = true;
             for (int i = 0; i < iters && e == cudaSuccess; ++i) e = launch_plane_conv_umma(U, h->stream, fuse);
         }
-        if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tcgen05 conv launch: ") + cudaGetErrorString(e));
+        if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tensor-core conv launch: ") + cudaGetErrorString(e));
         return WUN_OK;
     }
     if (h->phase == 1) return WUN_OK;
@@ -499,7 +494,7 @@ static int conv_forward(WunHandle* h, const ConvOp& op, int layer_index) {
         const bool ok0 = umma_plan_from_conv(L, &ch0), ok1 = umma_plan_from_conv(M, &ch);
         if (ok0 && ok1) {
             h->pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
-            if (!ch0.folded && pair_worthwhile(h, M, ch)) L = M;
+            if (pair_worthwhile(h, M, ch)) L = M;
         }
     }
     const int rc = launch_conv(h, L);
@@ -593,11 +588,11 @@ static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int 
                              (h->pair_dgrad == 4 && op.planes.size() == 2 && 2 * S.N <= 64);
         h->pack_floor = 0;
         if (h->pair_dgrad != 0 && S.ncls == 2 && h->umma_enabled && h->umma_pass[1] && merge_pair(S, &M)) {
-            UmmaChoice ch0, ch;       // the deep, few-row layers keep the batch-folded kernel (it has no pair-merged epilogue)
+            UmmaChoice ch0, ch;
             const bool ok0 = umma_plan_from_conv(S, &ch0), ok1 = umma_plan_from_conv(M, &ch);
             if (ok0 && ok1) {
                 h->pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
-                if (pair_on && !ch0.folded && pair_worthwhile(h, M, ch)) S = M;
+                if (pair_on && pair_worthwhile(h, M, ch)) S = M;
             }
         }
         // second (third ...) launch of this dgrad: on the helper stream, forked from the point the first launch was enqueued at
@@ -633,8 +628,11 @@ static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int 
 }
 
 static int64_t split_arena_half_bytes(const WunHandle* h, int64_t batch) {
-    return (int64_t)h->split_item_bytes * batch + 256 * (kSplitMaxJobs + 1);
+    return (int64_t)h->split_item_bytes * batch + 256 * (kSplitMaxJobs + 1) + (int64_t)h->wg_partial_bytes + 256;
 }
+
+static int64_t split_arena_bytes(const WunHandle* h, int64_t batch);
+static float* out_part_ptr(const WunHandle* h);
 
 static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale, int layer_index) {
     const Plan& P = h->plan;
@@ -643,8 +641,10 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
         FirstWgrad FW;
         if (first_layer_desc(h, op, &FW.L)) {          // one launch: dW and db of both classes
             if (h->phase == 1) return WUN_OK;
-            ++h->launches;
+            h->launches += 2;                             // per-CTA sums + their fixed-order total
             if (!h->dry) {
+                FW.part = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum +
+                                                   split_arena_bytes(h, h->batch));
                 FW.L.dec = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor]));
                 FW.L.odd = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor]));
                 FW.dW = grads + P.params[op.w_param].offset;
@@ -735,9 +735,9 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
             const WgGroup& G = U.grp[g];
             char line[512];
             snprintf(line, sizeof(line), "wgrad layer=%d group=%d Cp=%d Cg=%d swap=%d NT=%d mtiles=%d ntiles=%d ntaps=%d taps_per_cta=%d "
-                     "tapsets=%d tmem=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu",
+                     "tapsets=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu",
                      h->cur_layer, g, G.P.C, G.G.C, G.swap, G.NT, G.n_mtiles, G.n_ntiles, G.ntaps, G.taps_per_cta, G.n_tapsets,
-                     G.tmem_cols, G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages, umma_wgrad_smem_bytes(U));
+                     G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages, umma_wgrad_smem_bytes(U));
             h->audit->push_back(line);
         }
     }
@@ -761,7 +761,13 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
         int max_rows_g = 0;
         for (const auto& dp : class_dpre) max_rows_g = std::max(max_rows_g, dp.r_hi - dp.r_lo);
         const bool fused_colsum = colsum_mode == 1 || (colsum_mode == 2 && max_rows_g <= 4096);
-        if (bulk) { ++h->launches; if (h->dry) h->split_item_bytes = std::max(h->split_item_bytes, split_need); }
+        if (bulk) {      // + the split pass and the fixed-order reduction of the partial tiles / column sums
+            h->launches += 2;
+            if (h->dry) {
+                h->split_item_bytes = std::max(h->split_item_bytes, split_need);
+                h->wg_partial_bytes = std::max(h->wg_partial_bytes, umma_wgrad_partial_bytes(U));
+            }
+        }
         if (!bulk || !fused_colsum) colsum_launches();
         if (!h->dry) {
             cudaError_t e;
@@ -771,7 +777,8 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
                 if (ahead && (h->wg_index & 1)) arena += split_arena_half_bytes(h, h->batch);
                 arena += (256 - (reinterpret_cast<uintptr_t>(arena) & 255)) & 255;
                 WgSplit S; SplitJobs J;
-                umma_plan_wgrad_split(U, h->batch, arena, &S, &J);
+                const size_t used = umma_plan_wgrad_split(U, h->batch, arena, &S, &J);
+                U.partial = reinterpret_cast<float*>(arena + (used + 255) / 256 * 256);     // behind the split arrays of the same half
                 // the class-gradient views among the jobs also produce the bias gradient (their column sums)
                 J.colsum_scale = scale;
                 size_t matched = 0;
@@ -793,15 +800,17 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
                     if (e == cudaSuccess) e = cudaEventRecord(h->split_done[k], h->split_stream);
                     if (e == cudaSuccess) e = cudaStreamWaitEvent(h->wstream, h->split_done[k], 0);
                     if (e == cudaSuccess) e = launch_wgrad_umma_bulk(U, S, h->wstream);
+                    if (e == cudaSuccess) e = launch_wgrad_reduce(U, J, h->wstream);
                     if (e == cudaSuccess) e = cudaEventRecord(h->wg_done[k], h->wstream);
                 } else {
                     e = launch_split_views(J, h->wstream);      // same stream as the wgrad: the arena is reused layer after layer
                     if (e == cudaSuccess) e = launch_wgrad_umma_bulk(U, S, h->wstream);
+                    if (e == cudaSuccess) e = launch_wgrad_reduce(U, J, h->wstream);
                 }
             } else {
                 e = launch_wgrad_umma(U, h->wstream);
             }
-            if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tcgen05 wgrad launch: ") + cudaGetErrorString(e));
+            if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tensor-core wgrad launch: ") + cudaGetErrorString(e));
         }
         return WUN_OK;
     }
@@ -948,10 +957,11 @@ static int run_backward(WunHandle* h, const float* targets, float* grads, float 
     // fused forward (run_forward): dL/dpre and the feature gradient already exist; only the output convs' weight gradient is left
     // (mode 1), and it goes to the wgrad stream right after the first fork below
     const bool out_wgrad_late = h->out_fused && h->out_fuse_mode != 2;
-    if (h->phase != 1 && !h->out_fused) h->launches += 2;
-    if (h->phase != 1 && out_wgrad_late) h->launches += 1;
+    if (h->dry) h->out_part_bytes = std::max(h->out_part_bytes, output_wgrad_partial_bytes(O));
+    if (h->phase != 1 && !h->out_fused) h->launches += 3;
+    if (h->phase != 1 && out_wgrad_late) h->launches += 2;
     if (!h->dry && h->phase != 1 && !h->out_fused) {
-        launch_output_wgrad(O, grads, scale, h->stream);
+        launch_output_wgrad(O, grads, out_part_ptr(h), scale, h->stream);
         launch_output_dgrad(O, const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat])), h->stream);
     }
     if (h->phase != 1) h->bucket_next = 0;
@@ -960,7 +970,7 @@ static int run_backward(WunHandle* h, const float* targets, float* grads, float 
     for (int i = L - 1; i >= 0; --i) {
         const ConvOp& op = P.up[i];
         if ((rc = fork_side(h)) != WUN_OK) return rc;
-        if (i == L - 1 && out_wgrad_late && !h->dry && h->phase != 1) launch_output_wgrad(O, grads, scale, h->wstream);
+        if (i == L - 1 && out_wgrad_late && !h->dry && h->phase != 1) launch_output_wgrad(O, grads, out_part_ptr(h), scale, h->wstream);
         if ((rc = mark_grads_ready(h, ready_from, h->wstream)) != WUN_OK) return rc;
         ready_from = std::min(ready_from, op_first_offset(P, op, &P.ups[i]));
         if ((rc = conv_wgrad(h, op, grads, scale, L + 1 + i)) != WUN_OK) return rc;
@@ -1011,7 +1021,16 @@ static int check_device() {
 
 // bytes of the split arena behind the weight packs (bulk-fed wgrad only; per-item size from the dry run at create time)
 static int64_t split_arena_bytes(const WunHandle* h, int64_t batch) {
-    return (h && h->bulk_wgrad && h->split_item_bytes) ? 2 * ((int64_t)h->split_item_bytes * batch + 256 * (kSplitMaxJobs + 1)) : 0;     // two halves
+    return (h && h->bulk_wgrad && h->split_item_bytes) ? 2 * split_arena_half_bytes(h, batch) : 0;     // two halves
+}
+// training scratch behind the activations, the weight packs and the split arena: the first layer's per-CTA gradient sums
+static int64_t train_scratch_bytes(const WunHandle* h, int64_t batch) {
+    return split_arena_bytes(h, batch) + (int64_t)first_wgrad_partial_bytes((int)batch) + (int64_t)h->out_part_bytes;
+}
+// the output layer's per-CTA weight-gradient sums, behind the first layer's
+static float* out_part_ptr(const WunHandle* h) {
+    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum + split_arena_bytes(h, h->batch) +
+                                    first_wgrad_partial_bytes(h->batch));
 }
 
 static int begin_call(WunHandle* h, const float* params, const float* mix, int64_t batch, bool training, void* ws,
@@ -1026,7 +1045,7 @@ static int begin_call(WunHandle* h, const float* params, const float* mix, int64
     if (dry) return WUN_OK;
     { int rc0 = check_device(); if (rc0 != WUN_OK) return rc0; }
     if (!params || !mix || !ws) return set_err(WUN_E_INVALID, "null device pointer");
-    if (ws_bytes < h->lay.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + (training ? split_arena_bytes(h, batch) : 0))
+    if (ws_bytes < h->lay.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + (training ? train_scratch_bytes(h, batch) : 0))
         return set_err(WUN_E_INVALID, "workspace too small");
     if (reinterpret_cast<uintptr_t>(ws) % 256 != 0) return set_err(WUN_E_INVALID, "workspace must be 256-byte aligned");
     h->params = params; h->mix = mix; h->ws = (float*)ws; h->stream = (cudaStream_t)stream;
@@ -1039,7 +1058,7 @@ static int begin_call(WunHandle* h, const float* params, const float* mix, int64
 extern "C" {
 
 const char* wun_last_error(void) { return g_err.c_str(); }
-const char* wun_version(void) { return "wun-b200 0.1 (sm_100a)"; }
+const char* wun_version(void) { return "wun-b200 0.2 (sm_90a)"; }
 
 int wun_get_padding(const WunConfig* cfg, int64_t num_frames, int64_t* t_in, int64_t* t_out) {
     if (!cfg || !t_in || !t_out) return set_err(WUN_E_INVALID, "null argument");
@@ -1061,8 +1080,7 @@ int wun_create_for_input(const WunConfig* cfg, int64_t input_frames, WunHandle**
     { const char* names[3] = {"WUN_UMMA_FWD", "WUN_UMMA_DGRAD", "WUN_UMMA_WGRAD"};
       for (int i = 0; i < 3; ++i) { const char* v = getenv(names[i]); h->umma_pass[i] = !(v && v[0] == '0'); } }
     { const char* v = getenv("WUN_SIDE_STREAM"); h->use_side = !(v && v[0] == '0'); }
-    // default ON since round 2 (validated on B200: probes + the GPU parity suite with each switch; step 8.51 -> 7.39 ms);
-    // "=0" selects the round-1 path for A/B runs
+    // "=0" selects the generic path for A/B runs
     { const char* v = getenv("WUN_FIRST_LAYER"); h->first_fast = !(v && v[0] == '0'); }
     { const char* v = getenv("WUN_PACK_EVENTS"); h->pack_events_on = !(v && v[0] == '0'); }
     { const char* v = getenv("WUN_BULK_WGRAD"); h->bulk_wgrad = !(v && v[0] == '0'); }
@@ -1073,7 +1091,7 @@ int wun_create_for_input(const WunConfig* cfg, int64_t input_frames, WunHandle**
     { const char* v = getenv("WUN_OUT_FUSE"); h->out_fuse_mode = v ? atoi(v) : 1; }
     { const char* v = getenv("WUN_PAIR_FWD"); h->pair_fwd = !(v && v[0] == '0'); }
     h->kernel_used.assign((size_t)(2 * h->plan.cfg.num_layers + 1) * 3, "simt");
-    // dry run: which kernel each layer uses and how much pack scratch the tcgen05 launches need
+    // dry run: which kernel each layer uses and how much pack scratch the tensor-core launches need
     wun_launches_forward_backward(h);
     *out = h;
     return WUN_OK;
@@ -1122,7 +1140,7 @@ int wun_param_table(const WunHandle* h, WunParamInfo* out, int64_t capacity) {
 int64_t wun_workspace_bytes(const WunHandle* h, int64_t batch, int training) {
     if (!h || batch < 1) return -1;
     Layout l = make_layout(h->plan, batch, training != 0);
-    return l.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + 256 + (training ? split_arena_bytes(h, batch) : 0);
+    return l.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + 256 + (training ? train_scratch_bytes(h, batch) : 0);
 }
 
 double wun_forward_flops(const WunHandle* h, int64_t batch) { return h ? h->plan.fwd_flops_per_item * batch : 0; }

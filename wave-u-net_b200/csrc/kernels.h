@@ -61,17 +61,23 @@ struct FirstWgrad {
     float* db;                    // [N] or null
     float scale;
     int rows_per_cta;             // class rows one CTA reduces (multiple of 128; set by the launcher)
+    int grid_x;                   // row blocks per (item, class) (set by the launcher)
+    float* part;                  // per-CTA sums [class][item][row block][k*C*N + N], added up in a fixed order by a second kernel
 };
 
 void launch_plane_conv_simt(const ConvLaunch& L, cudaStream_t stream);
 bool first_layer_supported(int C, int N, int k);
 void launch_first_fwd(const FirstLayer& L, int C, int N, cudaStream_t stream);
 void launch_first_wgrad(FirstWgrad P, int C, int N, cudaStream_t stream);
+// bytes of FirstWgrad::part at `batch` (any supported C, N, k)
+size_t first_wgrad_partial_bytes(int batch);
 void launch_plane_wgrad_simt(WgradLaunch L, cudaStream_t stream);
 void launch_colsum(const PlaneView& V, int batch, float scale, float* out, cudaStream_t stream);
 void launch_output_fwd(const OutputLaunch& L, cudaStream_t stream);
 void launch_output_dgrad(const OutputLaunch& L, float* gfeat, cudaStream_t stream);
-void launch_output_wgrad(const OutputLaunch& L, float* grads, float scale, cudaStream_t stream);
+// part: the per-CTA sums (output_wgrad_partial_bytes), added into grads in a fixed order by a second kernel
+void launch_output_wgrad(const OutputLaunch& L, float* grads, float* part, float scale, cudaStream_t stream);
+size_t output_wgrad_partial_bytes(const OutputLaunch& L);
 void launch_upsample_bwd(UpsampleBwdLaunch L, cudaStream_t stream);
 void launch_sigmoid(const float* x, float* y, int n, cudaStream_t stream);
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, float lr_t, float b1, float b2,

@@ -102,7 +102,7 @@ cudaError_t launch_feed_batch(const float* pool, long long total_frames, const l
     F.seed = seed; F.step_state = step_state; F.mix_out = mix_out; F.targets_out = targets_out; F.chosen = chosen;
     const long long n_in = (long long)T_in * C;
     int bx = (int)((n_in + 255) / 256);
-    const int cap = (148 * 8 + batch - 1) / batch;                         // ~8 CTAs per SM over the whole batch
+    const int cap = (132 * 8 + batch - 1) / batch;                         // ~8 CTAs per SM over the whole batch
     if (bx > cap) bx = cap;
     if (bx < 1) bx = 1;
     feed_batch_kernel<<<dim3(bx, batch), 256, 0, stream>>>(F);

@@ -1,7 +1,6 @@
 // kernels_first.cu - dedicated CUDA-core kernels for the first down block (C_in = 1 | 2 waveform channels;
 // UnetAudioSeparator.py:97-100 with i = 0): forward and weight (+ bias) gradient.  Memory-shaped work (AI 13 FLOP/B) that
-// stays off the tensor cores; the generic plane kernels cost 6 % of the M4 step on it.  Default since round 2
-// (tools/first_layer_probe on B200, M4 B=16: forward 202 -> 71 us, weight + bias gradient 446 -> 220 us); WUN_FIRST_LAYER=0
+// stays off the tensor cores and is cheaper in these kernels than in the generic plane kernels; WUN_FIRST_LAYER=0
 // selects the generic plane kernels.
 //   first_fwd_kernel   thread = 2 output rows x all N filters in registers; x staged de-interleaved by parity so that the
 //                      stride-2 row reads are conflict-free; weights read as warp-broadcast float4 from shared memory
@@ -154,24 +153,51 @@ __global__ void __launch_bounds__(256) first_wgrad_kernel(const __grid_constant_
             }
         }
     }
-    __syncthreads();
-    if (active) {
+    // the 16 groups add their sums in group order (the threads of one group own distinct entries): the same bits on every run
+    for (int g = 0; g < 16; ++g) {
+        __syncthreads();
+        if (active && grp == g) {
 #pragma unroll
-        for (int u = 0; u < XT; ++u) {
-            const int jc = XT * xt + u;                         // = j*C + c
-            if (jc < XC) {
+            for (int u = 0; u < XT; ++u) {
+                const int jc = XT * xt + u;                     // = j*C + c
+                if (jc < XC) {
 #pragma unroll
-                for (int v = 0; v < NTL; ++v) atomicAdd(&red[jc * N + NTL * ntile + v], acc[u][v]);
+                    for (int v = 0; v < NTL; ++v) red[jc * N + NTL * ntile + v] += acc[u][v];
+                }
             }
-        }
-        if (xt == 0) {
+            if (xt == 0) {
 #pragma unroll
-            for (int v = 0; v < NTL; ++v) atomicAdd(&red[XC * N + NTL * ntile + v], accb[v]);
+                for (int v = 0; v < NTL; ++v) red[XC * N + NTL * ntile + v] += accb[v];
+            }
         }
     }
     __syncthreads();
-    for (int i = tid; i < XC * N; i += 256) atomicAdd(P.dW + i, red[i] * P.scale);
-    if (P.db) for (int i = tid; i < N; i += 256) atomicAdd(P.db + i, red[XC * N + i] * P.scale);
+    float* part = P.part + ((size_t)(q * gridDim.y + b) * gridDim.x + blockIdx.x) * (XC * N + N);
+    for (int i = tid; i < XC * N + N; i += 256) part[i] = red[i];
+}
+
+// dW / db = scale * the CTAs' sums of first_wgrad_kernel, added in (class, item, row block) order
+__global__ void __launch_bounds__(256) first_wgrad_sum_kernel(const __grid_constant__ FirstWgrad P, int C, int N) {
+    const FirstLayer& L = P.L;
+    const int len = L.k * C * N + N;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < len; i += gridDim.x * blockDim.x) {
+        float s = 0.f;
+        for (int q = 0; q < 2; ++q) {
+            const int m_lo = q == 0 ? 0 : L.mo_lo, m_hi = q == 0 ? L.Td : L.mo_hi;
+            for (int b = 0; b < L.batch; ++b)
+                for (int x = 0; x < P.grid_x && m_lo + x * P.rows_per_cta < m_hi; ++x)     // (CTAs without rows wrote nothing)
+                    s += P.part[((size_t)(q * L.batch + b) * P.grid_x + x) * len + i];
+        }
+        if (i < len - N) P.dW[i] += s * P.scale;
+        else if (P.db) P.db[i - (len - N)] += s * P.scale;
+    }
+}
+
+constexpr int kFirstCtas = 132 * 4;      // ~4 CTAs per SM
+
+size_t first_wgrad_partial_bytes(int batch) {
+    // launch_first_wgrad: rows_per_cta >= rows * batch / kFirstCtas, so <= kFirstCtas / batch + 1 row blocks per (item, class)
+    return (size_t)2 * (kFirstCtas + batch) * (16 * 2 * 24 + 24) * sizeof(float) + 256;
 }
 
 
@@ -193,15 +219,17 @@ void launch_first_fwd(const FirstLayer& L, int C, int N, cudaStream_t stream) {
 void launch_first_wgrad(FirstWgrad P, int C, int N, cudaStream_t stream) {
     const long long rows = max(P.L.Td, P.L.mo_hi - P.L.mo_lo);
     if (rows <= 0 || P.L.batch <= 0) return;
-    long long per = (rows * P.L.batch + 148 * 4 - 1) / (148 * 4);           // ~4 CTAs per SM
+    long long per = (rows * P.L.batch + kFirstCtas - 1) / kFirstCtas;
     per = (per + 127) / 128 * 128;
     if (per > rows) per = (rows + 127) / 128 * 128;
     P.rows_per_cta = (int)per;
-    dim3 grid((unsigned)((rows + per - 1) / per), P.L.batch, 2);
+    P.grid_x = (int)((rows + per - 1) / per);
+    dim3 grid((unsigned)P.grid_x, P.L.batch, 2);
     if (C == 2 && N == 24) first_wgrad_kernel<2, 24><<<grid, 256, 0, stream>>>(P);
     else if (C == 1 && N == 24) first_wgrad_kernel<1, 24><<<grid, 256, 0, stream>>>(P);
     else if (C == 2 && N == 16) first_wgrad_kernel<2, 16><<<grid, 256, 0, stream>>>(P);
     else if (C == 1 && N == 16) first_wgrad_kernel<1, 16><<<grid, 256, 0, stream>>>(P);
+    first_wgrad_sum_kernel<<<(P.L.k * C * N + N + 255) / 256, 256, 0, stream>>>(P, C, N);
 }
 
 }  // namespace wun

@@ -2,7 +2,7 @@
 //
 // These are the exact-fp32 kernels: they run every layer shape the reference allows (any filter size,
 // any channel count, 'same' or 'valid' padding) and are the path for the memory-bound / irregular
-// layers (down0 with C_in = 1|2, the 1x1 output layer, tiny test nets).  The tensor-core (tcgen05)
+// layers (down0 with C_in = 1|2, the 1x1 output layer, tiny test nets).  The tensor-core (wgmma)
 // kernels in kernels_umma.cu take over the regular, compute-bound layers.
 //
 // Reference semantics implemented here (file:line into /root/reference):
@@ -322,7 +322,7 @@ void launch_plane_wgrad_simt(WgradLaunch L, cudaStream_t stream) {
     const int rows = L.m_hi - L.m_lo;
     if (rows <= 0 || L.nterms <= 0) return;
     if (L.plane.C <= 4 && L.N <= 64 && L.nterms * L.plane.C * ((L.N + 3) / 4) <= 512) {
-        long long per = ((long long)rows * L.batch + 148 * 6 - 1) / (148 * 6);
+        long long per = ((long long)rows * L.batch + 132 * 6 - 1) / (132 * 6);
         per = ((per + 127) / 128) * 128;
         if (per > rows) per = ((rows + 127) / 128) * 128;
         L.rows_per_cta = (int)per;
@@ -332,7 +332,7 @@ void launch_plane_wgrad_simt(WgradLaunch L, cudaStream_t stream) {
     }
     const int tiles = ((L.plane.C + 15) / 16) * ((L.N + 63) / 64);
     // aim at ~8 CTAs per SM over the whole launch, at least 32 rows per CTA
-    long long target = 148LL * 8;
+    long long target = 132LL * 8;
     long long per = ((long long)rows * L.batch * tiles + target - 1) / target;
     per = ((per + 31) / 32) * 32;
     if (per < 32) per = 32;
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(PlaneView V, int batch, int
 void launch_colsum(const PlaneView& V, int batch, float scale, float* out, cudaStream_t stream) {
     const int rows = V.r_hi - V.r_lo;
     if (rows <= 0) return;
-    long long per = ((long long)rows * batch + 148 * 4 - 1) / (148 * 4);
+    long long per = ((long long)rows * batch + 132 * 4 - 1) / (132 * 4);
     if (per < 64) per = 64;
     if (per > rows) per = rows;
     const int chunks = (rows + (int)per - 1) / (int)per;
@@ -521,14 +521,17 @@ void launch_output_dgrad(const OutputLaunch& L, float* gfeat, cudaStream_t strea
     const long long total = (long long)L.batch * L.Tf * L.F;
     const size_t smem = (size_t)(L.nconv * L.ofs * L.F * L.C) * sizeof(float);
     int blocks = (int)((total + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     output_dgrad_kernel<<<blocks, 256, smem, stream>>>(L, gfeat);
 }
 
+constexpr int kOutWgradCtas = 132 * 4;     // row chunks of the output-layer weight gradient (~4 CTAs per SM)
+
 // dW[conv][j][c][oc] += scale * sum_{b,t} in[b, t+j-pad, c] * dpre[b,t,conv*C+oc];  db likewise.
-//   block = 8 row lanes x 32 channel lanes; grid.x = row chunks, grid.y = tap j
-__global__ void __launch_bounds__(256) output_wgrad_kernel(const __grid_constant__ OutputLaunch L,
-                                                            float* __restrict__ grads, float scale,
+//   block = 8 row lanes x 32 channel lanes; grid.x = row chunks, grid.y = tap j.  Every CTA stores its sums at
+//   part[(tap * gridDim.x + chunk) * (Cin + 1) * ncol ...]; output_wgrad_sum_kernel adds them in chunk order (the same bits on
+//   every run, unlike float atomics from the CTAs)
+__global__ void __launch_bounds__(256) output_wgrad_kernel(const __grid_constant__ OutputLaunch L, float* __restrict__ part,
                                                             int rows_per_cta) {
     __shared__ float red[8][32];
     const int lane = threadIdx.x % 32, rl = threadIdx.x / 32;
@@ -556,21 +559,40 @@ __global__ void __launch_bounds__(256) output_wgrad_kernel(const __grid_constant
             if (rl == 0 && c <= Cin && (c < Cin || j == 0)) {
                 float tot = 0.f;
                 for (int i = 0; i < 8; ++i) tot += red[i][lane];
-                const int conv = q / L.C, oc = q % L.C;
-                if (c < Cin) atomicAdd(grads + L.w_off[conv] + ((long long)j * Cin + c) * L.C + oc, tot * scale);
-                else atomicAdd(grads + L.b_off[conv] + oc, tot * scale);
+                part[((size_t)j * gridDim.x + blockIdx.x) * (Cin + 1) * ncol + (size_t)c * ncol + q] = tot;
             }
             __syncthreads();
         }
     }
 }
 
-void launch_output_wgrad(const OutputLaunch& L, float* grads, float scale, cudaStream_t stream) {
+// grads of the output convs = scale * the sums of output_wgrad_kernel's CTAs, added in chunk order
+__global__ void __launch_bounds__(256) output_wgrad_sum_kernel(const __grid_constant__ OutputLaunch L, const float* __restrict__ part,
+                                                                int nx, float* __restrict__ grads, float scale) {
+    const int Cin = L.C + L.F, ncol = L.nconv * L.C, per_tap = (Cin + 1) * ncol;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < L.ofs * per_tap; i += gridDim.x * blockDim.x) {
+        const int j = i / per_tap, c = (i % per_tap) / ncol, q = i % ncol;
+        if (c == Cin && j != 0) continue;                       // the bias "channel" exists for tap 0 only
+        float s = 0.f;
+        for (int x = 0; x < nx; ++x) s += part[((size_t)j * nx + x) * per_tap + (size_t)c * ncol + q];
+        const int conv = q / L.C, oc = q % L.C;
+        if (c < Cin) grads[L.w_off[conv] + ((long long)j * Cin + c) * L.C + oc] += s * scale;
+        else grads[L.b_off[conv] + oc] += s * scale;
+    }
+}
+
+size_t output_wgrad_partial_bytes(const OutputLaunch& L) {
+    return (size_t)(kOutWgradCtas + 1) * L.ofs * (L.C + L.F + 1) * L.nconv * L.C * sizeof(float) + 256;
+}
+
+void launch_output_wgrad(const OutputLaunch& L, float* grads, float* part, float scale, cudaStream_t stream) {
     const long long total = (long long)L.batch * L.T_out;
-    long long per = (total + 148 * 4 - 1) / (148 * 4);
+    long long per = (total + kOutWgradCtas - 1) / kOutWgradCtas;
     if (per < 64) per = 64;
-    dim3 grid((unsigned)((total + per - 1) / per), L.ofs);
-    output_wgrad_kernel<<<grid, 256, 0, stream>>>(L, grads, scale, (int)per);
+    const int nx = (int)((total + per - 1) / per);
+    output_wgrad_kernel<<<dim3(nx, L.ofs), 256, 0, stream>>>(L, part, (int)per);
+    const int len = L.ofs * (L.C + L.F + 1) * L.nconv * L.C;
+    output_wgrad_sum_kernel<<<(len + 255) / 256, 256, 0, stream>>>(L, part, nx, grads, scale);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -618,7 +640,7 @@ __global__ void __launch_bounds__(256) upsample_bwd_kernel(const __grid_constant
 }
 
 void launch_upsample_bwd(UpsampleBwdLaunch L, cudaStream_t stream) {
-    long long per = ((long long)L.N * L.batch + 148 * 4 - 1) / (148 * 4);
+    long long per = ((long long)L.N * L.batch + 132 * 4 - 1) / (132 * 4);
     if (per < 32) per = 32;
     if (per > L.N) per = L.N;
     L.rows_per_cta = (int)per;
@@ -682,7 +704,7 @@ __global__ void adam_advance_kernel(float* state, float b1, float b2) {
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, float lr_t, float b1, float b2,
                  float eps, float* state, cudaStream_t stream) {
     long long blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     adam_kernel<<<(unsigned)blocks, 256, 0, stream>>>(p, g, m, v, n, lr_t, b1, b2, eps, state);
     if (state) adam_advance_kernel<<<1, 1, 0, stream>>>(state, b1, b2);
@@ -707,7 +729,7 @@ void launch_gather_windows(const float* padded, long long n_padded, const long l
                            int T_in, int C, float* out, cudaStream_t stream) {
     long long total = (long long)T_in * C * n_windows;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) return;
     gather_windows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(padded, n_padded, starts, n_windows, T_in, C, out);
 }
@@ -733,7 +755,7 @@ void launch_scatter_windows(const float* outs, const long long* starts, int n_wi
                             int C, float* preds, long long n_frames, cudaStream_t stream) {
     long long total = (long long)T_out * C * n_windows * n_sources;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) return;
     scatter_windows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(outs, starts, n_windows, n_sources, T_out, C,
                                                                 preds, n_frames);

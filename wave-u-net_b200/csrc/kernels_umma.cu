@@ -1,36 +1,31 @@
-// kernels_umma.cu - tcgen05 (5th-gen tensor core) plane convolution for sm_100a.
+// kernels_umma.cu - tensor-core plane convolution and weight gradient for sm_90a (Hopper wgmma).
 //
 // One kernel serves the forward conv blocks and their dgrads (both are "plane convolutions", launch.h):
 //     out_cls[b, m, n] = epi( sum_terms  plane[b, m + d, :] . W_term[:, n] )
-// mapped onto tcgen05.mma as a shifted-tap implicit GEMM:
-//   * A operand: the CTA stages a SLAB of input rows once per 16-channel chunk in shared memory, as
-//     bf16 "channel-atom planes"  [hi|lo][atom(8 ch)][row][16 B]  (K-major, SWIZZLE_NONE canonical layout:
-//     8 rows x 16 B core matrices, SBO = 128 B between 8-row groups, LBO = atom-plane stride between the two
-//     K atoms of one MMA).  A conv tap is then just a descriptor START-ADDRESS shift of d*16 B - the slab is
-//     read by up to 8 taps x MT row tiles without ever being re-loaded or re-converted.  Decimation
-//     ([:, ::2, :], UnetAudioSeparator.py:100), the skip crop (:122), zero padding and the linear / learned
-//     upsampling (:109-118, InterpolationLayer.py:19-39) all happen in the fp32 -> bf16 converter warps that
-//     fill the slab, so none of those tensors ever exists in HBM.
-//   * fp32-level accuracy: every fp32 operand x is split x = hi + lo (two bf16), and each K step issues
-//     three MMAs  hi*hi + lo*hi + hi*lo  into the same fp32 TMEM accumulator (error ~2^-17 per operand;
-//     measured 5e-6 end to end vs the 1e-4 parity bar; single-pass bf16/tf32 fail it - BASELINE.md section 6).
-//   * B operand (weights): pre-packed once per optimizer step into the exact K-step streaming order, hi/lo
-//     bf16, core-matrix layout; streamed with cp.async.bulk (UBLKCP) through an mbarrier ring.
-//   * accumulators: MT row tiles x NPAD fp32 columns in TMEM; epilogue tcgen05.ld -> bias/LeakyReLU (fwd)
-//     or LeakyReLU-slope / accumulate (dgrad) -> a shared-memory staging tile -> coalesced global stores.
-// Kernels in this file (DESIGN.md section 4):
-//   plane_conv_umma_kernel<NTEAMS, DG>       one 128/256-row tile per CTA; 2 CTAs per SM (NTEAMS = 2) or one with 4 converter teams;
-//                                            both converter teams share the epilogue
-//   plane_conv_umma_persistent<PT, DG>       one CTA per SM loops over tiles, double-buffered TMEM accumulators, dedicated epilogue warps;
-//   plane_conv_umma_persistent_dg2           its dgrad form with two epilogue warp groups; plane_conv_umma_persistent_out<NCOL>: its
-//                                            forward form with the output layer + loss + dL/dpre + feature gradient in the epilogue
-//   plane_conv_umma_fold                     batch-folded row tiles + split-K over a thread-block cluster (deep, few-row layers)
-//   split_views_kernel, wgrad_umma_bulk_kernel   hi/lo split arrays of a layer's wgrad operands (+ bias column sums) and the
-//                                            bulk-copy-fed tcgen05 wgrad;  wgrad_umma_kernel<CW>: the converter-fed form (A/B switch)
-//   umma_pack_kernel                         fp32 weights -> hi/lo bf16 blocks in K-step streaming order (pair-merged classes: two taps
-//                                            side by side per row shift)
-// Warp roles of the conv kernels: converter teams of 4 warps (slab fill), one warp = TMEM alloc + single-thread MMA issue (elect.sync),
-// one warp = weight loader (cp.async.bulk through an mbarrier ring), epilogue warps (TMEM lane quarter = warp & 3).
+// mapped onto wgmma as a shifted-tap implicit GEMM:
+//   * A operand: the CTA stages a SLAB of input rows once per 16-channel chunk in shared memory, as bf16
+//     "channel-atom planes"  [hi a0|hi a1|lo a0|lo a1][row][16 B]  (K-major, no-swizzle canonical layout: 8 rows x 16 B
+//     core matrices, SBO = 128 B between 8-row groups, LBO = atom-plane stride between the two K atoms of one k16 MMA).
+//     A conv tap is then just a descriptor START-ADDRESS shift of d*16 B - the slab is read by every tap without being
+//     re-loaded or re-converted.  Decimation ([:, ::2, :], UnetAudioSeparator.py:100), the skip crop (:122), zero padding
+//     and the linear / learned upsampling (:109-118, InterpolationLayer.py:19-39) all happen in the fp32 -> bf16
+//     conversion that fills the slab, so none of those tensors ever exists in HBM.
+//   * fp32-level accuracy: every fp32 operand x is split x = hi + lo (two bf16), and each K step issues three MMAs
+//     lo*hi + hi*lo + hi*hi into the same fp32 accumulator (error ~2^-17 per operand; single-pass bf16 / tf32 miss the
+//     1e-4 parity bar - BASELINE.md section 6).
+//   * B operand (weights): pre-packed once per optimizer step into the exact K-step streaming order, hi/lo bf16, core-matrix
+//     layout (umma_pack_kernel); streamed with cp.async.bulk through an mbarrier ring.
+//   * a CTA is two warpgroups over a 128-row tile; each holds 64 rows x NPAD fp32 accumulators in registers.  The MMAs of a
+//     step are asynchronous (wgmma.mma_async): while they run, the same threads convert the next slab.  Epilogue: registers
+//     -> bias / LeakyReLU (fwd) -> a shared-memory staging tile -> coalesced global stores, with the LeakyReLU-slope /
+//     accumulate read-back of the dgrad.
+// Kernels in this file:
+//   plane_conv_umma_kernel<NPAD, DG>          the conv (forward: DG = false, dgrad: DG = true)
+//   split_views_kernel, wgrad_umma_bulk_kernel<NT>   hi/lo split arrays of a layer's wgrad operands (+ bias column sums) and
+//                                            the bulk-copy-fed wgrad;  wgrad_umma_kernel<NT>: the converter-fed form, for layers
+//                                            whose operand views do not fit one split pass
+//   umma_pack_kernel                         fp32 weights -> hi/lo bf16 blocks in K-step streaming order (pair-merged classes: two
+//                                            taps side by side per row shift)
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -76,35 +71,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (clock64() - t0 > 4000000000LL) asm volatile("trap;");
     }
 }
-// The same for the warps that are NOT the MMA issuer (converters waiting for a free slab, epilogue warps waiting for an
-// accumulator, the weight loader waiting for a free ring stage): back off with nanosleep between polls, so that their
-// polling does not take issue slots and shared-memory cycles from the single thread that feeds the tensor pipe.
-__device__ __forceinline__ void mbar_wait_bg(uint32_t bar, uint32_t parity) {
-#ifdef WUN_NO_BACKOFF
-    mbar_wait(bar, parity);
-#else
-    if (mbar_try_wait(bar, parity)) return;
-    const long long t0 = clock64();
-    unsigned ns = 20;
-    while (!mbar_try_wait(bar, parity)) {
-        __nanosleep(ns);
-        if (ns < 160) ns *= 2;
-        if (clock64() - t0 > 4000000000LL) asm volatile("trap;");
-    }
-#endif
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// One lane of a CONVERGED warp, chosen by the hardware.  Unlike `lane == 0` this tells the compiler that exactly one
-// thread runs the region, so every tcgen05.mma / commit / bulk copy inside is a plain instruction instead of an
-// ELECT + retry-branch sequence (measured on the single-thread issue loops, which are the critical path).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -112,116 +80,80 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                  : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// K-major / MN-major SWIZZLE_NONE shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout)
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// No-swizzle shared-memory matrix descriptor of wgmma: start address, leading / stride byte offsets (all >> 4).
+//   K-major operand:  LBO = bytes between the two 8-element K groups of a k16 step, SBO = bytes between 8-row M/N groups.
+//   MN-major operand: LBO = bytes between 8-row K groups, SBO = bytes between 8-element M/N groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46);
+           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// After wgmma_wait_all(): the accumulator registers are only now final.  The empty asm "redefines" each of them, so that
+// no read of an accumulator is scheduled above the wait.
+template <int N>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, M = 128, cta_group::1
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+#define WUN_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x N] += A[64 x 16] * B[16 x N], bf16 -> fp32; TA / TB = 1: that operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+        : WUN_F8(0)
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// The same MMA with the two 64-bit shared-memory descriptors given as (low word, high word) pairs: along a K loop only the
-// 14-bit start-address field in the LOW word changes (tap shift, row tile, weight block), so the single issuing thread
-// advances descriptors with one 32-bit add each instead of rebuilding 64-bit values.
-__device__ __forceinline__ void umma_bf16_w(uint32_t tmem_d, uint32_t a_w, uint32_t a_hw, uint32_t b_w, uint32_t b_hw, uint32_t idesc,
-                                            uint32_t accum) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "mov.b64 da, {%1, %2};\n\t"
-        "mov.b64 db, {%3, %4};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(a_w), "r"(a_hw), "r"(b_w), "r"(b_hw), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+        "%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
+        : WUN_F8(0), WUN_F8(8)
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ uint32_t umma_desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
-    return ((saddr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
-}
-constexpr uint32_t kDescHi128 = (128u >> 4) | (1u << 14);     // high word of a SWIZZLE_NONE descriptor with SBO = 128 B
-
-// One weight-ring stage of the conv K loop: nt <= 4 taps with CONSECUTIVE row shifts (shift0, shift0 + 1, ...) x MT row tiles
-// x the three split-precision MMAs, fully unrolled, every descriptor one word add away from the previous one.  The issue
-// loop is the critical path of every conv kernel (tools/umma_rate_bench: ~200 cycles of dependent uniform-datapath
-// arithmetic per tap in the generic loop, more than the 3 MMAs of a tap take for N <= 128), so nothing but adds and the
-// MMAs themselves remain here.  a_hi_w / a_lo_w: low words of the hi / lo sub-slab descriptors at row shift 0, tile 0;
-// b_hi_w / b_lo_w: low words of the stage's first weight block; blk16 = bytes of one tap's block / 16.
-template <int MT>
-__device__ __forceinline__ void issue_taps(uint32_t a_hi_w, uint32_t a_lo_w, uint32_t b_hi_w, uint32_t b_lo_w, uint32_t blk16, int nt,
-                                           uint32_t td, uint32_t acc_stride, uint32_t idesc, uint32_t& first) {
-#pragma unroll
-    for (int tt = 0; tt < 4; ++tt) {
-        if (tt < nt) {
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-                const uint32_t ah = a_hi_w + (uint32_t)(tt + 128 * mt), al = a_lo_w + (uint32_t)(tt + 128 * mt);
-                const uint32_t bh = b_hi_w + (uint32_t)tt * blk16, bl = b_lo_w + (uint32_t)tt * blk16;
-                const uint32_t t = td + (uint32_t)mt * acc_stride;
-                umma_bf16_w(t, al, kDescHi128, bh, kDescHi128, idesc, first);
-                umma_bf16_w(t, ah, kDescHi128, bl, kDescHi128, idesc, 1u);
-                umma_bf16_w(t, ah, kDescHi128, bh, kDescHi128, idesc, 1u);
-            }
-            first = 1u;
-        }
-    }
-}
-
-// Fused-N form of the same stage: per tap and row tile  D[:, 0:2N] += A_hi x [B_hi | B_lo]  (one MMA, N = 2*NPAD, the weight
-// block keeps B_hi and B_lo adjacent per K atom) and  D[:, 0:N] += A_lo x B_hi  - 2 MMAs per product instead of 3; the epilogue
-// adds the two accumulator halves.  tools/umma_rate_bench: 114 vs 153-173 cycles per K step and row tile for N <= 64.
-template <int MT>
-__device__ __forceinline__ void issue_taps_fused(uint32_t a_hi_w, uint32_t a_lo_w, uint32_t b_hi_w, uint32_t blk16, int nt, uint32_t td,
-                                                 uint32_t acc_stride, uint32_t idesc, uint32_t idesc2, uint32_t& first) {
-#pragma unroll
-    for (int tt = 0; tt < 4; ++tt) {
-        if (tt < nt) {
-#pragma unroll
-            for (int mt = 0; mt < MT; ++mt) {
-                const uint32_t ah = a_hi_w + (uint32_t)(tt + 128 * mt), al = a_lo_w + (uint32_t)(tt + 128 * mt);
-                const uint32_t bh = b_hi_w + (uint32_t)tt * blk16;
-                const uint32_t t = td + (uint32_t)mt * acc_stride;
-                umma_bf16_w(t, ah, kDescHi128, bh, kDescHi128, idesc2, first);
-                umma_bf16_w(t, al, kDescHi128, bh, kDescHi128, idesc, 1u);
-            }
-            first = 1u;
-        }
-    }
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
+        "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+        : WUN_F8(0), WUN_F8(8), WUN_F8(16), WUN_F8(24)
+        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
 }
+#undef WUN_F8
+
+// D[64 x N] += A * B for N = 64a + 32b + 16c columns, issued as n64 / n32 / n16 MMAs over consecutive column ranges;
+// b8 = descriptor units (16 B) between consecutive 8-column groups of B.  Accumulator register i of a thread holds
+// column (i/4)*8 + (lane%4)*2 + i%2 and row 16*(warp%4) + lane/4 + 8*((i/2)%2) of the warpgroup's 64 x N tile.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, uint32_t b8) {
+#pragma unroll
+    for (int i = 0; i < N / 64; ++i) wgmma_n64<TA, TB>(d + 32 * i, da, db + (uint64_t)(8u * b8 * i));
+    constexpr int o32 = N / 64 * 64, o16 = o32 + (N % 64) / 32 * 32;
+    if constexpr ((N % 64) >= 32) wgmma_n32<TA, TB>(d + o32 / 2, da, db + (uint64_t)(o32 / 8 * b8));
+    if constexpr ((N % 32) == 16) wgmma_n16<TA, TB>(d + o16 / 2, da, db + (uint64_t)(o16 / 8 * b8));
+}
+__device__ __forceinline__ int acc_col(int i, int lane) { return (i >> 2) * 8 + (lane & 3) * 2 + (i & 1); }
+__device__ __forceinline__ int acc_row(int i, int warp, int lane) { return 16 * (warp & 3) + (lane >> 2) + 8 * ((i >> 1) & 1); }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
     __nv_bfloat162 t = __floats2bfloat162_rn(lo_elem, hi_elem);   // .x = first (low address)
     return *reinterpret_cast<uint32_t*>(&t);
+}
+// 16 fp32 values -> 8 words of bf16 hi parts and 8 words of bf16 remainders (x = hi + lo to ~2^-17)
+__device__ __forceinline__ void split_hi_lo(const float* x, uint32_t* hi, uint32_t* lo) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const __nv_bfloat16 h0 = __float2bfloat16_rn(x[2 * i]), h1 = __float2bfloat16_rn(x[2 * i + 1]);
+        hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
+        lo[i] = pack_bf16x2(x[2 * i] - __bfloat162float(h0), x[2 * i + 1] - __bfloat162float(h1));
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -266,55 +198,20 @@ __device__ __forceinline__ void load_row16(const PlaneView& P, int b, int r, int
     }
 }
 
-// ------------------------------------------------------------------------------------------------
-// the kernel
-// ------------------------------------------------------------------------------------------------
-#ifdef WUN_UMMA_TIMING
-__device__ unsigned long long g_umma_timing[16];
-#define T_NOW() clock64()
-#define T_ADD(i, v) atomicAdd(&g_umma_timing[i], (unsigned long long)(v))
-#define T_WAIT(i, stmt) do { long long t__ = clock64(); stmt; T_ADD(i, clock64() - t__); } while (0)
-#define T_MARK(i) do { if (blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) g_fold_trace[i] = clock64(); } while (0)
-__device__ unsigned long long g_fold_trace[32];
-#else
-#define T_NOW() 0LL
-#define T_ADD(i, v) do { } while (0)
-#define T_WAIT(i, stmt) stmt
-#define T_MARK(i) do { } while (0)
-#endif
-
 // A (plane, tile) pair whose slab would hold nothing but zero rows - the tile's rows plus the group's tap span lie
-// entirely outside the plane's valid rows - contributes nothing: converters, MMA issuer and weight loader all skip the
-// group (same test, same order, so their job / ring counters stay in step).  This is what the dgrad of a down block
-// looks like outside the skip window: the gradient of the odd rows (g_odd) is zero there, i.e. for ~89 % of the tiles
-// 7-8 of the 15 taps have an all-zero operand.
+// entirely outside the plane's valid rows - contributes nothing: the K loop skips the group and its packed weights.  This
+// is what the dgrad of a down block looks like outside the skip window: the gradient of the odd rows (g_odd) is zero there.
 __device__ __forceinline__ bool group_is_empty(const UmmaLaunch& L, const UmmaGroup& G, int m_base) {
     const PlaneView& P = L.planes[G.plane];
     const int lo = m_base + G.dmin;
     return lo + L.rows_alloc <= P.r_lo || lo >= P.r_hi;
 }
 
-
-// Phase 2 of the conv epilogue for one warp: write out the 32 accumulator rows it staged (row r0 + 0..31 of the tile), lanes
-// running over (row, 4-column quad) pairs.  The LeakyReLU-slope read of the saved activation and the accumulate read of the
-// destination (dgrad) are issued for kEpiBatch items BEFORE any of them is used: the dgrad epilogue is a chain of dependent
-// global loads (measured: down1 dgrad 410 us with one load in flight per lane vs 175 us for the forward of the same layer,
-// whose epilogue only stores), so memory-level parallelism is what it needs.
-#ifndef WUN_KRB
-#define WUN_KRB 2            // slab rows a converter thread loads before converting any; measured (ms/step, same box): 4 -> 5.31, 3 -> 5.12, 2 -> 5.09
-#endif
-#ifndef WUN_EPI_BATCH
-#define WUN_EPI_BATCH 2      // measured with the lean addressing (same box, ms/step): 6 -> 5.82, 4 -> 5.38, 3 -> 5.23, 2 -> 5.21
-#endif
-constexpr int kEpiBatch = WUN_EPI_BATCH;
-// forward launches (nothing to read back) keep the straight loop; the two forms live in separate kernel instantiations
-// (template parameter DG) because the batched form's registers slowed the forward kernels down when both shared one body
-// (down1 forward 149 -> 195 us).
-// Phase 2 addressing.  The four epilogue warps are instruction-issue bound in the dgrad launches (measured: deleting the slope
-// read-back saved 0.4 ms of the step although its bytes are a third of the launch's traffic, while variants that ADDED
-// instructions to hide its latency - sign-bit masks, cp.async prefetch of the saved rows - were slower), so everything that
-// does not depend on the item is hoisted: per half (pair-merged classes have two, launch.h OutView::pairC) one base pointer that
-// already contains the batch item and the block's first column, then an item costs one 32-bit multiply-add.
+// ------------------------------------------------------------------------------------------------
+// conv epilogue: staged rows -> global memory
+// ------------------------------------------------------------------------------------------------
+// Per half (pair-merged classes have two, launch.h OutView::pairC) one base pointer that already contains the batch item and
+// the block's first column; an item then costs one 32-bit multiply-add.
 struct EpiHalf {
     float* dst;            // + m * rstride + 4 * (quad within the half)
     const float* saved;    // same geometry (null: no slope)
@@ -346,16 +243,11 @@ __device__ __forceinline__ EpiBlock epi_block(const OutView& O, int b, int col0,
     } else {
         B.h[1] = B.h[0];
     }
-#ifdef WUN_EXP_NOSLOPE          // timing experiment only (wrong gradients): what the slope read-back of the dgrad epilogue costs
-    B.h[0].saved = nullptr; B.h[1].saved = nullptr;
-#endif
     return B;
 }
 
-// Phase 2 of the conv epilogue for one warp: write out the 32 accumulator rows it staged (row r0 + 0..31 of the tile), lanes running
-// over (row, 4-column quad) pairs; (rl, q) advance incrementally (no division per item).  Forward form: nothing to read back.
-// (A separate one-view instantiation next to the pair-aware one was tried: the copies pushed the block descriptor into local
-//  memory - 352-byte stack frames - and the dgrad family from 2.2 to 3.5 ms.)
+// One warp writes out 32 staged rows (row r0 + 0..31 of the tile), lanes running over (row, 4-column quad) pairs so that narrow
+// layers (N = 24..48) still use every lane and a warp store covers several consecutive rows.  Forward form: nothing to read back.
 __device__ __forceinline__ void epi_write_rows_simple(const float* __restrict__ stage, int SW, int r0, int lane, int Q, int m0,
                                                       const EpiBlock& B) {
     const int dr = 32 / Q, dq = 32 - dr * Q;
@@ -370,7 +262,8 @@ __device__ __forceinline__ void epi_write_rows_simple(const float* __restrict__ 
     }
 }
 // dgrad form: the LeakyReLU-slope read of the saved activation and the accumulate read of the destination are issued for
-// kEpiBatch items BEFORE any of them is used (memory-level parallelism: the store loop is a chain of dependent global loads).
+// kEpiBatch items BEFORE any of them is used (memory-level parallelism: otherwise the store loop is a chain of dependent loads).
+constexpr int kEpiBatch = 2;
 __device__ __forceinline__ void epi_write_rows_vec(const float* __restrict__ stage, int SW, int r0, int lane, int Q, int m0,
                                                    const EpiBlock& B) {
     const int dr = 32 / Q, dq = 32 - dr * Q;
@@ -410,1373 +303,250 @@ __device__ __forceinline__ void epi_write_rows_vec(const float* __restrict__ sta
     }
 }
 
-constexpr int kSlabStages = 3;
-constexpr int kBStagesMax = 6;   // weight ring: L.nbs stages of L.TB taps each
-constexpr int kWorkerThreads = 128;
+// ------------------------------------------------------------------------------------------------
+// the conv kernel
+// ------------------------------------------------------------------------------------------------
+constexpr int kConvThreads = 256;      // two warpgroups: rows [0, 64) and [64, 128) of the tile
+constexpr int kBStagesMax = 6;         // weight ring: L.nbs stages of up to L.TB taps
 
-// NTEAMS converter teams (4 warps each) take jobs round-robin: 2 teams / 3 slab stages when two CTAs share an SM (dense
-// launches), 4 teams / 6 stages for the sparse deep-layer launches whose K loop is converter-latency bound.
-template <int NTEAMS, bool DG>
-__global__ void __launch_bounds__(NTEAMS * 128 + 64, (NTEAMS == 2) ? 2 : 1) plane_conv_umma_kernel(const __grid_constant__ UmmaLaunch L) {
-    constexpr int kSlabStages = (NTEAMS == 2) ? 3 : 6;
-    constexpr int kMmaWarp = NTEAMS * 4, kSlabMax = 6;
+// One step of a CTA's K loop = one weight-ring stage: taps [t0, t0 + nt) (relative to the group) of 16-channel chunk c of
+// group g; blk = index of its first packed weight block (pack order: group, chunk, term).
+struct ConvStep {
+    int g, c, t0, nt, blk;
+};
+// Moves s to the next step (from g = -1: to the first one), skipping groups whose slab would be all zeros together with
+// their packed blocks.  false = the K loop is done.
+__device__ __forceinline__ bool next_step(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
+    if (s.g >= 0) {
+        const UmmaGroup& G = K.groups[s.g];
+        const int nterm = G.term_end - G.term_begin;
+        s.blk += s.nt;
+        s.t0 += s.nt;
+        if (s.t0 < nterm) { s.nt = min(L.TB, nterm - s.t0); return true; }
+        s.t0 = 0;
+        if (++s.c < ((L.planes[G.plane].C + 15) >> 4)) { s.nt = min(L.TB, nterm); return true; }
+    }
+    for (++s.g; s.g < K.ngroups; ++s.g) {
+        const UmmaGroup& G = K.groups[s.g];
+        const int nterm = G.term_end - G.term_begin;
+        if (!group_is_empty(L, G, m_base)) { s.c = 0; s.t0 = 0; s.nt = min(L.TB, nterm); return true; }
+        s.blk += ((L.planes[G.plane].C + 15) >> 4) * nterm;
+    }
+    return false;
+}
+
+// slab of (group, chunk): rows m_base + dmin + [0, rows_alloc) of the plane, 16 channels, as hi / lo atom planes
+__device__ __forceinline__ void fill_slab(const UmmaLaunch& L, const UmmaGroup& G, int b, int m_base, int c, uint8_t* S) {
+    const PlaneView& P = L.planes[G.plane];
+    const uint32_t atom = 16u * L.rows_alloc;
+    for (int rr = threadIdx.x; rr < L.rows_alloc; rr += kConvThreads) {
+        float x[16];
+        uint32_t hi[8], lo[8];
+        load_row16(P, b, m_base + G.dmin + rr, c * 16, x);
+        split_hi_lo(x, hi, lo);
+        *reinterpret_cast<uint4*>(S + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+        *reinterpret_cast<uint4*>(S + atom + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+        *reinterpret_cast<uint4*>(S + 2 * atom + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        *reinterpret_cast<uint4*>(S + 3 * atom + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+    }
+}
+
+static __host__ __device__ size_t conv_smem_bytes(int NPAD, int rows_alloc, int TB, int nbs) {
+    const size_t pipe = 2 * 64 * (size_t)rows_alloc + (size_t)nbs * TB * 64 * NPAD;
+    const size_t epi = 128 * ((size_t)NPAD + 4) * 4;
+    return ((pipe > epi ? pipe : epi) + 127) / 128 * 128 + kBStagesMax * 8 + 4 * (size_t)NPAD;
+}
+
+// grid = (row tiles of 128, output-channel splits, batch * classes).  Shared memory: two slabs, the weight ring, the ring's
+// mbarriers, this split's bias; the epilogue re-uses the slabs + ring as a 128 x (NPAD + 4) fp32 staging tile.
+template <int NPAD, bool DG>
+__global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const __grid_constant__ UmmaLaunch L) {
     extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
     const int cls = blockIdx.z % L.ncls, b = blockIdx.z / L.ncls;
     const UmmaClass& K = L.cls[cls];
     const int split = blockIdx.y;
-    const int rows_tile = L.MT * 128;
-    const int m_base = K.out.m_lo + blockIdx.x * rows_tile;
+    const int m_base = K.out.m_lo + blockIdx.x * 128;
     if (m_base >= K.out.m_hi) return;
-    const long long t_start = T_NOW();
 
-    const int NPAD = L.NPAD;
-    const uint32_t slab_bytes = 64u * L.rows_alloc;          // [hi|lo][2 atoms][rows_alloc][16 B]
-    const uint32_t bblk_bytes = 64u * NPAD;                  // [hi|lo][2 atoms][NPAD/8][8][16 B]
-    uint8_t* slab0 = smem;
-    uint8_t* bring0 = smem + kSlabStages * slab_bytes;
-    const int TB = L.TB, nbs = L.nbs;
-    const uint32_t bstage_bytes = bblk_bytes * TB;
-    // the epilogue re-uses the (then idle) pipeline memory as a 128 x (CW+4) fp32 staging tile: barriers live
-    // behind whichever of the two is larger
-    const uint32_t pipe_bytes = kSlabStages * slab_bytes + nbs * bstage_bytes;
-    const uint32_t epi_bytes = 128u * ((uint32_t)(NPAD < 128 ? NPAD : 128) + 4u) * 4u;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((pipe_bytes > epi_bytes ? pipe_bytes : epi_bytes) + 127u) / 128u * 128u);
-    // bars: slab_full[3], slab_empty[3], b_full[6], b_empty[6], acc_full
+    const uint32_t atom = 16u * L.rows_alloc;
+    const uint32_t slab_bytes = 4u * atom;
+    constexpr uint32_t blk_bytes = 64u * NPAD;               // [hi a0|hi a1|lo a0|lo a1] x NPAD rows x 16 B ... see umma_pack_kernel
+    const uint32_t stage_bytes = blk_bytes * L.TB;
+    uint8_t* ring = smem + 2 * slab_bytes;
+    const size_t pipe = 2 * (size_t)slab_bytes + (size_t)L.nbs * stage_bytes, epi = 128u * (NPAD + 4) * 4u;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((pipe > epi ? pipe : epi) + 127) / 128 * 128);
+    float* bias_s = reinterpret_cast<float*>(bars + kBStagesMax);
     const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    const int SLAB_FULL = 0, SLAB_EMPTY = kSlabMax, B_FULL = 2 * kSlabMax, B_EMPTY = 2 * kSlabMax + kBStagesMax,
-              ACC_FULL = 2 * kSlabMax + 2 * kBStagesMax;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + ACC_FULL + 1);
-    float* bias_s = reinterpret_cast<float*>(tmem_holder + 4);       // NPAD floats: this split's bias
-    for (int i = tid; i < NPAD; i += blockDim.x) {
-        const int n = split * NPAD + i;
-        bias_s[i] = (L.bias && n < L.N) ? __ldg(L.bias + ((L.pairC > 0 && n >= L.pairC) ? n - L.pairC : n)) : 0.f;
-    }
-
-    if (tid == 0) {
-        for (int i = 0; i < kSlabStages; ++i) { mbar_init(BAR(SLAB_FULL + i), kWorkerThreads); mbar_init(BAR(SLAB_EMPTY + i), 1); }
-        for (int i = 0; i < kBStagesMax; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), 1); }
-        mbar_init(BAR(ACC_FULL), 1);
-        fence_barrier_init();
-    }
-    if (warp == kMmaWarp) tmem_alloc(smem_u32(tmem_holder), L.tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    if (tid == 0) { T_ADD(0, 1); T_ADD(2, T_NOW() - t_start); }
-
-    // job = (group, 16-channel chunk); K-step = (job, term)
-    if (warp < kMmaWarp) {
-        // ===================== converter: fill slabs =====================
-        // two teams of 4 warps take alternate jobs, so two jobs' global-load latencies are in flight at once
-        const int team = warp >> 2, ttid = tid & 127;
-        int ji = 0;
-        for (int g = 0; g < K.ngroups; ++g) {
-            const UmmaGroup& G = K.groups[g];
-            const PlaneView& P = L.planes[G.plane];
-            const int nchunk = (P.C + 15) >> 4;
-            if (group_is_empty(L, G, m_base)) continue;
-            for (int c = 0; c < nchunk; ++c, ++ji) {
-                if ((ji % NTEAMS) != team) continue;
-                const int st = ji % kSlabStages;
-                uint8_t* S = slab0 + st * slab_bytes;
-                const uint32_t atom_stride = 16u * L.rows_alloc;
-                const long long t_fill = T_NOW();
-                // Loads of up to kRB rows per thread are issued together and BEFORE the stage-free wait, so their
-                // latency overlaps the wait; only the convert + st.shared part needs the stage.
-                constexpr int kRB = WUN_KRB;
-                bool waited = false;
-                for (int rbase = 0; rbase < L.rows_alloc; rbase += kRB * kWorkerThreads) {
-                    float x[kRB][16];
-#pragma unroll
-                    for (int u = 0; u < kRB; ++u) {
-                        const int rr = rbase + u * kWorkerThreads + ttid;
-                        if (rr < L.rows_alloc) load_row16(P, b, m_base + G.dmin + rr, c * 16, x[u]);
-                    }
-                    if (!waited) {
-                        if (tid == 0) { T_WAIT(6, mbar_wait_bg(BAR(SLAB_EMPTY + st), ((ji / kSlabStages) & 1) ^ 1)); }
-                        else mbar_wait_bg(BAR(SLAB_EMPTY + st), ((ji / kSlabStages) & 1) ^ 1);
-                        waited = true;
-                    }
-#pragma unroll
-                    for (int u = 0; u < kRB; ++u) {
-                        const int rr = rbase + u * kWorkerThreads + ttid;
-                        if (rr >= L.rows_alloc) continue;
-                        uint32_t hi[8], lo[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const __nv_bfloat16 h0 = __float2bfloat16_rn(x[u][2 * i]), h1 = __float2bfloat16_rn(x[u][2 * i + 1]);
-                            hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                            lo[i] = pack_bf16x2(x[u][2 * i] - __bfloat162float(h0), x[u][2 * i + 1] - __bfloat162float(h1));
-                        }
-                        *reinterpret_cast<uint4*>(S + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);                       // hi, atom 0
-                        *reinterpret_cast<uint4*>(S + atom_stride + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);        // hi, atom 1
-                        *reinterpret_cast<uint4*>(S + 2 * atom_stride + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                        *reinterpret_cast<uint4*>(S + 3 * atom_stride + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                    }
-                }
-                fence_proxy_async();                 // generic-proxy smem writes -> visible to the tensor core (async proxy)
-                mbar_arrive(BAR(SLAB_FULL + st));
-                if (tid == 0) T_ADD(7, T_NOW() - t_fill);
-            }
-        }
-        // ===================== epilogue (teams 0 and 1: TMEM lane quarter = warp & 3) =====================
-        // Both teams are idle once their slabs are converted, and the epilogue is instruction-issue bound (DESIGN.md 4.1): the
-        // two teams split the 16-column chunks of every staged block between them (same rows, disjoint columns).
-        if (team < L.epi_teams) {
-        const int q4 = warp & 3, eg = (L.epi_teams == 2) ? team : 2;       // eg 2 = the only group: every chunk
-        if (tid == 0) { T_WAIT(8, mbar_wait_bg(BAR(ACC_FULL), 0)); }
-        else mbar_wait_bg(BAR(ACC_FULL), 0);
-        tc_fence_after();
-        const long long t_epi = T_NOW();
-        const int n0 = split * NPAD;
-        bool any_group = false;                          // all groups skipped as empty: the accumulator was never written = zeros
-        for (int g = 0; g < K.ngroups; ++g) any_group = any_group || !group_is_empty(L, K.groups[g], m_base);
-        // Stage each 128 x CW accumulator block in shared memory (the slab / weight ring is idle now: every MMA
-        // has retired), then write it out with one warp per output row: fully coalesced stores, and the
-        // LeakyReLU-slope / accumulate reads of the dgrad epilogue are coalesced too.
-        float* stage = reinterpret_cast<float*>(smem);
-        const int CW = (NPAD < 128) ? NPAD : 128;          // columns staged at a time
-        const int SW = CW + 4;                              // padded row stride (floats): conflict-free float4 rows
-        // each team owns a FIXED column range of the staging tile (its k-th chunk of any block goes to stage_ofs + 16k): the split
-        // of a block's chunks differs from block to block, and a team that runs ahead must never overwrite staged data the
-        // other team has not written out yet
-        const int stage_ofs = (eg == 1) ? 16 * (((CW >> 4) + 1) >> 1) : 0;
-        for (int mt = 0; mt < L.MT; ++mt) {
-            for (int c0 = 0; c0 < NPAD; c0 += CW) {
-                if (n0 + c0 >= L.N) break;
-                const int cw = min(CW, NPAD - c0);
-                const int nch_blk = (cw + 15) >> 4;
-                const int cb_lo = (eg == 1) ? 16 * ((nch_blk + 1) >> 1) : 0, cb_hi = (eg == 0) ? 16 * ((nch_blk + 1) >> 1) : 16 * nch_blk;
-                // phase 1: thread = accumulator row (TMEM lane)
-                for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-                    __syncwarp();
-                    float v[16];
-                    if (L.fuse) {
-                        float v2[16];
-                        tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(mt * 2 * NPAD + c0 + cb), v);
-                        tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(mt * 2 * NPAD + NPAD + c0 + cb), v2);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] += v2[j];
-                    } else {
-                        tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(mt * NPAD + c0 + cb), v);
-                    }
-                    if (!any_group) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = 0.f;
-                    }
-                    if (L.epilogue == EPI_BIAS_LRELU) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            const float y = v[j] + bias_s[c0 + cb + j];
-                            v[j] = fmaxf(0.2f * y, y);
-                        }
-                    }
-                    float4* dst = reinterpret_cast<float4*>(stage + (size_t)(q4 * 32 + lane) * SW + stage_ofs + (cb - cb_lo));
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                }
-                __syncwarp();
-                // phase 2: each warp writes out the 32 rows it staged itself (no block barrier needed); lanes run over
-                // (row, 4-column quad) pairs so that narrow layers (N = 24..48) still use every lane and a whole warp
-                // store covers several consecutive rows
-                const int ncols = min(cb_hi, L.N - (n0 + c0)) - cb_lo;      // real columns of this team's share
-                if (ncols > 0) {
-                const long long tile_off = (long long)b * K.out.bstride + n0 + c0 + cb_lo;
-                const bool vec = (ncols % 4 == 0) && (K.out.rstride % 4 == 0) && (((n0 + c0) & 3) == 0) &&
-                                 ((reinterpret_cast<uintptr_t>(K.out.base) & 15) == 0) && ((K.out.bstride & 3) == 0);
-                const float* stage_g = stage + stage_ofs;
-                if (vec) {      // (pair-merged classes always take this path: the planner checks both views)
-                    const EpiBlock EB = epi_block<true>(K.out, b, n0 + c0 + cb_lo, ncols >> 2, L.epilogue == EPI_SLOPE);
-                    if (DG) epi_write_rows_vec(stage_g, SW, q4 * 32, lane, ncols >> 2, m_base + mt * 128 + q4 * 32, EB);
-                    else epi_write_rows_simple(stage_g, SW, q4 * 32, lane, ncols >> 2, m_base + mt * 128 + q4 * 32, EB);
-                } else {
-                    for (int it = lane; it < 32 * ncols; it += 32) {
-                        const int rl = it / ncols, j = it - rl * ncols;
-                        const int r = q4 * 32 + rl;
-                        const int m = m_base + mt * 128 + r;
-                        if (m >= K.out.m_hi) continue;
-                        const long long roff = tile_off + (long long)m * K.out.rstride;
-                        float o = stage_g[(size_t)r * SW + j];
-                        if (L.epilogue == EPI_SLOPE && K.out.saved) o *= (__ldg(K.out.saved + roff + j) > 0.f) ? 1.f : 0.2f;
-                        float* dst = K.out.base + roff + j;
-                        if (m >= K.out.acc_lo && m < K.out.acc_hi) o += *dst;
-                        *dst = o;
-                    }
-                }
-                }
-                __syncwarp();                                     // the warp-private staging rows are overwritten by the next block
-            }
-        }
-        if (tid == 0) T_ADD(9, T_NOW() - t_epi);
-        }
-        tc_fence_before();
-    } else if (warp == kMmaWarp) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NPAD >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NPAD >> 2) << 17) | ((128u >> 4) << 24);   // N = 2*NPAD
-            const uint32_t atom_stride = 16u * L.rows_alloc;
-            const uint32_t b_lbo = 32u * NPAD;       // between the two K atoms of a weight block
-            int ji = 0, bi = 0;                      // bi counts weight STAGES (TB taps each)
-            const long long t_mma = T_NOW();
-            uint32_t first = 0;                      // accumulate flag: 0 for the very first K step
-            for (int g = 0; g < K.ngroups; ++g) {
-                const UmmaGroup& G = K.groups[g];
-                const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                if (group_is_empty(L, G, m_base)) continue;
-                for (int c = 0; c < nchunk; ++c, ++ji) {
-                    const int st = ji % kSlabStages;
-                    T_WAIT(4, mbar_wait(BAR(SLAB_FULL + st), (ji / kSlabStages) & 1));
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(slab0 + st * slab_bytes);
-                    // descriptor bases of this slab stage; a tap shift only adds (rows * 16 B) >> 4 to the address field
-                    const uint64_t a_hi0 = umma_desc(sa, atom_stride, 128), a_lo0 = umma_desc(sa + 2 * atom_stride, atom_stride, 128);
-                    for (int t0 = G.term_begin; t0 < G.term_end; t0 += TB, ++bi) {
-                        const int bs = bi % nbs;
-                        T_WAIT(5, mbar_wait(BAR(B_FULL + bs), (bi / nbs) & 1));
-                        tc_fence_after();
-                        const uint32_t sb = smem_u32(bring0 + bs * bstage_bytes);
-                        const uint64_t b_hi0 = umma_desc(sb, b_lbo, 128), b_lo0 = umma_desc(sb + 16u * NPAD, b_lbo, 128);
-                        const int nt = min(TB, G.term_end - t0);
-                        if (L.consec) {
-                            const uint32_t sh = (uint32_t)(t0 - G.term_begin);
-                            const uint32_t ahw = umma_desc_lo(sa, atom_stride) + sh, alw = umma_desc_lo(sa + 2 * atom_stride, atom_stride) + sh;
-                            const uint32_t bhw = umma_desc_lo(sb, b_lbo), blw = umma_desc_lo(sb + 16u * NPAD, b_lbo);
-                            if (L.fuse) {
-                                if (L.MT == 2) issue_taps_fused<2>(ahw, alw, bhw, bblk_bytes >> 4, nt, tmem_base, 2u * NPAD, idesc, idesc2, first);
-                                else issue_taps_fused<1>(ahw, alw, bhw, bblk_bytes >> 4, nt, tmem_base, 2u * NPAD, idesc, idesc2, first);
-                            } else if (L.MT == 2) issue_taps<2>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, tmem_base, (uint32_t)NPAD, idesc, first);
-                            else issue_taps<1>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, tmem_base, (uint32_t)NPAD, idesc, first);
-                        } else
-                        for (int tt = 0; tt < nt; ++tt) {
-                            const uint64_t boff = (uint64_t)((bblk_bytes >> 4) * tt);
-                            const uint64_t b_hi = b_hi0 + boff, b_lo = b_lo0 + boff;
-                            const uint64_t aoff = (uint64_t)(uint32_t)(L.d[t0 + tt] - G.dmin);
-                            for (int mt = 0; mt < L.MT; ++mt) {
-                                const uint64_t a_hi = a_hi0 + aoff + (uint64_t)(128u * mt), a_lo = a_lo0 + aoff + (uint64_t)(128u * mt);
-                                if (L.fuse) {
-                                    // fused-N: D[:, 0:NPAD] += A_hi B_hi, D[:, NPAD:2NPAD] += A_hi B_lo in ONE MMA over the
-                                    // [B_hi | B_lo] block, then D[:, 0:NPAD] += A_lo B_hi; the epilogue adds the two halves
-                                    const uint32_t td = tmem_base + (uint32_t)(mt * 2 * NPAD);
-                                    umma_bf16(td, a_hi, b_hi, idesc2, first);
-                                    umma_bf16(td, a_lo, b_hi, idesc, 1u);
-                                } else {
-                                    const uint32_t td = tmem_base + (uint32_t)(mt * NPAD);
-                                    umma_bf16(td, a_lo, b_hi, idesc, first);
-                                    umma_bf16(td, a_hi, b_lo, idesc, 1u);
-                                    umma_bf16(td, a_hi, b_hi, idesc, 1u);
-                                }
-                            }
-                            first = 1u;
-                        }
-                        umma_commit(BAR(B_EMPTY + bs));       // weight stage free once these MMAs retire
-                    }
-                    umma_commit(BAR(SLAB_EMPTY + st));        // slab stage free
-                }
-            }
-            umma_commit(BAR(ACC_FULL));
-            T_ADD(3, T_NOW() - t_mma);
-        }
-        __syncwarp();
-    } else {
-        // ===================== weight loader =====================
-        if (elect_one()) {
-            const uint8_t* src = K.wpack[split];
-            int bi = 0;
-            size_t blk = 0;                          // running block (tap) index into the packed stream
-            for (int g = 0; g < K.ngroups; ++g) {
-                const UmmaGroup& G = K.groups[g];
-                const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                const int nterm = G.term_end - G.term_begin;
-                if (group_is_empty(L, G, m_base)) { blk += (size_t)nchunk * nterm; continue; }
-                for (int c = 0; c < nchunk; ++c) {
-                    for (int t0 = 0; t0 < nterm; t0 += TB, ++bi) {
-                        const int nt = min(TB, nterm - t0);
-                        const int bs = bi % nbs;
-                        T_WAIT(10, mbar_wait_bg(BAR(B_EMPTY + bs), ((bi / nbs) & 1) ^ 1));
-                        mbar_arrive_expect_tx(BAR(B_FULL + bs), bblk_bytes * nt);
-                        bulk_g2s(smem_u32(bring0 + bs * bstage_bytes), src + blk * bblk_bytes, bblk_bytes * nt, BAR(B_FULL + bs));
-                        blk += nt;
-                    }
-                }
-            }
-        }
-        __syncwarp();
-    }
-    __syncthreads();
-    if (warp == kMmaWarp) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, L.tmem_cols);
-    }
-    if (tid == 0) T_ADD(1, T_NOW() - t_start);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Persistent variant for launches with many row tiles (the big layers): ONE CTA per SM loops over tiles,
-// the TMEM accumulator is double-buffered and a dedicated epilogue warp group drains tile k while the MMA
-// warp already issues tile k+1 - so the tensor pipe of an SM is fed by a single, never-interrupted issuer
-// (measured floor 56 cycles/MMA at N=96 vs ~70 with two interleaving CTAs) and there is no per-tile
-// prologue / TMEM allocation / wave tail.
-// Warps: 0-7 converters (two teams), 8 MMA issue + TMEM alloc, 9 weight loader, 10-13 epilogue.
-// ------------------------------------------------------------------------------------------------
-
-struct TileCoord { int cls, b, split, m_base; };
-
-__device__ __forceinline__ TileCoord decode_tile(const UmmaLaunch& L, int t) {
-    TileCoord tc;
-    tc.split = t % L.nsplit;
-    t /= L.nsplit;
-    const int rows_tile = L.MT * 128;
-    int q = 0;
-    for (; q < L.ncls - 1; ++q) {
-        const int nt = (L.cls[q].out.m_hi - L.cls[q].out.m_lo + rows_tile - 1) / rows_tile * L.batch;
-        if (t < nt) break;
-        t -= nt;
-    }
-    const int tiles_q = (L.cls[q].out.m_hi - L.cls[q].out.m_lo + rows_tile - 1) / rows_tile;
-    tc.cls = q;
-    tc.b = t / tiles_q;
-    tc.m_base = L.cls[q].out.m_lo + (t % tiles_q) * rows_tile;
-    return tc;
-}
-
-// PT converter teams (4 warps each): warps [0, 4PT) convert, warp 4PT issues MMAs, 4PT+1 streams weights, 4PT+2..4PT+5
-// run the epilogue (4PT+2 = 2 mod 4, so `warp & 3` covers the four TMEM lane quarters).  PT+1 slab stages.
-// NCOL = number of output-conv columns (nconv * C) of the fused output layer, 0 = plain conv.  The fused epilogue is compiled per
-// width: generic code predicated up to 8 columns was 6000 instructions (95 KB) that the four epilogue warps streamed through the
-// instruction cache once per row tile - 70k cycles per 128 rows, measured.
-// EPW = epilogue warps per TMEM lane quarter (1 or 2).  The dgrad launches are bound by the instruction issue of their epilogue
-// warps (DESIGN.md 4.1), so their instantiation trades one converter team for a second epilogue group: the two groups split the
-// 16-column chunks of every staged block between them (same rows, disjoint columns of the same staging tile - no extra shared
-// memory, no synchronisation between the groups beyond the accumulator-free barrier, which now counts 128 * EPW arrivals).
-template <int PT, bool DG, int NCOL, int EPW>
-__device__ __forceinline__ void persistent_body(const UmmaLaunch& L, int total_tiles, const OutputFuse* FP) {
-    constexpr bool OUTL = NCOL > 0;
-    constexpr int NC = OUTL ? NCOL : 1;          // array extent of the per-column registers
-    constexpr int kSlabStages = PT + 1;
-    constexpr int kMmaWarp = 4 * PT, kLoadWarp = 4 * PT + 1, kEpiWarp0 = 4 * PT + 2;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NPAD = L.NPAD;
-    const uint32_t slab_bytes = 64u * L.rows_alloc;
-    const uint32_t bblk_bytes = 64u * NPAD;
-    const int TB = L.TB, nbs = L.nbs;
-    const uint32_t bstage_bytes = bblk_bytes * TB;
-    const int CW = (NPAD < 128) ? NPAD : 128;
-    const int SW = CW + 4;
-    uint8_t* slab0 = smem;
-    uint8_t* bring0 = smem + kSlabStages * slab_bytes;
-    float* stage = reinterpret_cast<float*>(bring0 + nbs * bstage_bytes);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stage) + (size_t)128 * SW * 4);
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    const int SLAB_FULL = 0, SLAB_EMPTY = kSlabStages, B_FULL = 2 * kSlabStages, B_EMPTY = 2 * kSlabStages + kBStagesMax,
-              ACC_FULL = 2 * kSlabStages + 2 * kBStagesMax, ACC_EMPTY = ACC_FULL + 2;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + ACC_EMPTY + 2);
-    float* bias_s = reinterpret_cast<float*>(tmem_holder + 4);       // nsplit * NPAD floats
-    for (int i = tid; i < NPAD * L.nsplit; i += blockDim.x)
-        bias_s[i] = (L.bias && i < L.N) ? __ldg(L.bias + ((L.pairC > 0 && i >= L.pairC) ? i - L.pairC : i)) : 0.f;
-    // fused output layer (OUTL): [wout (C+F) x ncol | bout ncol | dpre 128 rows x 2 halves x ncol | wacc 4 warps x (C+F+1) x ncol]
-    float *wout_s = nullptr, *bout_s = nullptr, *dpre_s = nullptr, *wacc_s = nullptr;
-    int o_ncol = 0, o_cin = 0, o_nw = 0;
-    if (OUTL) {
-        const OutputLaunch& O = FP->O;
-        o_ncol = O.nconv * O.C; o_cin = O.C + O.F; o_nw = (o_cin + 1) * o_ncol;
-        wout_s = bias_s + ((NPAD * L.nsplit + 3) & ~3);
-        bout_s = wout_s + o_cin * o_ncol;
-        dpre_s = bout_s + ((o_ncol + 3) & ~3);
-        wacc_s = dpre_s + 128 * 2 * o_ncol;
-        for (int i = tid; i < o_cin * o_ncol; i += blockDim.x) {       // kernel [ofs = 1][C+F][C] per output conv (OutputLayer.py:8)
-            const int cin = i / o_ncol, q = i - cin * o_ncol, conv = q / O.C, oc = q - conv * O.C;
-            wout_s[i] = __ldg(O.params + O.w_off[conv] + (long long)cin * O.C + oc);
-        }
-        for (int i = tid; i < o_ncol; i += blockDim.x) bout_s[i] = __ldg(O.params + O.b_off[i / O.C] + (i % O.C));
-        for (int i = tid; i < 4 * o_nw; i += blockDim.x) wacc_s[i] = 0.f;
-    }
-    if (tid == 0) {
-        for (int i = 0; i < kSlabStages; ++i) { mbar_init(BAR(SLAB_FULL + i), kWorkerThreads); mbar_init(BAR(SLAB_EMPTY + i), 1); }
-        for (int i = 0; i < kBStagesMax; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(BAR(ACC_FULL + i), 1); mbar_init(BAR(ACC_EMPTY + i), 128 * EPW); }
-        fence_barrier_init();
-    }
-    if (warp == kMmaWarp) tmem_alloc(smem_u32(tmem_holder), L.tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    const uint32_t acc_w = (uint32_t)(L.fuse ? 2 * NPAD : NPAD);      // accumulator columns of one row tile (fused-N: two halves)
-    const uint32_t acc_cols = (uint32_t)L.MT * acc_w;                 // columns of one accumulator buffer
-
-    if (warp < kMmaWarp) {
-        // ===================== converters =====================
-        const int team = warp >> 2, ttid = tid & 127;
-        int jg = 0;                                                   // job counter across tiles
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-            const TileCoord tc = decode_tile(L, t);
-            const UmmaClass& K = L.cls[tc.cls];
-            for (int g = 0; g < K.ngroups; ++g) {
-                const UmmaGroup& G = K.groups[g];
-                const PlaneView& P = L.planes[G.plane];
-                const int nchunk = (P.C + 15) >> 4;
-                if (group_is_empty(L, G, tc.m_base)) continue;
-                for (int c = 0; c < nchunk; ++c, ++jg) {
-                    if ((jg % PT) != team) continue;
-                    const int st = jg % kSlabStages;
-                    uint8_t* S = slab0 + st * slab_bytes;
-                    const uint32_t atom_stride = 16u * L.rows_alloc;
-                    constexpr int kRB = WUN_KRB;
-                    bool waited = false;
-                    for (int rbase = 0; rbase < L.rows_alloc; rbase += kRB * kWorkerThreads) {
-                        float x[kRB][16];
-#pragma unroll
-                        for (int u = 0; u < kRB; ++u) {
-                            const int rr = rbase + u * kWorkerThreads + ttid;
-                            if (rr < L.rows_alloc) load_row16(P, tc.b, tc.m_base + G.dmin + rr, c * 16, x[u]);
-                        }
-                        if (!waited) { mbar_wait_bg(BAR(SLAB_EMPTY + st), ((jg / kSlabStages) & 1) ^ 1); waited = true; }
-#pragma unroll
-                        for (int u = 0; u < kRB; ++u) {
-                            const int rr = rbase + u * kWorkerThreads + ttid;
-                            if (rr >= L.rows_alloc) continue;
-                            uint32_t hi[8], lo[8];
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const __nv_bfloat16 h0 = __float2bfloat16_rn(x[u][2 * i]), h1 = __float2bfloat16_rn(x[u][2 * i + 1]);
-                                hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                                lo[i] = pack_bf16x2(x[u][2 * i] - __bfloat162float(h0), x[u][2 * i + 1] - __bfloat162float(h1));
-                            }
-                            *reinterpret_cast<uint4*>(S + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                            *reinterpret_cast<uint4*>(S + atom_stride + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                            *reinterpret_cast<uint4*>(S + 2 * atom_stride + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                            *reinterpret_cast<uint4*>(S + 3 * atom_stride + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                        }
-                    }
-                    fence_proxy_async();
-                    mbar_arrive(BAR(SLAB_FULL + st));
-                }
-            }
-        }
-    } else if (warp == kMmaWarp) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NPAD >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t atom_stride = 16u * L.rows_alloc;
-            const uint32_t b_lbo = 32u * NPAD;
-            int jg = 0, bg = 0, k = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++k) {
-                const TileCoord tc = decode_tile(L, t);
-                const UmmaClass& K = L.cls[tc.cls];
-                const int buf = k & 1;
-                mbar_wait(BAR(ACC_EMPTY + buf), ((k >> 1) & 1) ^ 1);          // epilogue has drained this accumulator buffer
-                tc_fence_after();
-                uint32_t first = 0;
-                for (int g = 0; g < K.ngroups; ++g) {
-                    const UmmaGroup& G = K.groups[g];
-                    const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                    if (group_is_empty(L, G, tc.m_base)) continue;
-                    for (int c = 0; c < nchunk; ++c, ++jg) {
-                        const int st = jg % kSlabStages;
-                        mbar_wait(BAR(SLAB_FULL + st), (jg / kSlabStages) & 1);
-                        tc_fence_after();
-                        const uint32_t sa = smem_u32(slab0 + st * slab_bytes);
-                        const uint64_t a_hi0 = umma_desc(sa, atom_stride, 128), a_lo0 = umma_desc(sa + 2 * atom_stride, atom_stride, 128);
-                        for (int t0 = G.term_begin; t0 < G.term_end; t0 += TB, ++bg) {
-                            const int bs = bg % nbs;
-                            mbar_wait(BAR(B_FULL + bs), (bg / nbs) & 1);
-                            tc_fence_after();
-                            const uint32_t sb = smem_u32(bring0 + bs * bstage_bytes);
-                            const uint64_t b_hi0 = umma_desc(sb, b_lbo, 128), b_lo0 = umma_desc(sb + 16u * NPAD, b_lbo, 128);
-                            const int nt = min(TB, G.term_end - t0);
-                            if (L.consec) {
-                                const uint32_t sh = (uint32_t)(t0 - G.term_begin);
-                                const uint32_t ahw = umma_desc_lo(sa, atom_stride) + sh, alw = umma_desc_lo(sa + 2 * atom_stride, atom_stride) + sh;
-                                const uint32_t bhw = umma_desc_lo(sb, b_lbo), blw = umma_desc_lo(sb + 16u * NPAD, b_lbo);
-                                const uint32_t td0 = tmem_base + buf * acc_cols;
-                                if (L.fuse) {
-                                    const uint32_t idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NPAD >> 2) << 17) | ((128u >> 4) << 24);
-                                    if (L.MT == 2) issue_taps_fused<2>(ahw, alw, bhw, bblk_bytes >> 4, nt, td0, acc_w, idesc, idesc2, first);
-                                    else issue_taps_fused<1>(ahw, alw, bhw, bblk_bytes >> 4, nt, td0, acc_w, idesc, idesc2, first);
-                                } else if (L.MT == 2) issue_taps<2>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, td0, (uint32_t)NPAD, idesc, first);
-                                else issue_taps<1>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, td0, (uint32_t)NPAD, idesc, first);
-                            } else
-                            for (int tt = 0; tt < nt; ++tt) {
-                                const uint64_t boff = (uint64_t)((bblk_bytes >> 4) * tt);
-                                const uint64_t b_hi = b_hi0 + boff, b_lo = b_lo0 + boff;
-                                const uint64_t aoff = (uint64_t)(uint32_t)(L.d[t0 + tt] - G.dmin);
-                                for (int mt = 0; mt < L.MT; ++mt) {
-                                    const uint64_t a_hi = a_hi0 + aoff + (uint64_t)(128u * mt), a_lo = a_lo0 + aoff + (uint64_t)(128u * mt);
-                                    const uint32_t td = tmem_base + buf * acc_cols + (uint32_t)(mt * NPAD);
-                                    umma_bf16(td, a_lo, b_hi, idesc, first);
-                                    umma_bf16(td, a_hi, b_lo, idesc, 1u);
-                                    umma_bf16(td, a_hi, b_hi, idesc, 1u);
-                                }
-                                first = 1u;
-                            }
-                            umma_commit(BAR(B_EMPTY + bs));
-                        }
-                        umma_commit(BAR(SLAB_EMPTY + st));
-                    }
-                }
-                umma_commit(BAR(ACC_FULL + buf));
-            }
-        }
-        __syncwarp();
-    } else if (warp == kLoadWarp) {
-        // ===================== weight loader =====================
-        if (elect_one()) {
-            int bg = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                const TileCoord tc = decode_tile(L, t);
-                const UmmaClass& K = L.cls[tc.cls];
-                const uint8_t* src = K.wpack[tc.split];
-                size_t blk = 0;
-                for (int g = 0; g < K.ngroups; ++g) {
-                    const UmmaGroup& G = K.groups[g];
-                    const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                    const int nterm = G.term_end - G.term_begin;
-                    if (group_is_empty(L, G, tc.m_base)) { blk += (size_t)nchunk * nterm; continue; }
-                    for (int c = 0; c < nchunk; ++c)
-                        for (int t0 = 0; t0 < nterm; t0 += TB, ++bg) {
-                            const int nt = min(TB, nterm - t0);
-                            const int bs = bg % nbs;
-                            mbar_wait_bg(BAR(B_EMPTY + bs), ((bg / nbs) & 1) ^ 1);
-                            mbar_arrive_expect_tx(BAR(B_FULL + bs), bblk_bytes * nt);
-                            bulk_g2s(smem_u32(bring0 + bs * bstage_bytes), src + blk * bblk_bytes, bblk_bytes * nt, BAR(B_FULL + bs));
-                            blk += nt;
-                        }
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue warps: TMEM lane quarter = warp & 3 =====================
-        const int q4 = warp & 3;
-        const int eg = (warp - kEpiWarp0) >> 2;                // epilogue group (0 .. EPW-1)
-        // each group owns a FIXED column range of the staging tile (its k-th chunk of any block goes to stage_ofs + 16k): the chunk
-        // split differs between column blocks, and a group that runs ahead must never overwrite data the other has not written out
-        const int stage_ofs = (EPW == 2 && eg == 1) ? 16 * (((CW >> 4) + 1) >> 1) : 0;
-        int k = 0;
-        float o_lsum = 0.f;                                    // OUTL: this thread's share of the squared error
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++k) {
-            const TileCoord tc = decode_tile(L, t);
-            const UmmaClass& K = L.cls[tc.cls];
-            const int buf = k & 1;
-            const int n0 = tc.split * NPAD;
-            mbar_wait_bg(BAR(ACC_FULL + buf), (k >> 1) & 1);
-            tc_fence_after();
-            bool any_group = false;                      // all groups skipped as empty: the accumulator was never written = zeros
-            for (int g = 0; g < K.ngroups; ++g) any_group = any_group || !group_is_empty(L, K.groups[g], tc.m_base);
-            const int c0_last = min((NPAD - 1) / CW, (L.N - n0 - 1) / CW) * CW;      // last column block that holds real channels
-            for (int mt = 0; mt < L.MT; ++mt) {
-                float o_pre0[NC], o_pre1[NC];     // OUTL: output-conv pre-activations of this thread's row (two frames when pair-merged)
-#pragma unroll
-                for (int q = 0; q < NC; ++q) { o_pre0[q] = 0.f; o_pre1[q] = 0.f; }
-                // OUTL: everything the row's frames need from global memory (mix at the feature / output crop, targets incl. the
-                // difference source's) is requested HERE, so that the latency hides under the accumulator read-out below
-                float o_x0[2] = {0.f, 0.f}, o_x1[2] = {0.f, 0.f}, o_mo0[2] = {0.f, 0.f}, o_mo1[2] = {0.f, 0.f};
-                float o_tg0[NC + 2], o_tg1[NC + 2];
-                bool o_ok0 = false, o_ok1 = false;
-                if (OUTL) {
-                    const OutputLaunch& O = FP->O;
-                    const bool o_two = O.C == 2;                  // (C is 1 or 2: no runtime divisions in the unrolled code)
-                    const int m = tc.m_base + mt * 128 + q4 * 32 + lane;
-                    const long long src_stride = (long long)O.batch * O.T_out * O.C;
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        const int tt = FP->t0[tc.cls] + FP->t_step * m + hh;
-                        bool ok = (L.pairC > 0) ? (m >= K.out.lo_h[hh] && m < K.out.hi_h[hh]) : (hh == 0 && m < K.out.m_hi);
-                        ok = ok && tt < O.T_out;
-                        float* xm = hh ? o_x1 : o_x0;
-                        float* mo = hh ? o_mo1 : o_mo0;
-                        float* tg = hh ? o_tg1 : o_tg0;
-                        if (hh) o_ok1 = ok; else o_ok0 = ok;
-                        if (ok) {
-                            const float* mixrow = O.mix + ((long long)tc.b * O.T_in + O.crop_feat + tt) * O.C;
-                            const float* mixout = O.mix + ((long long)tc.b * O.T_in + O.crop_out + tt) * O.C;
-                            xm[0] = __ldg(mixrow); if (O.C > 1) xm[1] = __ldg(mixrow + 1);
-                            if (O.output_type == 1) { mo[0] = __ldg(mixout); if (O.C > 1) mo[1] = __ldg(mixout + 1); }
-                            if (O.targets) {
-                                const long long frame = ((long long)tc.b * O.T_out + tt) * O.C;
-#pragma unroll
-                                for (int q = 0; q < NC; ++q)
-                                    tg[q] = __ldg(O.targets + (long long)(o_two ? (q >> 1) : q) * src_stride + frame + (o_two ? (q & 1) : 0));
-                                if (O.output_type == 1) {
-                                    tg[NC] = __ldg(O.targets + (long long)O.nconv * src_stride + frame);
-                                    if (O.C > 1) tg[NC + 1] = __ldg(O.targets + (long long)O.nconv * src_stride + frame + 1);
-                                }
-                            }
-                        }
-                    }
-                }
-                for (int c0 = 0; c0 < NPAD; c0 += CW) {
-                    const bool last_block = (mt == L.MT - 1) && (c0 == c0_last);
-                    // this group's 16-column chunks of the block: [cb_lo, cb_hi)
-                    const int nch_blk = (min(CW, NPAD - c0) + 15) >> 4;
-                    const int cb_lo = (EPW == 2 && eg == 1) ? 16 * ((nch_blk + 1) >> 1) : 0;
-                    const int cb_hi = (EPW == 2 && eg == 0) ? 16 * ((nch_blk + 1) >> 1) : 16 * nch_blk;
-                    if (n0 + c0 < L.N) {
-                        for (int cb = cb_lo; cb < cb_hi; cb += 16) {
-                            __syncwarp();
-                            float v[16];
-                            tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + buf * acc_cols + (uint32_t)mt * acc_w + (uint32_t)(c0 + cb), v);
-                            if (L.fuse) {                     // second accumulator half: A_hi x B_lo
-                                float v2[16];
-                                tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + buf * acc_cols + (uint32_t)mt * acc_w + (uint32_t)(NPAD + c0 + cb), v2);
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) v[j] += v2[j];
-                            }
-                            if (!any_group) {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) v[j] = 0.f;
-                            }
-                            if (L.epilogue == EPI_BIAS_LRELU) {
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) {
-                                    const float y = v[j] + bias_s[n0 + c0 + cb + j];
-                                    v[j] = fmaxf(0.2f * y, y);
-                                }
-                            }
-                            float4* dst = reinterpret_cast<float4*>(stage + (size_t)(q4 * 32 + lane) * SW + stage_ofs + (cb - cb_lo));
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                            if (OUTL) {                      // 1x1 output convs: feature part of [crop(mix) || features] . W
-                                const int o_C = FP->O.C;
-#pragma unroll
-                                for (int j = 0; j < 16; ++j) {
-                                    const int col = c0 + cb + j;              // (nsplit == 1: n0 == 0)
-                                    if (col < L.N) {
-                                        const bool h1 = L.pairC > 0 && col >= L.pairC;       // uniform over the warp
-                                        const float* w = wout_s + (o_C + (h1 ? col - L.pairC : col)) * o_ncol;
-                                        if (h1) {
-#pragma unroll
-                                            for (int q = 0; q < NC; ++q) o_pre1[q] = fmaf(v[j], w[q], o_pre1[q]);
-                                        } else {
-#pragma unroll
-                                            for (int q = 0; q < NC; ++q) o_pre0[q] = fmaf(v[j], w[q], o_pre0[q]);
-                                        }
-                                    }
-                                }
-                            }
-                        }
-                    }
-                    if (last_block) {                       // every tcgen05.ld of this buffer has completed: hand it back
-                        tc_fence_before();
-                        mbar_arrive(BAR(ACC_EMPTY + buf));
-                    }
-                    float o_g0[NC], o_g1[NC];     // OUTL: dL/dpre of the row's frames
-                    if (OUTL) {
-                        const OutputLaunch& O = FP->O;
-                        const bool o_two = O.C == 2;
-                        const int r = q4 * 32 + lane, m = tc.m_base + mt * 128 + r;
-                        const long long src_stride = (long long)O.batch * O.T_out * O.C;
-#pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            float* pre = hh ? o_pre1 : o_pre0;
-                            float* g = hh ? o_g1 : o_g0;
-                            const float* xm = hh ? o_x1 : o_x0;
-                            const float* mo = hh ? o_mo1 : o_mo0;
-                            const float* tg = hh ? o_tg1 : o_tg0;
-#pragma unroll
-                            for (int q = 0; q < NC; ++q) g[q] = 0.f;
-                            const int tt = FP->t0[tc.cls] + FP->t_step * m + hh;
-                            if (hh ? o_ok1 : o_ok0) {
-#pragma unroll
-                                for (int c = 0; c < 2; ++c) {
-                                    if (c < O.C) {
-#pragma unroll
-                                        for (int q = 0; q < NC; ++q) pre[q] = fmaf(xm[c], wout_s[c * o_ncol + q], pre[q]);
-                                    }
-                                }
-                                float est[NC];
-#pragma unroll
-                                for (int q = 0; q < NC; ++q) {
-                                    float e = pre[q] + bout_s[q];
-                                    if (O.activation == 0) e = tanhf(e);                              // UnetAudioSeparator.py:131-136
-                                    else if (!O.training) e = fminf(fmaxf(e, -1.f), 1.f);             // AudioClip, Utils.py:89-92
-                                    est[q] = e;
-                                }
-                                const long long frame = ((long long)tc.b * O.T_out + tt) * O.C;
-                                float g_last[2] = {0.f, 0.f};
-                                if (O.output_type == 1) {                                             // OutputLayer.py:17-22
-#pragma unroll
-                                    for (int oc = 0; oc < 2; ++oc) {
-                                        if (oc >= O.C) continue;
-                                        float sacc = 0.f;
-#pragma unroll
-                                        for (int q = 0; q < NC; ++q) if ((o_two ? (q & 1) : 0) == oc) sacc += est[q];
-                                        float last = mo[oc] - sacc;
-                                        if (!O.training) last = fminf(fmaxf(last, -1.f), 1.f);
-                                        if (O.outputs) O.outputs[(long long)O.nconv * src_stride + frame + oc] = last;
-                                        if (O.targets) {
-                                            const float e = last - tg[NC + oc];
-                                            o_lsum = fmaf(e, e, o_lsum);
-                                            g_last[oc] = 2.f * e * O.inv_count;
-                                        }
-                                    }
-                                }
-#pragma unroll
-                                for (int q = 0; q < NC; ++q) {
-                                    const int conv = o_two ? (q >> 1) : q, oc = o_two ? (q & 1) : 0;
-                                    if (O.outputs) O.outputs[(long long)conv * src_stride + frame + oc] = est[q];
-                                    if (O.targets) {
-                                        const float e = est[q] - tg[q];
-                                        o_lsum = fmaf(e, e, o_lsum);
-                                        float gg = 2.f * e * O.inv_count - ((oc == 0) ? g_last[0] : g_last[1]);   // Training.py:62-63 / OutputLayer.py:20
-                                        if (O.activation == 0) gg *= (1.f - est[q] * est[q]);         // tanh'
-                                        if (O.dpre) O.dpre[((long long)tc.b * O.T_out + tt) * o_ncol + q] = gg;
-                                        g[q] = gg;
-                                    }
-                                }
-                            }
-                            if (FP->gfeat) {
-#pragma unroll
-                                for (int q = 0; q < NC; ++q) dpre_s[(r * 2 + hh) * o_ncol + q] = g[q];
-                            }
-                        }
-                    }
-                    if (n0 + c0 + cb_lo < L.N && cb_lo < cb_hi) {
-                        __syncwarp();
-                        // real columns of this group's share: launch columns [n0 + c0 + cb_lo, ...)
-                        const int ncols = min(cb_hi, L.N - (n0 + c0)) - cb_lo;
-                        const long long tile_off = (long long)tc.b * K.out.bstride + n0 + c0 + cb_lo;
-                        const bool vec = (ncols % 4 == 0) && (K.out.rstride % 4 == 0) && (((n0 + c0) & 3) == 0) &&
-                                         ((reinterpret_cast<uintptr_t>(K.out.base) & 15) == 0) && ((K.out.bstride & 3) == 0);
-                        const EpiBlock EB = epi_block<true>(K.out, tc.b, n0 + c0 + cb_lo, ncols >> 2, L.epilogue == EPI_SLOPE);
-                        const float* stage_g = stage + stage_ofs;
-                        if (vec) {
-                            if (DG) epi_write_rows_vec(stage_g, SW, q4 * 32, lane, ncols >> 2, tc.m_base + mt * 128 + q4 * 32, EB);
-                            else epi_write_rows_simple(stage_g, SW, q4 * 32, lane, ncols >> 2, tc.m_base + mt * 128 + q4 * 32, EB);
-                        } else {
-                            for (int it = lane; it < 32 * ncols; it += 32) {
-                                const int rl = it / ncols, j = it - rl * ncols;
-                                const int r = q4 * 32 + rl;
-                                const int m = tc.m_base + mt * 128 + r;
-                                if (m >= K.out.m_hi) continue;
-                                const long long roff = tile_off + (long long)m * K.out.rstride;
-                                float o = stage_g[(size_t)r * SW + j];
-                                if (L.epilogue == EPI_SLOPE && K.out.saved) o *= (__ldg(K.out.saved + roff + j) > 0.f) ? 1.f : 0.2f;
-                                float* dst = K.out.base + roff + j;
-                                if (m >= K.out.acc_lo && m < K.out.acc_hi) o += *dst;
-                                *dst = o;
-                            }
-                        }
-                        __syncwarp();
-                        if (OUTL && FP->gfeat) {
-                            const OutputLaunch& O = FP->O;
-                            // (a) gradient w.r.t. the features' pre-activation: slope(feature) * dpre . W^T, written with the feature
-                            //     tensor's geometry into its gradient twin (lanes over (row, quad) like the feature store above)
-                            const int Q = ncols >> 2;
-                            for (int it = lane; it < 32 * Q; it += 32) {
-                                const int rl = it / Q, qd = it - rl * Q, col = 4 * qd;
-                                const EpiHalf& H = (qd < EB.qsplit) ? EB.h[0] : EB.h[1];
-                                const int mrow = tc.m_base + mt * 128 + q4 * 32 + rl;
-                                if (mrow < H.lo || mrow >= H.hi) continue;
-                                float* fdst = H.dst + mrow * H.rstride + 4 * qd;
-                                const bool h1 = L.pairC > 0 && col >= L.pairC;
-                                const float4 f = *reinterpret_cast<const float4*>(stage + (size_t)(q4 * 32 + rl) * SW + col);
-                                const float* dp = dpre_s + ((q4 * 32 + rl) * 2 + (h1 ? 1 : 0)) * o_ncol;
-                                const float* w = wout_s + (O.C + (h1 ? col - L.pairC : col)) * o_ncol;
-                                float sx = 0.f, sy = 0.f, sz = 0.f, sw = 0.f;
-                                #pragma unroll
-                                for (int q = 0; q < NC; ++q) {
-                                    const float dq = dp[q];
-                                    sx = fmaf(dq, w[q], sx); sy = fmaf(dq, w[o_ncol + q], sy);
-                                    sz = fmaf(dq, w[2 * o_ncol + q], sz); sw = fmaf(dq, w[3 * o_ncol + q], sw);
-                                }
-                                float4 go;
-                                go.x = sx * ((f.x > 0.f) ? 1.f : 0.2f); go.y = sy * ((f.y > 0.f) ? 1.f : 0.2f);
-                                go.z = sz * ((f.z > 0.f) ? 1.f : 0.2f); go.w = sw * ((f.w > 0.f) ? 1.f : 0.2f);
-                                *reinterpret_cast<float4*>(FP->gfeat + (fdst - O.feat)) = go;
-                            }
-                            // (b) output-conv weight / bias gradients: thread = its own row again, warp-reduced, summed per warp in shared memory
-                            const int r = q4 * 32 + lane;
-                            if (FP->grads)
-                            for (int cin = 0; cin <= o_cin; ++cin) {
-                                float x0, x1;
-                                if (cin < O.C) { x0 = (cin == 0) ? o_x0[0] : o_x0[1]; x1 = (cin == 0) ? o_x1[0] : o_x1[1]; }
-                                else if (cin < o_cin) {
-                                    x0 = stage[(size_t)r * SW + (cin - O.C)];
-                                    x1 = (L.pairC > 0) ? stage[(size_t)r * SW + L.pairC + (cin - O.C)] : 0.f;
-                                } else { x0 = 1.f; x1 = 1.f; }
-#pragma unroll
-                                for (int q = 0; q < NC; ++q) {
-                                    float val = fmaf(x0, o_g0[q], x1 * o_g1[q]);
-#pragma unroll
-                                    for (int off = 16; off > 0; off >>= 1) val += __shfl_xor_sync(0xffffffffu, val, off);
-                                    if (lane == 0) wacc_s[q4 * o_nw + cin * o_ncol + q] += val;
-                                }
-                            }
-                            __syncwarp();
-                        }
-                    }
-                }
-            }
-        }
-        if (OUTL) {
-            const OutputLaunch& O = FP->O;
-            if (O.targets && O.loss) {
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) o_lsum += __shfl_xor_sync(0xffffffffu, o_lsum, off);
-                if (lane == 0) atomicAdd(O.loss, o_lsum * O.inv_count);
-            }
-            if (FP->grads) {
-                __syncwarp();
-                for (int i = lane; i < o_nw; i += 32) {
-                    const int cin = i / o_ncol, q = i - cin * o_ncol, conv = q / O.C, oc = q - conv * O.C;
-                    const long long off = (cin < o_cin) ? O.w_off[conv] + (long long)cin * O.C + oc : O.b_off[conv] + oc;
-                    atomicAdd(FP->grads + off, wacc_s[q4 * o_nw + i] * FP->grad_scale);
-                }
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == kMmaWarp) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, L.tmem_cols);
-    }
-}
-
-template <int PT, bool DG>
-__global__ void __launch_bounds__(PT * 128 + 192, 1) plane_conv_umma_persistent(const __grid_constant__ UmmaLaunch L, int total_tiles) {
-    persistent_body<PT, DG, 0, 1>(L, total_tiles, nullptr);
-}
-// two epilogue warp groups and two converter teams (UmmaLaunch::epi2): the dgrad launches, optionally the forward ones
-__global__ void __launch_bounds__(2 * 128 + 64 + 256, 1) plane_conv_umma_persistent_dg2(const __grid_constant__ UmmaLaunch L, int total_tiles) {
-    persistent_body<2, true, 0, 2>(L, total_tiles, nullptr);
-}
-__global__ void __launch_bounds__(2 * 128 + 64 + 256, 1) plane_conv_umma_persistent_fw2(const __grid_constant__ UmmaLaunch L, int total_tiles) {
-    persistent_body<2, false, 0, 2>(L, total_tiles, nullptr);
-}
-// the last up block's forward conv with the output layer, the loss and the output layer's backward in its epilogue (OutputFuse);
-// NCOL = nconv * C of the output convs
-template <int NCOL>
-__global__ void __launch_bounds__(3 * 128 + 192, 1) plane_conv_umma_persistent_out(const __grid_constant__ UmmaLaunch L, int total_tiles,
-                                                                                 const __grid_constant__ OutputFuse F) {
-    persistent_body<3, false, NCOL, 1>(L, total_tiles, &F);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Batch-folded cluster split-K variant for the deep layers (down7 ... up7 at training batch sizes, everything at small
-// batch): a class there has only a handful of rows per batch item (M4: 23 + 8 at down11, 5 + 4 at the bottleneck), so
-// one 128-row tile per (item, class) wastes most of the M dimension, and the few CTAs each walk the whole
-// (plane, chunk, tap) K loop and stream the whole weight set on their own (64 CTAs x 75 us at 1-3 % of the FLOPs).
-//   * FOLDING: the rows of all batch items form one virtual row sequence, item b at [b*pitch, b*pitch + rows) with
-//     pitch = rows + widest tap span.  A slab row u maps to (item u / pitch, plane row m_lo + u % pitch + dmin); output
-//     row v of item v / pitch reads slab rows v + (d - dmin) which stay inside the same item's segment, so the tap shifts
-//     of the MMAs are unchanged; accumulator rows with v % pitch >= rows are discarded.  Tiles may straddle items.
-//   * SPLIT-K OVER A CLUSTER: the L.ksplit CTAs of a cluster share one tile; CTA k takes a contiguous range of the
-//     tile's (plane, 16-channel chunk) jobs (and only streams those jobs' weights), dumps its partial accumulator to its
-//     own shared memory, and after a cluster barrier every CTA reduces + finishes (bias / LeakyReLU / slope / accumulate)
-//     a 1/ksplit share of the tile's rows, reading the partials of its peers through distributed shared memory.
-// grid = (tiles * ksplit, nsplit, classes), cluster = (ksplit, 1, 1); warps as in plane_conv_umma_kernel<4>.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ float4 ld_dsmem_v4(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-
-constexpr int kFoldTeams = 4, kFoldSlabStages = 6, kFoldMaxSplit = 8;
-
-__global__ void __launch_bounds__(kFoldTeams * 128 + 64, 1) plane_conv_umma_fold(const __grid_constant__ UmmaLaunch L) {
-    constexpr int kMmaWarp = kFoldTeams * 4;
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (tid == 0) T_MARK(0);
-    const int cls = blockIdx.z, split = blockIdx.y;
-    const int S = L.ksplit;
-    const int tile = blockIdx.x / S;
-    const int krank = (int)cluster_ctarank();
-    const UmmaClass& K = L.cls[cls];
-    const int pitch = L.fold_pitch[cls];
-    const int rows_q = K.out.m_hi - K.out.m_lo;
-    const int RT = L.MT * 128;
-    const int v0 = tile * RT;
-    if (rows_q <= 0 || v0 >= L.batch * pitch) return;        // the whole cluster (same tile, same class) leaves together
-
-    int J = 0;                                               // (plane, chunk) jobs of this class; this CTA takes [j0, j1)
-    for (int g = 0; g < K.ngroups; ++g) J += (L.planes[K.groups[g].plane].C + 15) >> 4;
-    const int j0 = (int)((long long)J * krank / S), j1 = (int)((long long)J * (krank + 1) / S);
-    const bool has_work = j1 > j0;
-
-    const int NPAD = L.NPAD;
-    const uint32_t slab_bytes = 64u * L.rows_alloc;
-    const uint32_t bblk_bytes = 64u * NPAD;
-    uint8_t* slab0 = smem;
-    uint8_t* bring0 = smem + kFoldSlabStages * slab_bytes;
-    const int TB = L.TB, nbs = L.nbs;
-    const uint32_t bstage_bytes = bblk_bytes * TB;
-    // the partial-accumulator tile (RT x (NPAD+4) fp32) re-uses the pipeline memory once every MMA has retired
-    const int SWF = NPAD + 4;
-    const uint32_t pipe_bytes = kFoldSlabStages * slab_bytes + nbs * bstage_bytes;
-    const uint32_t part_bytes = (uint32_t)RT * (uint32_t)SWF * 4u;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((pipe_bytes > part_bytes ? pipe_bytes : part_bytes) + 127u) / 128u * 128u);
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    const int SLAB_FULL = 0, SLAB_EMPTY = kFoldSlabStages, B_FULL = 2 * kFoldSlabStages, B_EMPTY = 2 * kFoldSlabStages + kBStagesMax,
-              ACC_FULL = 2 * kFoldSlabStages + 2 * kBStagesMax;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + ACC_FULL + 1);
-    float* bias_s = reinterpret_cast<float*>(tmem_holder + 4);
-    for (int i = tid; i < NPAD; i += blockDim.x) {
+    for (int i = tid; i < NPAD; i += kConvThreads) {
         const int n = split * NPAD + i;
         bias_s[i] = (L.bias && n < L.N) ? __ldg(L.bias + ((L.pairC > 0 && n >= L.pairC) ? n - L.pairC : n)) : 0.f;
     }
     if (tid == 0) {
-        for (int i = 0; i < kFoldSlabStages; ++i) { mbar_init(BAR(SLAB_FULL + i), kWorkerThreads); mbar_init(BAR(SLAB_EMPTY + i), 1); }
-        for (int i = 0; i < kBStagesMax; ++i) { mbar_init(BAR(B_FULL + i), 1); mbar_init(BAR(B_EMPTY + i), 1); }
-        mbar_init(BAR(ACC_FULL), 1);
+        for (int i = 0; i < L.nbs; ++i) mbar_init(bar0 + 8u * i, 1);
         fence_barrier_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(smem_u32(tmem_holder), L.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    if (tid == 0) T_MARK(1);
 
-    if (warp < kMmaWarp) {
-        // ===================== converters: fill the slabs of this CTA's jobs =====================
-        const int team = warp >> 2, ttid = tid & 127;
-        int ji = 0;
-        for (int g = 0; g < K.ngroups; ++g) {
-            const UmmaGroup& G = K.groups[g];
-            const PlaneView& P = L.planes[G.plane];
-            const int nchunk = (P.C + 15) >> 4;
-            for (int c = 0; c < nchunk; ++c, ++ji) {
-                if (ji < j0 || ji >= j1) continue;
-                const int jl = ji - j0;
-                if ((jl % kFoldTeams) != team) continue;
-                const int st = jl % kFoldSlabStages;
-                uint8_t* Sl = slab0 + st * slab_bytes;
-                const uint32_t atom_stride = 16u * L.rows_alloc;
-                if (!(L.fold_flags & 1)) {
-                constexpr int kRB = WUN_KRB;
-                bool waited = false;
-                for (int rbase = 0; rbase < L.rows_alloc; rbase += kRB * kWorkerThreads) {
-                    float x[kRB][16];
+    const uint8_t* wsrc = K.wpack[split];
+    auto load_weights = [&](int stage, const ConvStep& s) {
+        const uint32_t bar = bar0 + 8u * stage;
+        mbar_arrive_expect_tx(bar, blk_bytes * s.nt);
+        bulk_g2s(smem_u32(ring + stage * stage_bytes), wsrc + (size_t)s.blk * blk_bytes, blk_bytes * s.nt, bar);
+    };
+    ConvStep cur = {-1, 0, 0, 0, 0};
+    bool more = next_step(L, K, m_base, cur);
+    ConvStep ld = cur;                  // thread 0: the next step whose weights are still to be loaded
+    bool ld_more = more;
+    if (tid == 0)
+        for (int i = 0; i < L.nbs - 1 && ld_more; ++i) { load_weights(i, ld); ld_more = next_step(L, K, m_base, ld); }
+    if (more) fill_slab(L, K.groups[cur.g], b, m_base, cur.c, smem);
+    fence_proxy_async();                // generic-proxy slab writes -> visible to the tensor core (async proxy)
+    __syncthreads();
+
+    float acc[NPAD / 2];
 #pragma unroll
-                    for (int w = 0; w < kRB; ++w) {
-                        const int rr = rbase + w * kWorkerThreads + ttid;
-                        if (rr < L.rows_alloc) {
-                            const int u = v0 + rr, bb = u / pitch, off = u - bb * pitch;     // virtual row -> (item, row)
-                            load_row16(P, bb, (bb < L.batch) ? K.out.m_lo + off + G.dmin : -(1 << 30), c * 16, x[w]);
-                        }
-                    }
-                    if (!waited) { mbar_wait_bg(BAR(SLAB_EMPTY + st), ((jl / kFoldSlabStages) & 1) ^ 1); waited = true; }
-#pragma unroll
-                    for (int w = 0; w < kRB; ++w) {
-                        const int rr = rbase + w * kWorkerThreads + ttid;
-                        if (rr >= L.rows_alloc) continue;
-                        uint32_t hi[8], lo[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const __nv_bfloat16 h0 = __float2bfloat16_rn(x[w][2 * i]), h1 = __float2bfloat16_rn(x[w][2 * i + 1]);
-                            hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                            lo[i] = pack_bf16x2(x[w][2 * i] - __bfloat162float(h0), x[w][2 * i + 1] - __bfloat162float(h1));
-                        }
-                        *reinterpret_cast<uint4*>(Sl + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                        *reinterpret_cast<uint4*>(Sl + atom_stride + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                        *reinterpret_cast<uint4*>(Sl + 2 * atom_stride + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                        *reinterpret_cast<uint4*>(Sl + 3 * atom_stride + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                    }
-                }
-                } else {
-                // One row per thread and pass, NOT the 3-row unrolled batches of the long-running kernels: these launches live
-                // ~20 us, and the cold instruction fetch of a 250-instruction straight-line body cost more than the load
-                // latency it hid (fold trace: first slab ready 7-14 k cycles after kernel start).
-                bool waited = false;
-#pragma unroll 1
-                for (int rr = ttid; rr < L.rows_alloc; rr += kWorkerThreads) {
-                    float x[16];
-                    const int u = v0 + rr, bb = u / pitch, off = u - bb * pitch;             // virtual row -> (item, row)
-                    load_row16(P, bb, (bb < L.batch) ? K.out.m_lo + off + G.dmin : -(1 << 30), c * 16, x);
-                    if (!waited) { mbar_wait_bg(BAR(SLAB_EMPTY + st), ((jl / kFoldSlabStages) & 1) ^ 1); waited = true; }
-                    uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const __nv_bfloat16 h0 = __float2bfloat16_rn(x[2 * i]), h1 = __float2bfloat16_rn(x[2 * i + 1]);
-                        hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                        lo[i] = pack_bf16x2(x[2 * i] - __bfloat162float(h0), x[2 * i + 1] - __bfloat162float(h1));
-                    }
-                    *reinterpret_cast<uint4*>(Sl + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-                    *reinterpret_cast<uint4*>(Sl + atom_stride + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                    *reinterpret_cast<uint4*>(Sl + 2 * atom_stride + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                    *reinterpret_cast<uint4*>(Sl + 3 * atom_stride + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                }
-                if (!waited) mbar_wait_bg(BAR(SLAB_EMPTY + st), ((jl / kFoldSlabStages) & 1) ^ 1);
-                }
-                fence_proxy_async();
-                mbar_arrive(BAR(SLAB_FULL + st));
-                if (tid == 0 && jl == 0) T_MARK(2);
-            }
+    for (int i = 0; i < NPAD / 2; ++i) acc[i] = 0.f;
+    int slab = 0;
+    for (int s = 0; more; ++s) {
+        // the ring stage of step s + nbs - 1 was last read by step s - 1, whose MMAs every thread has waited for
+        if (tid == 0 && ld_more) { load_weights((s + L.nbs - 1) % L.nbs, ld); ld_more = next_step(L, K, m_base, ld); }
+        const int st = s % L.nbs;
+        mbar_wait(bar0 + 8u * st, (s / L.nbs) & 1);
+        const UmmaGroup& G = K.groups[cur.g];
+        const uint32_t sa = smem_u32(smem + slab * slab_bytes) + 64u * 16u * wg;
+        const uint32_t sb = smem_u32(ring + st * stage_bytes);
+        wgmma_fence();
+        for (int tt = 0; tt < cur.nt; ++tt) {
+            const uint32_t a = sa + 16u * (uint32_t)(L.d[G.term_begin + cur.t0 + tt] - G.dmin);
+            const uint32_t bb = sb + tt * blk_bytes;
+            const uint64_t a_hi = gmma_desc(a, atom, 128), a_lo = gmma_desc(a + 2 * atom, atom, 128);
+            const uint64_t b_hi = gmma_desc(bb, 32u * NPAD, 128), b_lo = gmma_desc(bb + 16u * NPAD, 32u * NPAD, 128);
+            wgmma_tile<NPAD, 0, 0>(acc, a_lo, b_hi, 8);
+            wgmma_tile<NPAD, 0, 0>(acc, a_hi, b_lo, 8);
+            wgmma_tile<NPAD, 0, 0>(acc, a_hi, b_hi, 8);
         }
-        if (tid == 0) T_MARK(3);
-        // ===================== team 0: partial accumulator -> own shared memory (TMEM lane quarter = warp id) ==========
-        if (team == 0) {
-            float* part = reinterpret_cast<float*>(smem);
-            if (has_work) { mbar_wait_bg(BAR(ACC_FULL), 0); tc_fence_after(); }
-            if (tid == 0) T_MARK(4);
-            for (int mt = 0; mt < L.MT; ++mt)
-                for (int cb = 0; cb < NPAD; cb += 16) {
-                    __syncwarp();
-                    float v[16];
-                    if (has_work) tmem_ld16(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(mt * NPAD + cb), v);
-                    else {
+        wgmma_commit();
+        ConvStep nx = cur;
+        more = next_step(L, K, m_base, nx);
+        const bool new_slab = more && nx.t0 == 0;
+        // convert the next (group, chunk) into the other slab while the MMAs run; its last reader was the previous job
+        if (new_slab) fill_slab(L, K.groups[nx.g], b, m_base, nx.c, smem + (slab ^ 1) * slab_bytes);
+        wgmma_wait_all();
+        acc_fence<NPAD / 2>(acc);
+        fence_proxy_async();
+        __syncthreads();
+        if (new_slab) slab ^= 1;
+        cur = nx;
+    }
+
+    // ===================== epilogue =====================
+    // every MMA has retired and every weight copy has landed: the pipeline memory becomes the staging tile
+    float* stage = reinterpret_cast<float*>(smem);
+    constexpr int SW = NPAD + 4;                             // padded row stride (floats)
 #pragma unroll
-                        for (int j = 0; j < 16; ++j) v[j] = 0.f;
-                    }
-                    float4* dst = reinterpret_cast<float4*>(part + (size_t)(mt * 128 + warp * 32 + lane) * SWF + cb);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) dst[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                }
-            tc_fence_before();
-            if (tid == 0) T_MARK(5);
+    for (int i = 0; i < NPAD / 2; i += 2) {
+        const int col = acc_col(i, lane), row = 64 * wg + acc_row(i, warp, lane);
+        float v0 = acc[i], v1 = acc[i + 1];
+        if (L.epilogue == EPI_BIAS_LRELU) {
+            v0 += bias_s[col]; v1 += bias_s[col + 1];
+            v0 = fmaxf(0.2f * v0, v0); v1 = fmaxf(0.2f * v1, v1);
         }
-    } else if (warp == kMmaWarp) {
-        // ===================== MMA issuer =====================
-        if (has_work && elect_one()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NPAD >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t atom_stride = 16u * L.rows_alloc;
-            const uint32_t b_lbo = 32u * NPAD;
-            int ji = 0, bi = 0;
-            uint32_t first = 0;
-            for (int g = 0; g < K.ngroups; ++g) {
-                const UmmaGroup& G = K.groups[g];
-                const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                for (int c = 0; c < nchunk; ++c, ++ji) {
-                    if (ji < j0 || ji >= j1) continue;
-                    const int jl = ji - j0;
-                    const int st = jl % kFoldSlabStages;
-                    mbar_wait(BAR(SLAB_FULL + st), (jl / kFoldSlabStages) & 1);
-                    tc_fence_after();
-                    if (jl == 0) T_MARK(8);
-                    const uint32_t sa = smem_u32(slab0 + st * slab_bytes);
-                    const uint64_t a_hi0 = umma_desc(sa, atom_stride, 128), a_lo0 = umma_desc(sa + 2 * atom_stride, atom_stride, 128);
-                    for (int t0 = G.term_begin; t0 < G.term_end; t0 += TB, ++bi) {
-                        const int bs = bi % nbs;
-                        mbar_wait(BAR(B_FULL + bs), (bi / nbs) & 1);
-                        tc_fence_after();
-                        if (bi == 0) T_MARK(9);
-                        if (bi == 1) T_MARK(10);
-                        if (bi == 4) T_MARK(11);
-                        const uint32_t sb = smem_u32(bring0 + bs * bstage_bytes);
-                        const uint64_t b_hi0 = umma_desc(sb, b_lbo, 128), b_lo0 = umma_desc(sb + 16u * NPAD, b_lbo, 128);
-                        const int nt = min(TB, G.term_end - t0);
-                        if (L.consec) {
-                            const uint32_t sh = (uint32_t)(t0 - G.term_begin);
-                            const uint32_t ahw = umma_desc_lo(sa, atom_stride) + sh, alw = umma_desc_lo(sa + 2 * atom_stride, atom_stride) + sh;
-                            const uint32_t bhw = umma_desc_lo(sb, b_lbo), blw = umma_desc_lo(sb + 16u * NPAD, b_lbo);
-                            if (L.MT == 2) issue_taps<2>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, tmem_base, (uint32_t)NPAD, idesc, first);
-                            else issue_taps<1>(ahw, alw, bhw, blw, bblk_bytes >> 4, nt, tmem_base, (uint32_t)NPAD, idesc, first);
-                        } else
-                        for (int tt = 0; tt < nt; ++tt) {
-                            const uint64_t boff = (uint64_t)((bblk_bytes >> 4) * tt);
-                            const uint64_t b_hi = b_hi0 + boff, b_lo = b_lo0 + boff;
-                            const uint64_t aoff = (uint64_t)(uint32_t)(L.d[t0 + tt] - G.dmin);
-                            for (int mt = 0; mt < L.MT; ++mt) {
-                                const uint64_t a_hi = a_hi0 + aoff + (uint64_t)(128u * mt), a_lo = a_lo0 + aoff + (uint64_t)(128u * mt);
-                                const uint32_t td = tmem_base + (uint32_t)(mt * NPAD);
-                                umma_bf16(td, a_lo, b_hi, idesc, first);
-                                umma_bf16(td, a_hi, b_lo, idesc, 1u);
-                                umma_bf16(td, a_hi, b_hi, idesc, 1u);
-                            }
-                            first = 1u;
-                        }
-                        umma_commit(BAR(B_EMPTY + bs));
-                    }
-                    umma_commit(BAR(SLAB_EMPTY + st));
-                }
-            }
-            umma_commit(BAR(ACC_FULL));
-            T_MARK(12);
-        }
-        __syncwarp();
-    } else {
-        // ===================== weight loader: only the blocks of this CTA's jobs =====================
-        if (has_work && elect_one()) {
-            const uint8_t* src = K.wpack[split];
-            if (L.fold_flags & 2) {   // ask L2 for this CTA's whole weight range up front: the packs were written at the start of the step and have
-                // usually been evicted since; the ring below then streams L2 hits instead of waiting for HBM stage by stage
-                size_t b0 = 0, b1 = 0;
-                int jj = 0;
-                for (int g = 0; g < K.ngroups; ++g) {
-                    const int nchunk = (L.planes[K.groups[g].plane].C + 15) >> 4;
-                    const int nterm = K.groups[g].term_end - K.groups[g].term_begin;
-                    for (int c = 0; c < nchunk; ++c, ++jj) {
-                        if (jj < j0) b0 += nterm;
-                        if (jj < j1) b1 += nterm;
-                    }
-                }
-                for (size_t b = b0; b < b1; b += 4) {
-                    const uint32_t bytes = (uint32_t)((b1 - b < 4 ? b1 - b : 4) * bblk_bytes);
-                    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src + b * bblk_bytes), "r"(bytes) : "memory");
-                }
-            }
-            int bi = 0, ji = 0;
-            size_t blk = 0;
-            for (int g = 0; g < K.ngroups; ++g) {
-                const UmmaGroup& G = K.groups[g];
-                const int nchunk = (L.planes[G.plane].C + 15) >> 4;
-                const int nterm = G.term_end - G.term_begin;
-                for (int c = 0; c < nchunk; ++c, ++ji) {
-                    if (ji < j0 || ji >= j1) { blk += nterm; continue; }
-                    for (int t0 = 0; t0 < nterm; t0 += TB, ++bi) {
-                        const int nt = min(TB, nterm - t0);
-                        const int bs = bi % nbs;
-                        mbar_wait_bg(BAR(B_EMPTY + bs), ((bi / nbs) & 1) ^ 1);
-                        mbar_arrive_expect_tx(BAR(B_FULL + bs), bblk_bytes * nt);
-                        bulk_g2s(smem_u32(bring0 + bs * bstage_bytes), src + blk * bblk_bytes, bblk_bytes * nt, BAR(B_FULL + bs));
-                        blk += nt;
-                    }
-                }
-            }
-        }
-        __syncwarp();
+        *reinterpret_cast<float2*>(stage + row * SW + col) = make_float2(v0, v1);
     }
     __syncthreads();
-    if (warp == kMmaWarp) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, L.tmem_cols);
-    }
-    if (tid == 0) T_MARK(6);
-    cluster_sync_all();                                   // every CTA of the cluster has published its partial tile
-    if (tid == 0) T_MARK(7);
-    {
-        // ===================== reduce + finish a 1/S share of the tile's rows (all threads) =====================
-        uint32_t peer[kFoldMaxSplit];
-#pragma unroll
-        for (int s = 0; s < kFoldMaxSplit; ++s) peer[s] = (s < S) ? mapa_shared(smem_u32(smem), (uint32_t)s) : 0u;
-        const int r0 = RT * krank / S, r1 = RT * (krank + 1) / S;
-        const int n0 = split * NPAD;
-        const int Q = min(NPAD, L.N - n0) >> 2;              // real output columns of this split / 4 (host: N % 4 == 0)
-        for (int it = tid; it < (r1 - r0) * Q; it += blockDim.x) {
-            const int rl = it / Q, q = it - rl * Q;
-            const int r = r0 + rl;
-            const int v = v0 + r, bb = v / pitch, off = v - bb * pitch;
-            if (bb >= L.batch || off >= rows_q) continue;     // padding rows between the items' segments
-            const int m = K.out.m_lo + off;
-            const uint32_t eoff = ((uint32_t)r * (uint32_t)SWF + 4u * (uint32_t)q) * 4u;
-            float4 part[kFoldMaxSplit];                          // all peer loads in flight together, then the sum
-#pragma unroll
-            for (int s = 0; s < kFoldMaxSplit; ++s)
-                part[s] = (s < S) ? ld_dsmem_v4(peer[s] + eoff) : make_float4(0.f, 0.f, 0.f, 0.f);
-            float4 o = part[0];
-#pragma unroll
-            for (int s = 1; s < kFoldMaxSplit; ++s) { o.x += part[s].x; o.y += part[s].y; o.z += part[s].z; o.w += part[s].w; }
-            if (L.epilogue == EPI_BIAS_LRELU) {
-                o.x += bias_s[4 * q]; o.y += bias_s[4 * q + 1]; o.z += bias_s[4 * q + 2]; o.w += bias_s[4 * q + 3];
-                o.x = fmaxf(0.2f * o.x, o.x); o.y = fmaxf(0.2f * o.y, o.y); o.z = fmaxf(0.2f * o.z, o.z); o.w = fmaxf(0.2f * o.w, o.w);
-            }
-            const long long roff = (long long)bb * K.out.bstride + n0 + (long long)m * K.out.rstride;
-            if (L.epilogue == EPI_SLOPE && K.out.saved) {
-                const float4 sv = __ldg(reinterpret_cast<const float4*>(K.out.saved + roff) + q);
-                o.x *= (sv.x > 0.f) ? 1.f : 0.2f; o.y *= (sv.y > 0.f) ? 1.f : 0.2f;
-                o.z *= (sv.z > 0.f) ? 1.f : 0.2f; o.w *= (sv.w > 0.f) ? 1.f : 0.2f;
-            }
-            float4* dst = reinterpret_cast<float4*>(K.out.base + roff) + q;
-            if (m >= K.out.acc_lo && m < K.out.acc_hi) { const float4 old = *dst; o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w; }
+    const int n0 = split * NPAD;
+    const int ncols = min(NPAD, L.N - n0);
+    if (ncols <= 0) return;
+    const bool vec = (ncols % 4 == 0) && (K.out.rstride % 4 == 0) && ((reinterpret_cast<uintptr_t>(K.out.base) & 15) == 0) &&
+                     ((K.out.bstride & 3) == 0);
+    if (vec) {      // (pair-merged classes always take this path: the planner checks both views)
+        // warp w writes rows 32 (w % 4) + [0, 32) of one half of the column quads
+        const int Q = ncols >> 2, Qa = (Q + 1) >> 1;
+        const int q0 = (warp >= 4) ? Qa : 0, nq = (warp >= 4) ? Q - Qa : Qa;
+        if (nq <= 0) return;
+        const EpiBlock EB = epi_block<true>(K.out, b, n0 + 4 * q0, nq, L.epilogue == EPI_SLOPE);
+        if (DG) epi_write_rows_vec(stage + 4 * q0, SW, (warp & 3) * 32, lane, nq, m_base + (warp & 3) * 32, EB);
+        else epi_write_rows_simple(stage + 4 * q0, SW, (warp & 3) * 32, lane, nq, m_base + (warp & 3) * 32, EB);
+    } else {
+        const long long tile_off = (long long)b * K.out.bstride + n0;
+        for (int it = tid; it < 128 * ncols; it += kConvThreads) {
+            const int r = it / ncols, j = it - r * ncols;
+            const int m = m_base + r;
+            if (m >= K.out.m_hi) continue;
+            const long long roff = tile_off + (long long)m * K.out.rstride;
+            float o = stage[r * SW + j];
+            if (L.epilogue == EPI_SLOPE && K.out.saved) o *= (__ldg(K.out.saved + roff + j) > 0.f) ? 1.f : 0.2f;
+            float* dst = K.out.base + roff + j;
+            if (m >= K.out.acc_lo && m < K.out.acc_hi) o += *dst;
             *dst = o;
         }
     }
-    if (tid == 0) T_MARK(13);
-    cluster_sync_all();                                   // nobody leaves while a peer may still read its shared memory
-    if (tid == 0) T_MARK(14);
 }
 
-#ifdef WUN_UMMA_TIMING
-}  // namespace wun
-// timing builds only (tools/fold_trace.py): the clock64 marks CTA (0,0,0) of the last plane_conv_umma_fold launch left
-extern "C" int wun_debug_fold_trace(unsigned long long* out, int n) {
-    if (n > 32) n = 32;
-    return (int)cudaMemcpyFromSymbol(out, wun::g_fold_trace, sizeof(unsigned long long) * n);
-}
-namespace wun {
-#endif
+size_t umma_smem_bytes(const UmmaLaunch& L) { return conv_smem_bytes(L.NPAD, L.rows_alloc, L.TB, L.nbs); }
+size_t umma_choice_smem_bytes(const UmmaChoice& ch) { return conv_smem_bytes(ch.NPAD, ch.rows_alloc, ch.TB, ch.nbs); }
 
-static size_t umma_fold_smem_bytes(const UmmaLaunch& L) {
-    const size_t pipe = (size_t)kFoldSlabStages * 64u * L.rows_alloc + (size_t)L.nbs * L.TB * 64u * L.NPAD;
-    const size_t part = (size_t)L.MT * 128u * ((size_t)L.NPAD + 4u) * 4u;
-    return ((pipe > part ? pipe : part) + 127) / 128 * 128 + (2 * kFoldSlabStages + 2 * kBStagesMax + 1) * 8 + 32 + 4 * (size_t)L.NPAD;
-}
+// The output layer stays in its own kernels (kernels_simt.cu): the conv epilogue holds 64 x NPAD accumulators per warpgroup in
+// registers, which leaves no room for the output convs, the loss and their gradients.
+bool umma_output_fusable(const ConvLaunch&, const UmmaChoice&, const OutputLaunch&) { return false; }
 
-static cudaError_t launch_plane_conv_fold(const UmmaLaunch& L, cudaStream_t stream) {
+constexpr int kConvSmemMax = 200 * 1024;      // opt-in limit set for every conv instantiation (the planner stays far below)
+
+template <int NPAD>
+static cudaError_t launch_conv_npad(const UmmaLaunch& L, dim3 grid, size_t smem, cudaStream_t stream) {
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(plane_conv_umma_fold, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+        cudaError_t e = cudaFuncSetAttribute(plane_conv_umma_kernel<NPAD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmemMax);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(plane_conv_umma_kernel<NPAD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kConvSmemMax);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    int max_tiles = 0;
-    for (int q = 0; q < L.ncls; ++q) {
-        const int rows = L.cls[q].out.m_hi - L.cls[q].out.m_lo;
-        if (rows <= 0) continue;
-        max_tiles = max(max_tiles, (L.batch * L.fold_pitch[q] + L.MT * 128 - 1) / (L.MT * 128));
-    }
-    if (max_tiles <= 0) return cudaSuccess;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)(max_tiles * L.ksplit), (unsigned)L.nsplit, (unsigned)L.ncls);
-    cfg.blockDim = dim3(kFoldTeams * 128 + 64);
-    cfg.dynamicSmemBytes = umma_fold_smem_bytes(L);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr;
-    memset(&attr, 0, sizeof(attr));
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = (unsigned)L.ksplit; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-    cfg.attrs = &attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, plane_conv_umma_fold, L);
-}
-
-static size_t umma_pers_smem_bytes(const UmmaLaunch& L) {
-    const size_t CW = (L.NPAD < 128) ? L.NPAD : 128;
-    const size_t kSlabStages = (L.nteams == 3) ? 4 : 3;
-    return (size_t)kSlabStages * 64u * L.rows_alloc + (size_t)L.nbs * L.TB * 64u * L.NPAD + 128u * (CW + 4) * 4 +
-           (2 * kSlabStages + 2 * kBStagesMax + 4) * 8 + 32 + 4 * (size_t)L.NPAD * L.nsplit;
-}
-
-size_t umma_smem_bytes(const UmmaLaunch& L) {
-    const size_t nslab = (L.nteams == 4) ? 6 : 3;
-    const size_t pipe = nslab * 64u * L.rows_alloc + (size_t)L.nbs * L.TB * 64u * L.NPAD;
-    const size_t epi = 128u * ((size_t)(L.NPAD < 128 ? L.NPAD : 128) + 4u) * 4u;
-    return ((pipe > epi ? pipe : epi) + 127) / 128 * 128 + (2 * 6 + 2 * kBStagesMax + 1) * 8 + 32 + 4 * L.NPAD;
-}
-
-template <typename KernelT>
-static cudaError_t set_smem_limit(KernelT kernel, int bytes) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-
-static size_t umma_outfuse_smem_bytes(const OutputLaunch& O) {
-    const size_t ncol = (size_t)O.nconv * O.C, cin = (size_t)O.C + O.F;
-    return 4 * (cin * ncol + ncol + 8 + 128 * 2 * ncol + 4 * (cin + 1) * ncol) + 64;
-}
-
-bool umma_output_fusable(const ConvLaunch& L, const UmmaChoice& ch, const OutputLaunch& O) {
-    if (!ch.persistent || ch.folded || ch.nsplit != 1 || ch.NPAD > 128 || ch.nteams != 3) return false;
-    { const int ncol = O.nconv * O.C; if (ncol != 1 && ncol != 2 && ncol != 4 && ncol != 6) return false; }     // instantiated widths
-    if (O.ofs != 1 || O.pad_left != 0 || O.Tf != O.T_out || O.C < 1 || O.C > 2 || O.nconv < 1 || O.nconv * O.C > kOutFuseMaxCols) return false;
-    if (L.N != (L.pairC > 0 ? 2 : 1) * O.F || L.N % 4 != 0 || L.epilogue != EPI_BIAS_LRELU) return false;
-    for (int q = 0; q < L.ncls; ++q) {
-        const OutView& V = L.cls[q];
-        if (V.rstride % 4 || V.bstride % 4 || (reinterpret_cast<uintptr_t>(V.base) & 15)) return false;
-    }
-    UmmaLaunch U;
-    memset(&U, 0, sizeof(U));
-    U.NPAD = ch.NPAD; U.nsplit = ch.nsplit; U.rows_alloc = ch.rows_alloc; U.TB = ch.TB; U.nbs = ch.nbs; U.nteams = ch.nteams;
-    return umma_pers_smem_bytes(U) + umma_outfuse_smem_bytes(O) <= 220 * 1024;
-}
-
-cudaError_t launch_plane_conv_umma(const UmmaLaunch& L, cudaStream_t stream, const OutputFuse* fuse) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e0 = set_smem_limit(plane_conv_umma_persistent_out<1>, 220 * 1024);
-        if (e0 == cudaSuccess) e0 = set_smem_limit(plane_conv_umma_persistent_out<2>, 220 * 1024);
-        if (e0 == cudaSuccess) e0 = set_smem_limit(plane_conv_umma_persistent_out<4>, 220 * 1024);
-        if (e0 == cudaSuccess) e0 = set_smem_limit(plane_conv_umma_persistent_out<6>, 220 * 1024);
-        if (e0 == cudaSuccess) e0 = set_smem_limit(plane_conv_umma_persistent_dg2, 220 * 1024);
-        if (e0 == cudaSuccess) e0 = set_smem_limit(plane_conv_umma_persistent_fw2, 220 * 1024);
-        if (e0 != cudaSuccess) return e0;
-        cudaError_t e = set_smem_limit(plane_conv_umma_kernel<2, false>, 200 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_kernel<2, true>, 200 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_kernel<4, false>, 220 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_kernel<4, true>, 220 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_persistent<2, false>, 220 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_persistent<2, true>, 220 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_persistent<3, false>, 220 * 1024);
-        if (e == cudaSuccess) e = set_smem_limit(plane_conv_umma_persistent<3, true>, 220 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    if (L.folded) return launch_plane_conv_fold(L, stream);
-    int max_tiles = 0, total = 0;
-    for (int q = 0; q < L.ncls; ++q) {
-        const int rows = L.cls[q].out.m_hi - L.cls[q].out.m_lo;
-        const int tq = (rows + L.MT * 128 - 1) / (L.MT * 128);
-        max_tiles = max(max_tiles, tq);
-        total += tq * L.batch;
-    }
-    total *= L.nsplit;
-    if (max_tiles <= 0) return cudaSuccess;
-    const bool dg = L.epilogue == EPI_SLOPE;      // dgrad: batched read-back epilogue (separate instantiation)
-    if (fuse && !(L.persistent && !dg)) return cudaErrorInvalidValue;
-    if (L.persistent) {
-        const int grid = total < 148 ? total : 148;
-        const size_t smem = umma_pers_smem_bytes(L);
-        if (fuse) {
-            const size_t smem_o = smem + umma_outfuse_smem_bytes(fuse->O);
-            if (L.nteams != 3) return cudaErrorInvalidValue;
-            switch (fuse->O.nconv * fuse->O.C) {
-                case 1: plane_conv_umma_persistent_out<1><<<grid, 3 * 128 + 192, smem_o, stream>>>(L, total, *fuse); break;
-                case 2: plane_conv_umma_persistent_out<2><<<grid, 3 * 128 + 192, smem_o, stream>>>(L, total, *fuse); break;
-                case 4: plane_conv_umma_persistent_out<4><<<grid, 3 * 128 + 192, smem_o, stream>>>(L, total, *fuse); break;
-                case 6: plane_conv_umma_persistent_out<6><<<grid, 3 * 128 + 192, smem_o, stream>>>(L, total, *fuse); break;
-                default: return cudaErrorInvalidValue;
-            }
-            return cudaGetLastError();
-        }
-        if (L.epi2 && !fuse) {
-            if (L.nteams != 2) return cudaErrorInvalidValue;
-            if (dg) plane_conv_umma_persistent_dg2<<<grid, 2 * 128 + 64 + 256, smem, stream>>>(L, total);
-            else plane_conv_umma_persistent_fw2<<<grid, 2 * 128 + 64 + 256, smem, stream>>>(L, total);
-            return cudaGetLastError();
-        }
-        if (L.nteams == 3) {
-            if (dg) plane_conv_umma_persistent<3, true><<<grid, 3 * 128 + 192, smem, stream>>>(L, total);
-            else plane_conv_umma_persistent<3, false><<<grid, 3 * 128 + 192, smem, stream>>>(L, total);
-        } else {
-            if (dg) plane_conv_umma_persistent<2, true><<<grid, 2 * 128 + 192, smem, stream>>>(L, total);
-            else plane_conv_umma_persistent<2, false><<<grid, 2 * 128 + 192, smem, stream>>>(L, total);
-        }
-        return cudaGetLastError();
-    }
-    const size_t smem = umma_smem_bytes(L);
-    dim3 grid(max_tiles, L.nsplit, L.batch * L.ncls);
-    if (L.nteams == 4) {
-        if (dg) plane_conv_umma_kernel<4, true><<<grid, 4 * 128 + 64, smem, stream>>>(L);
-        else plane_conv_umma_kernel<4, false><<<grid, 4 * 128 + 64, smem, stream>>>(L);
-    } else {
-        if (dg) plane_conv_umma_kernel<2, true><<<grid, 2 * 128 + 64, smem, stream>>>(L);
-        else plane_conv_umma_kernel<2, false><<<grid, 2 * 128 + 64, smem, stream>>>(L);
-    }
+    // dgrad: batched read-back epilogue (separate instantiation)
+    if (L.epilogue == EPI_SLOPE) plane_conv_umma_kernel<NPAD, true><<<grid, kConvThreads, smem, stream>>>(L);
+    else plane_conv_umma_kernel<NPAD, false><<<grid, kConvThreads, smem, stream>>>(L);
     return cudaGetLastError();
 }
 
+cudaError_t launch_plane_conv_umma(const UmmaLaunch& L, cudaStream_t stream, const OutputFuse* fuse) {
+    if (fuse) return cudaErrorInvalidValue;
+    int max_tiles = 0;
+    for (int q = 0; q < L.ncls; ++q) max_tiles = max(max_tiles, (L.cls[q].out.m_hi - L.cls[q].out.m_lo + 127) / 128);
+    if (max_tiles <= 0) return cudaSuccess;
+    const size_t smem = umma_smem_bytes(L);
+    if (smem > (size_t)kConvSmemMax || L.nbs < 2 || L.nbs > kBStagesMax || L.MT != 1) return cudaErrorInvalidValue;
+    const dim3 grid(max_tiles, L.nsplit, L.batch * L.ncls);
+    switch (L.NPAD) {
+        case 16: return launch_conv_npad<16>(L, grid, smem, stream);
+        case 32: return launch_conv_npad<32>(L, grid, smem, stream);
+        case 48: return launch_conv_npad<48>(L, grid, smem, stream);
+        case 64: return launch_conv_npad<64>(L, grid, smem, stream);
+        case 80: return launch_conv_npad<80>(L, grid, smem, stream);
+        case 96: return launch_conv_npad<96>(L, grid, smem, stream);
+        case 112: return launch_conv_npad<112>(L, grid, smem, stream);
+        case 128: return launch_conv_npad<128>(L, grid, smem, stream);
+        default: return cudaErrorInvalidValue;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
-// wgrad kernel (MN-major operands: K = rows).  Slab layout per side: [hi|lo][atom (8 ch)][row][16 B]; for an
-// MN-major SWIZZLE_NONE operand the 8x8 core matrix is 8 rows (K) x 16 B, K groups LBO = 128 B apart, channel
-// atoms SBO = atom-plane stride apart.  A tap is again a start-address shift (d rows * 16 B) of the P side.
-// grid = (batch * chunks_per_batch, n_mtiles * n_ntiles, n_tapsets); 192 threads, roles as in the conv kernel.
+// wgrad kernels (MN-major operands: K = rows).  Stage layout per side: [hi|lo][atom (8 ch)][row][16 B]; for an MN-major
+// no-swizzle operand the 8x8 core matrix is 8 rows (K) x 16 B, K groups LBO = 128 B apart, channel atoms SBO = atom-plane
+// stride apart.  A tap is again a start-address shift (d rows * 16 B) of the P side.
+// grid = (batch * chunks_per_batch / chunks_per_cta, n_mtiles * n_ntiles, tap sets of all groups).  Warps 0-7: two
+// warpgroups over the 128-channel M tile (64 each), accumulators taps x NT in registers; warps 8..: the stage producer.
 // ------------------------------------------------------------------------------------------------
 constexpr int kWgRK = 64;          // rows per pipeline stage
 constexpr int kWgSpan = 16;        // extra P rows per stage (max tap shift span)
 constexpr int kWgStagesMax = 3;    // pipeline stages: as many as fit in shared memory (L.nstages)
+constexpr int kWgMmaThreads = 256;
+constexpr int kWgAccCols = 256;    // accumulator columns (taps x NT) per warpgroup: 128 fp32 registers per thread
+constexpr int kWgConvThreads = 128;                 // converter-fed kernel: 4 converter warps
+constexpr int kWgSmemMax = 200 * 1024;
+constexpr int kWgSlotFloats = 128 * kWgAccCols;     // one CTA's partial tile: [tap][128 M rows][NT]
 
-// CW converter warps (0..CW-1, a multiple of 4: TMEM lane quarters); warp CW = TMEM alloc + MMA issue
-
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-template <int CW>
-__global__ void __launch_bounds__(CW * 32 + 32, 1) wgrad_umma_kernel(const __grid_constant__ UmmaWgradLaunch L) {
-    constexpr int kWgConvThreads = CW * 32;
+template <bool BULK, int NT>
+__device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSplit* S) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     // group / tap set of this CTA
@@ -1784,7 +554,7 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) wgrad_umma_kernel(const __gri
     while (gi + 1 < L.ngroups && (int)blockIdx.z >= L.grp[gi + 1].z0) ++gi;
     const WgGroup& Gp = L.grp[gi];
     const int tapset = blockIdx.z - Gp.z0;
-    if ((int)blockIdx.x >= Gp.n_ctas_x || (int)blockIdx.y >= Gp.n_mtiles * Gp.n_ntiles) return;
+    if ((int)blockIdx.x >= Gp.n_ctas_x || (int)blockIdx.y >= Gp.n_mtiles * Gp.n_ntiles || Gp.NT != NT) return;
     const int total_chunks = L.batch * Gp.chunks_per_batch;
     const int g0 = blockIdx.x * Gp.chunks_per_cta;
     const int g1 = min(g0 + Gp.chunks_per_cta, total_chunks);
@@ -1792,14 +562,14 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) wgrad_umma_kernel(const __gri
     const int mtile = blockIdx.y / Gp.n_ntiles, ntile = blockIdx.y % Gp.n_ntiles;
     const int tap0 = tapset * Gp.taps_per_cta;
     const int ntap = min(Gp.taps_per_cta, Gp.ntaps - tap0);
-    const int NT = Gp.NT, swap = Gp.swap;
+    const int swap = Gp.swap;
     const PlaneView& SA = swap ? Gp.G : Gp.P;       // M side (128-channel tile)
     const PlaneView& SB = swap ? Gp.P : Gp.G;       // N side (NT-channel tile)
     const int ca0 = mtile * 128, cb0 = ntile * NT;
     const int rowsA = swap ? kWgRK : kWgRK + kWgSpan;
     const int rowsB = swap ? kWgRK + kWgSpan : kWgRK;
     const uint32_t planeA = 16u * rowsA, planeB = 16u * rowsB;           // atom-plane strides
-    const int atomsA = 16, atomsB = NT / 8;
+    constexpr int atomsA = 16, atomsB = NT / 8;
     const uint32_t bytesA = 2u * atomsA * planeA, bytesB = 2u * atomsB * planeB;
     const uint32_t stage_bytes = bytesA + bytesB;
     int dmin = Gp.d[tap0];
@@ -1809,40 +579,70 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) wgrad_umma_kernel(const __gri
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + nst * stage_bytes);
     const uint32_t bar0 = smem_u32(bars);
     auto BAR = [&](int i) { return bar0 + 8u * i; };
-    const int FULL = 0, EMPTY = kWgStagesMax, ACC = 2 * kWgStagesMax;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + ACC + 1);
+    const int FULL = 0, EMPTY = kWgStagesMax;
     if (tid == 0) {
-        for (int i = 0; i < kWgStagesMax; ++i) { mbar_init(BAR(FULL + i), kWgConvThreads); mbar_init(BAR(EMPTY + i), 1); }
-        mbar_init(BAR(ACC), 1);
+        for (int i = 0; i < kWgStagesMax; ++i) { mbar_init(BAR(FULL + i), BULK ? 1 : kWgConvThreads); mbar_init(BAR(EMPTY + i), kWgMmaThreads); }
         fence_barrier_init();
     }
-    if (warp == CW) tmem_alloc(smem_u32(tmem_holder), Gp.tmem_cols);
-    tc_fence_before();
+    // channel chunks the tensors really have inside this tile; the bulk copies leave the rest of the operand tile zero
+    const int chunksA = max(0, min(8, (SA.C - ca0 + 15) / 16)), chunksB = max(0, min(NT / 16, (SB.C - cb0 + 15) / 16));
+    if (BULK) {
+        for (uint32_t i = tid; i < (uint32_t)nst * stage_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
+        fence_proxy_async();
+    }
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
     const int nchunks = g1 - g0;
 
-    if (warp < CW) {
-        // ===================== converter =====================
-        // items of a chunk: (side, row, 16-channel group); A side = 8 groups (128 channels), B side = NT/16 groups
-        const int gA = 8, gB = (NT + 15) / 16;
-        const int itemsA = rowsA * gA, items = itemsA + rowsB * gB;
-        constexpr int kIB = 4;                                   // items in flight per thread
-        for (int ci = 0; ci < nchunks; ++ci) {
-            const int st = ci % nst;
-            uint8_t* S = smem + st * stage_bytes;
-            const int gch = g0 + ci;                              // batch-folded chunk index
-            const int b = gch / Gp.chunks_per_batch;
-            const int rc = Gp.m_lo + (gch % Gp.chunks_per_batch) * kWgRK;   // first G row of this chunk
-            const int rend = min(rc + kWgRK, Gp.m_hi);
-            bool waited = false;
-            for (int ibase = 0; ibase < items; ibase += kIB * kWgConvThreads) {
-                float x[kIB][16];
-#pragma unroll
-                for (int u = 0; u < kIB; ++u) {
-                    const int it = ibase + u * kWgConvThreads + tid;
-                    if (it >= items) continue;
+    if (warp >= kWgMmaThreads / 32) {
+        // ===================== producer =====================
+        if (BULK) {
+            if (warp == kWgMmaThreads / 32 && lane == 0) {
+                const uint8_t* baseA = swap ? S->G[gi] : S->P[gi];
+                const uint8_t* baseB = swap ? S->P[gi] : S->G[gi];
+                const long long a_ps = swap ? S->g_pstride[gi] : S->p_pstride[gi], b_ps = swap ? S->p_pstride[gi] : S->g_pstride[gi];
+                const long long a_cs = 4 * a_ps, b_cs = 4 * b_ps;
+                const long long a_bs = (swap ? S->g_nchunk[gi] : S->p_nchunk[gi]) * a_cs, b_bs = (swap ? S->p_nchunk[gi] : S->g_nchunk[gi]) * b_cs;
+                const int a_row0 = swap ? S->g_row0[gi] : S->p_row0[gi], b_row0 = swap ? S->p_row0[gi] : S->g_row0[gi];
+                const uint32_t tx = (uint32_t)(chunksA * 4) * planeA + (uint32_t)(chunksB * 4) * planeB;
+                for (int ci = 0; ci < nchunks; ++ci) {
+                    const int st = ci % nst;
+                    const int gch = g0 + ci;
+                    const int b = gch / Gp.chunks_per_batch;
+                    const int rc = Gp.m_lo + (gch % Gp.chunks_per_batch) * kWgRK;      // first G row of the chunk
+                    const int rowA = (swap ? rc : rc + dmin) - a_row0, rowB = (swap ? rc + dmin : rc) - b_row0;   // array indices
+                    mbar_wait(BAR(EMPTY + st), ((ci / nst) & 1) ^ 1);
+                    mbar_arrive_expect_tx(BAR(FULL + st), tx);
+                    const uint32_t sa = smem_u32(smem + st * stage_bytes), sb = sa + bytesA;
+                    for (int g = 0; g < chunksA; ++g) {
+                        const uint8_t* src = baseA + (long long)b * a_bs + (long long)(ca0 / 16 + g) * a_cs + (long long)rowA * 16;
+                        bulk_g2s(sa + (uint32_t)(2 * g) * planeA, src, planeA, BAR(FULL + st));                               // hi atom 2g
+                        bulk_g2s(sa + (uint32_t)(2 * g + 1) * planeA, src + a_ps, planeA, BAR(FULL + st));                    // hi atom 2g+1
+                        bulk_g2s(sa + (uint32_t)(atomsA + 2 * g) * planeA, src + 2 * a_ps, planeA, BAR(FULL + st));           // lo atom 2g
+                        bulk_g2s(sa + (uint32_t)(atomsA + 2 * g + 1) * planeA, src + 3 * a_ps, planeA, BAR(FULL + st));       // lo atom 2g+1
+                    }
+                    for (int g = 0; g < chunksB; ++g) {
+                        const uint8_t* src = baseB + (long long)b * b_bs + (long long)(cb0 / 16 + g) * b_cs + (long long)rowB * 16;
+                        bulk_g2s(sb + (uint32_t)(2 * g) * planeB, src, planeB, BAR(FULL + st));
+                        bulk_g2s(sb + (uint32_t)(2 * g + 1) * planeB, src + b_ps, planeB, BAR(FULL + st));
+                        bulk_g2s(sb + (uint32_t)(atomsB + 2 * g) * planeB, src + 2 * b_ps, planeB, BAR(FULL + st));
+                        bulk_g2s(sb + (uint32_t)(atomsB + 2 * g + 1) * planeB, src + 3 * b_ps, planeB, BAR(FULL + st));
+                    }
+                }
+            }
+        } else {
+            // items of a chunk: (side, row, 16-channel group); A side = 8 groups (128 channels), B side = NT/16 groups
+            const int ctid = tid - kWgMmaThreads;
+            const int gA = 8, gB = NT / 16;
+            const int itemsA = rowsA * gA, items = itemsA + rowsB * gB;
+            for (int ci = 0; ci < nchunks; ++ci) {
+                const int st = ci % nst;
+                uint8_t* Sm = smem + st * stage_bytes;
+                const int gch = g0 + ci;                              // batch-folded chunk index
+                const int b = gch / Gp.chunks_per_batch;
+                const int rc = Gp.m_lo + (gch % Gp.chunks_per_batch) * kWgRK;   // first G row of this chunk
+                const int rend = min(rc + kWgRK, Gp.m_hi);
+                mbar_wait(BAR(EMPTY + st), ((ci / nst) & 1) ^ 1);
+                for (int it = ctid; it < items; it += kWgConvThreads) {
                     const bool isA = it < itemsA;
                     const int k = isA ? it : it - itemsA;
                     const int nr = isA ? rowsA : rowsB;        // consecutive threads -> consecutive rows (conflict-free st.shared)
@@ -1851,122 +651,99 @@ __global__ void __launch_bounds__(CW * 32 + 32, 1) wgrad_umma_kernel(const __gri
                     const PlaneView& V = isA ? SA : SB;
                     const int c0 = (isA ? ca0 : cb0) + g * 16;
                     const int row = isP ? (rc + dmin + rr) : (rc + rr);
-                    bool valid = c0 < V.C;
-                    if (!isP && row >= rend) valid = false;       // G rows beyond the chunk / class contribute 0
-                    if (valid) load_row16(V, b, row, c0, x[u]);
+                    float x[16];
+                    if (c0 < V.C && (isP || row < rend)) load_row16(V, b, row, c0, x);    // G rows beyond the chunk / class contribute 0
                     else {
 #pragma unroll
-                        for (int i = 0; i < 16; ++i) x[u][i] = 0.f;
+                        for (int i = 0; i < 16; ++i) x[i] = 0.f;
                     }
-                }
-                if (!waited) {
-                    if (tid == 0) { T_WAIT(6, mbar_wait_bg(BAR(EMPTY + st), ((ci / nst) & 1) ^ 1)); }
-                    else mbar_wait_bg(BAR(EMPTY + st), ((ci / nst) & 1) ^ 1);
-                    waited = true;
-                }
-#pragma unroll
-                for (int u = 0; u < kIB; ++u) {
-                    const int it = ibase + u * kWgConvThreads + tid;
-                    if (it >= items) continue;
-                    const bool isA = it < itemsA;
-                    const int k = isA ? it : it - itemsA;
-                    const int nr = isA ? rowsA : rowsB;
-                    const int g = k / nr, rr = k - g * nr;
                     uint32_t hi[8], lo[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const __nv_bfloat16 h0 = __float2bfloat16_rn(x[u][2 * i]), h1 = __float2bfloat16_rn(x[u][2 * i + 1]);
-                        hi[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                        lo[i] = pack_bf16x2(x[u][2 * i] - __bfloat162float(h0), x[u][2 * i + 1] - __bfloat162float(h1));
-                    }
+                    split_hi_lo(x, hi, lo);
                     const uint32_t plane = isA ? planeA : planeB;
-                    uint8_t* base = S + (isA ? 0u : bytesA) + (uint32_t)(2 * g) * plane + 16u * rr;
+                    uint8_t* base = Sm + (isA ? 0u : bytesA) + (uint32_t)(2 * g) * plane + 16u * rr;
                     const uint32_t lo_off = (isA ? atomsA : atomsB) * plane;
                     *reinterpret_cast<uint4*>(base) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
                     *reinterpret_cast<uint4*>(base + lo_off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-                    if (isA || (2 * g + 1) < atomsB) {
-                        *reinterpret_cast<uint4*>(base + plane) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-                        *reinterpret_cast<uint4*>(base + plane + lo_off) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-                    }
+                    *reinterpret_cast<uint4*>(base + plane) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+                    *reinterpret_cast<uint4*>(base + plane + lo_off) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
                 }
-            }
-            fence_proxy_async();
-            mbar_arrive(BAR(FULL + st));
-        }
-        // ===================== epilogue: accumulators -> reductions into dW =====================
-        // TMEM lane quarter = warp % 4; the CW/4 warps of a quarter split the taps.
-        if (tid == 0) { T_WAIT(8, mbar_wait_bg(BAR(ACC), 0)); }
-        else mbar_wait_bg(BAR(ACC), 0);
-        tc_fence_after();
-        const long long t_epi = T_NOW();
-        const int q4 = warp & 3;
-        const int m = ca0 + q4 * 32 + lane;                      // M-side channel of this thread
-        const bool m_ok = m < SA.C;
-        const int sM = swap ? L.w_sg : L.w_sp, sN = swap ? L.w_sp : L.w_sg;
-        for (int t = (warp >> 2); t < ntap; t += CW / 4) {
-            float* dst_t = L.dW + (long long)Gp.woff[tap0 + t] + (long long)m * sM;
-            for (int cb = 0; cb < NT; cb += 16) {
-                if (cb0 + cb >= SB.C) break;
-                __syncwarp();
-                float v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(t * NT + cb), v);
-                if (!m_ok) continue;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] *= L.scale;
-                float* dst = dst_t + (long long)(cb0 + cb) * sN;
-                if (sN == 1 && cb0 + cb + 16 <= SB.C && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) red_add_v4(dst + 4 * q, v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (cb0 + cb + j < SB.C) atomicAdd(dst + (long long)j * sN, v[j]);
-                }
+                fence_proxy_async();
+                mbar_arrive(BAR(FULL + st));
             }
         }
-        if (tid == 0) { T_ADD(9, T_NOW() - t_epi); T_ADD(0, 1); T_ADD(7, nchunks); }
-        tc_fence_before();
-    } else {
-        if (elect_one()) {
-            const long long t_mma = T_NOW();
-            // both operands MN-major: idesc a_major (bit 15) = b_major (bit 16) = 1
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NT >> 3) << 17) | ((128u >> 4) << 24);
-            uint32_t accum = 0;
-            for (int ci = 0; ci < nchunks; ++ci) {
-                const int st = ci % nst;
-                T_WAIT(4, mbar_wait(BAR(FULL + st), (ci / nst) & 1));
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + st * stage_bytes), sb = sa + bytesA;
-                // tap-outer order: 12 consecutive MMAs per accumulator; descriptors advance by plain adds on the address field
-                const uint64_t a_hi0 = umma_desc(sa, 128, planeA), a_lo0 = umma_desc(sa + atomsA * planeA, 128, planeA);
-                const uint64_t b_hi0 = umma_desc(sb, 128, planeB), b_lo0 = umma_desc(sb + atomsB * planeB, 128, planeB);
-                for (int t = 0; t < ntap; ++t) {
-                    const uint64_t shift = (uint64_t)(uint32_t)(Gp.d[tap0 + t] - dmin);    // rows == 16-byte units
-                    const uint64_t sha = swap ? 0ull : shift, shb = swap ? shift : 0ull;
-                    const uint32_t td = tmem_base + (uint32_t)(t * NT);
-#pragma unroll
-                    for (int ks = 0; ks < kWgRK / 16; ++ks) {
-                        const uint64_t koff = (uint64_t)(16 * ks);           // 16 rows * 16 B >> 4
-                        const uint64_t a_hi = a_hi0 + sha + koff, a_lo = a_lo0 + sha + koff;
-                        const uint64_t b_hi = b_hi0 + shb + koff, b_lo = b_lo0 + shb + koff;
-                        umma_bf16(td, a_lo, b_hi, idesc, (ks == 0) ? accum : 1u);
-                        umma_bf16(td, a_hi, b_lo, idesc, 1u);
-                        umma_bf16(td, a_hi, b_hi, idesc, 1u);
-                    }
-                }
-                accum = 1u;
-                umma_commit(BAR(EMPTY + st));
-            }
-            umma_commit(BAR(ACC));
-            T_ADD(3, T_NOW() - t_mma);
-        }
-        __syncwarp();
+        return;
     }
-    __syncthreads();
-    if (warp == CW) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Gp.tmem_cols);
+
+    // ===================== MMA warpgroups =====================
+    constexpr int TMAX = kWgAccCols / NT;        // >= taps_per_cta (umma_plan_wgrad)
+    constexpr int NACC = TMAX * NT / 2;
+    const int wg = warp >> 2;
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    for (int ci = 0; ci < nchunks; ++ci) {
+        const int st = ci % nst;
+        mbar_wait(BAR(FULL + st), (ci / nst) & 1);
+        const uint32_t sa = smem_u32(smem + st * stage_bytes) + (uint32_t)(8 * wg) * planeA, sb = smem_u32(smem + st * stage_bytes) + bytesA;
+        wgmma_fence();
+#pragma unroll
+        for (int t = 0; t < TMAX; ++t) {
+            if (t < ntap) {
+                const uint32_t shift = 16u * (uint32_t)(Gp.d[tap0 + t] - dmin);          // rows * 16 B
+                const uint32_t sha = swap ? 0u : shift, shb = swap ? shift : 0u;
+#pragma unroll
+                for (int ks = 0; ks < kWgRK / 16; ++ks) {
+                    const uint32_t a = sa + sha + 256u * ks, bb = sb + shb + 256u * ks;
+                    const uint64_t a_hi = gmma_desc(a, 128, planeA), a_lo = gmma_desc(a + atomsA * planeA, 128, planeA);
+                    const uint64_t b_hi = gmma_desc(bb, 128, planeB), b_lo = gmma_desc(bb + atomsB * planeB, 128, planeB);
+                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_lo, b_hi, planeB >> 4);
+                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_hi, b_lo, planeB >> 4);
+                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_hi, b_hi, planeB >> 4);
+                }
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        acc_fence<NACC>(acc);
+        mbar_arrive(BAR(EMPTY + st));
     }
+    // ===================== epilogue: accumulators -> partial tile (or reductions into dW) =====================
+    if (L.partial) {
+        const int tiles = Gp.n_mtiles * Gp.n_ntiles;
+        float* part = L.partial + (size_t)(Gp.slot0 + (tapset * tiles + (int)blockIdx.y) * Gp.n_ctas_x + (int)blockIdx.x) * kWgSlotFloats;
+#pragma unroll
+        for (int t = 0; t < TMAX; ++t) {
+            if (t >= ntap) break;
+#pragma unroll
+            for (int i = 0; i < NT / 2; i += 2) {
+                const int row = 64 * wg + acc_row(i, warp, lane), col = acc_col(i, lane);
+                *reinterpret_cast<float2*>(part + (size_t)(t * 128 + row) * NT + col) =
+                    make_float2(acc[t * (NT / 2) + i] * L.scale, acc[t * (NT / 2) + i + 1] * L.scale);
+            }
+        }
+        return;
+    }
+    const int sM = swap ? L.w_sg : L.w_sp, sN = swap ? L.w_sp : L.w_sg;
+#pragma unroll
+    for (int t = 0; t < TMAX; ++t) {
+        if (t >= ntap) break;
+        float* dst_t = L.dW + Gp.woff[tap0 + t];
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) {
+            const int m = ca0 + 64 * wg + acc_row(i, warp, lane), n = cb0 + acc_col(i, lane);
+            if (m < SA.C && n < SB.C) atomicAdd(dst_t + (long long)m * sM + (long long)n * sN, acc[t * (NT / 2) + i] * L.scale);
+        }
+    }
+}
+
+template <int NT>
+__global__ void __launch_bounds__(kWgMmaThreads + 32, 1) wgrad_umma_bulk_kernel(const __grid_constant__ UmmaWgradLaunch L,
+                                                                                 const __grid_constant__ WgSplit S) {
+    wgrad_body<true, NT>(L, &S);
+}
+template <int NT>
+__global__ void __launch_bounds__(kWgMmaThreads + kWgConvThreads, 1) wgrad_umma_kernel(const __grid_constant__ UmmaWgradLaunch L) {
+    wgrad_body<false, NT>(L, nullptr);
 }
 
 static size_t wgrad_stage_bytes(int swap, int NT) {
@@ -1977,23 +754,14 @@ static size_t wgrad_stage_bytes(int swap, int NT) {
 static size_t wgrad_smem_bytes(const UmmaWgradLaunch& L) {
     size_t stage = 0;
     for (int g = 0; g < L.ngroups; ++g) stage = max(stage, wgrad_stage_bytes(L.grp[g].swap, L.grp[g].NT));
-    return L.nstages * stage + (2 * kWgStagesMax + 1) * 8 + 16;
+    return L.nstages * stage + 2 * kWgStagesMax * 8;
 }
 
 size_t umma_wgrad_smem_bytes(const UmmaWgradLaunch& L) { return wgrad_smem_bytes(L); }
 
-size_t umma_choice_smem_bytes(const UmmaChoice& ch) {
-    UmmaLaunch U;
-    memset(&U, 0, sizeof(U));
-    U.NPAD = ch.NPAD; U.nsplit = ch.nsplit; U.MT = ch.MT; U.rows_alloc = ch.rows_alloc; U.TB = ch.TB; U.nbs = ch.nbs;
-    U.nteams = ch.nteams; U.persistent = ch.persistent;
-    if (ch.folded) return umma_fold_smem_bytes(U);
-    return ch.persistent ? umma_pers_smem_bytes(U) : umma_smem_bytes(U);
-}
-
 bool umma_plan_wgrad(UmmaWgradLaunch* L) {
     if (L->ngroups < 1 || L->ngroups > kWgMaxGroups) return false;
-    long long work = 0;        // ~MMA work units of the launch, to size the K ranges
+    int NT = 16;               // one N-tile width for all groups: one kernel instantiation per launch
     for (int gi = 0; gi < L->ngroups; ++gi) {
         WgGroup& G = L->grp[gi];
         const int Cp = G.P.C, Cg = G.G.C;
@@ -2003,38 +771,36 @@ bool umma_plan_wgrad(UmmaWgradLaunch* L) {
         int dmin = G.d[0], dmax = G.d[0];
         for (int t = 1; t < G.ntaps; ++t) { dmin = min(dmin, G.d[t]); dmax = max(dmax, G.d[t]); }
         if (dmax - dmin > kWgSpan) return false;
-        const int rows = G.m_hi - G.m_lo;
-        if (rows <= 0) return false;
-        G.swap = (Cg > Cp) ? 1 : 0;                       // the wider side fills the 128-row M dimension
+        if (G.m_hi <= G.m_lo) return false;
+        G.swap = (Cg > Cp) ? 1 : 0;                       // the wider side fills the 128-channel M dimension
         const int Cm = G.swap ? Cg : Cp, Cn = G.swap ? Cp : Cg;
         G.n_mtiles = (Cm + 127) / 128;
-        int NT = (Cn + 15) / 16 * 16;
+        int nt = (Cn + 15) / 16 * 16;
         G.n_ntiles = 1;
-        while (NT > 128) { G.n_ntiles *= 2; NT = ((Cn + G.n_ntiles - 1) / G.n_ntiles + 15) / 16 * 16; }
+        while (nt > 128) { G.n_ntiles *= 2; nt = ((Cn + G.n_ntiles - 1) / G.n_ntiles + 15) / 16 * 16; }
+        NT = max(NT, nt);
+    }
+    long long work = 0;        // ~MMA work units of the launch, to size the K ranges
+    for (int gi = 0; gi < L->ngroups; ++gi) {
+        WgGroup& G = L->grp[gi];
         G.NT = NT;
-        int tpc = 512 / NT;
+        int tpc = kWgAccCols / NT;                        // the accumulators of all taps of a CTA live in registers
         if (tpc > kWgMaxTaps) tpc = kWgMaxTaps;
         if (tpc > G.ntaps) tpc = G.ntaps;
         G.n_tapsets = (G.ntaps + tpc - 1) / tpc;
         tpc = (G.ntaps + G.n_tapsets - 1) / G.n_tapsets;   // balance
         G.taps_per_cta = tpc;
-        {   // fused-N (bulk-fed kernel): only where it costs no extra tap set, i.e. the doubled accumulators still fit TMEM
-            static const int fuse_on = [] { const char* e = getenv("WUN_WG_FUSE"); return (e && e[0] == '0') ? 0 : 1; }();
-            G.fuse = (fuse_on && 2 * NT <= 256 && tpc * 2 * NT <= 512) ? 1 : 0;
-        }
-        int tm = 32;
-        while (tm < tpc * NT * (G.fuse ? 2 : 1)) tm *= 2;
-        G.tmem_cols = tm;
-        G.chunks_per_batch = (rows + kWgRK - 1) / kWgRK;
+        G.chunks_per_batch = (G.m_hi - G.m_lo + kWgRK - 1) / kWgRK;
         work += (long long)L->batch * G.chunks_per_batch * G.n_tapsets * G.n_mtiles * G.n_ntiles;
     }
-    // K range per CTA: the launch should be ONE full wave (1 CTA per SM, 148 SMs): every CTA runs concurrently and
-    // pays the dW reduction once.  Start from work/148 and grow until the (per-group rounded) CTA count fits.
-    const int kSMs = 148;
-    long long per = (work + kSMs - 1) / kSMs;
+    // K range per CTA: the launch should be ONE full wave (1 CTA per SM): every CTA runs concurrently and pays the dW
+    // reduction once.  Start from work/SMs and grow until the (per-group rounded) CTA count fits.
+    const int kSMs = 132;
+    long long per = (work + kSMs - 1) / kSMs, most = 1;
     if (per < 2) per = 2;
-    int z = 0, gx = 0, gy = 0;
-    for (int iter = 0; iter < 64; ++iter) {
+    for (int gi = 0; gi < L->ngroups; ++gi) most = max(most, (long long)L->batch * L->grp[gi].chunks_per_batch);
+    int z = 0, gx = 0, gy = 0, slots = 0;
+    for (;;) {              // ends with <= kSMs CTAs, or with one CTA per (group, tile, tap set): umma_wgrad_partial_bytes
         long long ctas = 0;
         for (int gi = 0; gi < L->ngroups; ++gi) {
             const WgGroup& G = L->grp[gi];
@@ -2042,8 +808,8 @@ bool umma_plan_wgrad(UmmaWgradLaunch* L) {
             const long long c = min(per, total);
             ctas += ((total + c - 1) / c) * G.n_tapsets * G.n_mtiles * G.n_ntiles;
         }
-        if (ctas <= kSMs) break;
-        per += (per + 15) / 16;
+        if (ctas <= kSMs || per >= most) break;
+        per = min(most, per + (per + 15) / 16);
     }
     for (int gi = 0; gi < L->ngroups; ++gi) {
         WgGroup& G = L->grp[gi];
@@ -2052,41 +818,58 @@ bool umma_plan_wgrad(UmmaWgradLaunch* L) {
         G.n_ctas_x = (int)((total + G.chunks_per_cta - 1) / G.chunks_per_cta);
         G.z0 = z;
         z += G.n_tapsets;
+        G.slot0 = slots;
+        slots += G.n_tapsets * G.n_mtiles * G.n_ntiles * G.n_ctas_x;
         gx = max(gx, G.n_ctas_x);
         gy = max(gy, G.n_mtiles * G.n_ntiles);
     }
     L->grid_x = gx; L->grid_y = gy; L->grid_z = z;
     L->nstages = kWgStagesMax;
-    while (L->nstages > 2 && wgrad_smem_bytes(*L) > 200 * 1024) --L->nstages;
-    return wgrad_smem_bytes(*L) <= 200 * 1024;
+    while (L->nstages > 2 && wgrad_smem_bytes(*L) > kWgSmemMax) --L->nstages;
+    return wgrad_smem_bytes(*L) <= kWgSmemMax;
 }
 
-cudaError_t launch_wgrad_umma(const UmmaWgradLaunch& L, cudaStream_t stream) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_umma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+// the instantiation of the launch's N-tile width (umma_plan_wgrad gives every group the same one)
+template <bool BULK>
+static cudaError_t launch_wgrad_any(const UmmaWgradLaunch& L, const WgSplit* S, cudaStream_t stream) {
+    const dim3 grid(L.grid_x, L.grid_y, L.grid_z);
+    const size_t smem = wgrad_smem_bytes(L);
+    const int threads = kWgMmaThreads + (BULK ? 32 : kWgConvThreads);
+    {
+        const int NT = L.grp[0].NT;
+        cudaError_t e = cudaSuccess;
+#define WUN_WG_CASE(W)                                                                                                      \
+    case W:                                                                                                                 \
+        if (BULK) {                                                                                                         \
+            static bool set = false;                                                                                        \
+            if (!set) { e = cudaFuncSetAttribute(wgrad_umma_bulk_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemMax); set = e == cudaSuccess; } \
+            if (e == cudaSuccess) wgrad_umma_bulk_kernel<W><<<grid, threads, smem, stream>>>(L, *S);                       \
+        } else {                                                                                                            \
+            static bool set = false;                                                                                        \
+            if (!set) { e = cudaFuncSetAttribute(wgrad_umma_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWgSmemMax); set = e == cudaSuccess; } \
+            if (e == cudaSuccess) wgrad_umma_kernel<W><<<grid, threads, smem, stream>>>(L);                                 \
+        }                                                                                                                   \
+        break;
+        switch (NT) {
+            WUN_WG_CASE(16) WUN_WG_CASE(32) WUN_WG_CASE(48) WUN_WG_CASE(64)
+            WUN_WG_CASE(80) WUN_WG_CASE(96) WUN_WG_CASE(112) WUN_WG_CASE(128)
+            default: return cudaErrorInvalidValue;
+        }
+#undef WUN_WG_CASE
         if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(wgrad_umma_kernel<12>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+        e = cudaGetLastError();
         if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(wgrad_umma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
     }
-    dim3 grid(L.grid_x, L.grid_y, L.grid_z);
-    static const int cw = [] { const char* env = getenv("WUN_WG_WARPS"); return env ? atoi(env) : 12; }();   // measured: 8 -> 12 converter warps = -22 % on down3 (converter-latency bound), 16 is slower
-    if (cw == 16) wgrad_umma_kernel<16><<<grid, 16 * 32 + 32, wgrad_smem_bytes(L), stream>>>(L);
-    else if (cw == 12) wgrad_umma_kernel<12><<<grid, 12 * 32 + 32, wgrad_smem_bytes(L), stream>>>(L);
-    else wgrad_umma_kernel<8><<<grid, 8 * 32 + 32, wgrad_smem_bytes(L), stream>>>(L);
-    return cudaGetLastError();
+    return cudaSuccess;
 }
+
+cudaError_t launch_wgrad_umma(const UmmaWgradLaunch& L, cudaStream_t stream) { return launch_wgrad_any<false>(L, nullptr, stream); }
 
 // ------------------------------------------------------------------------------------------------
-// Bulk-copy-fed wgrad (default; WUN_BULK_WGRAD=0 selects the converter-fed kernel above).  Validated on B200 by
-// tools/presplit_probe (down3: 241 -> 137 us) and the GPU parity suite.
-// A batched "split pass" materialises every plane view the layer's wgrad groups read (activation planes incl. interpolated
-// MID planes, and the class gradients) as hi/lo bf16 atom planes  [batch][16-ch chunk][hi a0|hi a1|lo a0|lo a1][row][16 B]
-// with zero rows around the valid range; the wgrad kernel then fills its stages with cp.async.bulk issued by ONE thread
-// instead of 12 converter warps re-converting the same rows in every (class, plane, tap-set) CTA.
+// Bulk-copy-fed wgrad (default).  A batched "split pass" materialises every plane view the layer's wgrad groups read
+// (activation planes incl. interpolated MID planes, and the class gradients) as hi/lo bf16 atom planes
+// [batch][16-ch chunk][hi a0|hi a1|lo a0|lo a1][row][16 B] with zero rows around the valid range; the wgrad kernel then fills
+// its stages with cp.async.bulk issued by ONE thread instead of re-converting the same rows in every (class, plane, tap-set) CTA.
 // ------------------------------------------------------------------------------------------------
 constexpr int kSplitRB = 2048;     // rows of one (item, 16-channel chunk) a CTA of the split pass covers (8 per thread)
 
@@ -2109,12 +892,7 @@ __global__ void __launch_bounds__(256) split_views_kernel(const __grid_constant_
         float x[16];
         load_row16(job.V, b, job.row0 + r, c * 16, x);      // zero outside the valid rows / channels; MID planes blended here
         uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const __nv_bfloat16 h0 = __float2bfloat16_rn(x[2 * k]), h1 = __float2bfloat16_rn(x[2 * k + 1]);
-            hi[k] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-            lo[k] = pack_bf16x2(x[2 * k] - __bfloat162float(h0), x[2 * k + 1] - __bfloat162float(h1));
-        }
+        split_hi_lo(x, hi, lo);
         uint8_t* o = obase + (long long)r * 16;
         *reinterpret_cast<uint4*>(o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
         *reinterpret_cast<uint4*>(o + ps) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
@@ -2140,7 +918,8 @@ __global__ void __launch_bounds__(256) split_views_kernel(const __grid_constant_
             float t = 0.f;
 #pragma unroll
             for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-            atomicAdd(job.colsum + c * 16 + threadIdx.x, t * J.colsum_scale);
+            if (job.colsum_part) job.colsum_part[(((long long)b * job.nchunk + c) * nrb + rbi) * 16 + threadIdx.x] = t;
+            else atomicAdd(job.colsum + c * 16 + threadIdx.x, t * J.colsum_scale);
         }
     }
 }
@@ -2155,186 +934,6 @@ cudaError_t launch_split_views(const SplitJobs& J, cudaStream_t stream) {
     split_views_kernel<<<dim3((unsigned)most, J.njobs), 256, 0, stream>>>(J);
     return cudaGetLastError();
 }
-
-constexpr int kWgBulkThreads = 384;   // warp 0 loader, warp 1 TMEM alloc + MMA issue, warps 4-11 epilogue
-
-
-
-__global__ void __launch_bounds__(kWgBulkThreads, 1) wgrad_umma_bulk_kernel(const __grid_constant__ UmmaWgradLaunch L,
-                                                                       const __grid_constant__ WgSplit S) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    int gi = 0;
-    while (gi + 1 < L.ngroups && (int)blockIdx.z >= L.grp[gi + 1].z0) ++gi;
-    const WgGroup& Gp = L.grp[gi];
-    const int tapset = blockIdx.z - Gp.z0;
-    if ((int)blockIdx.x >= Gp.n_ctas_x || (int)blockIdx.y >= Gp.n_mtiles * Gp.n_ntiles) return;
-    const int total_chunks = L.batch * Gp.chunks_per_batch;
-    const int g0 = blockIdx.x * Gp.chunks_per_cta;
-    const int g1 = min(g0 + Gp.chunks_per_cta, total_chunks);
-    if (g0 >= g1) return;
-    const int mtile = blockIdx.y / Gp.n_ntiles, ntile = blockIdx.y % Gp.n_ntiles;
-    const int tap0 = tapset * Gp.taps_per_cta;
-    const int ntap = min(Gp.taps_per_cta, Gp.ntaps - tap0);
-    const int NT = Gp.NT, swap = Gp.swap;
-    const PlaneView& SA = swap ? Gp.G : Gp.P;
-    const PlaneView& SB = swap ? Gp.P : Gp.G;
-    const int ca0 = mtile * 128, cb0 = ntile * NT;
-    const int rowsA = swap ? kWgRK : kWgRK + kWgSpan;
-    const int rowsB = swap ? kWgRK + kWgSpan : kWgRK;
-    const uint32_t planeA = 16u * rowsA, planeB = 16u * rowsB;
-    const int atomsA = 16, atomsB = NT / 8;
-    const uint32_t bytesA = 2u * atomsA * planeA, bytesB = 2u * atomsB * planeB;
-    const uint32_t stage_bytes = bytesA + bytesB;
-    int dmin = Gp.d[tap0];
-    for (int t = 1; t < ntap; ++t) dmin = min(dmin, Gp.d[tap0 + t]);
-
-    const int nst = L.nstages;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + nst * stage_bytes);
-    const uint32_t bar0 = smem_u32(bars);
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    const int FULL = 0, EMPTY = kWgStagesMax, ACC = 2 * kWgStagesMax;
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + ACC + 1);
-    if (tid == 0) {
-        for (int i = 0; i < kWgStagesMax; ++i) { mbar_init(BAR(FULL + i), 1); mbar_init(BAR(EMPTY + i), 1); }
-        mbar_init(BAR(ACC), 1);
-        fence_barrier_init();
-    }
-    // channel chunks the tensors really have inside this tile; the rest of the operand tile stays zero
-    const int chunksA = max(0, min(8, (SA.C - ca0 + 15) / 16)), chunksB = max(0, min(NT / 16, (SB.C - cb0 + 15) / 16));
-    for (uint32_t i = tid; i < (uint32_t)nst * stage_bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-    fence_proxy_async();
-    if (warp == 1) tmem_alloc(smem_u32(tmem_holder), Gp.tmem_cols);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_holder;
-    const int nchunks = g1 - g0;
-
-    if (warp == 0) {
-        // (all 32 lanes issuing the stage's up to 64 bulk copies was tried: every layer's wgrad got 10-30 % slower)
-        if (elect_one()) {
-            const uint8_t* baseA = swap ? S.G[gi] : S.P[gi];
-            const uint8_t* baseB = swap ? S.P[gi] : S.G[gi];
-            const long long a_ps = swap ? S.g_pstride[gi] : S.p_pstride[gi], b_ps = swap ? S.p_pstride[gi] : S.g_pstride[gi];
-            const long long a_cs = 4 * a_ps, b_cs = 4 * b_ps;
-            const long long a_bs = (swap ? S.g_nchunk[gi] : S.p_nchunk[gi]) * a_cs, b_bs = (swap ? S.p_nchunk[gi] : S.g_nchunk[gi]) * b_cs;
-            const int a_row0 = swap ? S.g_row0[gi] : S.p_row0[gi], b_row0 = swap ? S.p_row0[gi] : S.g_row0[gi];
-            const uint32_t tx = (uint32_t)(chunksA * 4) * planeA + (uint32_t)(chunksB * 4) * planeB;
-            for (int ci = 0; ci < nchunks; ++ci) {
-                const int st = ci % nst;
-                const int gch = g0 + ci;
-                const int b = gch / Gp.chunks_per_batch;
-                const int rc = Gp.m_lo + (gch % Gp.chunks_per_batch) * kWgRK;      // first G row of the chunk
-                const int rowA = (swap ? rc : rc + dmin) - a_row0, rowB = (swap ? rc + dmin : rc) - b_row0;   // array indices
-                mbar_wait_bg(BAR(EMPTY + st), ((ci / nst) & 1) ^ 1);
-                mbar_arrive_expect_tx(BAR(FULL + st), tx);
-                const uint32_t sa = smem_u32(smem + st * stage_bytes), sb = sa + bytesA;
-                for (int g = 0; g < chunksA; ++g) {
-                    const uint8_t* src = baseA + (long long)b * a_bs + (long long)(ca0 / 16 + g) * a_cs + (long long)rowA * 16;
-                    bulk_g2s(sa + (uint32_t)(2 * g) * planeA, src, planeA, BAR(FULL + st));                               // hi atom 2g
-                    bulk_g2s(sa + (uint32_t)(2 * g + 1) * planeA, src + a_ps, planeA, BAR(FULL + st));                    // hi atom 2g+1
-                    bulk_g2s(sa + (uint32_t)(atomsA + 2 * g) * planeA, src + 2 * a_ps, planeA, BAR(FULL + st));           // lo atom 2g
-                    bulk_g2s(sa + (uint32_t)(atomsA + 2 * g + 1) * planeA, src + 3 * a_ps, planeA, BAR(FULL + st));       // lo atom 2g+1
-                }
-                for (int g = 0; g < chunksB; ++g) {
-                    const uint8_t* src = baseB + (long long)b * b_bs + (long long)(cb0 / 16 + g) * b_cs + (long long)rowB * 16;
-                    bulk_g2s(sb + (uint32_t)(2 * g) * planeB, src, planeB, BAR(FULL + st));
-                    bulk_g2s(sb + (uint32_t)(2 * g + 1) * planeB, src + b_ps, planeB, BAR(FULL + st));
-                    bulk_g2s(sb + (uint32_t)(atomsB + 2 * g) * planeB, src + 2 * b_ps, planeB, BAR(FULL + st));
-                    bulk_g2s(sb + (uint32_t)(atomsB + 2 * g + 1) * planeB, src + 3 * b_ps, planeB, BAR(FULL + st));
-                }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (elect_one()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NT >> 3) << 17) | ((128u >> 4) << 24);
-            const uint32_t idesc2 = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NT >> 2) << 17) | ((128u >> 4) << 24);   // N = 2*NT
-            const uint32_t accw = (uint32_t)(Gp.fuse ? 2 * NT : NT);
-            uint32_t accum = 0;
-            for (int ci = 0; ci < nchunks; ++ci) {
-                const int st = ci % nst;
-                mbar_wait(BAR(FULL + st), (ci / nst) & 1);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + st * stage_bytes), sb = sa + bytesA;
-                // descriptors as (low word, high word): along the taps and K steps only the start-address field of the low word moves
-                // (+1 per row), so the issuing thread advances them with one 32-bit add per MMA (the same lean form as the conv kernels)
-                const uint32_t hiA = (planeA >> 4) | (1u << 14), hiB = (planeB >> 4) | (1u << 14);
-                const uint32_t a_hi0 = umma_desc_lo(sa, 128), a_lo0 = umma_desc_lo(sa + atomsA * planeA, 128);
-                const uint32_t b_hi0 = umma_desc_lo(sb, 128), b_lo0 = umma_desc_lo(sb + atomsB * planeB, 128);
-                for (int t = 0; t < ntap; ++t) {
-                    const uint32_t shift = (uint32_t)(Gp.d[tap0 + t] - dmin);
-                    const uint32_t sha = swap ? 0u : shift, shb = swap ? shift : 0u;
-                    const uint32_t td = tmem_base + (uint32_t)t * accw;
-                    if (Gp.fuse) {
-                        // fused-N: the B stage keeps the lo atom planes right behind the hi atom planes at the same stride, so one
-                        // descriptor with N = 2*NT covers [B_hi | B_lo]: 2 MMAs per product, halves summed in the epilogue
-#pragma unroll
-                        for (int ks = 0; ks < kWgRK / 16; ++ks) {
-                            const uint32_t koff = (uint32_t)(16 * ks);
-                            umma_bf16_w(td, a_hi0 + sha + koff, hiA, b_hi0 + shb + koff, hiB, idesc2, (ks == 0) ? accum : 1u);
-                            umma_bf16_w(td, a_lo0 + sha + koff, hiA, b_hi0 + shb + koff, hiB, idesc, 1u);
-                        }
-                    } else {
-#pragma unroll
-                        for (int ks = 0; ks < kWgRK / 16; ++ks) {
-                            const uint32_t koff = (uint32_t)(16 * ks);
-                            umma_bf16_w(td, a_lo0 + sha + koff, hiA, b_hi0 + shb + koff, hiB, idesc, (ks == 0) ? accum : 1u);
-                            umma_bf16_w(td, a_hi0 + sha + koff, hiA, b_lo0 + shb + koff, hiB, idesc, 1u);
-                            umma_bf16_w(td, a_hi0 + sha + koff, hiA, b_hi0 + shb + koff, hiB, idesc, 1u);
-                        }
-                    }
-                }
-                accum = 1u;
-                umma_commit(BAR(EMPTY + st));
-            }
-            umma_commit(BAR(ACC));
-        }
-        __syncwarp();
-    } else if (warp >= 4) {
-        mbar_wait_bg(BAR(ACC), 0);
-        tc_fence_after();
-        const int q4 = warp & 3;
-        const int m = ca0 + q4 * 32 + lane;
-        const bool m_ok = m < SA.C;
-        const int sM = swap ? L.w_sg : L.w_sp, sN = swap ? L.w_sp : L.w_sg;
-        for (int t = (warp - 4) >> 2; t < ntap; t += 2) {
-            float* dst_t = L.dW + (long long)Gp.woff[tap0 + t] + (long long)m * sM;
-            for (int cb = 0; cb < NT; cb += 16) {
-                if (cb0 + cb >= SB.C) break;
-                __syncwarp();
-                float v[16];
-                tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(t * (Gp.fuse ? 2 * NT : NT) + cb), v);
-                if (Gp.fuse) {
-                    float v2[16];
-                    tmem_ld16(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(t * 2 * NT + NT + cb), v2);
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] += v2[j];
-                }
-                if (!m_ok) continue;
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] *= L.scale;
-                float* dst = dst_t + (long long)(cb0 + cb) * sN;
-                if (sN == 1 && cb0 + cb + 16 <= SB.C && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-#pragma unroll
-                    for (int q = 0; q < 4; ++q) red_add_v4(dst + 4 * q, v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (cb0 + cb + j < SB.C) atomicAdd(dst + (long long)j * sN, v[j]);
-                }
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Gp.tmem_cols);
-    }
-}
-
 
 // Split arena of one layer's bulk-fed wgrad: one array per DISTINCT plane view the groups read (activation planes are shared
 // by the classes, class gradients by the planes), covering the union of the row ranges the CTAs touch.  Returns the bytes
@@ -2367,6 +966,13 @@ size_t umma_plan_wgrad_split(const UmmaWgradLaunch& U, int batch, uint8_t* arena
         sl.off = cur;
         cur += (size_t)batch * nchunk * 4 * rows * 16;
     }
+    std::vector<size_t> part_off(slots.size());       // per-CTA column sums of the views that turn out to be class gradients
+    for (size_t i = 0; i < slots.size(); ++i) {
+        const int nchunk = (slots[i].V.C + 15) / 16, rows = (slots[i].hi - slots[i].lo + 7) / 8 * 8;
+        cur = (cur + 255) / 256 * 256;
+        part_off[i] = cur;
+        cur += (size_t)batch * nchunk * ((rows + kSplitRB - 1) / kSplitRB) * 16 * sizeof(float);
+    }
     if (arena) {
         memset(S, 0, sizeof(*S));
         memset(J, 0, sizeof(*J));
@@ -2375,6 +981,7 @@ size_t umma_plan_wgrad_split(const UmmaWgradLaunch& U, int batch, uint8_t* arena
             SplitJob& job = J->job[i];
             job.V = slots[i].V; job.out = arena + slots[i].off;
             job.nchunk = (slots[i].V.C + 15) / 16; job.rows = (slots[i].hi - slots[i].lo + 7) / 8 * 8; job.row0 = slots[i].lo;
+            job.colsum_part = reinterpret_cast<float*>(arena + part_off[i]);
         }
         for (int g = 0; g < U.ngroups; ++g) {
             const SplitJob& jp = J->job[p_slot[g]];
@@ -2387,28 +994,77 @@ size_t umma_plan_wgrad_split(const UmmaWgradLaunch& U, int batch, uint8_t* arena
 }
 
 cudaError_t launch_wgrad_umma_bulk(const UmmaWgradLaunch& L, const WgSplit& S, cudaStream_t stream) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(wgrad_umma_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
+    return launch_wgrad_any<true>(L, &S, stream);
+}
+
+size_t umma_wgrad_partial_bytes(const UmmaWgradLaunch& U) {
+    long long tiles = 0;                // umma_plan_wgrad: <= kSMs CTAs, or one per (group, tile, tap set)
+    for (int g = 0; g < U.ngroups; ++g) tiles += (long long)U.grp[g].n_tapsets * U.grp[g].n_mtiles * U.grp[g].n_ntiles;
+    return (size_t)max(tiles, 132LL) * kWgSlotFloats * sizeof(float) + 256;
+}
+
+// blockIdx.y < ngroups: the weight gradient of group y, one element of its tap-set tiles per thread iteration, the partial
+// tiles of its CTAs along x added in x order; blockIdx.y == ngroups: the bias gradients of the split jobs, their CTAs' column
+// sums added in (item, row block) order.
+__global__ void __launch_bounds__(256) wgrad_reduce_kernel(const __grid_constant__ UmmaWgradLaunch L, const __grid_constant__ SplitJobs J) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if ((int)blockIdx.y < L.ngroups) {
+        if (!L.partial) return;
+        const WgGroup& G = L.grp[blockIdx.y];
+        const int NT = G.NT, tpc = G.taps_per_cta, tiles = G.n_mtiles * G.n_ntiles;
+        const PlaneView& SA = G.swap ? G.G : G.P;
+        const PlaneView& SB = G.swap ? G.P : G.G;
+        const int sM = G.swap ? L.w_sg : L.w_sp, sN = G.swap ? L.w_sp : L.w_sg;
+        const long long total = (long long)G.n_tapsets * tiles * tpc * 128 * NT;
+        for (long long e = i0; e < total; e += stride) {
+            long long r = e;
+            const int n = (int)(r % NT); r /= NT;
+            const int mrow = (int)(r % 128); r /= 128;
+            const int t = (int)(r % tpc); r /= tpc;
+            const int y = (int)(r % tiles), tapset = (int)(r / tiles);
+            const int tap = tapset * tpc + t;
+            const int m = (y / G.n_ntiles) * 128 + mrow, nn = (y % G.n_ntiles) * NT + n;
+            if (tap >= G.ntaps || m >= SA.C || nn >= SB.C) continue;
+            const float* p = L.partial + (size_t)(G.slot0 + (tapset * tiles + y) * G.n_ctas_x) * kWgSlotFloats + (size_t)(t * 128 + mrow) * NT + n;
+            float sum = 0.f;
+            for (int x = 0; x < G.n_ctas_x; ++x) sum += p[(size_t)x * kWgSlotFloats];
+            atomicAdd(L.dW + G.woff[tap] + (long long)m * sM + (long long)nn * sN, sum);
+        }
+        return;
     }
-    dim3 grid(L.grid_x, L.grid_y, L.grid_z);
-    wgrad_umma_bulk_kernel<<<grid, kWgBulkThreads, wgrad_smem_bytes(L), stream>>>(L, S);
+    long long total = 0;
+    for (int j = 0; j < J.njobs; ++j) if (J.job[j].colsum) total += J.job[j].V.C;
+    for (long long e = i0; e < total; e += stride) {
+        int j = 0;
+        long long c = e;
+        for (;; ++j) {
+            if (!J.job[j].colsum) continue;
+            if (c < J.job[j].V.C) break;
+            c -= J.job[j].V.C;
+        }
+        const SplitJob& job = J.job[j];
+        const int nrb = (job.rows + kSplitRB - 1) / kSplitRB;
+        float sum = 0.f;
+        for (int b = 0; b < J.batch; ++b)
+            for (int rb = 0; rb < nrb; ++rb) sum += job.colsum_part[(((long long)b * job.nchunk + c / 16) * nrb + rb) * 16 + c % 16];
+        atomicAdd(job.colsum + c, sum * J.colsum_scale);
+    }
+}
+
+cudaError_t launch_wgrad_reduce(const UmmaWgradLaunch& U, const SplitJobs& J, cudaStream_t stream) {
+    wgrad_reduce_kernel<<<dim3(132 * 2, U.ngroups + 1), 256, 0, stream>>>(U, J);
     return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight pre-pack: fp32 W -> hi/lo bf16 blocks in K-step streaming order.  blockIdx.y = job (class, split);
-// one thread per (block, n, k) element.  Block bi = ((group, chunk), term) in the kernel's loop order; element
-// (a, n, kk) of the hi half sits at byte a*32*NPAD + (n/8)*128 + (n%8)*16 + kk*2, the lo half 16*NPAD bytes later:
-// per K atom the block is a K-major [hi rows 0..NPAD) | lo rows NPAD..2*NPAD) matrix, so ONE descriptor with
-// N = 2*NPAD covers [B_hi | B_lo] (fused-N mode) and N = NPAD covers B_hi alone.
-// ------------------------------------------------------------------------------------------------
+// weight pre-pack: fp32 W -> hi/lo bf16 blocks in K-step streaming order.  blockIdx.y = job (class, split).
+// Block bi = ((group, chunk), term) in the kernel's loop order; element (a, n, kk) of the hi half sits at byte
+// a*32*NPAD + (n/8)*128 + (n%8)*16 + kk*2, the lo half 16*NPAD bytes later: per K atom the block is a K-major
+// [hi rows 0..NPAD) | lo rows NPAD..2*NPAD) matrix.
 // One thread per (block, K atom, n): 8 k-values -> one 16-byte hi store and one 16-byte lo store (consecutive n = consecutive
 // 16 B: coalesced); the fp32 reads are coalesced along n (forward: w_sn = 1) or 32 B contiguous per thread (dgrad: w_sk = 1).
-// (Round 1 used one thread per bf16 element with 2-byte stores: 448 us per step for the 60 packs; this form moves the same
-// bytes with 1/16 of the threads.)
+// ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) umma_pack_kernel(const __grid_constant__ UmmaPackLaunch PL) {
     const UmmaPackJob& J = PL.jobs[blockIdx.y];
     const long long total = (long long)J.nblocks * PL.NPAD * 2;
@@ -2456,15 +1112,28 @@ cudaError_t launch_umma_pack(const UmmaPackLaunch& PL, cudaStream_t stream) {
     const long long total = (long long)maxblk * PL.NPAD * 2;
     if (total <= 0 || PL.njobs <= 0) return cudaSuccess;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 4) blocks = 148 * 4;
+    if (blocks > 132 * 4) blocks = 132 * 4;
     dim3 grid((unsigned)blocks, PL.njobs);
     umma_pack_kernel<<<grid, 256, 0, stream>>>(PL);
     return cudaGetLastError();
 }
 
 // ------------------------------------------------------------------------------------------------
-// host: turn a generic plane-convolution launch (launch.h ConvLaunch) into a tcgen05 launch
+// host: turn a generic plane-convolution launch (launch.h ConvLaunch) into a tensor-core launch
 // ------------------------------------------------------------------------------------------------
+constexpr int kNpadMax = 128;      // accumulator columns per CTA: 64 fp32 registers per thread of each warpgroup
+constexpr int kSMs = 132;
+
+// output-channel splits of a launch: enough for NPAD <= kNpadMax, doubled once when the row tiles alone leave SMs idle (each
+// CTA then runs cheaper MMAs; the K loop of a tile is the critical path of those latency-bound launches)
+static int conv_nsplit(int N, long long tiles128) {
+    const int npad_total = (N + 15) / 16 * 16;
+    int s = (npad_total + kNpadMax - 1) / kNpadMax;
+    if (s * 2 <= kUmmaMaxSplit && tiles128 * s * 2 <= kSMs && (N + s * 2 - 1) / (s * 2) >= 48) s *= 2;
+    return s;
+}
+static int conv_npad(int N, int nsplit) { return ((N + nsplit - 1) / nsplit + 15) / 16 * 16; }
+
 bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* ch) {
     memset(ch, 0, sizeof(*ch));
     if (L.N < 16 || L.ncls < 1 || L.ncls > kMaxClasses) return false;
@@ -2483,29 +1152,20 @@ bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* ch) {
         if (P.C % 8 != 0 || P.C < 8) return false;
         if (P.rstride % 4 != 0 || P.bstride % 4 != 0 || (reinterpret_cast<uintptr_t>(P.base) & 15) != 0) return false;
     }
-    const int npad_total = (L.N + 15) / 16 * 16;
-    if (npad_total > 512) return false;
-    ch->nsplit = (npad_total <= 256) ? 1 : 2;
-    {   // deep layers have fewer row tiles than there are SMs: split the output channels over more CTAs (each CTA then
-        // runs cheaper MMAs; the K loop of a tile is the critical path of these latency-bound launches)
-        long long tiles128 = 0;
-        for (int q = 0; q < L.ncls; ++q) tiles128 += (long long)((L.cls[q].m_hi - L.cls[q].m_lo + 127) / 128) * L.batch;
-        const char* env = getenv("WUN_NSPLIT_MAX");
-        const int smax = env ? atoi(env) : 2;        // measured: 2 helps (10.72 -> 10.56 ms/step), 4 hurts
-        while (ch->nsplit * 2 <= smax && tiles128 * ch->nsplit * 2 <= 148 && (L.N + ch->nsplit * 2 - 1) / (ch->nsplit * 2) >= 48)
-            ch->nsplit *= 2;
-    }
-    ch->NPAD = (ch->nsplit == 1) ? npad_total : (((L.N + ch->nsplit - 1) / ch->nsplit + 15) / 16 * 16);
+    if ((L.N + 15) / 16 * 16 > kUmmaMaxSplit * kNpadMax) return false;
+    long long tiles128 = 0;
+    for (int q = 0; q < L.ncls; ++q) tiles128 += (long long)((L.cls[q].m_hi - L.cls[q].m_lo + 127) / 128) * L.batch;
+    ch->nsplit = conv_nsplit(L.N, tiles128);
+    ch->NPAD = conv_npad(L.N, ch->nsplit);
     int maxspan = 0, max_rows = 0;
-    int cls_span[kMaxClasses], cls_jobs[kMaxClasses];
     size_t bytes = 0;
-    // packed-weight columns reserved per block: independent of the batch-dependent tiling below (the arena is sized by a
-    // batch-1 dry run), i.e. the widest of the 1- and 2-way output-channel splits
-    const int pack_cols = max(npad_total, 2 * (((L.N + 1) / 2 + 15) / 16 * 16));
+    // packed-weight columns reserved per block: independent of the batch-dependent split above (the arena is sized by a
+    // batch-1 dry run), i.e. the widest of the two split counts conv_nsplit can choose
+    const int s0 = conv_nsplit(L.N, 1LL << 40);
+    const int pack_cols = (s0 * 2 <= kUmmaMaxSplit) ? max(s0 * conv_npad(L.N, s0), 2 * s0 * conv_npad(L.N, 2 * s0)) : s0 * conv_npad(L.N, s0);
     for (int q = 0; q < L.ncls; ++q) {
         const OutView& O = L.cls[q];
         max_rows = max(max_rows, O.m_hi - O.m_lo);
-        cls_span[q] = 0; cls_jobs[q] = 0;
         int ngroups = 0, t = O.term_begin;
         while (t < O.term_end) {
             const int p = L.terms[t].plane;
@@ -2513,8 +1173,6 @@ bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* ch) {
             while (t1 < O.term_end && L.terms[t1].plane == p) { dmin = min(dmin, L.terms[t1].d); dmax = max(dmax, L.terms[t1].d); ++t1; }
             if (dmax - dmin > 24) return false;
             maxspan = max(maxspan, dmax - dmin);
-            cls_span[q] = max(cls_span[q], dmax - dmin);
-            cls_jobs[q] += (L.planes[p].C + 15) / 16;
             bytes += (size_t)((L.planes[p].C + 15) / 16) * (t1 - t) * 64u * pack_cols;
             ++ngroups; t = t1;
         }
@@ -2522,159 +1180,13 @@ bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* ch) {
     }
     if (max_rows <= 0) return false;
     ch->pack_bytes = (bytes + 255) / 256 * 256;
-    {   // batch-folded cluster split-K kernel (plane_conv_umma_fold): launches whose row tiles leave SMs idle.
-        // WUN_FOLD: 0 = never, 1 (default) = launches the unfolded tiling would run on <= 148 CTAs, 2 = whenever it fits.
-        const char* env = getenv("WUN_FOLD");
-        const int mode = env ? atoi(env) : 1;
-        bool ok = mode != 0 && (L.N % 4 == 0) && L.pairC == 0;     // (the folded kernel's epilogue has no pair-merged form)
-        long long old_ctas = 0;
-        int jmin = 1 << 30;
-        for (int q = 0; q < L.ncls; ++q) {
-            const OutView& O = L.cls[q];
-            if (O.m_hi <= O.m_lo) continue;
-            if (O.rstride % 4 || O.bstride % 4 || (reinterpret_cast<uintptr_t>(O.base) & 15) ||
-                (O.saved && (reinterpret_cast<uintptr_t>(O.saved) & 15))) ok = false;
-            old_ctas += (long long)((O.m_hi - O.m_lo + 127) / 128) * L.batch;
-            jmin = min(jmin, cls_jobs[q]);
-        }
-        if (ok && mode == 1 && old_ctas > 148) ok = false;
-        if (ok) {
-            const int nsplit = (npad_total <= 256) ? 1 : 2;
-            const int NPAD = (nsplit == 1) ? npad_total : (((L.N + 1) / 2 + 15) / 16 * 16);
-            int best_mt = 0, best_s = 0; long long best_ctas = 0;
-            for (int MT = 2; MT >= 1; --MT) {
-                if ((size_t)MT * 128 * (NPAD + 4) * 4 > 160 * 1024 || MT * NPAD > 512) continue;
-                long long T = 0;
-                for (int q = 0; q < L.ncls; ++q) {
-                    const int rows = L.cls[q].m_hi - L.cls[q].m_lo;
-                    if (rows > 0) T += ((long long)L.batch * (rows + cls_span[q]) + MT * 128 - 1) / (MT * 128);
-                }
-                T *= nsplit;
-                for (int S = 1; S <= kFoldMaxSplit && S <= jmin; ++S) {
-                    const long long ctas = T * S;
-                    // One CTA per SM and a cluster lives inside one GPC: resident clusters of this kernel's footprint as
-                    // cudaOccupancyMaxActiveClusters reports them on B200 (tools/cluster_probe: 148 74 45 33 26 22 15 15),
-                    // one less for S >= 3 as margin for parts with other SM harvesting.  More clusters than slots = a second
-                    // wave (seen: S = 7 x 18 tiles, 50 us vs 32 us for its neighbours).
-                    static const int kClusterSlots[kFoldMaxSplit + 1] = {0, 148, 74, 44, 32, 25, 21, 14, 14};
-                    if (T > kClusterSlots[S]) continue;
-                    (void)ctas;
-                    if (ctas > best_ctas) { best_ctas = ctas; best_mt = MT; best_s = S; }   // ties: the larger MT / smaller S seen first
-                }
-            }
-            if (best_ctas > 0) {
-                const int rows_alloc = best_mt * 128 + (maxspan + 7) / 8 * 8;
-                const int blk = 64 * NPAD;
-                int TB = 36864 / blk;
-                if (TB > 4) TB = 4;
-                if (TB < 1) TB = 1;
-                int nbs = 147456 / (TB * blk);
-                if (nbs > kBStagesMax) nbs = kBStagesMax;
-                const long long left = 200 * 1024 - (long long)kFoldSlabStages * 64 * rows_alloc - 4096;
-                while (nbs > 2 && (long long)nbs * TB * blk > left) --nbs;
-                if (nbs < 2) nbs = 2;
-                if ((long long)nbs * TB * blk <= left) {        // else: fall through to the unfolded kernels
-                    ch->folded = 1; ch->ksplit = best_s; ch->nsplit = nsplit; ch->NPAD = NPAD; ch->MT = best_mt;
-                    ch->rows_alloc = rows_alloc;
-                    int tm = 32;
-                    while (tm < best_mt * NPAD) tm *= 2;
-                    ch->tmem_cols = tm;
-                    ch->nteams = 4; ch->persistent = 0; ch->fuse = 0;
-                    ch->TB = TB; ch->nbs = nbs;
-                    return true;
-                }
-            }
-        }
-    }
-    // two co-resident CTAs per SM beat one big one (measured): keep TMEM <= 256 columns and smem <= ~110 KB
-    int MT = 256 / ch->NPAD;
-    if (MT > 2) MT = 2;
-    if (MT < 1) MT = 1;
-    if (max_rows <= 128) MT = 1;
-    ch->MT = MT;
-    ch->rows_alloc = MT * 128 + (maxspan + 7) / 8 * 8;
-    int tm = 32;
-    while (tm < MT * ch->NPAD) tm *= 2;
-    ch->tmem_cols = tm;
-    {   // fused-N mode (2 MMAs per product instead of 3): pays when the MMA is at its shared-memory floor (small N)
-        // WUN_FUSE_N: 0 (default) = off, 1 = launches the persistent kernel does not take, 2 = preferred over persistent.
-        // Measured: no step-time gain (8.583 vs 8.584 ms) - those launches are not MMA-bound - but the separate hi*lo
-        // accumulator halves the worst-case rounding error, so the mode stays available.
-        const char* env = getenv("WUN_FUSE_N");
-        const int mode = env ? atoi(env) : 1;       // round 2: default on (lean issue loop made the small-N launches MMA-bound)
-        ch->fuse = (mode > 0 && ch->NPAD <= 64) ? 1 : 0;
-    }
-    // weight ring: stages of TB taps (fewer barrier round trips for the single MMA-issuing thread).  Launches that
-    // fill the GPU keep it at ~48 KB so two CTAs fit per SM; launches with fewer CTAs than SMs (the deep layers) are
-    // weight-stream-latency bound, so they get a deep ring instead.
-    long long n_ctas = 0;
-    for (int q = 0; q < L.ncls; ++q)
-        n_ctas += (long long)((L.cls[q].m_hi - L.cls[q].m_lo + MT * 128 - 1) / (MT * 128)) * ch->nsplit * L.batch;
-    const bool sparse = n_ctas <= 148;
+    ch->MT = 1;
+    ch->rows_alloc = 128 + (maxspan + 7) / 8 * 8;
+    // weight ring: stages of TB taps (~16 KB) and ~64 KB in all, so that two CTAs share an SM (one hides the other's epilogue
+    // and slab conversion)
     const int blk = 64 * ch->NPAD;
-    int TB = (sparse ? 36864 : 24576) / blk;
-    if (TB > 4) TB = 4;
-    if (TB < 1) TB = 1;
-    int nbs = (sparse ? 147456 : 49152) / (TB * blk);
-    if (nbs > kBStagesMax) nbs = kBStagesMax;
-    if (nbs < 2) nbs = 2;
-    ch->TB = TB; ch->nbs = nbs;
-    {
-        const char* env = getenv("WUN_TEAMS");
-        ch->nteams = (sparse && !(env && env[0] == '2')) ? 4 : 2;
-        if (ch->nteams == 4) {      // 6 slab stages: keep the ring within what is left of ~200 KB
-            const long long left = 200 * 1024 - 6LL * 64 * ch->rows_alloc - 4096;
-            while (ch->nbs > 2 && (long long)ch->nbs * TB * blk > left) --ch->nbs;
-            if ((long long)ch->nbs * TB * blk > left) ch->nteams = 2;
-        }
-    }
-    // persistent one-CTA-per-SM kernel for launches with at least ~3 tiles per SM whose double-buffered accumulators fit TMEM
-    ch->persistent = 0;
-    {
-        // WUN_PERSISTENT: 0 = never, 1 = forward launches with NPAD <= 80, 2 (default) = every eligible launch incl. dgrad,
-        // 3..6 = experiment subsets.  Measured after the elect_one() issue-loop fix (ms/step, M4 B=16): 0: 9.17, 1: 9.13,
-        // 2: 8.99, 3: 9.17, 5 (fwd, any NPAD): 9.13, 6: 9.12; with 12 wgrad converter warps 1: 8.76, 2: 8.58.
-        const char* env = getenv("WUN_PERSISTENT");
-        const int mode = env ? atoi(env) : 2;
-        const bool allow = (mode == 2) || (mode == 1 && L.epilogue == EPI_BIAS_LRELU && ch->NPAD <= 80) ||
-                           (mode == 3 && ch->NPAD <= 80) || (mode == 4 && ch->NPAD <= 48) ||
-                           (mode == 5 && L.epilogue == EPI_BIAS_LRELU) ||
-                           (mode == 6 && (L.epilogue == EPI_BIAS_LRELU || ch->NPAD > 80));
-        const char* envm = getenv("WUN_PERS_MIN");
-        const int min_per_sm = envm ? atoi(envm) : 3;
-        if (allow && n_ctas >= (long long)min_per_sm * 148 && 2 * MT * ch->NPAD * (ch->fuse ? 2 : 1) <= 512) {
-            ch->persistent = 1;
-            // (128-row tiles for better last-round balance were tried - rounds x height cost model - and lost badly:
-            //  9.04 vs 8.51 ms/step; the 256-row tile amortises the slab halo and the per-tile pipeline ramp.)
-            {   // converter teams of the persistent kernel (WUN_PERS_TEAMS = 2 | 3)
-                const char* envt = getenv("WUN_PERS_TEAMS");
-                ch->nteams = (envt && envt[0] == '2') ? 2 : 3;
-            }
-            {   // dgrad: two epilogue warp groups + two converter teams (WUN_EPI2=0: one group, three teams)
-                const char* enve = getenv("WUN_EPI2");
-                const char* envf = getenv("WUN_EPI2_FWD");          // forward launches too (experiment; the fused-output conv keeps one group)
-                ch->epi2 = ((L.epilogue == EPI_SLOPE && !(enve && enve[0] == '0')) || (L.epilogue != EPI_SLOPE && envf && envf[0] == '1')) ? 1 : 0;
-                if (ch->epi2) ch->nteams = 2;
-            }
-            // one CTA per SM: a deeper weight ring fits next to the slab stages and the epilogue staging tile
-            const long long cw = (ch->NPAD < 128) ? ch->NPAD : 128;
-            long long left = 218 * 1024 - (long long)(ch->nteams + 1) * 64 * ch->rows_alloc - 128 * (cw + 4) * 4 - 1024 - 4LL * ch->NPAD * ch->nsplit;
-            if (left > 98304) left = 98304;
-            ch->nbs = (int)(left / (TB * blk));
-            if (ch->nbs > kBStagesMax) ch->nbs = kBStagesMax;
-            if (ch->nbs < 2) { ch->nbs = 2; ch->nteams = 2; }
-            if (ch->nteams != 2) ch->epi2 = 0;
-            int tm2 = 32;
-            while (tm2 < 2 * MT * ch->NPAD * (ch->fuse ? 2 : 1)) tm2 *= 2;
-            ch->tmem_cols = tm2;
-        }
-    }
-    if (ch->fuse && !ch->persistent) {
-        int tmf = 32;
-        while (tmf < 2 * MT * ch->NPAD) tmf *= 2;
-        if (ch->nteams == 2 && tmf > 256) ch->fuse = 0;      // two CTAs per SM share the 512 TMEM columns
-        else ch->tmem_cols = tmf;
-    }
+    ch->TB = min(4, max(1, 16384 / blk));
+    ch->nbs = min(kBStagesMax, max(2, 65536 / (ch->TB * blk)));
     return true;
 }
 
@@ -2695,20 +1207,7 @@ cudaError_t umma_build(const ConvLaunch& L, const UmmaChoice& ch, uint8_t* arena
     memset(&PL, 0, sizeof(PL));
     for (int p = 0; p < L.nplanes; ++p) U.planes[p] = L.planes[p];
     U.ncls = L.ncls; U.N = L.N; U.NPAD = ch.NPAD; U.nsplit = ch.nsplit; U.MT = ch.MT; U.rows_alloc = ch.rows_alloc;
-    U.tmem_cols = ch.tmem_cols; U.TB = ch.TB; U.nbs = ch.nbs; U.persistent = ch.persistent; U.nteams = ch.nteams; U.fuse = ch.fuse; U.bias = L.bias; U.epilogue = L.epilogue; U.batch = L.batch;
-    U.folded = ch.folded; U.ksplit = ch.ksplit; U.epi2 = ch.epi2;
-    { static const int et = [] { const char* e = getenv("WUN_EPI_TEAMS"); return (e && e[0] == '1') ? 1 : 2; }(); U.epi_teams = et; }
-    {   // A/B switches of the folded kernel: WUN_FOLD_COMPACT (bit 0: one-row converter passes), WUN_FOLD_PREFETCH (bit 1: L2 prefetch)
-        static const int flags = [] {
-            const char* a = getenv("WUN_FOLD_COMPACT"); const char* b = getenv("WUN_FOLD_PREFETCH");
-            return ((a && a[0] == '1') ? 1 : 0) | ((b && b[0] == '1') ? 2 : 0);
-        }();
-        U.fold_flags = flags;
-    }
-    {   // every group's taps sorted with consecutive row shifts (checked below): lean issue loop; WUN_LEAN=0 = generic loop (A/B)
-        static const int lean = [] { const char* e = getenv("WUN_LEAN"); return (e && e[0] == '0') ? 0 : 1; }();
-        U.consec = lean;
-    }
+    U.TB = ch.TB; U.nbs = ch.nbs; U.bias = L.bias; U.epilogue = L.epilogue; U.batch = L.batch;
     PL.W = L.W; PL.w_sk = L.w_sk; PL.w_sn = L.w_sn; PL.N = L.N; PL.NPAD = ch.NPAD;
     int nterm_total = 0;
     for (int q = 0; q < L.ncls; ++q) nterm_total = max(nterm_total, L.cls[q].term_end);
@@ -2730,21 +1229,11 @@ cudaError_t umma_build(const ConvLaunch& L, const UmmaChoice& ch, uint8_t* arena
             int t1 = t;
             while (t1 < K.out.term_end && L.terms[t1].plane == p) { G.dmin = min(G.dmin, L.terms[t1].d); ++t1; }
             G.term_end = t1;
-            for (int tt = t; tt < t1; ++tt) if (L.terms[tt].d != L.terms[t].d + (tt - t)) U.consec = 0;
             const int g = K.ngroups++;
             K.groups[g] = G;
             J0.g_nchunk[g] = (L.planes[p].C + 15) / 16; J0.g_nterm[g] = t1 - t; J0.g_term_begin[g] = t; J0.g_C[g] = L.planes[p].C;
             nblocks += J0.g_nchunk[g] * J0.g_nterm[g];
             t = t1;
-        }
-        {   // folded launches: virtual rows per batch item = the class's rows + its widest tap span
-            int span = 0;
-            for (int g = 0; g < K.ngroups; ++g) {
-                int dmax = K.groups[g].dmin;
-                for (int tt = K.groups[g].term_begin; tt < K.groups[g].term_end; ++tt) dmax = max(dmax, L.terms[tt].d);
-                span = max(span, dmax - K.groups[g].dmin);
-            }
-            U.fold_pitch[q] = max(1, K.out.m_hi - K.out.m_lo + span);
         }
         J0.ngroups = K.ngroups; J0.nblocks = nblocks;
         for (int sp = 0; sp < ch.nsplit; ++sp) {

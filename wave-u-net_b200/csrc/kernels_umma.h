@@ -1,4 +1,4 @@
-// kernels_umma.h - parameter blocks and launchers of the tcgen05 plane-convolution kernel.
+// kernels_umma.h - parameter blocks and launchers of the tensor-core (wgmma) plane-convolution and wgrad kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -30,26 +30,15 @@ struct UmmaLaunch {
     int d[kMaxTerms];       // row shift of every term (grouped per class/plane)
     int ncls;
     int N;                  // real output channels
-    int NPAD;               // channels handled per split, multiple of 16, <= 256
-    int nsplit;             // output-channel splits (N > 256, or to spread sparse launches over more SMs)
-    int MT;                 // 128-row tiles per CTA
-    int rows_alloc;         // slab rows per stage  (>= MT*128 + max row-shift span)
-    int tmem_cols;          // power of two >= MT*NPAD
+    int NPAD;               // channels handled per split, multiple of 16, <= 128
+    int nsplit;             // output-channel splits (N > 128, or to spread sparse launches over more SMs)
+    int MT;                 // 128-row tiles per CTA (1)
+    int rows_alloc;         // slab rows  (>= MT*128 + max row-shift span)
     int TB, nbs;            // weight ring: nbs stages of TB taps
-    int nteams;             // converter teams of the non-persistent kernel: 2 (dense launches) or 4 (sparse)
-    int persistent;         // 1: one-CTA-per-SM tile loop with double-buffered TMEM (big layers)
-    int fuse;               // 1: fused-N MMAs over [B_hi | B_lo] (2 per product; accumulator tile = 2*NPAD columns)
-    int consec;             // 1: within every group the terms are sorted by row shift, d = dmin, dmin+1, ... (issue_taps path)
-    int folded;             // 1: batch-folded row tiles + cluster split-K (plane_conv_umma_fold; the deep, few-row layers)
-    int fold_flags;         // folded: bit 0 = one-row converter passes (compact code), bit 1 = L2 prefetch of the CTA's weights
-    int ksplit;             // folded: CTAs per cluster; each takes a contiguous range of the tile's (plane, chunk) jobs
-    int fold_pitch[kMaxClasses];   // folded: virtual rows per batch item of a class = its rows + its widest tap span
     const float* bias;
     int epilogue;
     int batch;
     int pairC;              // > 0: pair-merged classes (launch.h OutView::pairC); the bias repeats with this period
-    int epi2;               // persistent dgrad: two epilogue warp groups (and two converter teams) - plane_conv_umma_persistent_dg2
-    int epi_teams;          // 2-CTA / sparse kernel: converter teams that share the epilogue (2; WUN_EPI_TEAMS=1 = team 0 alone)
 };
 
 constexpr int kUmmaMaxPackJobs = kMaxClasses * kUmmaMaxSplit;
@@ -74,9 +63,7 @@ struct UmmaPackLaunch {
 };
 
 struct UmmaChoice {         // tiling decisions for one ConvLaunch
-    int NPAD, nsplit, MT, rows_alloc, tmem_cols, TB, nbs, persistent, nteams, fuse;
-    int folded, ksplit;     // batch-folded cluster split-K kernel (sparse launches)
-    int epi2;               // see UmmaLaunch
+    int NPAD, nsplit, MT, rows_alloc, TB, nbs;
     size_t pack_bytes;      // arena bytes the packed weights of this launch need
 };
 
@@ -95,15 +82,14 @@ struct WgGroup {
     int woff[kWgMaxTaps];
     // tiling (filled by umma_plan_wgrad)
     int swap;               // 0: A (M side) = P, B (N side) = G;  1: A = G, B = P
-    int NT;                 // N-tile width (multiple of 16, <= 128)
+    int NT;                 // N-tile width (multiple of 16, <= 128; the same for every group of a launch)
     int n_mtiles, n_ntiles; // tiles of 128 / NT channels
     int taps_per_cta, n_tapsets;
     int chunks_per_batch;   // 64-row chunks per batch element
     int chunks_per_cta;     // consecutive (batch-folded) chunks one CTA reduces
     int n_ctas_x;           // ceil(batch*chunks_per_batch / chunks_per_cta)
-    int tmem_cols;
-    int fuse;               // bulk-fed kernel: fused-N MMAs (A_hi x [B_hi|B_lo], A_lo x B_hi); accumulator stride 2*NT per tap
     int z0;                 // first blockIdx.z of this group (one z per tap set)
+    int slot0;              // first partial-tile slot of this group (UmmaWgradLaunch::partial)
 };
 
 struct UmmaWgradLaunch {
@@ -111,14 +97,18 @@ struct UmmaWgradLaunch {
     int ngroups;
     int batch;
     float* dW;
+    // not null: every CTA stores its scaled 128 x (taps x NT) tile at slot (slot0 + (tapset * tiles + y) * n_ctas_x + x) and
+    //   launch_wgrad_reduce adds the slots in a fixed order (a run-to-run reproducible dW); null: CTAs add into dW atomically
+    float* partial;
     int w_sp, w_sg;         // element strides of dW along the P-channel / G-channel index
     float scale;
     int grid_x, grid_y, grid_z;
     int nstages;            // shared-memory pipeline stages (2 or 3)
 };
 
+// converter-fed wgrad: for layers whose operand views do not fit one split pass (umma_plan_wgrad_split returns 0)
 cudaError_t launch_wgrad_umma(const UmmaWgradLaunch& L, cudaStream_t stream);
-// ---- bulk-copy-fed wgrad (experimental, WUN_BULK_WGRAD=1) --------------------------------------------------------
+// ---- bulk-copy-fed wgrad (default) ------------------------------------------------------------------------------------
 constexpr int kSplitMaxJobs = 2 * kWgMaxGroups;
 
 struct SplitJob {           // materialise plane rows [row0, row0 + rows) of V as hi/lo bf16 atom planes at `out`
@@ -126,6 +116,7 @@ struct SplitJob {           // materialise plane rows [row0, row0 + rows) of V a
     uint8_t* out;           // [batch][nchunk][4][rows][16 B]
     int nchunk, rows, row0;
     float* colsum;          // class-gradient views: bias gradient [V.C] that receives colsum_scale * column sums (else null)
+    float* colsum_part;     // the per-CTA column sums [batch][nchunk][row blocks][16]; launch_wgrad_reduce adds them into colsum
 };
 
 struct SplitJobs {
@@ -146,6 +137,13 @@ struct WgSplit {            // where the wgrad groups find their operands (fille
 // when `arena` (256-B aligned, that many bytes) is given.
 size_t umma_plan_wgrad_split(const UmmaWgradLaunch& U, int batch, uint8_t* arena, WgSplit* S, SplitJobs* J);
 cudaError_t launch_split_views(const SplitJobs& J, cudaStream_t stream);
+// Bytes of the partial tiles of a bulk-fed wgrad launch (U.partial), at any batch.
+size_t umma_wgrad_partial_bytes(const UmmaWgradLaunch& U);
+// The fixed-order sums of a layer's weight gradient (U.partial) and bias gradient (the colsum jobs of J) into dW / colsum:
+// float atomics would add the CTAs' contributions in a different order on every run.  A dW or bias element receives one sum
+// per forward class (<= 2 in every launch the engine plans), and two float additions onto zero commute, so the result is the
+// same bits on every run.
+cudaError_t launch_wgrad_reduce(const UmmaWgradLaunch& U, const SplitJobs& J, cudaStream_t stream);
 cudaError_t launch_wgrad_umma_bulk(const UmmaWgradLaunch& L, const WgSplit& S, cudaStream_t stream);
 // rows one wgrad CTA can read past the last valid row of a group: G side / P side (chunk rounding + tap span)
 constexpr int kWgOverreachG = 64, kWgOverreachP = 64 + 16;
@@ -153,12 +151,10 @@ constexpr int kWgOverreachG = 64, kWgOverreachP = 64 + 16;
 // fills the tiling fields (groups' P, G, taps and the common fields already set); false = not eligible
 bool umma_plan_wgrad(UmmaWgradLaunch* L);
 
-// Output layer fused into the epilogue of the last up block's forward conv (persistent kernel only; north_star "the per-source
-// tanh / difference OutputLayer is fused into the final conv").  The conv epilogue holds one feature row per thread: it applies the
-// 1x1 output convs over [crop(mix) || features] (OutputLayer.py:8,15), the activation, the difference source (:17-22) and the test-time
-// clip, writes the source estimates, and - when targets are given - the MSE loss (Training.py:50-63), dL/dpre of the output
-// convs, their weight / bias gradients and the gradient w.r.t. the features' pre-activation, so that output_fwd / output_dgrad /
-// output_wgrad launch nothing.
+// Output layer fused into the epilogue of the last up block's forward conv: the 1x1 output convs over [crop(mix) || features]
+// (OutputLayer.py:8,15), the activation, the difference source (:17-22), the test-time clip, the MSE loss (Training.py:50-63) and
+// their gradients.  The wgmma conv kernel keeps its accumulators in registers and has no room for this epilogue, so
+// umma_output_fusable() is false and the output layer runs in its own kernels; the block stays the engine's description of it.
 constexpr int kOutFuseMaxCols = 8;    // nconv * C the fused epilogue supports (registers); wider heads use the separate kernels
 struct OutputFuse {
     OutputLaunch O;
@@ -177,9 +173,9 @@ size_t umma_choice_smem_bytes(const UmmaChoice& ch);
 size_t umma_wgrad_smem_bytes(const UmmaWgradLaunch& L);
 cudaError_t launch_plane_conv_umma(const UmmaLaunch& L, cudaStream_t stream, const OutputFuse* fuse = nullptr);
 cudaError_t launch_umma_pack(const UmmaPackLaunch& PL, cudaStream_t stream);
-// Decide whether / how a generic plane-convolution launch runs on tcgen05; false = not eligible (SIMT).
+// Decide whether / how a generic plane-convolution launch runs on the tensor cores; false = not eligible (SIMT).
 bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* choice);
-// Pack the weights into `arena` (choice.pack_bytes, 256-B aligned) and enqueue the tcgen05 kernel.
+// Pack the weights into `arena` (choice.pack_bytes, 256-B aligned) and enqueue the tensor-core kernel.
 cudaError_t umma_run_conv(const ConvLaunch& L, const UmmaChoice& choice, uint8_t* arena, cudaStream_t stream);
 // The two parameter blocks umma_run_conv launches (exposed for the probe / per-kernel timing).
 cudaError_t umma_build(const ConvLaunch& L, const UmmaChoice& choice, uint8_t* arena, UmmaLaunch* U, UmmaPackLaunch* PL);
