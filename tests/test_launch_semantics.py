@@ -1,6 +1,6 @@
 """Host-only check of the planner's launch algebra (no GPU): the engine exports the full description of every plane-convolution
 launch of a training step (wun_debug_launches: planes, classes, terms - csrc/launch.h), and a numpy interpreter executes those
-descriptions on a random workspace.  A pair-merged launch (launch.h OutView::pairC: two classes of equal width issued as one class
+descriptions (tests/launch_interp.py) on a random workspace.  A pair-merged launch (launch.h OutView::pairC: two classes of equal width issued as one class
 of 2C columns, round 2) must write exactly what the two-class form of the same launch writes - forward (bias + LeakyReLU with the
 bias repeated per half) and dgrad (slope from the saved activation, skip-window accumulate ranges, per-half row ranges), for
 context ('valid'), 'same'-padding and learned-upsampling nets.  The interpreter follows plane_conv_kernel (csrc/kernels_simt.cu),
@@ -10,100 +10,8 @@ import pytest
 
 import Config
 import wun
+from launch_interp import decode, plane_rows, run_launch, run_wgrad_group
 from oracle import wave_unet_oracle as O
-
-WS_BASE, PAR_BASE, MIX_BASE = 1 << 40, 1 << 41, 1 << 42
-SLACK = 1 << 38
-
-
-def decode(addr):
-    """raw exported address -> (buffer name, element offset); offsets may be negative (views that start before their tensor)."""
-    if addr >= MIX_BASE - SLACK:
-        return "mix", (addr - MIX_BASE) // 4
-    if addr >= PAR_BASE - SLACK:
-        return "par", (addr - PAR_BASE) // 4
-    return "ws", (addr - WS_BASE) // 4
-
-
-def plane_rows(mem, P, b, rows):
-    """[len(rows), C] float64: plane rows `rows` of batch item b, zero outside [r_lo, r_hi); MID planes blend two tensor rows
-    (plane_load, kernels_simt.cu)."""
-    name, base = decode(P["base"])
-    buf = mem[name]
-    C = P["C"]
-    out = np.zeros((len(rows), C))
-    ok = (rows >= P["r_lo"]) & (rows < P["r_hi"])
-    r = rows[ok]
-    idx = base + b * P["bstride"] + r[:, None] * P["rstride"] + np.arange(C)[None, :]
-    x = buf[idx]
-    if P["kind"] == 1:                                   # PLANE_MID
-        if P["mid_mode"] == 0:                           # MID_VALID: r + 1 always exists
-            nx = buf[idx + P["rstride"]]
-        else:
-            has_next = (r + 1 < P["xrows"])[:, None]
-            nxt = buf[np.where(has_next, idx + P["rstride"], idx)]
-            nx = np.where(has_next, nxt, x if P["mid_mode"] == 1 else 0.0)      # MID_CLAMP / MID_ZERO
-        if P["blend"] >= 0:
-            bname, boff = decode(P["blend"])
-            w = mem[bname][boff + np.arange(C)][None, :]
-            x = w * x + (1.0 - w) * nx
-        else:
-            x = x + (nx - x) * 0.5
-    out[ok] = x
-    return out
-
-
-def run_launch(mem, D):
-    """Execute one exported ConvLaunch on mem = {"ws", "par", "mix"} (float64 arrays); writes go to mem["ws"]."""
-    L, planes, classes, terms = D["launch"], D["planes"], D["cls"], D["terms"]
-    N, pairC = L["N"], L["pairC"]
-    wname, wbase = decode(L["W"])
-    W = mem[wname]
-    ws = mem["ws"]
-    for q in classes:
-        if q["m_hi"] <= q["m_lo"]:
-            continue
-        rows = np.arange(q["m_lo"], q["m_hi"])
-        for b in range(L["batch"]):
-            acc = np.zeros((len(rows), N))
-            for t in terms[q["term_begin"]:q["term_end"]]:
-                P = planes[t["plane"]]
-                X = plane_rows(mem, P, b, rows + t["d"])
-                Wt = np.zeros((P["C"], N))
-                c = np.arange(P["C"])[:, None]
-                if pairC == 0:
-                    Wt[:] = W[wbase + t["woff"] + c * L["w_sk"] + np.arange(N)[None, :] * L["w_sn"]]
-                else:
-                    n = np.arange(pairC)[None, :]
-                    if t["woff"] >= 0:
-                        Wt[:, :pairC] = W[wbase + t["woff"] + c * L["w_sk"] + n * L["w_sn"]]
-                    if t["woff2"] >= 0:
-                        Wt[:, pairC:] = W[wbase + t["woff2"] + c * L["w_sk"] + n * L["w_sn"]]
-                acc += X @ Wt
-            halves = [(0, N, q["base"], q["bstride"], q["rstride"], q["saved"], q["acc_lo"], q["acc_hi"], q["m_lo"], q["m_hi"])]
-            if pairC > 0:
-                assert q["pairC"] == pairC and N == 2 * pairC
-                halves = [(0, pairC, q["base"], q["bstride"], q["rstride"], q["saved"], q["acc_lo"], q["acc_hi"], q["lo0"], q["hi0"]),
-                          (pairC, N, q["base2"], q["bstride2"], q["rstride2"], q["saved2"], q["acc_lo2"], q["acc_hi2"], q["lo1"], q["hi1"])]
-            for (n0, n1, base, bstride, rstride, saved, acc_lo, acc_hi, lo, hi) in halves:
-                sel = (rows >= lo) & (rows < hi)
-                m = rows[sel]
-                v = acc[sel][:, n0:n1].copy()
-                _, dbase = decode(base)
-                didx = dbase + b * bstride + m[:, None] * rstride + np.arange(n1 - n0)[None, :]
-                if L["epilogue"] == 0:                                   # EPI_BIAS_LRELU
-                    if L["bias"] >= 0:
-                        bname, boff = decode(L["bias"])
-                        v += mem[bname][boff + np.arange(n1 - n0)][None, :]      # pair: the bias repeats per half
-                    v = np.maximum(0.2 * v, v)
-                elif L["epilogue"] == 1 and saved >= 0:                  # EPI_SLOPE
-                    sname, sbase = decode(saved)
-                    sidx = sbase + b * bstride + m[:, None] * rstride + np.arange(n1 - n0)[None, :]
-                    v *= np.where(mem[sname][sidx] > 0.0, 1.0, 0.2)
-                accum = ((m >= acc_lo) & (m < acc_hi))[:, None]
-                v = np.where(accum, v + ws[didx], v)
-                ws[didx] = v
-
 
 CASES = [
     ("context_stereo", ["baseline_stereo"], dict(num_layers=4), 2, 700),
@@ -359,20 +267,6 @@ def test_exported_dgrad_chain_reproduces_the_oracle(name, named, ov, batch, nf, 
             np.testing.assert_allclose(got / scale, want_full[:, rows, :] / scale, rtol=1e-8, atol=1e-10, err_msg="g_" + tname)
             checked += 1
     assert checked == 3 * L + 1
-
-
-def run_wgrad_group(mem, G, dW):
-    """One exported (class, plane) weight-gradient group (launch.h WgradLaunch; plane_wgrad_kernel, kernels_simt.cu):
-    dW[woff_t + c * w_sk + n * w_sn] += sum_{b, m in [m_lo, m_hi)} plane[b, m + d_t, c] * dpre[b, m, n]."""
-    g = G["wgrad"]
-    rows = np.arange(g["m_lo"], g["m_hi"])
-    C, N = G["plane"]["C"], g["N"]
-    c, n = np.arange(C)[:, None], np.arange(N)[None, :]
-    for b in range(g["batch"]):
-        Y = plane_rows(mem, G["dpre"], b, rows)[:, :N]
-        for t in G["terms"]:
-            X = plane_rows(mem, G["plane"], b, rows + t["d"])
-            dW[g["dW"] + t["woff"] + c * g["w_sk"] + n * g["w_sn"]] += X.T @ Y
 
 
 @pytest.mark.parametrize("name,named,ov,batch,nf", FWD_CASES, ids=[c[0] for c in FWD_CASES])

@@ -776,17 +776,12 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
                 uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum;
                 if (ahead && (h->wg_index & 1)) arena += split_arena_half_bytes(h, h->batch);
                 arena += (256 - (reinterpret_cast<uintptr_t>(arena) & 255)) & 255;
+                // split arrays, then the partial tiles, in this half; the class-gradient views among the jobs also produce the
+                // bias gradient (their column sums)
                 WgSplit S; SplitJobs J;
-                const size_t used = umma_plan_wgrad_split(U, h->batch, arena, &S, &J);
-                U.partial = reinterpret_cast<float*>(arena + (used + 255) / 256 * 256);     // behind the split arrays of the same half
-                // the class-gradient views among the jobs also produce the bias gradient (their column sums)
-                J.colsum_scale = scale;
-                size_t matched = 0;
-                for (int j = 0; j < J.njobs; ++j)
-                    for (const auto& dp : class_dpre)
-                        if (memcmp(&J.job[j].V, &dp, sizeof(PlaneView)) == 0) { J.job[j].colsum = bias_grad; ++matched; break; }
-                if (!fused_colsum) for (int j = 0; j < J.njobs; ++j) J.job[j].colsum = nullptr;
-                if (matched != class_dpre.size()) return set_err(WUN_E_INVALID, "wgrad split pass: class gradient view not among the split jobs");
+                if (!umma_wgrad_bulk_setup(&U, h->batch, arena, class_dpre.data(), (int)class_dpre.size(), fused_colsum ? bias_grad : nullptr,
+                                           scale, &S, &J))
+                    return set_err(WUN_E_INVALID, "wgrad split pass: class gradient view not among the split jobs");
                 if (ahead) {
                     const int k = h->wg_index++;
                     while ((int)h->split_done.size() <= k) {

@@ -502,8 +502,8 @@ static cudaError_t launch_conv_npad(const UmmaLaunch& L, dim3 grid, size_t smem,
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    // dgrad: batched read-back epilogue (separate instantiation)
-    if (L.epilogue == EPI_SLOPE) plane_conv_umma_kernel<NPAD, true><<<grid, kConvThreads, smem, stream>>>(L);
+    // dgrad (EPI_SLOPE / EPI_PLAIN): batched read-back epilogue with the accumulate ranges (separate instantiation)
+    if (L.epilogue != EPI_BIAS_LRELU) plane_conv_umma_kernel<NPAD, true><<<grid, kConvThreads, smem, stream>>>(L);
     else plane_conv_umma_kernel<NPAD, false><<<grid, kConvThreads, smem, stream>>>(L);
     return cudaGetLastError();
 }
@@ -995,6 +995,18 @@ size_t umma_plan_wgrad_split(const UmmaWgradLaunch& U, int batch, uint8_t* arena
 
 cudaError_t launch_wgrad_umma_bulk(const UmmaWgradLaunch& L, const WgSplit& S, cudaStream_t stream) {
     return launch_wgrad_any<true>(L, &S, stream);
+}
+
+bool umma_wgrad_bulk_setup(UmmaWgradLaunch* U, int batch, uint8_t* arena, const PlaneView* class_dpre, int ncls, float* db,
+                           float colsum_scale, WgSplit* S, SplitJobs* J) {
+    const size_t used = umma_plan_wgrad_split(*U, batch, arena, S, J);
+    U->partial = reinterpret_cast<float*>(arena + (used + 255) / 256 * 256);     // behind the split arrays
+    J->colsum_scale = colsum_scale;
+    int matched = 0;
+    for (int j = 0; j < J->njobs; ++j)
+        for (int q = 0; q < ncls; ++q)
+            if (memcmp(&J->job[j].V, &class_dpre[q], sizeof(PlaneView)) == 0) { J->job[j].colsum = db; ++matched; break; }
+    return matched == ncls;
 }
 
 size_t umma_wgrad_partial_bytes(const UmmaWgradLaunch& U) {

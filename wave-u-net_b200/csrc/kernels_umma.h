@@ -145,6 +145,12 @@ size_t umma_wgrad_partial_bytes(const UmmaWgradLaunch& U);
 // same bits on every run.
 cudaError_t launch_wgrad_reduce(const UmmaWgradLaunch& U, const SplitJobs& J, cudaStream_t stream);
 cudaError_t launch_wgrad_umma_bulk(const UmmaWgradLaunch& L, const WgSplit& S, cudaStream_t stream);
+// Everything a bulk-fed wgrad launch needs before the split pass / wgrad / reduce launches: the split arena at `arena` (256-B
+// aligned; umma_plan_wgrad_split(*U, batch, ...) bytes, rounded up to 256, then umma_wgrad_partial_bytes(*U)), U->partial behind
+// it, and the bias gradient `db` (scaled by colsum_scale) on the jobs that split one of the layer's class-gradient views
+// class_dpre[0..ncls) - `db` null: no fused column sums.  false: a class-gradient view is not among the split jobs.
+bool umma_wgrad_bulk_setup(UmmaWgradLaunch* U, int batch, uint8_t* arena, const PlaneView* class_dpre, int ncls, float* db,
+                           float colsum_scale, WgSplit* S, SplitJobs* J);
 // rows one wgrad CTA can read past the last valid row of a group: G side / P side (chunk rounding + tap span)
 constexpr int kWgOverreachG = 64, kWgOverreachP = 64 + 16;
 
