@@ -89,8 +89,10 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// After wgmma_wait_all(): the accumulator registers are only now final.  The empty asm "redefines" each of them, so that
+// waits until at most N committed MMA groups of this warpgroup are still running
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// After wgmma_wait<0>(): the accumulator registers are only now final.  The empty asm "redefines" each of them, so that
 // no read of an accumulator is scheduled above the wait.
 template <int N>
 __device__ __forceinline__ void acc_fence(float* d) {
@@ -98,47 +100,61 @@ __device__ __forceinline__ void acc_fence(float* d) {
     for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// One m64nNk16 MMA for every N the kernels use (16..128 in steps of 16), from one asm template: the N/2 accumulators are
+// read-write operands %0 .. %(N/2 - 1) (WUN_ACC<N> lists them, WUN_D<N> binds them) and the two descriptors are the input
+// operands that follow (WUN_DESC<N>).
 #define WUN_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
-// D[64 x N] += A[64 x 16] * B[16 x N], bf16 -> fp32; TA / TB = 1: that operand is MN-major
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n16(float* d, uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
-        : WUN_F8(0)
-        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n32(float* d, uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-        "%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
-        : WUN_F8(0), WUN_F8(8)
-        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n64(float* d, uint64_t da, uint64_t db) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, "
-        "%15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
-        : WUN_F8(0), WUN_F8(8), WUN_F8(16), WUN_F8(24)
-        : "l"(da), "l"(db), "r"(1), "n"(TA), "n"(TB));
-}
-#undef WUN_F8
+#define WUN_ACC16 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define WUN_ACC32 WUN_ACC16 ", %8, %9, %10, %11, %12, %13, %14, %15"
+#define WUN_ACC48 WUN_ACC32 ", %16, %17, %18, %19, %20, %21, %22, %23"
+#define WUN_ACC64 WUN_ACC48 ", %24, %25, %26, %27, %28, %29, %30, %31"
+#define WUN_ACC80 WUN_ACC64 ", %32, %33, %34, %35, %36, %37, %38, %39"
+#define WUN_ACC96 WUN_ACC80 ", %40, %41, %42, %43, %44, %45, %46, %47"
+#define WUN_ACC112 WUN_ACC96 ", %48, %49, %50, %51, %52, %53, %54, %55"
+#define WUN_ACC128 WUN_ACC112 ", %56, %57, %58, %59, %60, %61, %62, %63"
+#define WUN_D16 WUN_F8(0)
+#define WUN_D32 WUN_D16, WUN_F8(8)
+#define WUN_D48 WUN_D32, WUN_F8(16)
+#define WUN_D64 WUN_D48, WUN_F8(24)
+#define WUN_D80 WUN_D64, WUN_F8(32)
+#define WUN_D96 WUN_D80, WUN_F8(40)
+#define WUN_D112 WUN_D96, WUN_F8(48)
+#define WUN_D128 WUN_D112, WUN_F8(56)
+#define WUN_DESC16 "%8, %9"
+#define WUN_DESC32 "%16, %17"
+#define WUN_DESC48 "%24, %25"
+#define WUN_DESC64 "%32, %33"
+#define WUN_DESC80 "%40, %41"
+#define WUN_DESC96 "%48, %49"
+#define WUN_DESC112 "%56, %57"
+#define WUN_DESC128 "%64, %65"
+#define WUN_WGMMA(N, T)                                                                                                     \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"                                                           \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 {" WUN_ACC##N "}, " WUN_DESC##N ", p, 1, 1, " T ", " T ";\n\t}" \
+                 : WUN_D##N                                                                                             \
+                 : "l"(da), "l"(db))
+#define WUN_WGMMA_ANY_N(T)                                                                                                  \
+    if constexpr (N == 16) WUN_WGMMA(16, T);                                                                                \
+    else if constexpr (N == 32) WUN_WGMMA(32, T);                                                                           \
+    else if constexpr (N == 48) WUN_WGMMA(48, T);                                                                           \
+    else if constexpr (N == 64) WUN_WGMMA(64, T);                                                                           \
+    else if constexpr (N == 80) WUN_WGMMA(80, T);                                                                           \
+    else if constexpr (N == 96) WUN_WGMMA(96, T);                                                                           \
+    else if constexpr (N == 112) WUN_WGMMA(112, T);                                                                         \
+    else WUN_WGMMA(128, T);
 
-// D[64 x N] += A * B for N = 64a + 32b + 16c columns, issued as n64 / n32 / n16 MMAs over consecutive column ranges;
-// b8 = descriptor units (16 B) between consecutive 8-column groups of B.  Accumulator register i of a thread holds
-// column (i/4)*8 + (lane%4)*2 + i%2 and row 16*(warp%4) + lane/4 + 8*((i/2)%2) of the warpgroup's 64 x N tile.
-template <int N, int TA, int TB>
-__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, uint32_t b8) {
-#pragma unroll
-    for (int i = 0; i < N / 64; ++i) wgmma_n64<TA, TB>(d + 32 * i, da, db + (uint64_t)(8u * b8 * i));
-    constexpr int o32 = N / 64 * 64, o16 = o32 + (N % 64) / 32 * 32;
-    if constexpr ((N % 64) >= 32) wgmma_n32<TA, TB>(d + o32 / 2, da, db + (uint64_t)(o32 / 8 * b8));
-    if constexpr ((N % 32) == 16) wgmma_n16<TA, TB>(d + o16 / 2, da, db + (uint64_t)(o16 / 8 * b8));
+// D[64 x N] += A[64 x 16] * B[16 x N], bf16 -> fp32, as ONE wgmma (A is read from shared memory once per k16 step).  MN = 1:
+// both operands are MN-major, else both K-major.  Accumulator register i of a thread holds column (i/4)*8 + (lane%4)*2 + i%2 and
+// row 16*(warp%4) + lane/4 + 8*((i/2)%2) of the warpgroup's 64 x N tile.
+template <int N, int MN>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db) {
+    static_assert(N % 16 == 0 && N >= 16 && N <= 128, "m64nNk16: N = 16..128 in steps of 16");
+    if constexpr (MN) { WUN_WGMMA_ANY_N("1") }
+    else { WUN_WGMMA_ANY_N("0") }
 }
+#undef WUN_WGMMA_ANY_N
+#undef WUN_WGMMA
+#undef WUN_F8
 __device__ __forceinline__ int acc_col(int i, int lane) { return (i >> 2) * 8 + (lane & 3) * 2 + (i & 1); }
 __device__ __forceinline__ int acc_row(int i, int warp, int lane) { return 16 * (warp & 3) + (lane >> 2) + 8 * ((i >> 1) & 1); }
 
@@ -362,7 +378,9 @@ static __host__ __device__ size_t conv_smem_bytes(int NPAD, int rows_alloc, int 
 template <int NPAD, bool DG>
 __global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const __grid_constant__ UmmaLaunch L) {
     extern __shared__ __align__(128) uint8_t smem[];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // warp-uniform for the compiler: an MMA operand it thinks may diverge makes it serialize the MMAs
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
     const int cls = blockIdx.z % L.ncls, b = blockIdx.z / L.ncls;
     const UmmaClass& K = L.cls[cls];
     const int split = blockIdx.y;
@@ -422,9 +440,9 @@ __global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const 
             const uint32_t bb = sb + tt * blk_bytes;
             const uint64_t a_hi = gmma_desc(a, atom, 128), a_lo = gmma_desc(a + 2 * atom, atom, 128);
             const uint64_t b_hi = gmma_desc(bb, 32u * NPAD, 128), b_lo = gmma_desc(bb + 16u * NPAD, 32u * NPAD, 128);
-            wgmma_tile<NPAD, 0, 0>(acc, a_lo, b_hi, 8);
-            wgmma_tile<NPAD, 0, 0>(acc, a_hi, b_lo, 8);
-            wgmma_tile<NPAD, 0, 0>(acc, a_hi, b_hi, 8);
+            wgmma_tile<NPAD, 0>(acc, a_lo, b_hi);
+            wgmma_tile<NPAD, 0>(acc, a_hi, b_lo);
+            wgmma_tile<NPAD, 0>(acc, a_hi, b_hi);
         }
         wgmma_commit();
         ConvStep nx = cur;
@@ -432,7 +450,7 @@ __global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const 
         const bool new_slab = more && nx.t0 == 0;
         // convert the next (group, chunk) into the other slab while the MMAs run; its last reader was the previous job
         if (new_slab) fill_slab(L, K.groups[nx.g], b, m_base, nx.c, smem + (slab ^ 1) * slab_bytes);
-        wgmma_wait_all();
+        wgmma_wait<0>();
         acc_fence<NPAD / 2>(acc);
         fence_proxy_async();
         __syncthreads();
@@ -696,17 +714,19 @@ __device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSpl
                     const uint32_t a = sa + sha + 256u * ks, bb = sb + shb + 256u * ks;
                     const uint64_t a_hi = gmma_desc(a, 128, planeA), a_lo = gmma_desc(a + atomsA * planeA, 128, planeA);
                     const uint64_t b_hi = gmma_desc(bb, 128, planeB), b_lo = gmma_desc(bb + atomsB * planeB, 128, planeB);
-                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_lo, b_hi, planeB >> 4);
-                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_hi, b_lo, planeB >> 4);
-                    wgmma_tile<NT, 1, 1>(acc + t * (NT / 2), a_hi, b_hi, planeB >> 4);
+                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_lo, b_hi);
+                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_lo);
+                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_hi);
                 }
             }
         }
         wgmma_commit();
-        wgmma_wait_all();
-        acc_fence<NACC>(acc);
-        mbar_arrive(BAR(EMPTY + st));
+        // chunk ci stays in flight while the next stage is awaited: only chunk ci - 1 has surely finished reading its stage
+        wgmma_wait<1>();
+        if (ci > 0) mbar_arrive(BAR(EMPTY + (ci - 1) % nst));
     }
+    wgmma_wait<0>();
+    acc_fence<NACC>(acc);
     // ===================== epilogue: accumulators -> partial tile (or reductions into dW) =====================
     if (L.partial) {
         const int tiles = Gp.n_mtiles * Gp.n_ntiles;
