@@ -79,6 +79,16 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                  ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
+// mbar_arrive_expect_tx + bulk_g2s of `bytes`, issued by the thread with tid == 0 only.  The predicate lives inside the asm, so
+// the code has no branch on the thread index: between MMAs still in flight and the next ones, such a branch makes ptxas
+// serialise the MMAs (C7520).
+__device__ __forceinline__ void bulk_g2s_thread0(uint32_t tid, uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, %0, 0;\n\t"
+                 "@p mbarrier.arrive.expect_tx.shared::cta.b64 _, [%1], %2;\n\t"
+                 "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%3], [%4], %2, [%1];\n\t}"
+                 ::"r"(tid), "r"(bar), "r"(bytes), "r"(dst), "l"(src)
+                 : "memory");
+}
 
 // No-swizzle shared-memory matrix descriptor of wgmma: start address, leading / stride byte offsets (all >> 4).
 //   K-major operand:  LBO = bytes between the two 8-element K groups of a k16 step, SBO = bytes between 8-row M/N groups.
@@ -175,6 +185,17 @@ __device__ __forceinline__ void split_hi_lo(const float* x, uint32_t* hi, uint32
 // ------------------------------------------------------------------------------------------------
 // slab fill helpers
 // ------------------------------------------------------------------------------------------------
+// Interpolated row of a MID plane from row x and its successor nx (channels [c0, c0 + nv)): learned or linear upsampling.
+__device__ __forceinline__ void mid_blend(const PlaneView& P, int c0, int nv, float* x, const float* nx) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        if (i < nv) {
+            if (P.blend) { const float w = __ldg(P.blend + c0 + i); x[i] = w * x[i] + (1.f - w) * nx[i]; }
+            else x[i] = x[i] + (nx[i] - x[i]) * 0.5f;
+        }
+    }
+}
+
 // 16 channels [c0, c0+16) of plane row r of batch b, fp32, zero where invalid.
 __device__ __forceinline__ void load_row16(const PlaneView& P, int b, int r, int c0, float* x) {
 #pragma unroll
@@ -204,13 +225,7 @@ __device__ __forceinline__ void load_row16(const PlaneView& P, int b, int r, int
 #pragma unroll
             for (int i = 0; i < 16; ++i) nx[i] = x[i];
         }
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-            if (i < nv) {
-                if (P.blend) { const float w = __ldg(P.blend + c0 + i); x[i] = w * x[i] + (1.f - w) * nx[i]; }
-                else x[i] = x[i] + (nx[i] - x[i]) * 0.5f;
-            }
-        }
+        mid_blend(P, c0, nv, x, nx);
     }
 }
 
@@ -351,20 +366,91 @@ __device__ __forceinline__ bool next_step(const UmmaLaunch& L, const UmmaClass& 
     return false;
 }
 
-// slab of (group, chunk): rows m_base + dmin + [0, rows_alloc) of the plane, 16 channels, as hi / lo atom planes
-__device__ __forceinline__ void fill_slab(const UmmaLaunch& L, const UmmaGroup& G, int b, int m_base, int c, uint8_t* S) {
-    const PlaneView& P = L.planes[G.plane];
-    const uint32_t atom = 16u * L.rows_alloc;
-    for (int rr = threadIdx.x; rr < L.rows_alloc; rr += kConvThreads) {
-        float x[16];
-        uint32_t hi[8], lo[8];
-        load_row16(P, b, m_base + G.dmin + rr, c * 16, x);
-        split_hi_lo(x, hi, lo);
-        *reinterpret_cast<uint4*>(S + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(S + atom + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-        *reinterpret_cast<uint4*>(S + 2 * atom + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        *reinterpret_cast<uint4*>(S + 3 * atom + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+// Moves s from any step of its (group, chunk) to the first step of the next non-empty (group, chunk).  false = none left.
+__device__ __forceinline__ bool next_chunk(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
+    const UmmaGroup& G = K.groups[s.g];
+    s.nt = (G.term_end - G.term_begin) - s.t0;      // as if this step ran to the chunk's last tap
+    return next_step(L, K, m_base, s);
+}
+
+// The slab of (group, chunk) holds plane rows m_base + dmin + [0, rows_alloc), 16 channels, as hi / lo atom planes.  Each thread
+// owns one slab row (rows_alloc <= 152 < kConvThreads; threads past the slab redo its last row: the same bits to the same
+// address), and nothing branches on the thread index: a row outside the plane's valid rows has its loads predicated off and is
+// zeroed by a select.  slab_load only issues the global loads and slab_store converts and stores them, so that a step can keep
+// the next chunk's loads in flight while it waits for its previous step's MMAs.
+struct SlabRow {
+    float x[16], nx[16];       // the row, and (MID planes) its successor
+    bool valid, has_next;
+};
+// 4 floats at q if ld, else zeros: a predicated load (no branch; rows outside the plane cost no memory traffic)
+__device__ __forceinline__ void ldg4_if(bool ld, const float* q, float* x) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %5, 0;\n\t"
+                 "mov.b32 %0, 0;\n\tmov.b32 %1, 0;\n\tmov.b32 %2, 0;\n\tmov.b32 %3, 0;\n\t"
+                 "@p ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];\n\t}"
+                 : "=f"(x[0]), "=f"(x[1]), "=f"(x[2]), "=f"(x[3])
+                 : "l"(q), "r"((int)ld));
+}
+__device__ __forceinline__ void load16(bool ld, const float* p, int nv, float* x) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        if (i < 2 || nv >= 16) ldg4_if(ld, p + 4 * i, x + 4 * i);
+        else { x[4 * i] = 0.f; x[4 * i + 1] = 0.f; x[4 * i + 2] = 0.f; x[4 * i + 3] = 0.f; }
     }
+}
+__device__ __forceinline__ void slab_load(const PlaneView& P, int b, int r, int c0, SlabRow& R) {
+    const int nv = min(16, P.C - c0);      // 8 or 16 (eligibility: C % 8 == 0)
+    R.valid = r >= P.r_lo && r < P.r_hi;
+    const int rc = min(max(r, P.r_lo), P.r_hi - 1);      // a group's slab has a valid row (group_is_empty)
+    const float* p = P.base + (long long)b * P.bstride + (long long)rc * P.rstride + c0;
+    load16(R.valid, p, nv, R.x);
+    if (P.kind == PLANE_MID) {
+        R.has_next = (P.mid_mode == MID_VALID) || (rc + 1 < P.xrows);
+        load16(R.valid && R.has_next, p + P.rstride, nv, R.nx);
+    }
+}
+__device__ __forceinline__ void slab_store(const PlaneView& P, int c0, SlabRow& R, uint8_t* S, uint32_t atom, int rr) {
+    const int nv = min(16, P.C - c0);
+    if (P.kind == PLANE_MID) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) R.nx[i] = R.has_next ? R.nx[i] : (P.mid_mode == MID_CLAMP ? R.x[i] : 0.f);
+        mid_blend(P, c0, nv, R.x, R.nx);
+    }
+    uint32_t hi[8], lo[8];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) R.x[i] = R.valid ? R.x[i] : 0.f;
+    split_hi_lo(R.x, hi, lo);
+    *reinterpret_cast<uint4*>(S + 16u * rr) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    *reinterpret_cast<uint4*>(S + atom + 16u * rr) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
+    *reinterpret_cast<uint4*>(S + 2 * atom + 16u * rr) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    *reinterpret_cast<uint4*>(S + 3 * atom + 16u * rr) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
+}
+
+// Taps per weight-ring stage: ~16 KB of packed weights, 1..4 taps.  A function of NPAD alone, so that the kernel's tap loop has a
+// trip count fixed at compile time; the planner reports the same value.
+constexpr __host__ __device__ int conv_stage_taps(int NPAD) {
+    return 16384 / (64 * NPAD) > 4 ? 4 : (16384 / (64 * NPAD) < 1 ? 1 : 16384 / (64 * NPAD));
+}
+
+// The MMAs of one K step, nt taps (1 <= nt <= NT) with row shifts d[0 .. nt), committed as one group.  Every tap count gets its
+// own straight-line sequence: ptxas closes an MMA group at the end of every basic block that issues MMAs, so taps behind a
+// per-tap `if` would each be a group, and wait_group 1 after the step would then retire all but the last of them.
+template <int NPAD, int NT>
+__device__ __forceinline__ void conv_step_mmas(int nt, float* acc, uint32_t sa, uint32_t sb, uint32_t atom, const int* d, int dmin) {
+    if constexpr (NT > 1) {
+        if (nt < NT) { conv_step_mmas<NPAD, NT - 1>(nt, acc, sa, sb, atom, d, dmin); return; }
+    }
+    constexpr uint32_t blk_bytes = 64u * NPAD;
+#pragma unroll
+    for (int tt = 0; tt < NT; ++tt) {
+        const uint32_t a = sa + 16u * (uint32_t)(d[tt] - dmin);
+        const uint32_t bb = sb + tt * blk_bytes;
+        const uint64_t a_hi = gmma_desc(a, atom, 128), a_lo = gmma_desc(a + 2 * atom, atom, 128);
+        const uint64_t b_hi = gmma_desc(bb, 32u * NPAD, 128), b_lo = gmma_desc(bb + 16u * NPAD, 32u * NPAD, 128);
+        wgmma_tile<NPAD, 0>(acc, a_lo, b_hi);
+        wgmma_tile<NPAD, 0>(acc, a_hi, b_lo);
+        wgmma_tile<NPAD, 0>(acc, a_hi, b_hi);
+    }
+    wgmma_commit();
 }
 
 static __host__ __device__ size_t conv_smem_bytes(int NPAD, int rows_alloc, int TB, int nbs) {
@@ -390,7 +476,8 @@ __global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const 
     const uint32_t atom = 16u * L.rows_alloc;
     const uint32_t slab_bytes = 4u * atom;
     constexpr uint32_t blk_bytes = 64u * NPAD;               // [hi a0|hi a1|lo a0|lo a1] x NPAD rows x 16 B ... see umma_pack_kernel
-    const uint32_t stage_bytes = blk_bytes * L.TB;
+    constexpr int TB = conv_stage_taps(NPAD);                // == L.TB (launch_plane_conv_umma checks)
+    constexpr uint32_t stage_bytes = blk_bytes * TB;
     uint8_t* ring = smem + 2 * slab_bytes;
     const size_t pipe = 2 * (size_t)slab_bytes + (size_t)L.nbs * stage_bytes, epi = 128u * (NPAD + 4) * 4u;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ((pipe > epi ? pipe : epi) + 127) / 128 * 128);
@@ -406,57 +493,71 @@ __global__ void __launch_bounds__(kConvThreads, 2) plane_conv_umma_kernel(const 
     }
     __syncthreads();
 
+    // Everything the K loop branches on (cur, ld, the fill target) depends only on L, blockIdx and the step counter.
     const uint8_t* wsrc = K.wpack[split];
-    auto load_weights = [&](int stage, const ConvStep& s) {
-        const uint32_t bar = bar0 + 8u * stage;
-        mbar_arrive_expect_tx(bar, blk_bytes * s.nt);
-        bulk_g2s(smem_u32(ring + stage * stage_bytes), wsrc + (size_t)s.blk * blk_bytes, blk_bytes * s.nt, bar);
-    };
     ConvStep cur = {-1, 0, 0, 0, 0};
     bool more = next_step(L, K, m_base, cur);
-    ConvStep ld = cur;                  // thread 0: the next step whose weights are still to be loaded
+    ConvStep ld = cur;                  // the next step whose weights are still to be loaded
     bool ld_more = more;
-    if (tid == 0)
-        for (int i = 0; i < L.nbs - 1 && ld_more; ++i) { load_weights(i, ld); ld_more = next_step(L, K, m_base, ld); }
-    if (more) fill_slab(L, K.groups[cur.g], b, m_base, cur.c, smem);
+    for (int i = 0; i < L.nbs && ld_more; ++i) {
+        bulk_g2s_thread0(tid, smem_u32(ring + i * stage_bytes), wsrc + (size_t)ld.blk * blk_bytes, blk_bytes * ld.nt, bar0 + 8u * i);
+        ld_more = next_step(L, K, m_base, ld);
+    }
+    const int row = min(tid, L.rows_alloc - 1);       // this thread's slab row
+    SlabRow R;
+    if (more) {
+        const UmmaGroup& G = K.groups[cur.g];
+        slab_load(L.planes[G.plane], b, m_base + G.dmin + row, cur.c * 16, R);
+        slab_store(L.planes[G.plane], cur.c * 16, R, smem, atom, row);
+    }
     fence_proxy_async();                // generic-proxy slab writes -> visible to the tensor core (async proxy)
     __syncthreads();
 
+    // Step s = one ring stage: TB taps (fewer at the end of a group) of one chunk, 3 MMAs per tap.  The MMAs of step s stay in
+    // flight until step s + 1 has issued its own: wait_group 1 retires step s - 1 only, and after the block barrier that follows
+    // it, step s - 1's ring stage takes the weights of step s - 1 + nbs.  The first step of a chunk issues the loads of the
+    // next chunk's slab rows before that wait and converts them into the other slab after the barrier, once the previous
+    // chunk's last step (its last reader) has retired in both warpgroups.
     float acc[NPAD / 2];
 #pragma unroll
     for (int i = 0; i < NPAD / 2; ++i) acc[i] = 0.f;
-    int slab = 0;
+    int slab = 0, st = 0, phase = 0, st_prev = -1;     // ring stage of step s, its mbarrier phase, the stage of step s - 1
     for (int s = 0; more; ++s) {
-        // the ring stage of step s + nbs - 1 was last read by step s - 1, whose MMAs every thread has waited for
-        if (tid == 0 && ld_more) { load_weights((s + L.nbs - 1) % L.nbs, ld); ld_more = next_step(L, K, m_base, ld); }
-        const int st = s % L.nbs;
-        mbar_wait(bar0 + 8u * st, (s / L.nbs) & 1);
+        mbar_wait(bar0 + 8u * st, phase);
         const UmmaGroup& G = K.groups[cur.g];
         const uint32_t sa = smem_u32(smem + slab * slab_bytes) + 64u * 16u * wg;
         const uint32_t sb = smem_u32(ring + st * stage_bytes);
         wgmma_fence();
-        for (int tt = 0; tt < cur.nt; ++tt) {
-            const uint32_t a = sa + 16u * (uint32_t)(L.d[G.term_begin + cur.t0 + tt] - G.dmin);
-            const uint32_t bb = sb + tt * blk_bytes;
-            const uint64_t a_hi = gmma_desc(a, atom, 128), a_lo = gmma_desc(a + 2 * atom, atom, 128);
-            const uint64_t b_hi = gmma_desc(bb, 32u * NPAD, 128), b_lo = gmma_desc(bb + 16u * NPAD, 32u * NPAD, 128);
-            wgmma_tile<NPAD, 0>(acc, a_lo, b_hi);
-            wgmma_tile<NPAD, 0>(acc, a_hi, b_lo);
-            wgmma_tile<NPAD, 0>(acc, a_hi, b_hi);
-        }
-        wgmma_commit();
+        conv_step_mmas<NPAD, TB>(cur.nt, acc, sa, sb, atom, L.d + G.term_begin + cur.t0, G.dmin);
+        ConvStep fc = cur;              // the chunk whose slab this step fills
+        const bool fill = cur.t0 == 0 && next_chunk(L, K, m_base, fc);
+        const PlaneView& FP = L.planes[K.groups[fc.g].plane];
+        if (fill) slab_load(FP, b, m_base + K.groups[fc.g].dmin + row, fc.c * 16, R);
+        // the bookkeeping of this step runs while the MMAs do
         ConvStep nx = cur;
         more = next_step(L, K, m_base, nx);
         const bool new_slab = more && nx.t0 == 0;
-        // convert the next (group, chunk) into the other slab while the MMAs run; its last reader was the previous job
-        if (new_slab) fill_slab(L, K.groups[nx.g], b, m_base, nx.c, smem + (slab ^ 1) * slab_bytes);
-        wgmma_wait<0>();
-        acc_fence<NPAD / 2>(acc);
-        fence_proxy_async();
+        const bool refill = st_prev >= 0 && ld_more;
+        const ConvStep lw = ld;
+        if (refill) ld_more = next_step(L, K, m_base, ld);
+        wgmma_wait<1>();
         __syncthreads();
+        if (refill)
+            bulk_g2s_thread0(tid, smem_u32(ring + st_prev * stage_bytes), wsrc + (size_t)lw.blk * blk_bytes, blk_bytes * lw.nt,
+                             bar0 + 8u * st_prev);
+        st_prev = st;
+        if (++st == L.nbs) { st = 0; phase ^= 1; }
+        if (fill) {
+            slab_store(FP, fc.c * 16, R, smem + (slab ^ 1) * slab_bytes, atom, row);
+            fence_proxy_async();
+            if (new_slab) __syncthreads();      // read by the very next step (otherwise the next step's barrier orders it)
+        }
         if (new_slab) slab ^= 1;
         cur = nx;
     }
+    wgmma_wait<0>();
+    acc_fence<NPAD / 2>(acc);
+    __syncthreads();
 
     // ===================== epilogue =====================
     // every MMA has retired and every weight copy has landed: the pipeline memory becomes the staging tile
@@ -532,7 +633,8 @@ cudaError_t launch_plane_conv_umma(const UmmaLaunch& L, cudaStream_t stream, con
     for (int q = 0; q < L.ncls; ++q) max_tiles = max(max_tiles, (L.cls[q].out.m_hi - L.cls[q].out.m_lo + 127) / 128);
     if (max_tiles <= 0) return cudaSuccess;
     const size_t smem = umma_smem_bytes(L);
-    if (smem > (size_t)kConvSmemMax || L.nbs < 2 || L.nbs > kBStagesMax || L.MT != 1) return cudaErrorInvalidValue;
+    if (smem > (size_t)kConvSmemMax || L.nbs < 2 || L.nbs > kBStagesMax || L.MT != 1 || L.TB != conv_stage_taps(L.NPAD))
+        return cudaErrorInvalidValue;
     const dim3 grid(max_tiles, L.nsplit, L.batch * L.ncls);
     switch (L.NPAD) {
         case 16: return launch_conv_npad<16>(L, grid, smem, stream);
@@ -1217,7 +1319,7 @@ bool umma_plan_from_conv(const ConvLaunch& L, UmmaChoice* ch) {
     // weight ring: stages of TB taps (~16 KB) and ~64 KB in all, so that two CTAs share an SM (one hides the other's epilogue
     // and slab conversion)
     const int blk = 64 * ch->NPAD;
-    ch->TB = min(4, max(1, 16384 / blk));
+    ch->TB = conv_stage_taps(ch->NPAD);
     ch->nbs = min(kBStagesMax, max(2, 65536 / (ch->TB * blk)));
     return true;
 }
