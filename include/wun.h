@@ -171,6 +171,25 @@ int wun_feed_batch(WunHandle* h, const float* pool, int64_t total_frames, const 
                    const int64_t* track_length, int64_t n_tracks, int64_t batch, int augmentation, uint64_t seed,
                    int64_t* step_state, float* mix_out, float* targets_out, int64_t* chosen, void* stream);
 
+/* --- separation scoring (no handle) -------------------------------------------------------------
+ * BSS Eval v4 as museval 0.2.0 evaluate(references, estimates, win, hop, mode="v4") computes it - the "images"
+ * decomposition with 512-tap distortion filters solved once over the whole track and applied frame by frame - in float64.
+ * Replaces the museval.eval_mus_track call at the reference's Evaluate.py:71.
+ *   references, estimates  DEVICE float32 [nsrc][nsampl][nchan] (estimate k is scored against reference k; pad or truncate
+ *                          the estimates to nsampl first)
+ *   metrics   DEVICE float64 [4][nsrc][nwin]: SDR, ISR, SIR, SAR per frame, nwin = floor((nsampl - win + hop) / hop) >= 0;
+ *             NaN for frames where some reference or estimate is silent, +inf for a zero denominator
+ *   filters   optional DEVICE float64: the filters for all sources, C[j][e][k][c][l] (target j, estimate channel e, reference
+ *             source k and channel c, tap l < 512), then those for source j alone, Cj[j][e][c][l]; NULL skips the copy
+ * 1 <= nsrc <= WUN_MAX_SOURCES, nchan 1 or 2, nsampl, win, hop >= 1, workspace 256-byte aligned and at least
+ * wun_bss_eval_workspace_bytes(...) bytes; otherwise WUN_E_INVALID (and wun_bss_eval_workspace_bytes returns WUN_E_INVALID).
+ * Enqueued on `stream`; no allocation, no synchronisation.  The same inputs give the same bits on every call.  These two
+ * functions do not set wun_last_error(): the return code is the whole report. */
+int64_t wun_bss_eval_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop);
+int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                 int64_t win, int64_t hop, double* metrics, double* filters, void* workspace, int64_t workspace_bytes,
+                 void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

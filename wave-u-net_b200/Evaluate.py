@@ -8,9 +8,14 @@ predict_track() keeps the semantics of /root/reference/Evaluate.py:82-145 exactl
 through the network as batches, and scattered back on the device; with torch.distributed initialised the window list
 is split over the ranks (no collective on the data path, results all-gathered at the end).
 
-Audio file I/O, resampling and museval scoring of the reference (librosa / musdb / museval, Evaluate.py:16-80,147-231)
-are out of scope (SURVEY section 2): predict_track works on arrays already at model_config["expected_sr"].
+Audio file I/O, resampling and musdb loading of the reference (librosa / musdb, Evaluate.py:16-80,147-193) are out of
+scope (SURVEY section 2): predict_track works on arrays already at model_config["expected_sr"].  Scoring is here:
+evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS Eval v4 on the GPU
+(wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).
 """
+import glob
+import json
+import os
 from collections import OrderedDict
 
 import numpy as np
@@ -90,3 +95,88 @@ def produce_source_estimates(model_config, load_model, mix_audio, separator=None
             import TFCheckpoint
             TFCheckpoint.restore_separator(load_model, separator, int(in_shape[1]), with_optimizer=False)
     return predict_track(model_config, separator, mix_audio)
+
+
+def _device_bss_eval(references, estimates, win, hop):
+    """[nsrc, N, nchan] float arrays -> numpy float64 [4 (SDR, ISR, SIR, SAR), nsrc, nwin] from wun.bss_eval."""
+    import torch
+    import wun
+    ref = torch.from_numpy(np.ascontiguousarray(references, dtype=np.float32)).cuda()
+    est = torch.from_numpy(np.ascontiguousarray(estimates, dtype=np.float32)).cuda()
+    return torch.stack(wun.bss_eval(ref, est, win, hop)).cpu().numpy()
+
+
+def _pad_or_truncate(estimates, n):
+    if estimates.shape[1] >= n:
+        return estimates[:, :n]
+    return np.pad(estimates, ((0, 0), (0, n - estimates.shape[1]), (0, 0)))
+
+
+def evaluate(references, estimates, win=44100, hop=44100):
+    """museval.evaluate(references, estimates, win, hop, mode="v4", padding=True): arrays [nsrc, n_samples, nchan];
+    estimates are cut or zero-extended to the references' length.  Returns SDR, ISR, SIR, SAR, each [nsrc, nwin]."""
+    references = np.asarray(references)
+    estimates = _pad_or_truncate(np.asarray(estimates), references.shape[1])
+    sdr, isr, sir, sar = _device_bss_eval(references, estimates, int(win), int(hop))
+    return sdr, isr, sir, sar
+
+
+def eval_track(references, estimates, rate, output_dir=None, track_name=None):
+    """museval.eval_mus_track with arrays: `references` and `estimates` map source names to [n_samples, nchan] arrays;
+    the references' order plays the role of track.targets, and only names present in both are scored.  When vocals and
+    accompaniment are both present, accompaniment leaves the list and the pair is scored as its own 2-source problem,
+    reported last; the remaining targets (vocals included) are scored together if there are at least two of them, and
+    all but vocals are reported from that problem.  Frames are one second at `rate` (win = hop).  Returns
+    {"targets": [...]} in museval's JSON layout (NaN for silent frames) and writes it to <output_dir>/<track_name>.json
+    when output_dir is given."""
+    win = hop = int(rate)
+    names = [n for n in references if n in estimates]
+    has_acc = "vocals" in names and "accompaniment" in names
+    scenarios = []                  # (scored together, reported)
+    rest = [n for n in names if not (has_acc and n == "accompaniment")]
+    if len(rest) >= 2:
+        scenarios.append((rest, [n for n in rest if not (has_acc and n == "vocals")]))
+    if has_acc:
+        scenarios.append((["vocals", "accompaniment"], ["vocals", "accompaniment"]))
+    targets = []
+    for group, report in scenarios:
+        ref = np.stack([np.asarray(references[n]) for n in group])
+        est = np.stack([_pad_or_truncate(np.asarray(estimates[n])[None], ref.shape[1])[0] for n in group])
+        sdr, isr, sir, sar = evaluate(ref, est, win, hop)
+        for k, name in enumerate(group):
+            if name not in report:
+                continue
+            frames = [{"time": float(t * hop) / rate, "duration": float(win) / rate,
+                       "metrics": {"SDR": float(sdr[k, t]), "SIR": float(sir[k, t]), "SAR": float(sar[k, t]),
+                                   "ISR": float(isr[k, t])}}
+                      for t in range(sdr.shape[1])]
+            targets.append({"name": name, "frames": frames})
+    scores = {"targets": targets}
+    if output_dir is not None:
+        os.makedirs(output_dir, exist_ok=True)
+        with open(os.path.join(output_dir, "%s.json" % (track_name or "track")), "w") as f:
+            json.dump(scores, f, indent=2, allow_nan=True)
+    return scores
+
+
+def compute_mean_metrics(json_folder, compute_averages=True, metric="SDR"):
+    """The reference's compute_mean_metrics (Evaluate.py:195-232): per target, (median, MAD, mean, SD) of `metric` over
+    every frame of every <track>.json in json_folder, ignoring NaN; with compute_averages=False the frame values."""
+    files = glob.glob(os.path.join(json_folder, "*.json"))
+    inst_list = None
+    print("Found " + str(len(files)) + " JSON files to evaluate...")
+    for path in files:
+        if "test.json" in path:
+            print("Found test JSON, skipping...")
+            continue
+        with open(path, "r") as f:
+            js = json.load(f)
+        if inst_list is None:
+            inst_list = [list() for _ in range(len(js["targets"]))]
+        for i in range(len(js["targets"])):
+            inst_list[i].extend([float(f["metrics"][metric]) for f in js["targets"][i]["frames"]])
+    inst_list = [np.array(perf) for perf in inst_list]
+    if compute_averages:
+        return [(np.nanmedian(perf), np.nanmedian(np.abs(perf - np.nanmedian(perf))), np.nanmean(perf), np.nanstd(perf))
+                for perf in inst_list]
+    return inst_list

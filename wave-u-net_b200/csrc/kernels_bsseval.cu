@@ -1,0 +1,509 @@
+// BSS Eval v4 ("images" decomposition, filters solved once over the whole track, applied frame by frame) in fp64:
+// museval 0.2.0 evaluate(references, estimates, win, hop, mode="v4"), which the reference calls through
+// museval.eval_mus_track (Evaluate.py:71).  DESIGN.md §4.5 describes the stages; oracle/bsseval_oracle.py restates them
+// in numpy.
+//
+// Every sum runs in a fixed order (per-CTA partial slots, then an ordered second pass; no float atomics), so a call
+// returns the same bits on every run.  fp32 inputs are widened to fp64 when staged: each product of two of them is exact.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "../../include/wun.h"
+
+namespace {
+
+constexpr int kL = 512;              // museval filters_len
+constexpr int kR = 8;                // outputs (lags or samples) per thread, kept in registers
+constexpr int kXcThreads = kL / kR;  // one CTA covers all L lags of a signal pair
+constexpr int kXcChunk = 1024;       // samples staged per step
+constexpr int kMaxSegs = 256;        // sample segments of the correlation (partial slots per lag)
+constexpr int kPanel = 64;           // LDL^T panel width
+constexpr int kFrThreads = 128;
+constexpr int kFrTile = kFrThreads * kR;  // output samples per framewise CTA
+constexpr int kEnergies = 7;
+
+__host__ __device__ constexpr int skew(int i) { return i + (i >> 4); }  // one pad double per 16: stride-8 reads hit distinct banks
+
+// ---- stage 1: lag correlations corr(x, y, tau) = sum_m x[m] y[m + tau], tau in [0, L) ----------------------------------------
+// Task t = a * 2nref + s pairs reference signal a = (k, c) with signal s: references 0..nref-1, then estimates.  G needs
+// every ordered reference pair (corr(a, b, -tau) = corr(b, a, tau)), D every (reference, estimate) pair.  CTA (seg, t) sums
+// its segment of samples; thread i owns lags 8i .. 8i+7 and slides a window of y through registers.
+__global__ void __launch_bounds__(kXcThreads) bss_xcorr_kernel(const float* __restrict__ ref, const float* __restrict__ est,
+                                                                int nsrc, int nchan, int64_t N, int64_t seg_len,
+                                                                double* __restrict__ slots) {
+    __shared__ double xs[kXcChunk];
+    __shared__ double ys[skew(kXcChunk + kL)];
+    const int nref = nsrc * nchan, task = blockIdx.y, tid = threadIdx.x;
+    const int a = task / (2 * nref), s = task % (2 * nref), b = s % nref;
+    const float* xp = ref + (int64_t)(a / nchan) * N * nchan + a % nchan;
+    const float* yp = (s < nref ? ref : est) + (int64_t)(b / nchan) * N * nchan + b % nchan;
+    const int64_t lo = (int64_t)blockIdx.x * seg_len, hi = min(N, lo + seg_len);
+    double acc[kR];
+#pragma unroll
+    for (int i = 0; i < kR; ++i) acc[i] = 0.0;
+    for (int64_t m0 = lo; m0 < hi; m0 += kXcChunk) {
+        __syncthreads();
+        for (int i = tid; i < kXcChunk; i += kXcThreads) {
+            const int64_t m = m0 + i;
+            xs[i] = m < hi ? (double)xp[m * nchan] : 0.0;
+        }
+        for (int i = tid; i < kXcChunk + kL; i += kXcThreads) {
+            const int64_t m = m0 + i;
+            ys[skew(i)] = m < N ? (double)yp[m * nchan] : 0.0;
+        }
+        __syncthreads();
+        double w[2 * kR];
+#pragma unroll
+        for (int k = 0; k < kR; ++k) w[k] = ys[skew(kR * tid + k)];
+        for (int mb = 0; mb < kXcChunk; mb += kR) {
+#pragma unroll
+            for (int k = 0; k < kR; ++k) w[kR + k] = ys[skew(mb + kR * tid + kR + k)];
+#pragma unroll
+            for (int st = 0; st < kR; ++st) {
+                const double xm = xs[mb + st];
+#pragma unroll
+                for (int i = 0; i < kR; ++i) acc[i] = fma(xm, w[st + i], acc[i]);
+            }
+#pragma unroll
+            for (int k = 0; k < kR; ++k) w[k] = w[kR + k];
+        }
+    }
+    double* out = slots + ((int64_t)blockIdx.x * gridDim.y + task) * kL + kR * tid;
+#pragma unroll
+    for (int i = 0; i < kR; ++i) out[i] = acc[i];
+}
+
+// lags[t][tau] = sum over segments in order
+__global__ void bss_lag_reduce_kernel(const double* __restrict__ slots, int64_t nseg, int64_t nvals, double* __restrict__ lags) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= nvals) return;
+    double s = 0.0;
+    for (int64_t g = 0; g < nseg; ++g) s += slots[g * nvals + v];
+    lags[v] = s;
+}
+
+// ---- stage 2: assembly --------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double lag(const double* lags, int nref, int a, int s, int tau) {
+    return lags[((int64_t)a * 2 * nref + s) * kL + tau];
+}
+
+// <S_p r_a, S_q r_b> = corr(a, b, p - q)
+__device__ __forceinline__ double gram(const double* lags, int nref, int a, int p, int b, int q) {
+    return p >= q ? lag(lags, nref, a, b, p - q) : lag(lags, nref, b, a, q - p);
+}
+
+// Lower triangle of G + eps I (z = 0, order nref*L) and of the diagonal blocks G[j,j] + eps I (z = 1 + j, order nchan*L).
+// The epsilon is museval's: numpy's float64 eps, added to the whole diagonal.
+__global__ void bss_assemble_gram_kernel(const double* __restrict__ lags, int nsrc, int nchan, double* __restrict__ G,
+                                         double* __restrict__ Gjj) {
+    const int nref = nsrc * nchan, z = blockIdx.z;
+    const int n = (z == 0 ? nref : nchan) * kL, a0 = z == 0 ? 0 : (z - 1) * nchan;
+    const int i = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || j > i) return;
+    double* A = z == 0 ? G : Gjj + (int64_t)(z - 1) * n * n;
+    double v = gram(lags, nref, a0 + i / kL, i % kL, a0 + j / kL, j % kL);
+    if (i == j) v += 2.220446049250313e-16;
+    A[(int64_t)i * n + j] = v;
+}
+
+// Right-hand sides, one contiguous column per (target j, estimate channel e):
+//   C  [j][e][(k, c, l)] = D_j[(k, c, l), e] = <S_l r_{k,c}, est_{j,e}>
+//   Cj [j][e][(c, l)]    = D_j[(j, c, l), e]   (source j's rows: the single-source system against G[j,j])
+__global__ void bss_assemble_rhs_kernel(const double* __restrict__ lags, int nsrc, int nchan, double* __restrict__ C,
+                                        double* __restrict__ Cj) {
+    const int nref = nsrc * nchan, col = blockIdx.y, j = col / nchan, e = col % nchan;
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= nref * kL) return;
+    const int a = r / kL, l = r % kL;
+    const double v = lag(lags, nref, a, nref + j * nchan + e, l);
+    C[(int64_t)col * nref * kL + r] = v;
+    if (a / nchan == j) Cj[(int64_t)col * nchan * kL + (a % nchan) * kL + l] = v;
+}
+
+// ---- stage 3: blocked LDL^T without pivoting, in place on the lower triangle ------------------------------------------------
+// After panel k0: L (unit diagonal implied) below the diagonal, D on it; the panel's columns of L are mirrored into the upper
+// triangle (A[p][i] = L[i][p], i beyond the panel's diagonal block) so that back substitution reads them coalesced.
+// Batch z: A + z * n * n.  n is a multiple of 64.
+__global__ void __launch_bounds__(256) bss_ldl_diag_kernel(double* __restrict__ A0, int n, int k0) {
+    __shared__ double S[kPanel][kPanel + 1];
+    double* A = A0 + (int64_t)blockIdx.x * n * n;
+    const int tid = threadIdx.x;
+    for (int idx = tid; idx < kPanel * kPanel; idx += 256) {
+        const int r = idx / kPanel, c = idx % kPanel;
+        S[r][c] = c <= r ? A[(int64_t)(k0 + r) * n + k0 + c] : 0.0;
+    }
+    __syncthreads();
+    for (int j = 0; j < kPanel; ++j) {
+        const double d = S[j][j];
+        for (int idx = tid; idx < kPanel * kPanel; idx += 256) {
+            const int r = idx / kPanel, c = idx % kPanel;
+            if (c > j && c <= r) S[r][c] -= S[r][j] * S[c][j] / d;
+        }
+        __syncthreads();
+        if (tid > j && tid < kPanel) S[tid][j] /= d;
+        __syncthreads();
+    }
+    for (int idx = tid; idx < kPanel * kPanel; idx += 256) {
+        const int r = idx / kPanel, c = idx % kPanel;
+        if (c <= r) A[(int64_t)(k0 + r) * n + k0 + c] = S[r][c];
+    }
+}
+
+// Rows below the diagonal block: l_i = (L11^{-1} a_i) / d, one row per thread.
+__global__ void __launch_bounds__(128) bss_ldl_panel_kernel(double* __restrict__ A0, int n, int k0) {
+    extern __shared__ double sm[];
+    double* Ld = sm;                          // [64][65]: L11 below, d on the diagonal
+    double* R = sm + kPanel * (kPanel + 1);   // [64][129]: the CTA's rows, transposed
+    double* A = A0 + (int64_t)blockIdx.y * n * n;
+    const int tid = threadIdx.x, k1 = k0 + kPanel, row0 = k1 + blockIdx.x * 128;
+    for (int idx = tid; idx < kPanel * kPanel; idx += 128) {
+        const int r = idx / kPanel, c = idx % kPanel;
+        Ld[r * (kPanel + 1) + c] = c <= r ? A[(int64_t)(k0 + r) * n + k0 + c] : 0.0;
+    }
+    for (int idx = tid; idx < 128 * kPanel; idx += 128) {
+        const int rl = idx / kPanel, c = idx % kPanel, i = row0 + rl;
+        R[c * 129 + rl] = i < n ? A[(int64_t)i * n + k0 + c] : 0.0;
+    }
+    __syncthreads();
+    for (int c = 0; c < kPanel; ++c) {
+        double s = R[c * 129 + tid];
+        for (int p = 0; p < c; ++p) s -= Ld[c * (kPanel + 1) + p] * R[p * 129 + tid];
+        R[c * 129 + tid] = s;
+    }
+    for (int c = 0; c < kPanel; ++c) R[c * 129 + tid] /= Ld[c * (kPanel + 1) + c];
+    __syncthreads();
+    for (int idx = tid; idx < 128 * kPanel; idx += 128) {
+        const int rl = idx / kPanel, c = idx % kPanel, i = row0 + rl;
+        if (i < n) A[(int64_t)i * n + k0 + c] = R[c * 129 + rl];
+    }
+    for (int idx = tid; idx < 128 * kPanel; idx += 128) {
+        const int c = idx / 128, rl = idx % 128, i = row0 + rl;
+        if (i < n) A[(int64_t)(k0 + c) * n + i] = R[c * 129 + rl];
+    }
+}
+
+// Trailing update A22 -= L21 D L21^T on 64x64 lower tiles; 4x4 outputs per thread.
+__global__ void __launch_bounds__(256) bss_ldl_update_kernel(double* __restrict__ A0, int n, int k0) {
+    const int ti = blockIdx.y, tj = blockIdx.x;
+    if (tj > ti) return;
+    constexpr int kK = kPanel / 2;   // the panel's columns in two halves (static shared memory)
+    __shared__ double Li[kK][kPanel + 4];
+    __shared__ double Lj[kK][kPanel + 4];
+    double* A = A0 + (int64_t)blockIdx.z * n * n;
+    const int tid = threadIdx.x, k1 = k0 + kPanel, i0 = k1 + ti * kPanel, j0 = k1 + tj * kPanel;
+    const int ty = tid / 16, tx = tid % 16;
+    double acc[4][4] = {};
+    for (int kh = 0; kh < kPanel; kh += kK) {
+        __syncthreads();
+        for (int idx = tid; idx < kPanel * kK; idx += 256) {
+            const int r = idx / kK, k = idx % kK, kk = k0 + kh + k;
+            Li[k][r] = A[(int64_t)(i0 + r) * n + kk];
+            Lj[k][r] = A[(int64_t)(j0 + r) * n + kk] * A[(int64_t)kk * n + kk];
+        }
+        __syncthreads();
+        for (int k = 0; k < kK; ++k) {
+            double x[4], y[4];
+#pragma unroll
+            for (int r = 0; r < 4; ++r) { x[r] = Li[k][ty * 4 + r]; y[r] = Lj[k][tx * 4 + r]; }
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) acc[r][c] = fma(x[r], y[c], acc[r][c]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int i = i0 + ty * 4 + r, j = j0 + tx * 4 + c;
+            if (j <= i) A[(int64_t)i * n + j] -= acc[r][c];
+        }
+}
+
+__device__ __forceinline__ double warp_sum(double s) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    return s;
+}
+
+// L D L^T x = b for one right-hand side column per CTA (grid: columns x batch), solved in place.  Left-looking: each
+// panel's rows first subtract the finished part as warp dot products (coalesced along a row of L, or along the mirrored
+// row of L^T), then the 64x64 unit-triangular block is solved column by column.
+__global__ void __launch_bounds__(256) bss_ldl_solve_kernel(const double* __restrict__ A0, int n, double* __restrict__ B0) {
+    extern __shared__ double y[];
+    const double* A = A0 + (int64_t)blockIdx.y * n * n;
+    double* b = B0 + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * n;
+    const int tid = threadIdx.x, lane = tid % 32, warp = tid / 32;
+    for (int i = tid; i < n; i += 256) y[i] = b[i];
+    __syncthreads();
+    for (int k0 = 0; k0 < n; k0 += kPanel) {
+        for (int r = warp; r < kPanel; r += 8) {
+            const double* row = A + (int64_t)(k0 + r) * n;
+            double s = 0.0;
+            for (int p = lane; p < k0; p += 32) s = fma(row[p], y[p], s);
+            s = warp_sum(s);
+            if (lane == 0) y[k0 + r] -= s;
+        }
+        __syncthreads();
+        for (int j = 0; j < kPanel; ++j) {
+            if (tid > j && tid < kPanel) y[k0 + tid] -= A[(int64_t)(k0 + tid) * n + k0 + j] * y[k0 + j];
+            __syncthreads();
+        }
+    }
+    for (int i = tid; i < n; i += 256) y[i] /= A[(int64_t)i * n + i];
+    __syncthreads();
+    for (int k0 = n - kPanel; k0 >= 0; k0 -= kPanel) {
+        for (int r = warp; r < kPanel; r += 8) {
+            const double* row = A + (int64_t)(k0 + r) * n;   // upper mirror: row[i] = L[i][k0 + r]
+            double s = 0.0;
+            for (int i = k0 + kPanel + lane; i < n; i += 32) s = fma(row[i], y[i], s);
+            s = warp_sum(s);
+            if (lane == 0) y[k0 + r] -= s;
+        }
+        __syncthreads();
+        for (int j = kPanel - 1; j > 0; --j) {
+            if (tid < j) y[k0 + tid] -= A[(int64_t)(k0 + j) * n + k0 + tid] * y[k0 + j];
+            __syncthreads();
+        }
+    }
+    for (int i = tid; i < n; i += 256) b[i] = y[i];
+}
+
+// ---- stage 4: framewise decomposition ---------------------------------------------------------------------------------------
+// CTA (tile, target j, frame t): output samples w = tile*1024 + 8*tid + i of P_all = sum_{k,c} C_j * frame slice of r_{k,c}
+// and P_j = sum_c Cj_j * slice of r_{j,c}, over the frame's W = win + L - 1 samples (slices zero-extended, no context from
+// neighbouring frames).  Only the seven energies leave the CTA, as one ordered partial per tile.  Samples past W come out as
+// zero (every tap reads beyond the slice there) and add nothing.
+template <int NCH>
+__global__ void __launch_bounds__(kFrThreads) bss_frame_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est,
+                                                                       const double* __restrict__ C, const double* __restrict__ Cj,
+                                                                       int nsrc, int64_t N, int64_t win, int64_t hop, int ntile,
+                                                                       double* __restrict__ energies) {
+    __shared__ double xs[skew(kFrTile + kL)];
+    __shared__ double h[NCH][kL], hj[NCH][kL];
+    __shared__ double red[kEnergies][kFrThreads];
+    const int nref = nsrc * NCH, tid = threadIdx.x, j = blockIdx.y;
+    const int tile = blockIdx.x % ntile;
+    const int64_t t = blockIdx.x / ntile, f0 = t * hop, w0 = (int64_t)tile * kFrTile;
+    double pa[NCH][kR], pj[NCH][kR];
+#pragma unroll
+    for (int e = 0; e < NCH; ++e)
+#pragma unroll
+        for (int i = 0; i < kR; ++i) pa[e][i] = pj[e][i] = 0.0;
+    for (int a = 0; a < nref; ++a) {
+        const bool own = a / NCH == j;
+        const float* xp = ref + (int64_t)(a / NCH) * N * NCH + a % NCH;
+        __syncthreads();
+        // xs[u] = slice[w0 - (L-1) + u]; taps reversed so that P[w] = sum_u h[u] xs[w - w0 + u]
+        for (int u = tid; u < kFrTile + kL; u += kFrThreads) {
+            const int64_t v = w0 - (kL - 1) + u;
+            xs[skew(u)] = (v >= 0 && v < win) ? (double)xp[(f0 + v) * NCH] : 0.0;
+        }
+        for (int u = tid; u < NCH * kL; u += kFrThreads) {
+            const int e = u / kL, l = u % kL;
+            h[e][kL - 1 - l] = C[((int64_t)(j * NCH + e) * nref + a) * kL + l];
+            if (own) hj[e][kL - 1 - l] = Cj[((int64_t)(j * NCH + e) * NCH + a % NCH) * kL + l];
+        }
+        __syncthreads();
+        double w[2 * kR];
+#pragma unroll
+        for (int k = 0; k < kR; ++k) w[k] = xs[skew(kR * tid + k)];
+        for (int ub = 0; ub < kL; ub += kR) {
+#pragma unroll
+            for (int k = 0; k < kR; ++k) w[kR + k] = xs[skew(ub + kR * tid + kR + k)];
+#pragma unroll
+            for (int st = 0; st < kR; ++st) {
+#pragma unroll
+                for (int e = 0; e < NCH; ++e) {
+                    const double he = h[e][ub + st];
+#pragma unroll
+                    for (int i = 0; i < kR; ++i) pa[e][i] = fma(he, w[st + i], pa[e][i]);
+                }
+                if (own) {
+#pragma unroll
+                    for (int e = 0; e < NCH; ++e) {
+                        const double he = hj[e][ub + st];
+#pragma unroll
+                        for (int i = 0; i < kR; ++i) pj[e][i] = fma(he, w[st + i], pj[e][i]);
+                    }
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < kR; ++k) w[k] = w[kR + k];
+        }
+    }
+    // E0 |P_j|^2, E1 |est - r_j|^2, E2 |r_j|^2, E3 |P_j - r_j|^2, E4 |P_all - P_j|^2, E5 |P_all|^2, E6 |est - P_all|^2
+    double en[kEnergies] = {};
+#pragma unroll
+    for (int i = 0; i < kR; ++i) {
+        const int64_t v = w0 + kR * tid + i;
+#pragma unroll
+        for (int e = 0; e < NCH; ++e) {
+            const int64_t off = ((int64_t)j * N + f0 + v) * NCH + e;
+            const double s = v < win ? (double)est[off] : 0.0, r = v < win ? (double)ref[off] : 0.0;
+            const double p = pj[e][i], q = pa[e][i];
+            en[0] += p * p;
+            en[1] += (s - r) * (s - r);
+            en[2] += r * r;
+            en[3] += (p - r) * (p - r);
+            en[4] += (q - p) * (q - p);
+            en[5] += q * q;
+            en[6] += (s - q) * (s - q);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < kEnergies; ++k) red[k][tid] = en[k];
+    __syncthreads();
+    if (tid < kEnergies) {
+        double s = 0.0;
+        for (int i = 0; i < kFrThreads; ++i) s += red[tid][i];
+        energies[(((int64_t)t * nsrc + j) * ntile + tile) * kEnergies + tid] = s;
+    }
+}
+
+__device__ __forceinline__ double safe_db(double num, double den) {
+    return den == 0.0 ? __longlong_as_double(0x7ff0000000000000LL) : 10.0 * log10(num / den);
+}
+
+// One CTA per frame: museval's silence rule, then the four metrics of every target from its tiles' energies (in order).
+__global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __restrict__ ref, const float* __restrict__ est,
+                                                                int nsrc, int nchan, int64_t N, int64_t win, int64_t hop,
+                                                                int64_t nwin, int ntile, const double* __restrict__ energies,
+                                                                double* __restrict__ metrics) {
+    const int64_t t = blockIdx.x, f0 = t * hop;
+    // A frame is NaN for every target if some reference or some estimate has sum_c x[n][c] == 0 on every sample of it.
+    bool silent = false;
+    for (int k = 0; k < 2 * nsrc; ++k) {
+        const float* x = (k < nsrc ? ref : est) + (int64_t)(k % nsrc) * N * nchan;
+        int nonzero = 0;
+        for (int64_t v = threadIdx.x; v < win && !nonzero; v += blockDim.x) {
+            double s = 0.0;
+            for (int c = 0; c < nchan; ++c) s += (double)x[(f0 + v) * nchan + c];
+            nonzero = s != 0.0;
+        }
+        silent |= !__syncthreads_or(nonzero);
+    }
+    const int j = threadIdx.x;
+    if (j >= nsrc) return;
+    double E[kEnergies] = {};
+    for (int tile = 0; tile < ntile; ++tile)
+#pragma unroll
+        for (int k = 0; k < kEnergies; ++k) E[k] += energies[(((int64_t)t * nsrc + j) * ntile + tile) * kEnergies + k];
+    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    // images decomposition: s_true = r_j, e_spat = P_j - r_j, e_interf = P_all - P_j, e_artif = est - P_all
+    const double sdr = silent ? nan : safe_db(E[2], E[1]);   // |s_true|^2 / |e_spat + e_interf + e_artif|^2
+    const double isr = silent ? nan : safe_db(E[2], E[3]);
+    const double sir = silent ? nan : safe_db(E[0], E[4]);
+    const double sar = silent ? nan : safe_db(E[5], E[6]);
+    const int64_t o = (int64_t)j * nwin + t, m = (int64_t)nsrc * nwin;
+    metrics[o] = sdr;
+    metrics[m + o] = isr;
+    metrics[2 * m + o] = sir;
+    metrics[3 * m + o] = sar;
+}
+
+// ---- host side --------------------------------------------------------------------------------------------------------------
+struct Layout {
+    int64_t nref, ntask, n, m, nseg, seg_len, nwin, ntile;
+    int64_t slots, lags, G, Gjj, C, Cj, E, total;   // byte offsets into the workspace
+};
+
+bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, Layout* o) {
+    if (nsrc < 1 || nsrc > WUN_MAX_SOURCES || (nchan != 1 && nchan != 2) || N < 1 || win < 1 || hop < 1) return false;
+    if (win > (int64_t)1 << 40 || hop > (int64_t)1 << 40 || N > (int64_t)1 << 40) return false;
+    Layout& L = *o;
+    L.nref = nsrc * nchan;
+    L.ntask = 2 * L.nref * L.nref;
+    L.n = L.nref * kL;
+    L.m = nchan * kL;
+    const int64_t nchunks = (N + kXcChunk - 1) / kXcChunk, per_seg = (nchunks + kMaxSegs - 1) / kMaxSegs;
+    L.nseg = (nchunks + per_seg - 1) / per_seg;
+    L.seg_len = per_seg * kXcChunk;
+    L.nwin = N >= win ? (N - win) / hop + 1 : 0;   // floor((N - win + hop) / hop), at least 0
+    L.ntile = (win + kL - 1 + kFrTile - 1) / kFrTile;
+    if (L.nwin * L.ntile >= ((int64_t)1 << 31)) return false;
+    int64_t off = 0;
+    auto take = [&](int64_t doubles) { const int64_t at = off; off += (doubles * 8 + 255) / 256 * 256; return at; };
+    L.slots = take(L.nseg * L.ntask * kL);
+    L.lags = take(L.ntask * kL);
+    L.G = take(L.n * L.n);
+    L.Gjj = take(nsrc * L.m * L.m);
+    L.C = take(L.nref * L.n);
+    L.Cj = take(L.nref * L.m);
+    L.E = take(L.nwin * nsrc * L.ntile * kEnergies);
+    L.total = off;
+    return true;
+}
+
+// Blocked LDL^T of `batch` matrices of order n, then solve for ncol right-hand-side columns each.
+cudaError_t ldl_solve(double* A, int n, int batch, double* B, int ncol, cudaStream_t st) {
+    const int panel_smem = (kPanel * (kPanel + 1) + kPanel * 129) * 8;
+    cudaError_t e = cudaFuncSetAttribute(bss_ldl_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, panel_smem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(bss_ldl_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n * 8);
+    if (e != cudaSuccess) return e;
+    for (int k0 = 0; k0 < n; k0 += kPanel) {
+        bss_ldl_diag_kernel<<<batch, 256, 0, st>>>(A, n, k0);
+        const int rest = n - k0 - kPanel;
+        if (rest > 0) {
+            bss_ldl_panel_kernel<<<dim3((rest + 127) / 128, batch), 128, panel_smem, st>>>(A, n, k0);
+            const int nt = rest / kPanel;
+            bss_ldl_update_kernel<<<dim3(nt, nt, batch), 256, 0, st>>>(A, n, k0);
+        }
+    }
+    bss_ldl_solve_kernel<<<dim3(ncol, batch), 256, n * 8, st>>>(A, n, B);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+extern "C" int64_t wun_bss_eval_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop) {
+    Layout L;
+    return make_layout(nsrc, nchan, nsampl, win, hop, &L) ? L.total : WUN_E_INVALID;
+}
+
+extern "C" int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                            int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+    Layout L;
+    if (!make_layout(nsrc, nchan, nsampl, win, hop, &L)) return WUN_E_INVALID;
+    if (!references || !estimates || !workspace || (!metrics && L.nwin > 0)) return WUN_E_INVALID;
+    if (workspace_bytes < L.total || reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return WUN_E_INVALID;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        return WUN_E_NOGPU;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    double *slots = (double*)(ws + L.slots), *lags = (double*)(ws + L.lags), *G = (double*)(ws + L.G),
+           *Gjj = (double*)(ws + L.Gjj), *C = (double*)(ws + L.C), *Cj = (double*)(ws + L.Cj), *E = (double*)(ws + L.E);
+    const int ns = (int)nsrc, nc = (int)nchan, nref = (int)L.nref;
+
+    bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)L.ntask), kXcThreads, 0, st>>>(references, estimates, ns, nc, nsampl,
+                                                                                        L.seg_len, slots);
+    const int64_t nvals = L.ntask * kL;
+    bss_lag_reduce_kernel<<<(unsigned)((nvals + 255) / 256), 256, 0, st>>>(slots, L.nseg, nvals, lags);
+    bss_assemble_gram_kernel<<<dim3((unsigned)(L.n + 255) / 256, (unsigned)L.n, 1 + ns), 256, 0, st>>>(lags, ns, nc, G, Gjj);
+    bss_assemble_rhs_kernel<<<dim3((unsigned)(L.n + 255) / 256, nref), 256, 0, st>>>(lags, ns, nc, C, Cj);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = ldl_solve(G, (int)L.n, 1, C, nref, st);
+    if (e == cudaSuccess) e = ldl_solve(Gjj, (int)L.m, ns, Cj, nc, st);
+    if (e == cudaSuccess && L.nwin > 0) {
+        const dim3 grid((unsigned)(L.nwin * L.ntile), ns);
+        if (nc == 1)
+            bss_frame_energy_kernel<1><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
+                                                                    (int)L.ntile, E);
+        else
+            bss_frame_energy_kernel<2><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
+                                                                    (int)L.ntile, E);
+        bss_frame_metrics_kernel<<<(unsigned)L.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, L.nwin,
+                                                                   (int)L.ntile, E, metrics);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && filters) {
+        e = cudaMemcpyAsync(filters, C, L.nref * L.n * 8, cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(filters + L.nref * L.n, Cj, L.nref * L.m * 8, cudaMemcpyDeviceToDevice, st);
+    }
+    return e == cudaSuccess ? WUN_OK : WUN_E_CUDA;
+}

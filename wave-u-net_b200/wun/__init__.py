@@ -19,6 +19,7 @@ SYMBOLS = [
     "wun_launches_forward_backward", "wun_forward", "wun_forward_backward", "wun_adam_step", "wun_adam_step_device", "wun_set_grad_buckets", "wun_stream_wait_grad_bucket",
     "wun_gather_windows", "wun_scatter_windows", "wun_feed_batch", "wun_last_error", "wun_version", "wun_describe",
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
+    "wun_bss_eval_workspace_bytes", "wun_bss_eval",
 ]
 
 
@@ -87,6 +88,10 @@ def _load():
     lib.wun_debug_launches.restype = I64
     lib.wun_crc32c.argtypes = [ctypes.c_uint32, VP, ctypes.c_uint64]
     lib.wun_crc32c.restype = ctypes.c_uint32
+    if hasattr(lib, "wun_bss_eval"):        # the host-simulation build (tests/hostsim, WUN_LIB) leaves the scoring kernels out
+        lib.wun_bss_eval_workspace_bytes.argtypes = [I64, I64, I64, I64, I64]
+        lib.wun_bss_eval_workspace_bytes.restype = I64
+        lib.wun_bss_eval.argtypes = [VP, VP, I64, I64, I64, I64, I64, VP, VP, VP, I64, VP]
     return lib
 
 
@@ -110,6 +115,45 @@ def check(rc):
         if rc == WUN_E_SHAPE:
             raise AssertionError(msg)               # reference: asserts :55, :121, Utils.py:114-117
         raise WunError(rc, msg)
+
+
+BSS_FILTER_LEN = 512
+
+
+def bss_eval(references, estimates, win, hop, filters=False):
+    """BSS Eval v4 of `estimates` against `references` (include/wun.h wun_bss_eval): both contiguous float32 CUDA tensors
+    [nsrc, nsampl, nchan] on one device.  Returns float64 CUDA tensors (SDR, ISR, SIR, SAR), each [nsrc, nwin]; with
+    filters=True also (C [nsrc, nchan, nsrc, nchan, 512], Cj [nsrc, nchan, nchan, 512]): the filters for all sources and
+    for each source alone, indexed [target, estimate channel, (source,) reference channel, tap]."""
+    import torch
+    for t in (references, estimates):
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 3, \
+            "references / estimates must be contiguous float32 CUDA tensors [nsrc, nsampl, nchan]"
+    assert estimates.shape == references.shape and estimates.device == references.device, "estimates must match references"
+    nsrc, n, nchan = (int(s) for s in references.shape)
+    nbytes = lib.wun_bss_eval_workspace_bytes(nsrc, nchan, n, int(win), int(hop))
+    if nbytes < 0:
+        raise WunError(WUN_E_INVALID, "bss_eval: need 1 <= nsrc <= 8, nchan 1 or 2, nsampl, win, hop >= 1 (got %d, %d, %d, %d, %d)"
+                       % (nsrc, nchan, n, win, hop))
+    nwin = (n - win) // hop + 1 if n >= win else 0
+    dev = references.device
+    metrics = torch.empty((4, nsrc, nwin), dtype=torch.float64, device=dev)
+    filt = None
+    if filters:
+        filt = torch.empty(nsrc * nchan * (nsrc * nchan + nchan) * BSS_FILTER_LEN, dtype=torch.float64, device=dev)
+    ws = torch.empty((nbytes + 255) // 256 * 32, dtype=torch.float64, device=dev)      # torch allocations are 256-B aligned
+    with torch.cuda.device(dev):
+        rc = lib.wun_bss_eval(references.data_ptr(), estimates.data_ptr(), nsrc, nchan, n, int(win), int(hop),
+                              metrics.data_ptr() if nwin else None, filt.data_ptr() if filt is not None else None,
+                              ws.data_ptr(), ws.numel() * 8, Engine._stream(dev))
+    if rc != WUN_OK:
+        raise WunError(rc, "wun_bss_eval failed")
+    out = tuple(metrics)
+    if filters:
+        nc = nsrc * nchan * nsrc * nchan * BSS_FILTER_LEN
+        out += (filt[:nc].view(nsrc, nchan, nsrc, nchan, BSS_FILTER_LEN),
+                filt[nc:].view(nsrc, nchan, nchan, BSS_FILTER_LEN))
+    return out
 
 
 _UPSAMPLING = {"linear": 0, "learned": 1}
