@@ -190,6 +190,24 @@ int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, 
                  int64_t win, int64_t hop, double* metrics, double* filters, void* workspace, int64_t workspace_bytes,
                  void* stream);
 
+/* --- resampling (no handle) ----------------------------------------------------------------------
+ * librosa 0.6.2 resample(y, sr_in, sr_out) with res_type='kaiser_best', which the reference applies to every track before and
+ * after separation (Evaluate.py:64,104, Utils.resample): resampy 0.2's resample_f bit for bit, then fix_length's zero
+ * padding.  Frames t < floor(n_in * ratio), ratio = (double)sr_out / sr_in, are resampy's output; the frames from there up to
+ * n_out are zero.
+ *   x      DEVICE float32 [n_in][nchan]          y  DEVICE float32 [n_out][nchan], n_out = wun_resample_frames(...)
+ *   win, delta  DEVICE float64 [nwin]: the half filter table, already multiplied by the ratio when downsampling (as
+ *          resampy.resample scales it before calling resample_f), and its forward difference with a trailing zero;
+ *   precision   table entries per zero crossing (512 for kaiser_best)
+ * nchan 1 or 2, rates > 0, n_out == wun_resample_frames(n_in, sr_in, sr_out) and floor(n_in * ratio) >= 1 (resampy raises
+ * ValueError there); otherwise WUN_E_INVALID (and wun_resample_frames returns WUN_E_INVALID for a rate <= 0 or n_in < 0).
+ * Enqueued on `stream`; no allocation, no synchronisation.  The same inputs give the same bits on every call.  These two
+ * functions do not set wun_last_error(). */
+/* librosa.resample(y, sr_in, sr_out) output length: ceil(n_in * ((double)sr_out / sr_in)) */
+int64_t wun_resample_frames(int64_t n_in, int64_t sr_in, int64_t sr_out);
+int wun_resample(const float* x, int64_t n_in, int64_t nchan, int64_t sr_in, int64_t sr_out, const double* win,
+                 const double* delta, int64_t nwin, int64_t precision, float* y, int64_t n_out, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

@@ -8,10 +8,11 @@ predict_track() keeps the semantics of /root/reference/Evaluate.py:82-145 exactl
 through the network as batches, and scattered back on the device; with torch.distributed initialised the window list
 is split over the ranks (no collective on the data path, results all-gathered at the end).
 
-Audio file I/O, resampling and musdb loading of the reference (librosa / musdb, Evaluate.py:16-80,147-193) are out of
-scope (SURVEY section 2): predict_track works on arrays already at model_config["expected_sr"].  Scoring is here:
-evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS Eval v4 on the GPU
-(wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).
+predict_track works on arrays already at model_config["expected_sr"]; predict() is the reference's predict() (Evaluate.py:
+60-71) on an array at any rate, resampling on the GPU with librosa's kaiser_best (wun.resample) on the way in and out.
+Scoring is here: evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS
+Eval v4 on the GPU (wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).  Audio decoding
+beyond WAV (Predict.py) and musdb loading are out of scope (SURVEY section 2).
 """
 import glob
 import json
@@ -38,19 +39,31 @@ def predict_track(model_config, separator, mix_audio, batch_windows=16, device="
     Models.UnetAudioSeparator.UnetAudioSeparator holding variables.  Returns OrderedDict name -> [n_frames, C]."""
     import torch
     assert len(mix_audio.shape) == 2
+    mix_audio = _model_channels(model_config, mix_audio)
+    preds = _separate_on_device(model_config, separator, torch.from_numpy(np.ascontiguousarray(mix_audio)), batch_windows,
+                                device)
+    result = preds.cpu().numpy()
+    return OrderedDict((name, result[k]) for k, name in enumerate(model_config["source_names"]))
+
+
+def _model_channels(model_config, mix_audio):
+    """The mono downmix, or the tiling of a mono input to stereo, that predict_track applies (Evaluate.py:98-102)."""
     mix_audio = np.asarray(mix_audio, dtype=np.float32)
     if model_config["mono_downmix"]:
-        mix_audio = np.mean(mix_audio, axis=1, keepdims=True)
-    elif mix_audio.shape[1] == 1:
-        mix_audio = np.tile(mix_audio, [1, 2])
+        return np.mean(mix_audio, axis=1, keepdims=True)
+    if mix_audio.shape[1] == 1:
+        return np.tile(mix_audio, [1, 2])
+    return mix_audio
 
+
+def _separate_on_device(model_config, separator, mix, batch_windows=16, device="cuda"):
+    """predict_track's device half: `mix` a float32 tensor [n_frames, C] at expected_sr with the model's channel count
+    (host or device).  Returns the estimates as a float32 CUDA tensor [K, n_frames, C] in source_names order."""
+    import torch
     in_shape, out_shape = separator.get_padding(np.array([1, model_config["num_frames"], 0]))
     t_in, t_out = int(in_shape[1]), int(out_shape[1])
-    extra_pad = 0
-    if mix_audio.shape[0] < t_in:
-        extra_pad = t_in - mix_audio.shape[0]
-        mix_audio = np.pad(mix_audio, [(0, extra_pad), (0, 0)], mode="constant", constant_values=0.0)
-    n_frames, C = mix_audio.shape
+    n_mix, C = int(mix.shape[0]), int(mix.shape[1])
+    n_frames = max(n_mix, t_in)          # zero-extension of short inputs, cut off again at the end (Evaluate.py:107-111,142-143)
     pad = (t_in - t_out) // 2                                   # context on both sides (Evaluate.py:121-122), zero-filled ON the device
 
     eng = separator.engine(input_frames=t_in)
@@ -61,8 +74,8 @@ def predict_track(model_config, separator, mix_audio, batch_windows=16, device="
     lo, hi = parallel.shard_range(len(starts_all), rank, ws)
 
     padded_d = torch.zeros((n_frames + 2 * pad, C), dtype=torch.float32, device=device)
-    padded_d[pad:pad + n_frames].copy_(torch.from_numpy(np.ascontiguousarray(mix_audio)))      # (a host-side np.pad of a 3-minute
-    # track costs as much as a third of the whole separation)
+    padded_d[pad:pad + n_mix].copy_(mix)        # (a host-side np.pad of a 3-minute track costs as much as a third of the
+    # whole separation)
     preds_local = torch.empty((K, hi - lo, t_out, C), dtype=torch.float32, device=device)
     st_all = torch.tensor(starts_all, dtype=torch.int64, device=device)          # one upload; the batches take slices of it
     for b0 in range(lo, hi, batch_windows):
@@ -77,23 +90,57 @@ def predict_track(model_config, separator, mix_audio, batch_windows=16, device="
     # scatter (overwrite; the shifted last window wins where it overlaps its predecessor)
     preds = torch.zeros((K, n_frames, C), dtype=torch.float32, device=device)
     eng.scatter_windows(preds_all.contiguous(), st_all, preds)
-    result = preds.cpu().numpy()
-    if extra_pad > 0:
-        result = result[:, :-extra_pad, :]
-    return OrderedDict((name, result[k]) for k, name in enumerate(names))
+    return preds[:, :n_mix]
+
+
+def predict(model_config, separator, audio, rate, references=None, results_dir=None, track_name=None):
+    """The reference's predict() (Evaluate.py:60-71) on an array: `audio` float [n_frames, n_channels] at `rate` Hz.
+    The mixture is downmixed or tiled to the model's channels, resampled to expected_sr with wun.resample (librosa's
+    kaiser_best, Evaluate.py:104), separated, and every estimate is resampled back to `rate`, cut to n_frames and, for a
+    mono model and a multichannel input, tiled to the input's channels (:64-67).  The track stays on the device from the
+    upload to the download.  Returns OrderedDict name -> float32 [n_frames, n_channels].
+
+    With `references` (name -> [n_frames, n_channels] at `rate`) the estimates are scored by eval_track at `rate` (the
+    reference's museval.eval_mus_track, :71), written to <results_dir>/<track_name>.json when results_dir is given, and the
+    per-target median SDR / ISR / SIR / SAR is printed."""
+    import torch
+    import wun
+    assert len(audio.shape) == 2
+    n_frames, mix_channels = int(audio.shape[0]), int(audio.shape[1])
+    sr = int(model_config["expected_sr"])
+    mix = torch.from_numpy(np.ascontiguousarray(_model_channels(model_config, audio))).cuda()
+    preds = _separate_on_device(model_config, separator, wun.resample(mix, rate, sr))
+    back = torch.stack([wun.resample(preds[k].contiguous(), sr, rate)[:n_frames] for k in range(preds.shape[0])])
+    result = back.cpu().numpy()
+    if model_config["mono_downmix"] and mix_channels > 1:
+        result = np.tile(result, [1, 1, mix_channels])
+    pred_audio = OrderedDict((name, result[k]) for k, name in enumerate(model_config["source_names"]))
+    if references is not None:
+        scores = eval_track(references, pred_audio, rate, output_dir=results_dir, track_name=track_name)
+        for target in scores["targets"]:
+            print("%s ==> %s" % (target["name"], "  ".join(
+                "%s: %.3f" % (m, np.nanmedian([f["metrics"][m] for f in target["frames"]]))
+                for m in ("SDR", "ISR", "SIR", "SAR"))))
+    return pred_audio
+
+
+def load_separator(model_config, load_model):
+    """A separator holding the variables of `load_model` (a TF-V2 checkpoint prefix - written by Training.train or by the
+    reference - or a round-1 .npz; reference restore: Evaluate.py:55-57); None leaves them uninitialised."""
+    from Models.UnetAudioSeparator import UnetAudioSeparator
+    separator = UnetAudioSeparator(model_config)
+    in_shape, _ = separator.get_padding(np.array([1, model_config["num_frames"], 0]))
+    if load_model is not None:
+        import TFCheckpoint
+        TFCheckpoint.restore_separator(load_model, separator, int(in_shape[1]), with_optimizer=False)
+    return separator
 
 
 def produce_source_estimates(model_config, load_model, mix_audio, separator=None):
-    """Predict.py's work-horse (reference Evaluate.py:161-193 minus file I/O): builds the separator, loads variables
-    from `load_model` (a TF-V2 checkpoint prefix - written by Training.train or by the reference - or a round-1 .npz;
-    reference restore: Evaluate.py:55-57) and separates `mix_audio`."""
-    from Models.UnetAudioSeparator import UnetAudioSeparator
+    """Predict.py's work-horse for arrays already at expected_sr (reference Evaluate.py:161-193 minus file I/O): builds
+    the separator with load_separator and separates `mix_audio`."""
     if separator is None:
-        separator = UnetAudioSeparator(model_config)
-        in_shape, _ = separator.get_padding(np.array([1, model_config["num_frames"], 0]))
-        if load_model is not None:
-            import TFCheckpoint
-            TFCheckpoint.restore_separator(load_model, separator, int(in_shape[1]), with_optimizer=False)
+        separator = load_separator(model_config, load_model)
     return predict_track(model_config, separator, mix_audio)
 
 

@@ -1,53 +1,103 @@
 """Prediction entry point (stand-in for /root/reference/Predict.py:1-17):
 
-    python Predict.py with cfg.full_44KHz model_path=checkpoints/123/123-2000 input_path=mix.npy [output_path=out]
+    python Predict.py with cfg.full_44KHz model_path=checkpoints/123/123-2000 input_path=song.wav [output_path=out]
 
 model_path:  a TF-V2 checkpoint prefix (written by Training.py here or by the reference's Saver) or a round-1 .npz.
-input_path: a .npy float array [n_frames, n_channels] already at model_config["expected_sr"] (decoding / resampling
-audio files needs librosa + ffmpeg, which the reference uses at Evaluate.py:172 and which are out of scope here).
-Writes <output_path or input_path>_<source>.npy per source (reference writes _<source>.wav, Evaluate.py:193).
+input_path:
+  *.wav  16-bit PCM (scaled by 1/32768, as librosa 0.6 loads it) or 32-bit float, mono or multichannel, at any rate.  The
+         track is separated at its own rate through Evaluate.predict - resampled to expected_sr and back on the GPU with
+         librosa's kaiser_best, as the reference's predict() does (Evaluate.py:60-71) - and every estimate is written to
+         <output_path or input_path>_<source>.wav as 32-bit float WAV at the input's rate (librosa.output.write_wav,
+         Evaluate.py:193).
+  *.npy  a float array [n_frames, n_channels] already at model_config["expected_sr"]; estimates are written to
+         <output_path or input_path>_<source>.npy.
+Other audio formats (mp3 and friends need ffmpeg, Evaluate.py:172) are out of scope.
 
-With references_path=<refs.npz> (one [n_frames, n_channels] array per source name, at the mixture's rate) and
-results_dir=<dir>, the predictions are also scored with BSS Eval v4 on the GPU (Evaluate.eval_track, the reference's
-museval.eval_mus_track at Evaluate.py:71) and written to <results_dir>/<input file name>.json, which
-Evaluate.compute_mean_metrics reads.  Mono-model estimates are tiled to the references' channel count (Evaluate.py:66-67).
+With references_path= and results_dir=<dir>, the predictions are also scored with BSS Eval v4 on the GPU
+(Evaluate.eval_track, the reference's museval.eval_mus_track at Evaluate.py:71) at the input's rate and written to
+<results_dir>/<input file name>.json, which Evaluate.compute_mean_metrics reads.  references_path is a directory of
+<source>.wav stems at the input's rate, or a .npz with one [n_frames, n_channels] array per source name.  Mono-model
+estimates are tiled to the references' channel count (Evaluate.py:66-67).
 """
+import glob
 import os
 import sys
 
 import numpy as np
+import scipy.io.wavfile
 
 import Config
 import Evaluate
 
 
+def read_wav(path):
+    """(rate, float32 [n_frames, n_channels]) of a WAV file, as the reference's Utils.load(path, sr=None, mono=False) gives
+    it: 16-bit PCM divided by 32768 (librosa 0.6's buf_to_float), 32-bit float unchanged.  Other sample formats raise."""
+    rate, data = scipy.io.wavfile.read(path)
+    if data.dtype == np.int16:
+        audio = data.astype(np.float32) / np.float32(32768)
+    elif data.dtype == np.float32:
+        audio = data
+    else:
+        raise ValueError("%s: %s WAV samples are not supported (16-bit PCM or 32-bit float only)" % (path, data.dtype))
+    return int(rate), np.ascontiguousarray(audio.reshape(audio.shape[0], -1))
+
+
+def write_wav(path, audio, rate):
+    """32-bit float WAV of `audio` [n_frames, n_channels] at `rate`, as librosa.output.write_wav writes float32 audio."""
+    audio = np.asarray(audio, np.float32)
+    scipy.io.wavfile.write(path, int(rate), audio[:, 0] if audio.shape[1] == 1 else audio)
+
+
+def load_references(references_path, rate):
+    """name -> [n_frames, n_channels] from a directory of <source>.wav stems at `rate`, or from a .npz."""
+    if os.path.isdir(references_path):
+        refs = {}
+        for path in sorted(glob.glob(os.path.join(references_path, "*.wav"))):
+            sr, audio = read_wav(path)
+            if sr != rate:
+                raise ValueError("%s is at %d Hz, the mixture at %d Hz" % (path, sr, rate))
+            refs[os.path.splitext(os.path.basename(path))[0]] = audio
+        return refs
+    with np.load(references_path) as z:
+        return {name: z[name] for name in z.files}
+
+
 def main(cfg, model_path, input_path, output_path=None, references_path=None, results_dir=None):
     model_config = cfg["model_config"]
+    base = output_path if output_path is not None else input_path
+    track = os.path.splitext(os.path.basename(input_path))[0]
+    score = references_path is not None and results_dir is not None
+    if input_path.lower().endswith(".wav"):
+        rate, mix = read_wav(input_path)
+        refs = load_references(references_path, rate) if score else None
+        preds = Evaluate.predict(model_config, Evaluate.load_separator(model_config, model_path), mix, rate,
+                                 references=refs, results_dir=results_dir, track_name=track)
+        for name, audio in preds.items():
+            write_wav("%s_%s.wav" % (base, name), audio, rate)
+        return preds
     mix = np.load(input_path)
     preds = Evaluate.produce_source_estimates(model_config, model_path, mix)
-    base = output_path if output_path is not None else input_path
     for name, audio in preds.items():
         np.save("%s_%s.npy" % (base, name), audio)
-    if references_path is not None and results_dir is not None:
-        with np.load(references_path) as z:
-            refs = {name: z[name] for name in z.files}
+    if score:
+        refs = load_references(references_path, model_config["expected_sr"])
         nchan = next(iter(refs.values())).shape[1]
         est = {name: np.tile(audio, [1, nchan]) if audio.shape[1] == 1 and nchan > 1 else audio
                for name, audio in preds.items()}
-        track = os.path.splitext(os.path.basename(input_path))[0]
         Evaluate.eval_track(refs, est, model_config["expected_sr"], output_dir=results_dir, track_name=track)
     return preds
 
 
-# the reference's defaults (Predict.py:9-13); its default input is an mp3 - decoding audio files is out of scope here, so
-# input_path has to be given
+# the reference's defaults (Predict.py:9-13); its default input is an mp3 - decoding mp3 needs ffmpeg, so input_path has to
+# be given
 DEFAULT_MODEL_PATH = os.path.join("checkpoints", "full_44KHz", "full_44KHz-236118")
 
 
 if __name__ == "__main__":
     cfg, extras = Config.parse_command_line(sys.argv[1:])
     if "input_path" not in extras:
-        raise SystemExit("Predict.py: input_path=<mix.npy> is required (a float array [n_frames, n_channels] at expected_sr; the "
-                         "reference's default, an mp3 of audio_examples/, needs librosa + ffmpeg)\n" + __doc__)
+        raise SystemExit("Predict.py: input_path=<song.wav or mix.npy> is required (the reference's default, an mp3 of "
+                         "audio_examples/, needs ffmpeg)\n" + __doc__)
     main(cfg, extras.get("model_path", DEFAULT_MODEL_PATH), extras["input_path"], extras.get("output_path"),
          extras.get("references_path"), extras.get("results_dir"))

@@ -19,7 +19,7 @@ SYMBOLS = [
     "wun_launches_forward_backward", "wun_forward", "wun_forward_backward", "wun_adam_step", "wun_adam_step_device", "wun_set_grad_buckets", "wun_stream_wait_grad_bucket",
     "wun_gather_windows", "wun_scatter_windows", "wun_feed_batch", "wun_last_error", "wun_version", "wun_describe",
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
-    "wun_bss_eval_workspace_bytes", "wun_bss_eval",
+    "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_resample_frames", "wun_resample",
 ]
 
 
@@ -92,6 +92,10 @@ def _load():
         lib.wun_bss_eval_workspace_bytes.argtypes = [I64, I64, I64, I64, I64]
         lib.wun_bss_eval_workspace_bytes.restype = I64
         lib.wun_bss_eval.argtypes = [VP, VP, I64, I64, I64, I64, I64, VP, VP, VP, I64, VP]
+    if hasattr(lib, "wun_resample"):        # likewise the resampling kernel
+        lib.wun_resample_frames.argtypes = [I64, I64, I64]
+        lib.wun_resample_frames.restype = I64
+        lib.wun_resample.argtypes = [VP, I64, I64, I64, I64, VP, VP, I64, I64, VP, I64, VP]
     return lib
 
 
@@ -154,6 +158,83 @@ def bss_eval(references, estimates, win, hop, filters=False):
         out += (filt[:nc].view(nsrc, nchan, nsrc, nchan, BSS_FILTER_LEN),
                 filt[nc:].view(nsrc, nchan, nchan, BSS_FILTER_LEN))
     return out
+
+
+# resampy 0.2's 'kaiser_best' filter, which librosa 0.6.2 resample() uses by default: sinc_window(num_zeros=64, precision=9,
+# window=kaiser(beta), rolloff).  These constants and the symmetric window below are recalled from resampy, not read from it.
+KAISER_BEST_ZEROS = 64
+KAISER_BEST_PRECISION = 2 ** 9
+KAISER_BEST_ROLLOFF = 0.9475937167399596
+KAISER_BEST_BETA = 14.769656459379492
+_kaiser_best = None
+_resample_tables = {}
+
+
+def kaiser_best_filter():
+    """(half window float64 [32769], precision): rolloff * sinc(rolloff * x) for x = 0 .. 64 zero crossings in steps of
+    1/512, times the right half of a symmetric Kaiser window of length 65537 (resampy.filters.sinc_window).  Built once."""
+    global _kaiser_best
+    if _kaiser_best is None:
+        import numpy as np
+        import scipy.signal
+        n = KAISER_BEST_PRECISION * KAISER_BEST_ZEROS
+        sinc = KAISER_BEST_ROLLOFF * np.sinc(KAISER_BEST_ROLLOFF * np.linspace(0, KAISER_BEST_ZEROS, num=n + 1, endpoint=True))
+        taper = scipy.signal.windows.kaiser(2 * n + 1, KAISER_BEST_BETA, sym=True)[n:]
+        _kaiser_best = (taper * sinc, KAISER_BEST_PRECISION)
+    return _kaiser_best
+
+
+def resample_tables(sr_in, sr_out):
+    """(win, delta) float64 numpy arrays as resampy.resample hands them to resample_f: the kaiser_best half window, times
+    the ratio when downsampling, and its np.diff with a trailing zero."""
+    import numpy as np
+    win, _ = kaiser_best_filter()
+    ratio = float(sr_out) / sr_in
+    if ratio < 1:
+        win = win * ratio
+    delta = np.zeros_like(win)
+    delta[:-1] = np.diff(win)
+    return win, delta
+
+
+def resample_frames(n_in, sr_in, sr_out):
+    """librosa.resample's output length, ceil(n_in * sr_out / sr_in) (include/wun.h wun_resample_frames)."""
+    n = lib.wun_resample_frames(int(n_in), int(sr_in), int(sr_out))
+    if n < 0:
+        raise ValueError("resample: need n_in >= 0 and positive rates (got %d, %d, %d)" % (n_in, sr_in, sr_out))
+    return n
+
+
+def resample(x, sr_in, sr_out):
+    """librosa.resample(x.T, sr_in, sr_out).T with res_type='kaiser_best' (resampy 0.2) on the GPU, bit for bit
+    (include/wun.h wun_resample): `x` a contiguous float32 CUDA tensor [n, C], C 1 or 2.  Returns `x` itself when the rates
+    are equal, as librosa does; raises ValueError when the input is too short to give one output frame."""
+    import torch
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2 and x.shape[1] in (1, 2), \
+        "x must be a contiguous float32 CUDA tensor [n, 1 or 2]"
+    sr_in, sr_out = int(sr_in), int(sr_out)
+    if sr_in <= 0 or sr_out <= 0:
+        raise ValueError("resample: sample rates must be positive (got %d, %d)" % (sr_in, sr_out))
+    if sr_in == sr_out:
+        return x
+    n_in, nchan = (int(s) for s in x.shape)
+    if int(n_in * (float(sr_out) / sr_in)) < 1:
+        raise ValueError("resample: an input of %d frames is too short to resample from %d to %d Hz" % (n_in, sr_in, sr_out))
+    dev = x.device
+    key = (str(dev), sr_in, sr_out)
+    tables = _resample_tables.get(key)
+    if tables is None:
+        tables = tuple(torch.from_numpy(t).to(dev) for t in resample_tables(sr_in, sr_out))
+        _resample_tables[key] = tables
+    win, delta = tables
+    n_out = resample_frames(n_in, sr_in, sr_out)
+    y = torch.empty((n_out, nchan), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        rc = lib.wun_resample(x.data_ptr(), n_in, nchan, sr_in, sr_out, win.data_ptr(), delta.data_ptr(), win.numel(),
+                              KAISER_BEST_PRECISION, y.data_ptr(), n_out, Engine._stream(dev))
+    if rc != WUN_OK:
+        raise WunError(rc, "wun_resample failed")
+    return y
 
 
 _UPSAMPLING = {"linear": 0, "learned": 1}
