@@ -735,9 +735,10 @@ static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale,
             const WgGroup& G = U.grp[g];
             char line[512];
             snprintf(line, sizeof(line), "wgrad layer=%d group=%d Cp=%d Cg=%d swap=%d NT=%d mtiles=%d ntiles=%d ntaps=%d taps_per_cta=%d "
-                     "tapsets=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu",
+                     "tapsets=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu issued_macs=%lld useful_macs=%lld",
                      h->cur_layer, g, G.P.C, G.G.C, G.swap, G.NT, G.n_mtiles, G.n_ntiles, G.ntaps, G.taps_per_cta, G.n_tapsets,
-                     G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages, umma_wgrad_smem_bytes(U));
+                     G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages, umma_wgrad_smem_bytes(U),
+                     umma_wgrad_issued_macs(G, U.batch), (long long)U.batch * G.chunks_per_batch * 64 * G.ntaps * G.P.C * G.G.C);
             h->audit->push_back(line);
         }
     }

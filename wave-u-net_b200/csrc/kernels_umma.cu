@@ -654,7 +654,8 @@ cudaError_t launch_plane_conv_umma(const UmmaLaunch& L, cudaStream_t stream, con
 // no-swizzle operand the 8x8 core matrix is 8 rows (K) x 16 B, K groups LBO = 128 B apart, channel atoms SBO = atom-plane
 // stride apart.  A tap is again a start-address shift (d rows * 16 B) of the P side.
 // grid = (batch * chunks_per_batch / chunks_per_cta, n_mtiles * n_ntiles, tap sets of all groups).  Warps 0-7: two
-// warpgroups over the 128-channel M tile (64 each), accumulators taps x NT in registers; warps 8..: the stage producer.
+// warpgroups, each owning one 64-channel M block of the 128-channel tile and a subset of the CTA's taps (wgrad_body),
+// accumulators taps x NT in registers; warps 8..: the stage producer.
 // ------------------------------------------------------------------------------------------------
 constexpr int kWgRK = 64;          // rows per pipeline stage
 constexpr int kWgSpan = 16;        // extra P rows per stage (max tap shift span)
@@ -664,6 +665,35 @@ constexpr int kWgAccCols = 256;    // accumulator columns (taps x NT) per warpgr
 constexpr int kWgConvThreads = 128;                 // converter-fed kernel: 4 converter warps
 constexpr int kWgSmemMax = 200 * 1024;
 constexpr int kWgSlotFloats = 128 * kWgAccCols;     // one CTA's partial tile: [tap][128 M rows][NT]
+
+// Taps one CTA (and so one warpgroup) holds accumulators for: as many NT-column tiles as 128 registers per thread take, at most
+// a group's kWgMaxTaps.
+constexpr __host__ __device__ int wgrad_max_taps(int NT) { return kWgAccCols / NT < kWgMaxTaps ? kWgAccCols / NT : kWgMaxTaps; }
+
+// The MMAs of one 64-row chunk for one warpgroup: nt taps (0 <= nt <= T), 4 k16 steps x 3 MMAs per tap, committed as one group.
+// As in conv_step_mmas, every tap count gets its own straight-line sequence, so that wait_group 1 after the chunk really keeps
+// this chunk in flight instead of retiring all its taps but the last.  offA / offB: per tap, the byte shift of each operand.
+template <int NT, int T>
+__device__ __forceinline__ void wgrad_chunk_mmas(int nt, float* acc, uint32_t sa, uint32_t sb, uint32_t planeA, uint32_t planeB,
+                                                 const uint32_t* offA, const uint32_t* offB) {
+    if constexpr (T > 0) {
+        if (nt < T) { wgrad_chunk_mmas<NT, T - 1>(nt, acc, sa, sb, planeA, planeB, offA, offB); return; }
+    }
+    constexpr uint32_t atomsA = 16, atomsB = NT / 8;
+#pragma unroll
+    for (int t = 0; t < T; ++t) {
+#pragma unroll
+        for (int ks = 0; ks < kWgRK / 16; ++ks) {
+            const uint32_t a = sa + offA[t] + 256u * ks, bb = sb + offB[t] + 256u * ks;
+            const uint64_t a_hi = gmma_desc(a, 128, planeA), a_lo = gmma_desc(a + atomsA * planeA, 128, planeA);
+            const uint64_t b_hi = gmma_desc(bb, 128, planeB), b_lo = gmma_desc(bb + atomsB * planeB, 128, planeB);
+            wgmma_tile<NT, 1>(acc + t * (NT / 2), a_lo, b_hi);
+            wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_lo);
+            wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_hi);
+        }
+    }
+    wgmma_commit();
+}
 
 template <bool BULK, int NT>
 __device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSplit* S) {
@@ -795,34 +825,34 @@ __device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSpl
     }
 
     // ===================== MMA warpgroups =====================
-    constexpr int TMAX = kWgAccCols / NT;        // >= taps_per_cta (umma_plan_wgrad)
+    constexpr int TMAX = wgrad_max_taps(NT);     // >= taps_per_cta (umma_plan_wgrad)
     constexpr int NACC = TMAX * NT / 2;
-    const int wg = warp >> 2;
+    // warp-uniform for the compiler: an MMA operand it thinks may diverge makes it serialize the MMAs
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
+    // What this warpgroup owns: a tile whose two 64-channel M blocks both hold real channels gives block wg to warpgroup wg, with
+    // all the CTA's taps; a tile with one such block (an M side of <= 64 channels, or the last block of a 144-channel side) gives
+    // that block to both warpgroups and splits the taps between them.  No warpgroup multiplies a block of padding.
+    const bool tsplit = SA.C - ca0 <= 64;
+    const int th = (ntap + 1) >> 1;
+    const int wt0 = (tsplit && wg) ? th : 0;                  // first of this warpgroup's taps, relative to tap0
+    const int wnt = tsplit ? (wg ? ntap - th : th) : ntap;   // its tap count (0 for warpgroup 1 of a one-tap tile split)
+    const int mrow0 = tsplit ? 0 : 64 * wg;                  // its first M row in the tile
+    uint32_t offA[TMAX], offB[TMAX];                         // per tap: the row shift (16 B per row) of the P side's operand
+#pragma unroll
+    for (int t = 0; t < TMAX; ++t) {
+        const uint32_t shift = t < wnt ? 16u * (uint32_t)(Gp.d[tap0 + wt0 + t] - dmin) : 0u;
+        offA[t] = swap ? 0u : shift;
+        offB[t] = swap ? shift : 0u;
+    }
     float acc[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
     for (int ci = 0; ci < nchunks; ++ci) {
         const int st = ci % nst;
         mbar_wait(BAR(FULL + st), (ci / nst) & 1);
-        const uint32_t sa = smem_u32(smem + st * stage_bytes) + (uint32_t)(8 * wg) * planeA, sb = smem_u32(smem + st * stage_bytes) + bytesA;
+        const uint32_t sa = smem_u32(smem + st * stage_bytes) + (uint32_t)(mrow0 / 8) * planeA, sb = smem_u32(smem + st * stage_bytes) + bytesA;
         wgmma_fence();
-#pragma unroll
-        for (int t = 0; t < TMAX; ++t) {
-            if (t < ntap) {
-                const uint32_t shift = 16u * (uint32_t)(Gp.d[tap0 + t] - dmin);          // rows * 16 B
-                const uint32_t sha = swap ? 0u : shift, shb = swap ? shift : 0u;
-#pragma unroll
-                for (int ks = 0; ks < kWgRK / 16; ++ks) {
-                    const uint32_t a = sa + sha + 256u * ks, bb = sb + shb + 256u * ks;
-                    const uint64_t a_hi = gmma_desc(a, 128, planeA), a_lo = gmma_desc(a + atomsA * planeA, 128, planeA);
-                    const uint64_t b_hi = gmma_desc(bb, 128, planeB), b_lo = gmma_desc(bb + atomsB * planeB, 128, planeB);
-                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_lo, b_hi);
-                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_lo);
-                    wgmma_tile<NT, 1>(acc + t * (NT / 2), a_hi, b_hi);
-                }
-            }
-        }
-        wgmma_commit();
+        wgrad_chunk_mmas<NT, TMAX>(wnt, acc, sa, sb, planeA, planeB, offA, offB);
         // chunk ci stays in flight while the next stage is awaited: only chunk ci - 1 has surely finished reading its stage
         wgmma_wait<1>();
         if (ci > 0) mbar_arrive(BAR(EMPTY + (ci - 1) % nst));
@@ -830,16 +860,17 @@ __device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSpl
     wgmma_wait<0>();
     acc_fence<NACC>(acc);
     // ===================== epilogue: accumulators -> partial tile (or reductions into dW) =====================
+    // A tap-split tile leaves rows [64, 128) of its slot unwritten: they are channels >= SA.C, which the reduction skips.
     if (L.partial) {
         const int tiles = Gp.n_mtiles * Gp.n_ntiles;
         float* part = L.partial + (size_t)(Gp.slot0 + (tapset * tiles + (int)blockIdx.y) * Gp.n_ctas_x + (int)blockIdx.x) * kWgSlotFloats;
 #pragma unroll
         for (int t = 0; t < TMAX; ++t) {
-            if (t >= ntap) break;
+            if (t >= wnt) break;
 #pragma unroll
             for (int i = 0; i < NT / 2; i += 2) {
-                const int row = 64 * wg + acc_row(i, warp, lane), col = acc_col(i, lane);
-                *reinterpret_cast<float2*>(part + (size_t)(t * 128 + row) * NT + col) =
+                const int row = mrow0 + acc_row(i, warp, lane), col = acc_col(i, lane);
+                *reinterpret_cast<float2*>(part + (size_t)((wt0 + t) * 128 + row) * NT + col) =
                     make_float2(acc[t * (NT / 2) + i] * L.scale, acc[t * (NT / 2) + i + 1] * L.scale);
             }
         }
@@ -848,11 +879,11 @@ __device__ __forceinline__ void wgrad_body(const UmmaWgradLaunch& L, const WgSpl
     const int sM = swap ? L.w_sg : L.w_sp, sN = swap ? L.w_sp : L.w_sg;
 #pragma unroll
     for (int t = 0; t < TMAX; ++t) {
-        if (t >= ntap) break;
-        float* dst_t = L.dW + Gp.woff[tap0 + t];
+        if (t >= wnt) break;
+        float* dst_t = L.dW + Gp.woff[tap0 + wt0 + t];
 #pragma unroll
         for (int i = 0; i < NT / 2; ++i) {
-            const int m = ca0 + 64 * wg + acc_row(i, warp, lane), n = cb0 + acc_col(i, lane);
+            const int m = ca0 + mrow0 + acc_row(i, warp, lane), n = cb0 + acc_col(i, lane);
             if (m < SA.C && n < SB.C) atomicAdd(dst_t + (long long)m * sM + (long long)n * sN, acc[t * (NT / 2) + i] * L.scale);
         }
     }
@@ -881,9 +912,20 @@ static size_t wgrad_smem_bytes(const UmmaWgradLaunch& L) {
 
 size_t umma_wgrad_smem_bytes(const UmmaWgradLaunch& L) { return wgrad_smem_bytes(L); }
 
+// N tiles of an N side of Cn channels: at most 128 wide, 16-multiples
+static void wgrad_ntiles(int Cn, int* nt, int* ntiles) {
+    *nt = (Cn + 15) / 16 * 16;
+    *ntiles = 1;
+    while (*nt > 128) { *ntiles *= 2; *nt = ((Cn + *ntiles - 1) / *ntiles + 15) / 16 * 16; }
+}
+
+long long umma_wgrad_issued_macs(const WgGroup& G, int batch) {
+    const int Cm = G.swap ? G.G.C : G.P.C;
+    return (long long)batch * G.chunks_per_batch * kWgRK * G.ntaps * (64LL * ((Cm + 63) / 64)) * G.NT * G.n_ntiles;
+}
+
 bool umma_plan_wgrad(UmmaWgradLaunch* L) {
     if (L->ngroups < 1 || L->ngroups > kWgMaxGroups) return false;
-    int NT = 16;               // one N-tile width for all groups: one kernel instantiation per launch
     for (int gi = 0; gi < L->ngroups; ++gi) {
         WgGroup& G = L->grp[gi];
         const int Cp = G.P.C, Cg = G.G.C;
@@ -894,25 +936,30 @@ bool umma_plan_wgrad(UmmaWgradLaunch* L) {
         for (int t = 1; t < G.ntaps; ++t) { dmin = min(dmin, G.d[t]); dmax = max(dmax, G.d[t]); }
         if (dmax - dmin > kWgSpan) return false;
         if (G.m_hi <= G.m_lo) return false;
-        G.swap = (Cg > Cp) ? 1 : 0;                       // the wider side fills the 128-channel M dimension
-        const int Cm = G.swap ? Cg : Cp, Cn = G.swap ? Cp : Cg;
+        G.chunks_per_batch = (G.m_hi - G.m_lo + kWgRK - 1) / kWgRK;
+    }
+    // The wider side fills M.  Putting the narrower side on M when that issues fewer MMAs (down2: Cp 48 on one M block, Cg 72
+    // in N tiles of 80) measured slower on H100: the wider NT leaves room for fewer taps per CTA, so more tap sets re-stage the
+    // same rows (down2's wgrad kernel 393 -> 454 us).
+    int NT = 16;               // one N-tile width for all groups: one kernel instantiation per launch
+    for (int gi = 0; gi < L->ngroups; ++gi) {
+        WgGroup& G = L->grp[gi];
+        G.swap = (G.G.C > G.P.C) ? 1 : 0;
+        const int Cm = G.swap ? G.G.C : G.P.C, Cn = G.swap ? G.P.C : G.G.C;
         G.n_mtiles = (Cm + 127) / 128;
-        int nt = (Cn + 15) / 16 * 16;
-        G.n_ntiles = 1;
-        while (nt > 128) { G.n_ntiles *= 2; nt = ((Cn + G.n_ntiles - 1) / G.n_ntiles + 15) / 16 * 16; }
+        int nt;
+        wgrad_ntiles(Cn, &nt, &G.n_ntiles);
         NT = max(NT, nt);
     }
     long long work = 0;        // ~MMA work units of the launch, to size the K ranges
     for (int gi = 0; gi < L->ngroups; ++gi) {
         WgGroup& G = L->grp[gi];
         G.NT = NT;
-        int tpc = kWgAccCols / NT;                        // the accumulators of all taps of a CTA live in registers
-        if (tpc > kWgMaxTaps) tpc = kWgMaxTaps;
+        int tpc = wgrad_max_taps(NT);                     // the accumulators of all taps of a CTA live in registers
         if (tpc > G.ntaps) tpc = G.ntaps;
         G.n_tapsets = (G.ntaps + tpc - 1) / tpc;
         tpc = (G.ntaps + G.n_tapsets - 1) / G.n_tapsets;   // balance
         G.taps_per_cta = tpc;
-        G.chunks_per_batch = (G.m_hi - G.m_lo + kWgRK - 1) / kWgRK;
         work += (long long)L->batch * G.chunks_per_batch * G.n_tapsets * G.n_mtiles * G.n_ntiles;
     }
     // K range per CTA: the launch should be ONE full wave (1 CTA per SM): every CTA runs concurrently and pays the dW

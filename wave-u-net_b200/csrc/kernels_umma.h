@@ -83,7 +83,7 @@ struct WgGroup {
     // tiling (filled by umma_plan_wgrad)
     int swap;               // 0: A (M side) = P, B (N side) = G;  1: A = G, B = P
     int NT;                 // N-tile width (multiple of 16, <= 128; the same for every group of a launch)
-    int n_mtiles, n_ntiles; // tiles of 128 / NT channels
+    int n_mtiles, n_ntiles; // tiles of 128 / NT channels (a CTA's M tile: two 64-channel blocks, one per warpgroup)
     int taps_per_cta, n_tapsets;
     int chunks_per_batch;   // 64-row chunks per batch element
     int chunks_per_cta;     // consecutive (batch-folded) chunks one CTA reduces
@@ -156,6 +156,8 @@ constexpr int kWgOverreachG = 64, kWgOverreachP = 64 + 16;
 
 // fills the tiling fields (groups' P, G, taps and the common fields already set); false = not eligible
 bool umma_plan_wgrad(UmmaWgradLaunch* L);
+// MACs a planned group issues at `batch` (every 64-row chunk, tap, 64-channel M block with a real channel and N tile)
+long long umma_wgrad_issued_macs(const WgGroup& G, int batch);
 
 // Output layer fused into the epilogue of the last up block's forward conv: the 1x1 output convs over [crop(mix) || features]
 // (OutputLayer.py:8,15), the activation, the difference source (:17-22), the test-time clip, the MSE loss (Training.py:50-63) and
