@@ -208,6 +208,34 @@ int64_t wun_resample_frames(int64_t n_in, int64_t sr_in, int64_t sr_out);
 int wun_resample(const float* x, int64_t n_in, int64_t nchan, int64_t sr_in, int64_t sr_out, const double* win,
                  const double* delta, int64_t nwin, int64_t precision, float* y, int64_t n_out, void* stream);
 
+/* --- validation / test loss (no handle) -----------------------------------------------------------
+ * The data path of the reference's Test.test (Test.py:57-79) over a partition pool laid out as wun_feed_batch's.
+ *
+ * wun_snippet_batch: one evaluation batch, no augmentation (Datasets.py:21-25 take_all_snippets, :207 crop_sample).
+ *   pool         DEVICE float32 [num_sources + 1][total_frames][nchan]: sources in source_names order, then the mix
+ *   positions    DEVICE int64 [n_positions]: absolute pool frame of every snippet start, n_positions a multiple of batch
+ *   batch_state  DEVICE int64[1]: batch counter; batch i = counter mod (n_positions / batch) reads positions[i * batch ..];
+ *                advanced by one by this call (on the stream), so the call can sit inside a captured CUDA graph
+ *   mix_out      DEVICE float32 [batch][input_frames][nchan]: the recorded mix
+ *   targets_out  DEVICE float32 [num_sources][batch][output_frames][nchan]: the centre output_frames of every source
+ *                ((input_frames - output_frames) / 2 frames cut at the front), the layout wun_forward returns
+ * Pure data movement: the outputs are copies of pool values, bit for bit.
+ *
+ * wun_eval_batch_loss: curr = sum_k mean((targets[k] - outputs[k])^2) / num_sources in float64, then the running mean
+ * state[0] += (1 / state[1]') * (curr - state[0]) with state[1]' = state[1] + 1 (Test.py:76).
+ *   outputs, targets  DEVICE float32 [num_sources][n]      state  DEVICE float64[2] {total, n}, {0, 0} before a partition
+ *   batch_loss        optional DEVICE float64[1] receiving curr
+ *   workspace         DEVICE, 8-byte aligned, >= num_sources * WUN_EVAL_LOSS_CTAS * 8 bytes (per-CTA partial sums)
+ * The grid and every reduction order are fixed, so the same inputs give the same bits on every call and on every GPU.
+ * Both functions: WUN_E_INVALID on a bad argument; enqueued on `stream`; no allocation, no synchronisation; they do not set
+ * wun_last_error(). */
+#define WUN_EVAL_LOSS_CTAS 264
+int wun_snippet_batch(const float* pool, int64_t total_frames, int64_t num_sources, int64_t nchan, int64_t input_frames,
+                      int64_t output_frames, const int64_t* positions, int64_t n_positions, int64_t batch,
+                      int64_t* batch_state, float* mix_out, float* targets_out, void* stream);
+int wun_eval_batch_loss(const float* outputs, const float* targets, int64_t num_sources, int64_t n, double* state,
+                        double* batch_loss, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

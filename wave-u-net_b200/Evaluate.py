@@ -11,8 +11,9 @@ is split over the ranks (no collective on the data path, results all-gathered at
 predict_track works on arrays already at model_config["expected_sr"]; predict() is the reference's predict() (Evaluate.py:
 60-71) on an array at any rate, resampling on the GPU with librosa's kaiser_best (wun.resample) on the way in and out.
 Scoring is here: evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS
-Eval v4 on the GPU (wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).  Audio decoding
-beyond WAV (Predict.py) and musdb loading are out of scope (SURVEY section 2).
+Eval v4 on the GPU (wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).
+produce_musdb_source_estimates runs them over the MUSDB18 WAV layout.  Audio decoding beyond WAV (Predict.py) and the musdb
+package are out of scope (SURVEY section 2).
 """
 import glob
 import json
@@ -134,6 +135,40 @@ def load_separator(model_config, load_model):
         import TFCheckpoint
         TFCheckpoint.restore_separator(load_model, separator, int(in_shape[1]), with_optimizer=False)
     return separator
+
+
+def produce_musdb_source_estimates(model_config, load_model, musdb_path, output_path, subsets=None):
+    """The reference's produce_musdb_source_estimates (Evaluate.py:147-159) over the MUSDB18 WAV layout: every track of
+    `subsets` (both, as mus.run(subsets=None) does) is separated at its own rate with predict(), scored against its stems,
+    and written as musdb and museval would: float32 WAV estimates in <output_path>/<subset>/<track>/<source>.wav and the BSS
+    Eval JSON in <output_path>/<subset>/<track>.json (Datasets.estimate_path / museval_json_dir).  The reference
+    accompaniment is bass + drums + other, unclipped.  With torch.distributed every rank separates its share of the windows
+    and rank 0 writes."""
+    import Datasets
+    from Predict import read_wav, write_wav
+    print("Evaluating trained model saved at " + str(load_model) + " on MUSDB and saving source estimate audio to "
+          + str(output_path))
+    rank, _ = parallel.world()
+    separator = load_separator(model_config, load_model)
+    for subset in (subsets or Datasets.MUSDB_SUBSETS):
+        for track in Datasets.musdb_tracks(musdb_path, subset):
+            rate, mix = read_wav(track["mix"])
+            if mix.shape[1] == 1 and not model_config["mono_downmix"]:
+                raise ValueError("%s is mono: a stereo model's estimates cannot be scored against it (MUSDB18 is stereo)"
+                                 % track["mix"])
+            refs = OrderedDict((s, read_wav(track[s])[1]) for s in Datasets.MUSDB_STEMS)
+            acc = refs[Datasets.ACCOMPANIMENT_STEMS[0]]
+            for s in Datasets.ACCOMPANIMENT_STEMS[1:]:
+                acc = acc + refs[s]
+            refs["accompaniment"] = acc
+            results_dir = Datasets.museval_json_dir(output_path, subset) if rank == 0 else None
+            preds = predict(model_config, separator, mix, rate, references=refs, results_dir=results_dir,
+                            track_name=track["name"])
+            if rank == 0:
+                for name, audio in preds.items():
+                    path = Datasets.estimate_path(output_path, subset, track["name"], name)
+                    os.makedirs(os.path.dirname(path), exist_ok=True)
+                    write_wav(path, audio, rate)
 
 
 def produce_source_estimates(model_config, load_model, mix_audio, separator=None):

@@ -1,0 +1,72 @@
+"""The reference's Test.test (Test.py:11-93): the mean MSE of a model over every snippet of a partition.
+
+    loss = Test.test(model_config, "valid", model_folder, load_model, dataset=ds, separator=sep)
+
+Snippets start every T_out frames (take_all_snippets, Datasets.py:21-25), the mix is the recorded mixture, the targets are
+centre-cropped, batches of model_config["batch_size"] cross track boundaries and the last incomplete batch is dropped.  Per
+batch, curr = sum_k mean((target_k - estimate_k)^2) / K with the forward in test mode (output clip on), and the result is
+the running mean total += (1 / n) * (curr - total) (Test.py:57-79).
+
+On the device: one CUDA graph of wun_snippet_batch -> wun_forward -> wun_eval_batch_loss, replayed once per batch; the
+batch counter and the fp64 running mean live on the device, so the partition costs one host synchronisation, at the end,
+and gives the same bits on every run.  The reference's test_loss TensorBoard summary is not written.
+"""
+import numpy as np
+
+
+def test(model_config, partition, model_folder, load_model, dataset=None, separator=None):
+    """Running-mean MSE over the full batches of `partition` ("valid" or "test") of `dataset` (a Datasets.Dataset; staged
+    from model_config["musdb_path"] when None), with `separator` or else the variables of checkpoint `load_model`.
+    Raises ValueError when the partition has fewer snippets than one batch."""
+    import torch
+    import Datasets
+    import Evaluate
+    import wun
+    if model_config["network"] != "unet":
+        raise NotImplementedError
+    if separator is None:
+        separator = Evaluate.load_separator(model_config, load_model)
+    B = int(model_config["batch_size"])
+    in_shape, out_shape = separator.get_padding(np.array([B, model_config["num_frames"], 0]))
+    t_in, t_out = int(in_shape[1]), int(out_shape[1])
+    if dataset is None:
+        dataset = Datasets.load_musdb(model_config, t_in, t_out)
+    assert (dataset.t_in, dataset.t_out) == (t_in, t_out), "the dataset was staged for other input / output lengths"
+    pool = dataset.partitions[partition].pool
+    positions = dataset.positions(partition, B)
+    n_batches = positions.numel() // B
+    dev = pool.device
+    eng = separator.engine(input_frames=t_in)
+    separator._ensure_params(eng, dev, create=False)
+    K, C = len(model_config["source_names"]), int(pool.shape[2])
+    print("Testing...")
+
+    counter = torch.zeros(1, dtype=torch.int64, device=dev)
+    mix = torch.empty((B, t_in, C), dtype=torch.float32, device=dev)
+    targets = torch.empty((K, B, t_out, C), dtype=torch.float32, device=dev)
+    outputs = torch.empty_like(targets)
+    state = torch.zeros(2, dtype=torch.float64, device=dev)
+    slots = torch.empty(K * wun.EVAL_LOSS_CTAS, dtype=torch.float64, device=dev)
+
+    def batch():
+        wun.snippet_batch(pool, positions, B, counter, mix, targets)
+        eng.forward(separator.params, mix, False, out=outputs)
+        wun.eval_batch_loss(outputs, targets, state, slots)
+
+    with torch.cuda.device(dev):
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(dev)                # a graph is captured on a stream other than the default one
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            batch()                                  # batch 0 eagerly: the engine sets up its workspace outside the capture
+            if n_batches > 1:
+                graph = torch.cuda.CUDAGraph()
+                graph.capture_begin()
+                batch()
+                graph.capture_end()
+                for _ in range(n_batches - 1):
+                    graph.replay()
+        cur.wait_stream(side)
+        total = float(state[0].item())
+    print("Finished testing - Mean MSE: " + str(total))
+    return total

@@ -12,9 +12,14 @@ train()    one "epoch" of model_config["epoch_it"] steps (reference :103-109): e
            "separator/..." variables, Adam slots and global_step, as the reference's Saver does (:98,113).
 optimise() early stopping on a validation loss + fine-tuning stage with doubled batch and lr 1e-5 (:123-150).
 
-The MUSDB/CCMixter TFRecord pipeline (Datasets.py) is out of scope; batches come from `batch_source`, by default the
-synthetic generator of SURVEY 8(d) (uniform sources, random gains as Utils.random_amplify :26-36, centre-cropped
-targets as Utils.crop_sample :38-42).
+By default batches come from `batch_source`, by default the synthetic generator of SURVEY 8(d) (uniform sources, random
+gains as Utils.random_amplify :26-36, centre-cropped targets as Utils.crop_sample :38-42).  Training on real music is
+opt-in with a top-level extra:
+
+    python Training.py with cfg.full model_config.musdb_path=/data/musdb18 dataset=musdb [ccmixter_xml=...] [valid_tracks=N]
+
+which stages the MUSDB18 WAV dataset on the device (Datasets.py), validates with Test.test, returns the best checkpoint's
+test loss and writes its estimates and BSS Eval JSONs (Evaluate.produce_musdb_source_estimates), as the reference does.
 """
 import os
 import sys
@@ -73,12 +78,21 @@ def _to_device(batch, names, device):
     return mix, tg
 
 
-def _device_feeder(model_config, sep, eng, device, rank, world, local_batch):
+def _device_feeder(model_config, sep, eng, device, rank, world, local_batch, dataset=None):
     """The training data source when none is given: synthetic tracks resident in HBM + wun.feeder.DeviceFeeder (snippet
     sampling, random_amplify, centre crop in ONE kernel per batch: Datasets.py:196-214 / Utils.py:26-42 on the device).
-    Built once per separator and input length, re-used by every later epoch; rank r draws its own shard of the batch."""
+    Built once per separator and input length, re-used by every later epoch; rank r draws its own shard of the batch.
+    With `dataset` (a Datasets.Dataset) the feeder draws from its staged train partition instead."""
     from wun.feeder import DeviceFeeder, synthetic_tracks
     key = (eng.T_in, local_batch, str(device), bool(model_config["augmentation"]))
+    if dataset is not None:
+        key += (id(dataset),)
+        if getattr(sep, "_feeder_key", None) != key:
+            sep.last_feeder_tracks = None
+            sep.last_feeder = dataset.train_feeder(eng, local_batch, augmentation=model_config["augmentation"],
+                                                   seed=1337 + 7919 * rank)
+            sep._feeder_key = key
+        return sep.last_feeder
     if getattr(sep, "_feeder_key", None) != key:
         tracks = synthetic_tracks(model_config["source_names"], model_config["num_channels"], 8,
                                   (eng.T_in + 1 + eng.T_in // 4, 2 * eng.T_in), seed=4321)
@@ -89,10 +103,12 @@ def _device_feeder(model_config, sep, eng, device, rank, world, local_batch):
     return sep.last_feeder
 
 
-def train(model_config, experiment_id, load_model=None, batch_source=None, sep=None, device=None, log_every=100, feeder=None):
+def train(model_config, experiment_id, load_model=None, batch_source=None, sep=None, device=None, log_every=100, feeder=None,
+          dataset=None):
     """One epoch (reference train(), :24-121).  Returns (checkpoint path, separator).
     Data: `batch_source` (an iterator of host numpy batches, e.g. SyntheticBatches) if given; otherwise, on a CUDA device,
-    the device-side feeder (`feeder="device"`, the default there); `feeder="host"` forces the numpy generator."""
+    the device-side feeder (`feeder="device"`, the default there); `feeder="host"` forces the numpy generator.  With
+    `dataset` (a Datasets.Dataset) the device-side feeder draws from its train partition."""
     import torch
     rank, world = parallel.world()
     if device is None:
@@ -117,8 +133,10 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
     if batch_source is None and feeder != "host" and device.type == "cuda":
         lo, hi = parallel.shard_range(global_batch, rank, world)
         local_batch = hi - lo
-        dev_feeder = _device_feeder(model_config, sep, eng, device, rank, world, local_batch)
+        dev_feeder = _device_feeder(model_config, sep, eng, device, rank, world, local_batch, dataset)
     elif batch_source is None:
+        if dataset is not None:
+            raise ValueError("training on a dataset needs the device-side feeder on a CUDA device")
         batch_source = SyntheticBatches(model_config, in_shape, out_shape, seed=1337 + sep.global_step)
     running, t0 = 0.0, time.time()
     # N > 1: the gradient all-reduce runs bucketed on a communication stream while backward still computes
@@ -163,8 +181,13 @@ def validation_loss(model_config, sep, batches=4, seed=99):
     return tot / n
 
 
-def optimise(model_config, experiment_id, max_epochs=None):
-    """Early stopping + fine-tuning (reference optimise(), :123-150)."""
+def optimise(model_config, experiment_id, max_epochs=None, dataset=None):
+    """Early stopping + fine-tuning (reference optimise(), :123-150).  Without `dataset`: synthetic batches, validated by
+    validation_loss, returns (best checkpoint, its validation loss).  With `dataset` (a Datasets.Dataset): trained on its
+    train partition, validated by Test.test on "valid" at the current batch size, and, as the reference does, returns
+    (best checkpoint, Test.test of that checkpoint on "test")."""
+    if dataset is not None:
+        return _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset)
     epoch, best_loss, model_path, best_model_path, sep = 0, 10000, None, None, None
     for i in range(2):
         worse_epochs = 0
@@ -189,7 +212,66 @@ def optimise(model_config, experiment_id, max_epochs=None):
     return best_model_path, best_loss
 
 
-def run(cfg, max_epochs=None):
+def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset):
+    import Test
+    rank, world = parallel.world()
+    epoch, best_loss, model_path, best_model_path, best_step, sep = 0, 10000, None, None, None, None
+    for i in range(2):
+        worse_epochs = 0
+        if i == 1:
+            print("Finished first round of training, now entering fine-tuning stage")
+            model_config["batch_size"] *= 2
+            model_config["init_sup_sep_lr"] = 1e-5
+        while worse_epochs < model_config["worse_epochs"]:
+            if max_epochs is not None and epoch >= max_epochs:
+                break
+            print("EPOCH: " + str(epoch))
+            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, dataset=dataset)
+            # every rank evaluates the whole partition; the loss has the same bits on every rank, so they all take the
+            # same early-stopping decision without a collective
+            curr_loss = Test.test(model_config, "valid", str(experiment_id), model_path, dataset=dataset, separator=sep)
+            epoch += 1
+            if curr_loss < best_loss:
+                worse_epochs = 0
+                print("Performance on validation set improved from " + str(best_loss) + " to " + str(curr_loss))
+                best_model_path, best_loss, best_step = model_path, curr_loss, sep.global_step
+            else:
+                worse_epochs += 1
+                print("Performance on validation set worsened to " + str(curr_loss))
+    if best_step is None:
+        raise RuntimeError("no epoch was trained, so there is no checkpoint to test")
+    # only rank 0 writes checkpoints (train()); every rank knows the best one's path from its global step
+    best_model_path = os.path.join(model_config["model_base_dir"], str(experiment_id), "%s-%d" % (experiment_id, best_step))
+    if world > 1:
+        import torch.distributed as dist
+        dist.barrier()
+    print("TRAINING FINISHED - TESTING WITH BEST MODEL " + best_model_path)
+    test_loss = Test.test(model_config, "test", str(experiment_id), best_model_path, dataset=dataset)
+    return best_model_path, test_loss
+
+
+def dataset_options(extras):
+    """The dataset extras of the command line: dataset=musdb [ccmixter_xml=<path>] [valid_tracks=N].  Returns the keyword
+    arguments of run(); no dataset= gives {} (synthetic training, as without the extras)."""
+    if "dataset" not in extras:
+        unused = [k for k in ("ccmixter_xml", "valid_tracks") if k in extras]
+        if unused:
+            raise ValueError("%s need dataset=musdb" % ", ".join(unused))
+        return {}
+    if extras["dataset"] != "musdb":
+        raise ValueError("dataset=%r: only dataset=musdb (the MUSDB18 WAV layout) is supported" % (extras["dataset"],))
+    opts = {"dataset": "musdb", "valid_tracks": int(extras.get("valid_tracks", 25))}
+    if extras.get("ccmixter_xml") is not None:
+        opts["ccmixter_xml"] = str(extras["ccmixter_xml"])
+    return opts
+
+
+def run(cfg, max_epochs=None, dataset=None, ccmixter_xml=None, valid_tracks=25):
+    """The reference's run() (:152-166).  With dataset="musdb" the MUSDB18 WAV dataset at model_config["musdb_path"] (and
+    CCMixter's tracks for the voice task, from `ccmixter_xml`) is staged on the device once, trained and validated on,
+    and the best checkpoint's estimates and BSS Eval JSONs are written under model_config["estimates_path"]."""
+    if dataset is not None:
+        return _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks)
     model_config = cfg["model_config"]
     print("SCRIPT START")
     for d in [model_config["model_base_dir"], model_config["log_dir"]]:
@@ -204,6 +286,32 @@ def run(cfg, max_epochs=None):
     return sup_model_path, sup_loss
 
 
+def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks):
+    import torch
+    import Datasets
+    import Evaluate
+    if dataset != "musdb":
+        raise ValueError("dataset=%r: only dataset=musdb is supported" % (dataset,))
+    model_config = cfg["model_config"]
+    print("SCRIPT START")
+    for d in [model_config["model_base_dir"], model_config["log_dir"]]:
+        os.makedirs(d, exist_ok=True)
+    if "WORLD_SIZE" in os.environ and int(os.environ["WORLD_SIZE"]) > 1:
+        import torch.distributed as dist
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
+        dist.init_process_group("nccl")
+    device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
+    probe = UnetAudioSeparator(model_config)
+    in_shape, out_shape = probe.get_padding(np.array([model_config["batch_size"], model_config["num_frames"], 0]))
+    ds = Datasets.load_musdb(model_config, int(in_shape[1]), int(out_shape[1]), model_config["musdb_path"], ccmixter_xml,
+                             valid_tracks, device)
+    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, dataset=ds)
+    print("Supervised training finished! Saved model at " + str(sup_model_path) + ". Performance: " + str(sup_loss))
+    Evaluate.produce_musdb_source_estimates(model_config, sup_model_path, model_config["musdb_path"],
+                                            model_config["estimates_path"])
+    return sup_model_path, sup_loss
+
+
 if __name__ == "__main__":
     cfg, extras = Config.parse_command_line(sys.argv[1:])
-    run(cfg, max_epochs=extras.get("max_epochs"))
+    run(cfg, max_epochs=extras.get("max_epochs"), **dataset_options(extras))

@@ -20,6 +20,7 @@ SYMBOLS = [
     "wun_gather_windows", "wun_scatter_windows", "wun_feed_batch", "wun_last_error", "wun_version", "wun_describe",
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
     "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_resample_frames", "wun_resample",
+    "wun_snippet_batch", "wun_eval_batch_loss",
 ]
 
 
@@ -96,6 +97,9 @@ def _load():
         lib.wun_resample_frames.argtypes = [I64, I64, I64]
         lib.wun_resample_frames.restype = I64
         lib.wun_resample.argtypes = [VP, I64, I64, I64, I64, VP, VP, I64, I64, VP, I64, VP]
+    if hasattr(lib, "wun_snippet_batch"):   # likewise the validation-loss kernels
+        lib.wun_snippet_batch.argtypes = [VP, I64, I64, I64, I64, I64, VP, I64, I64, VP, VP, VP, VP]
+        lib.wun_eval_batch_loss.argtypes = [VP, VP, I64, I64, VP, VP, VP, I64, VP]
     return lib
 
 
@@ -235,6 +239,65 @@ def resample(x, sr_in, sr_out):
     if rc != WUN_OK:
         raise WunError(rc, "wun_resample failed")
     return y
+
+
+EVAL_LOSS_CTAS = 264        # include/wun.h WUN_EVAL_LOSS_CTAS
+
+
+def _check_f32(name, t, dim):
+    import torch
+    assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == dim, \
+        "%s must be a contiguous float32 CUDA tensor with %d dimensions" % (name, dim)
+
+
+def snippet_batch(pool, positions, batch, batch_state, mix_out, targets_out):
+    """One evaluation batch cut out of a partition pool (include/wun.h wun_snippet_batch): `pool` float32 [K + 1, frames, C]
+    (sources, then the mix), `positions` int64 [n_batches * batch] absolute snippet frames, `batch_state` int64 [1] the batch
+    counter the call advances, `mix_out` [batch, T_in, C] and `targets_out` [K, batch, T_out, C] (centre crop).  All contiguous
+    CUDA tensors on one device; the call is enqueued on its current stream."""
+    import torch
+    _check_f32("pool", pool, 3)
+    _check_f32("mix_out", mix_out, 3)
+    _check_f32("targets_out", targets_out, 4)
+    for name, t in (("positions", positions), ("batch_state", batch_state)):
+        assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous(), "%s must be a contiguous int64 CUDA tensor" % name
+    dev = pool.device
+    assert all(t.device == dev for t in (positions, batch_state, mix_out, targets_out)), "tensors on different devices"
+    K, C = int(pool.shape[0]) - 1, int(pool.shape[2])
+    t_in, t_out = int(mix_out.shape[1]), int(targets_out.shape[2])
+    assert tuple(mix_out.shape) == (batch, t_in, C), ("mix_out shape", tuple(mix_out.shape))
+    assert tuple(targets_out.shape) == (K, batch, t_out, C), ("targets_out shape", tuple(targets_out.shape))
+    with torch.cuda.device(dev):
+        rc = lib.wun_snippet_batch(pool.data_ptr(), int(pool.shape[1]), K, C, t_in, t_out, positions.data_ptr(),
+                                   positions.numel(), int(batch), batch_state.data_ptr(), mix_out.data_ptr(),
+                                   targets_out.data_ptr(), Engine._stream(dev))
+    if rc != WUN_OK:
+        raise WunError(rc, "wun_snippet_batch failed (K %d, C %d, T_in %d, T_out %d, %d positions, batch %d)"
+                       % (K, C, t_in, t_out, positions.numel(), batch))
+
+
+def eval_batch_loss(outputs, targets, state, workspace, batch_loss=None):
+    """Test.test's per-batch loss and running mean on the device (include/wun.h wun_eval_batch_loss): `outputs` and
+    `targets` float32 [K, ...] of one shape; `state` float64 [2] {total, n}, updated in place; `workspace` float64 with at
+    least K * EVAL_LOSS_CTAS elements; `batch_loss` optional float64 [1] receiving this batch's loss."""
+    import torch
+    assert outputs.is_cuda and outputs.dtype == torch.float32 and outputs.is_contiguous(), "outputs: contiguous float32 CUDA"
+    assert targets.shape == outputs.shape and targets.dtype == torch.float32 and targets.is_contiguous(), "targets must match outputs"
+    for name, t in (("state", state), ("workspace", workspace), ("batch_loss", batch_loss)):
+        if t is not None:
+            assert t.is_cuda and t.dtype == torch.float64 and t.is_contiguous(), "%s must be a contiguous float64 CUDA tensor" % name
+    dev = outputs.device
+    assert all(t.device == dev for t in (targets, state, workspace) + ((batch_loss,) if batch_loss is not None else ())), \
+        "tensors on different devices"
+    assert state.numel() == 2, "state is {total, n}"
+    K = int(outputs.shape[0])
+    with torch.cuda.device(dev):
+        rc = lib.wun_eval_batch_loss(outputs.data_ptr(), targets.data_ptr(), K, outputs.numel() // K, state.data_ptr(),
+                                     batch_loss.data_ptr() if batch_loss is not None else None, workspace.data_ptr(),
+                                     workspace.numel() * 8, Engine._stream(dev))
+    if rc != WUN_OK:
+        raise WunError(rc, "wun_eval_batch_loss failed (K %d, %d elements, workspace %d doubles)"
+                       % (K, outputs.numel(), workspace.numel()))
 
 
 _UPSAMPLING = {"linear": 0, "learned": 1}

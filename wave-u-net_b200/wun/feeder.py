@@ -44,13 +44,27 @@ class DeviceFeeder(object):
         import torch
         if not torch.cuda.is_available():
             raise RuntimeError("DeviceFeeder needs a CUDA device: the feeder has no host fallback")
+        pool, offsets, lengths = build_pool(tracks, list(source_names))
+        self._setup(engine, torch.from_numpy(pool).to(torch.device(device)), offsets, lengths, source_names, batch,
+                    augmentation, seed, record_choice)
+
+    @classmethod
+    def from_pool(cls, engine, pool, offsets, lengths, source_names, batch, augmentation=True, seed=1337, record_choice=False):
+        """A feeder over an already staged device pool (Datasets.stage_partition): `pool` a float32 CUDA tensor
+        [K + 1, total_frames, C], `offsets` / `lengths` int64 arrays of the tracks to draw from (each > T_in frames)."""
+        self = cls.__new__(cls)
+        self._setup(engine, pool, np.asarray(offsets, np.int64), np.asarray(lengths, np.int64), source_names, batch,
+                    augmentation, seed, record_choice)
+        return self
+
+    def _setup(self, engine, pool, offsets, lengths, source_names, batch, augmentation, seed, record_choice):
+        import torch
         self.eng, self.batch, self.augmentation, self.seed = engine, int(batch), bool(augmentation), int(seed)
         self.source_names = list(source_names)
-        pool, offsets, lengths = build_pool(tracks, self.source_names)
-        if int(lengths.min()) <= engine.T_in:
+        if len(lengths) == 0 or int(lengths.min()) <= engine.T_in:
             raise ValueError("every track needs more than T_in = %d frames (Datasets.py:18 draws start < length - T_in)" % engine.T_in)
-        self.device = torch.device(device)
-        self.pool = torch.from_numpy(pool).to(self.device)
+        self.device = pool.device
+        self.pool = pool
         self.track_offset = torch.from_numpy(offsets).to(self.device)
         self.track_length = torch.from_numpy(lengths).to(self.device)
         K, C = len(self.source_names), pool.shape[2]
