@@ -319,7 +319,12 @@ Acc decode(const std::string& name, void** args, bool* known) {
         a.plane(V, *static_cast<const int*>(args[1]), V.r_lo, V.r_hi);
         a.flat('A', *static_cast<float* const*>(args[4]), 4LL * V.C);
     } else if (has(name, "output_fwd_kernel")) {
-        decode_output(a, *static_cast<const OutputLaunch*>(args[0]), true, true);
+        const OutputLaunch& O = *static_cast<const OutputLaunch*>(args[0]);
+        decode_output(a, O, true, true);
+        if (O.targets && O.loss) {                                      // per-CTA loss sums + the CTA counter of their fixed-order total
+            a.flat('W', O.loss_part, 4 * (((long long)O.batch * O.T_out + 127) / 128));
+            a.flat('A', O.loss_count, 4);
+        }
     } else if (has(name, "output_dgrad_kernel")) {
         const OutputLaunch& O = *static_cast<const OutputLaunch*>(args[0]);
         decode_output(a, O, true, false);
@@ -351,7 +356,12 @@ Acc decode(const std::string& name, void** args, bool* known) {
         a.flat('R', U.x, 4LL * U.batch * U.N * U.C);
         a.flat('W', U.gx, 4LL * U.batch * U.N * U.C);
         if (U.blend) a.flat('R', U.blend, 4LL * U.C);
-        if (U.dvar) a.flat('A', U.dvar, 4LL * U.C);
+        if (U.dvar) {
+            a.flat('A', U.dvar, 4LL * U.C);
+            // per-CTA sums [item * row chunks][C] + the CTA counter of their fixed-order total (rows_per_cta: set by the launcher)
+            a.flat('W', U.part, 4LL * U.batch * ((U.N + U.rows_per_cta - 1) / U.rows_per_cta) * U.C);
+            a.flat('A', U.count, 4);
+        }
     } else if (has(name, "sigmoid_kernel")) {
         const int n = *static_cast<const int*>(args[2]);
         a.flat('R', *static_cast<const float* const*>(args[0]), 4LL * n);

@@ -1,7 +1,9 @@
 // harness.cu - runs ONE plane-convolution launch or ONE layer's weight gradient, given as text in the format
-// wun_debug_launches writes (engine.cu export_launch / conv_wgrad), through the product's own planner and launchers.
-// Test infrastructure (tests/test_kernels_gpu.py): linked with the product's kernel sources into libwun_kernels.so, never
-// loaded by the product.
+// wun_debug_launches writes (engine.cu export_launch / conv_wgrad), through the product's own planner and launchers; and
+// ONE launch of the step's other kernels (first layer, output layer, upsampling backward, sigmoid, Adam, window gather /
+// scatter) on buffers the caller passes.
+// Test infrastructure (tests/test_kernels_gpu.py, tests/test_step_kernels_gpu.py): linked with the product's kernel sources into
+// libwun_kernels.so, never loaded by the product.
 //
 // Addresses in a description are offsets from the fake bases of the dry run (workspace 1 << 40, parameters 1 << 41, mix
 // 1 << 42; -1 = null); the harness moves them onto the device buffers the caller passes.  The wgrad lines' dW / db are
@@ -298,6 +300,134 @@ int wkh_run_wgrad(const char* desc, void* ws, void* par, void* mix, float* grads
         if (e == cudaSuccess) e = launch_wgrad_reduce(U, J, s);
         return (int)e;
     } catch (const std::string& e) { g_err = e; return -1; } catch (const std::exception& e) { g_err = e.what(); return -1; }
+}
+
+// ---- the step's other launches (kernels_first.cu, kernels_simt.cu): each through the product's own launcher ----------------------
+// Geometry comes as an array of integers (the fields of the engine's `first` / `output` / `upsample` export lines), buffers as
+// device pointers; partial-sum arenas must be at least as long as the product's own size functions say.
+
+long long wkh_first_partial_bytes(int batch) { return (long long)first_wgrad_partial_bytes(batch); }
+int wkh_first_supported(int C, int N, int k) { return first_layer_supported(C, N, k) ? 1 : 0; }
+
+// g: C, N, k, pad_left, batch, x_bstride, T, dec_bstride, Td, odd_bstride, mo_lo, mo_hi
+static bool first_from(const long long* g, const float* x, float* dec, float* odd, const float* W, const float* bias, FirstLayer* F,
+                       int* C, int* N) {
+    memset(F, 0, sizeof(*F));
+    *C = (int)g[0]; *N = (int)g[1];
+    F->k = (int)g[2]; F->pad_left = (int)g[3]; F->batch = (int)g[4];
+    F->x = x; F->x_bstride = g[5]; F->T = (int)g[6];
+    F->dec = dec; F->dec_bstride = g[7]; F->Td = (int)g[8];
+    F->odd = odd; F->odd_bstride = g[9]; F->mo_lo = (int)g[10]; F->mo_hi = (int)g[11];
+    F->W = W; F->bias = bias;
+    if (!first_layer_supported(*C, *N, F->k)) { g_err = "first layer shape not supported"; return false; }
+    return true;
+}
+
+int wkh_first_fwd(const long long* g, const float* x, float* dec, float* odd, const float* W, const float* bias, void* stream) {
+    FirstLayer F;
+    int C, N;
+    if (!first_from(g, x, dec, odd, W, bias, &F, &C, &N)) return -1;
+    launch_first_fwd(F, C, N, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_first_wgrad(const long long* g, const float* x, float* gdec, float* godd, float* dW, float* db, float scale, float* part,
+                    long long part_bytes, void* stream) {
+    FirstWgrad P;
+    memset(&P, 0, sizeof(P));
+    int C, N;
+    if (!first_from(g, x, gdec, godd, nullptr, nullptr, &P.L, &C, &N)) return -1;
+    if (part_bytes < (long long)first_wgrad_partial_bytes(P.L.batch)) { g_err = "first-layer partial arena too small"; return -1; }
+    P.dW = dW; P.db = db; P.scale = scale; P.part = part;
+    launch_first_wgrad(P, C, N, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+// g: batch, T_in, Tf, T_out, C, F, nconv, K, ofs, pad_left, crop_feat, crop_out, output_type, activation, training, then w_off[8],
+// b_off[8] (flat parameter offsets)
+static void output_from(const long long* g, float inv_count, const float* params, const float* mix, const float* feat, OutputLaunch* O) {
+    memset(O, 0, sizeof(*O));
+    O->batch = (int)g[0]; O->T_in = (int)g[1]; O->Tf = (int)g[2]; O->T_out = (int)g[3]; O->C = (int)g[4]; O->F = (int)g[5];
+    O->nconv = (int)g[6]; O->K = (int)g[7]; O->ofs = (int)g[8]; O->pad_left = (int)g[9]; O->crop_feat = (int)g[10];
+    O->crop_out = (int)g[11]; O->output_type = (int)g[12]; O->activation = (int)g[13]; O->training = (int)g[14];
+    for (int s = 0; s < 8; ++s) { O->w_off[s] = g[15 + s]; O->b_off[s] = g[23 + s]; }
+    O->inv_count = inv_count; O->params = params; O->mix = mix; O->feat = feat;
+}
+
+// out[0]: output_wgrad_partial_bytes, out[1]: output_loss_partial_bytes
+int wkh_output_partial_bytes(const long long* g, long long* out) {
+    OutputLaunch O;
+    output_from(g, 1.f, nullptr, nullptr, nullptr, &O);
+    out[0] = (long long)output_wgrad_partial_bytes(O);
+    out[1] = (long long)output_loss_partial_bytes(O.batch, O.T_out);
+    return 0;
+}
+
+// loss_count: the CTA counter of the loss sum (0 before; the launch leaves it 0)
+int wkh_output_fwd(const long long* g, float inv_count, const float* params, const float* mix, const float* feat, const float* targets,
+                   float* outputs, float* dpre, float* loss, float* loss_part, long long part_bytes, unsigned* loss_count, void* stream) {
+    OutputLaunch O;
+    output_from(g, inv_count, params, mix, feat, &O);
+    if (O.nconv * O.C > WUN_MAX_OUT_COLS) { g_err = "nconv * C above WUN_MAX_OUT_COLS"; return -1; }
+    if (targets && loss && (!loss_count || part_bytes < (long long)output_loss_partial_bytes(O.batch, O.T_out))) { g_err = "loss needs a counter and a partial arena"; return -1; }
+    O.targets = targets; O.outputs = outputs; O.dpre = dpre; O.loss = loss; O.loss_part = loss_part; O.loss_count = loss_count;
+    launch_output_fwd(O, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_output_dgrad(const long long* g, const float* params, const float* feat, float* dpre, float* gfeat, void* stream) {
+    OutputLaunch O;
+    output_from(g, 1.f, params, nullptr, feat, &O);
+    O.dpre = dpre;
+    launch_output_dgrad(O, gfeat, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_output_wgrad(const long long* g, const float* params, const float* mix, const float* feat, float* dpre, float* grads, float scale,
+                     float* part, long long part_bytes, void* stream) {
+    OutputLaunch O;
+    output_from(g, 1.f, params, mix, feat, &O);
+    O.dpre = dpre;
+    if (part_bytes < (long long)output_wgrad_partial_bytes(O)) { g_err = "output partial arena too small"; return -1; }
+    launch_output_wgrad(O, grads, part, scale, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+long long wkh_upsample_partial_bytes(int batch, int C) { return (long long)upsample_dvar_partial_bytes(batch, C); }
+
+// g: batch, N, nmid, C, mid_mode; count: the CTA counter of the interp-gradient sum (0 before; the launch leaves it 0)
+int wkh_upsample_bwd(const long long* g, const float* due, const float* dmid, const float* x, float* gx, const float* blend, float* dvar,
+                     float scale, float* part, long long part_bytes, unsigned* count, void* stream) {
+    UpsampleBwdLaunch U;
+    memset(&U, 0, sizeof(U));
+    U.batch = (int)g[0]; U.N = (int)g[1]; U.nmid = (int)g[2]; U.C = (int)g[3]; U.mid_mode = (int)g[4];
+    U.due = due; U.dmid = dmid; U.x = x; U.gx = gx; U.blend = blend; U.dvar = dvar; U.scale = scale; U.part = part; U.count = count;
+    if (dvar && (!blend || !count || part_bytes < (long long)upsample_dvar_partial_bytes(U.batch, U.C))) { g_err = "dvar needs blend, a counter and a partial arena"; return -1; }
+    launch_upsample_bwd(U, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_sigmoid(const float* x, float* y, int n, void* stream) {
+    launch_sigmoid(x, y, n, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+// state == null: lr_t as given (folded on the host); else lr_t = lr * sqrt(1 - state[1]) / (1 - state[0]) on the device, then advanced
+int wkh_adam(float* p, const float* g, float* m, float* v, long long n, float lr, float b1, float b2, float eps, float* state, void* stream) {
+    launch_adam(p, g, m, v, n, lr, b1, b2, eps, state, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_gather_windows(const float* padded, long long n_padded, const long long* starts, int n_windows, int T_in, int C, float* out,
+                       void* stream) {
+    launch_gather_windows(padded, n_padded, starts, n_windows, T_in, C, out, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
+}
+
+int wkh_scatter_windows(const float* outs, const long long* starts, int n_windows, int n_sources, int T_out, int C, float* preds,
+                        long long n_frames, void* stream) {
+    launch_scatter_windows(outs, starts, n_windows, n_sources, T_out, C, preds, n_frames, reinterpret_cast<cudaStream_t>(stream));
+    return (int)cudaGetLastError();
 }
 
 }  // extern "C"

@@ -18,7 +18,8 @@ BUILD = os.path.join(HERE, "_build")
 LIB = os.path.join(BUILD, "libwun_kernels.so")
 # WUN_KERNELS_LIB: run the tests against another build of the harness (e.g. one made from modified kernel sources)
 OVERRIDE = os.environ.get("WUN_KERNELS_LIB")
-SOURCES = [os.path.join(HERE, "harness.cu"), os.path.join(CSRC, "kernels_umma.cu"), os.path.join(CSRC, "kernels_simt.cu")]
+SOURCES = [os.path.join(HERE, "harness.cu"), os.path.join(CSRC, "kernels_umma.cu"), os.path.join(CSRC, "kernels_simt.cu"),
+           os.path.join(CSRC, "kernels_first.cu")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 
 
@@ -71,7 +72,56 @@ def _bind(lib):
     lib.wkh_run_wgrad.argtypes = [S, P, P, P, P, ctypes.c_float, ctypes.c_int, P, I64, P]
     for f in (lib.wkh_plan_conv, lib.wkh_plan_wgrad, lib.wkh_run_conv, lib.wkh_run_wgrad):
         f.restype = ctypes.c_int
+    G, F, I = ctypes.POINTER(I64), ctypes.c_float, ctypes.c_int
+    sig = {
+        "wkh_first_partial_bytes": (I64, [I]), "wkh_first_supported": (I, [I, I, I]),
+        "wkh_first_fwd": (I, [G, P, P, P, P, P, P]), "wkh_first_wgrad": (I, [G, P, P, P, P, P, F, P, I64, P]),
+        "wkh_output_partial_bytes": (I, [G, G]), "wkh_output_fwd": (I, [G, F, P, P, P, P, P, P, P, P, I64, P, P]),
+        "wkh_output_dgrad": (I, [G, P, P, P, P, P]), "wkh_output_wgrad": (I, [G, P, P, P, P, P, F, P, I64, P]),
+        "wkh_upsample_partial_bytes": (I64, [I, I]), "wkh_upsample_bwd": (I, [G, P, P, P, P, P, P, F, P, I64, P, P]),
+        "wkh_sigmoid": (I, [P, P, I, P]), "wkh_adam": (I, [P, P, P, P, I64, F, F, F, F, P, P]),
+        "wkh_gather_windows": (I, [P, I64, P, I, I, I, P, P]), "wkh_scatter_windows": (I, [P, P, I, I, I, I, P, I64, P]),
+    }
+    for name, (res, args) in sig.items():
+        if hasattr(lib, name):                   # (a harness built from older sources lacks them: the step-kernel tests fail by name)
+            getattr(lib, name).restype = res
+            getattr(lib, name).argtypes = args
     return lib
+
+
+def geom(values):
+    """A list of integers -> the int64 array the step-kernel entry points take as geometry."""
+    return (ctypes.c_longlong * len(values))(*[int(v) for v in values])
+
+
+FIRST_KEYS = ["C", "N", "k", "pad_left", "batch", "x_bstride", "T", "dec_bstride", "Td", "odd_bstride", "mo_lo", "mo_hi"]
+OUTPUT_KEYS = ["batch", "T_in", "Tf", "T_out", "C", "F", "nconv", "K", "ofs", "pad_left", "crop_feat", "crop_out", "output_type",
+               "activation", "training"]
+UPSAMPLE_KEYS = ["batch", "N", "nmid", "C", "mid_mode"]
+
+
+def first_geom(d):
+    return geom([d[k] for k in FIRST_KEYS])
+
+
+def output_geom(d):
+    return geom([d[k] for k in OUTPUT_KEYS] + [d["w_off%d" % s] for s in range(8)] + [d["b_off%d" % s] for s in range(8)])
+
+
+def upsample_geom(d):
+    return geom([d[k] for k in UPSAMPLE_KEYS])
+
+
+def output_partial_bytes(d):
+    """-> (output_wgrad_partial_bytes, output_loss_partial_bytes) of an output-layer geometry."""
+    out = (ctypes.c_longlong * 2)()
+    _check(load().wkh_output_partial_bytes(output_geom(d), out), "wkh_output_partial_bytes")
+    return int(out[0]), int(out[1])
+
+
+def call(name, *args):
+    """Runs one step-kernel entry point (wkh_<name>); raises on a malformed call or a CUDA error."""
+    _check(getattr(load(), "wkh_" + name)(*args), "wkh_" + name)
 
 
 CONV_KEYS = {

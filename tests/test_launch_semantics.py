@@ -76,6 +76,17 @@ def test_exported_launches_cover_the_step():
     for d in L:
         assert len(d["planes"]) == d["launch"]["nplanes"] and len(d["cls"]) == d["launch"]["ncls"]
         assert all(0 <= t["plane"] < d["launch"]["nplanes"] for t in d["terms"])
+    # the step's other launches: the dedicated first layer, the output layer, one upsampling backward per level, Adam
+    kinds = [k for k, _ in eng.step_launches]
+    assert kinds.count("first") == 1 and kinds.count("output") == 1 and kinds.count("adam") == 1
+    ups = [d for k, d in eng.step_launches if k == "upsample"]
+    assert len(ups) == 3 and all(d["dvar"] == -1 for d in ups)                  # linear upsampling: no interp gradient
+    cfg = Config.build_config(["full"], dict(num_layers=3), experiment_id=0)["model_config"]
+    t_in, _ = O.get_padding(cfg, 300)
+    eng = wun.Engine(wun.config_from_model_config(cfg), input_frames=t_in)
+    eng.launch_descriptions(2)
+    ups = [d for k, d in eng.step_launches if k == "upsample"]
+    assert len(ups) == 3 and all(d["dvar"] >= 0 and d["mid_mode"] != 1 for d in ups)      # learned: dvar, never MID_CLAMP
 
 
 def _tensor_view(eng, name, batch, training=True):

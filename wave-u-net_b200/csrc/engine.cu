@@ -124,6 +124,7 @@ struct WunHandle {
     int bucket_next = 0;
     // per-call state
     bool dry = false;
+    bool train_call = false;             // a training step (or its dry run): the CTA counters of the loss sums are zeroed
     int64_t launches = 0;
     cudaStream_t stream = nullptr;
     const float* params = nullptr;
@@ -456,6 +457,18 @@ static int conv_forward(WunHandle* h, const ConvOp& op, int layer_index) {
         FirstLayer F;
         if (first_layer_desc(h, op, &F)) {
             if (h->phase == 1) return WUN_OK;
+            if (h->dry && h->export_launches) {   // wun_debug_launches: the first layer (its weight gradient has the same geometry;
+                char line[768];                   // gdec / godd = the gradient tensors it reads, dW / db = flat parameter offsets)
+                auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
+                const Plan& P = h->plan;
+                snprintf(line, sizeof(line), "first C=%d N=%d k=%d pad_left=%d batch=%d x=%lld x_bstride=%lld T=%d dec=%lld dec_bstride=%lld Td=%d "
+                         "odd=%lld odd_bstride=%lld mo_lo=%d mo_hi=%d gdec=%lld godd=%lld dW=%lld db=%lld",
+                         P.cfg.num_channels, op.cout, F.k, F.pad_left, F.batch, addr(F.x), F.x_bstride, F.T, addr(F.dec), F.dec_bstride, F.Td,
+                         addr(F.odd), F.odd_bstride, F.mo_lo, F.mo_hi, addr(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor])),
+                         addr(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor])), (long long)P.params[op.w_param].offset,
+                         (long long)P.params[op.b_param].offset);
+                h->export_launches->push_back(line);
+            }
             ++h->launches;
             if (!h->dry) launch_first_fwd(F, h->plan.cfg.num_channels, op.cout, h->stream);
             return WUN_OK;
@@ -633,6 +646,9 @@ static int64_t split_arena_half_bytes(const WunHandle* h, int64_t batch) {
 
 static int64_t split_arena_bytes(const WunHandle* h, int64_t batch);
 static float* out_part_ptr(const WunHandle* h);
+static unsigned* counters_ptr(const WunHandle* h);
+static float* loss_part_ptr(const WunHandle* h);
+static float* dvar_part_ptr(const WunHandle* h);
 
 static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale, int layer_index) {
     const Plan& P = h->plan;
@@ -877,6 +893,8 @@ static void fill_output_launch(const WunHandle* h, OutputLaunch* O, const float*
     O->outputs = outputs;
     O->dpre = (h->lay.off[P.t_dpre_out] >= 0) ? const_cast<float*>(tensor_ptr(h, P.t_dpre_out)) : nullptr;
     O->loss = loss;
+    O->loss_part = (loss && !h->dry) ? loss_part_ptr(h) : nullptr;
+    O->loss_count = (loss && !h->dry) ? counters_ptr(h) : nullptr;
     O->batch = h->batch; O->T_in = (int)P.T_in; O->Tf = (int)P.Tf; O->T_out = (int)P.T_out;
     O->C = P.cfg.num_channels; O->F = P.cfg.num_initial_filters;
     O->nconv = P.nconv; O->K = P.cfg.num_sources;
@@ -932,8 +950,25 @@ static int run_forward(WunHandle* h, const float* targets, float* outputs, float
         if (rc != WUN_OK) return rc;
     }
     if (h->out_fused) return WUN_OK;
-    if (h->phase != 1) ++h->launches;
-    if (!h->dry && h->phase != 1) launch_output_fwd(O, h->stream);
+    if (h->dry && h->export_launches) {      // wun_debug_launches: the output layer's geometry (caller buffers: include/wun.h layouts)
+        char line[768];
+        auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
+        int n = snprintf(line, sizeof(line), "output batch=%d T_in=%d Tf=%d T_out=%d C=%d F=%d nconv=%d K=%d ofs=%d pad_left=%d crop_feat=%d "
+                         "crop_out=%d output_type=%d activation=%d feat=%lld dpre=%lld gfeat=%lld",
+                         O.batch, O.T_in, O.Tf, O.T_out, O.C, O.F, O.nconv, O.K, O.ofs, O.pad_left, O.crop_feat, O.crop_out, O.output_type,
+                         O.activation, addr(O.feat), addr(O.dpre), addr(tensor_ptr(h, P.grad_twin[P.t_feat])));
+        for (int s = 0; s < 8; ++s)
+            n += snprintf(line + n, sizeof(line) - n, " w_off%d=%lld b_off%d=%lld", s, s < O.nconv ? O.w_off[s] : -1LL, s,
+                          s < O.nconv ? O.b_off[s] : -1LL);
+        h->export_launches->push_back(line);
+    }
+    if (h->phase != 1) h->launches += h->train_call ? 2 : 1;       // + a training step's memset of the CTA counters
+    if (!h->dry && h->phase != 1) {
+        // the loss and interp-gradient sums count their CTAs here; each sum's last CTA sets its counter back to 0, this makes
+        // sure they start from 0 whatever the workspace held before
+        if (h->train_call) WUN_CUDA_OK(cudaMemsetAsync(counters_ptr(h), 0, 2 * sizeof(unsigned), h->stream));
+        launch_output_fwd(O, h->stream);
+    }
     return WUN_OK;
 }
 
@@ -980,7 +1015,17 @@ static int run_backward(WunHandle* h, const float* targets, float* grads, float 
         U.gx = const_cast<float*>(tensor_ptr(h, P.grad_twin[us.src_tensor]));
         U.blend = (us.wsig_tensor >= 0) ? tensor_ptr(h, us.wsig_tensor) : nullptr;
         U.dvar = (us.interp_param >= 0) ? grads + P.params[us.interp_param].offset : nullptr;
+        U.part = U.dvar ? dvar_part_ptr(h) : nullptr;
+        U.count = U.dvar ? counters_ptr(h) + 1 : nullptr;
         U.batch = h->batch; U.N = us.N; U.nmid = us.nmid; U.C = us.C; U.mid_mode = us.mid_mode; U.scale = scale;
+        if (h->dry && h->export_launches) {  // wun_debug_launches: dvar = the interp parameter's flat offset (gradient buffer) or -1
+            char line[512];
+            auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
+            snprintf(line, sizeof(line), "upsample level=%d batch=%d N=%d nmid=%d C=%d mid_mode=%d due=%lld dmid=%lld x=%lld gx=%lld blend=%lld dvar=%lld",
+                     i, U.batch, U.N, U.nmid, U.C, U.mid_mode, addr(U.due), addr(U.dmid), addr(U.x), addr(U.gx), U.blend ? addr(U.blend) : -1LL,
+                     us.interp_param >= 0 ? (long long)P.params[us.interp_param].offset : -1LL);
+            h->export_launches->push_back(line);
+        }
         if (h->phase != 1) ++h->launches;
         if (!h->dry && h->phase != 1) launch_upsample_bwd(U, h->stream);
     }
@@ -1019,14 +1064,37 @@ static int check_device() {
 static int64_t split_arena_bytes(const WunHandle* h, int64_t batch) {
     return (h && h->bulk_wgrad && h->split_item_bytes) ? 2 * split_arena_half_bytes(h, batch) : 0;     // two halves
 }
-// training scratch behind the activations, the weight packs and the split arena: the first layer's per-CTA gradient sums
+// bytes of the per-CTA sums of the interp gradients: one level at a time, all on the caller's stream (0 without learned upsampling)
+static int64_t dvar_part_bytes(const WunHandle* h, int64_t batch) {
+    int C = 0;
+    for (int i = 0; i < h->plan.cfg.num_layers; ++i)
+        if (h->plan.ups[i].interp_param >= 0) C = std::max(C, h->plan.ups[i].C);
+    return C ? (int64_t)upsample_dvar_partial_bytes((int)batch, C) : 0;
+}
+constexpr int64_t kCounterBytes = 256;     // the CTA counters of the loss and interp-gradient sums: [0] loss, [1] interp
+// training scratch behind the activations, the weight packs and the split arena: the per-CTA sums of the first layer's and the
+// output layer's weight gradients, then the counters and the per-CTA sums of the loss and of the interp gradients (each added up
+// in a fixed order)
 static int64_t train_scratch_bytes(const WunHandle* h, int64_t batch) {
-    return split_arena_bytes(h, batch) + (int64_t)first_wgrad_partial_bytes((int)batch) + (int64_t)h->out_part_bytes;
+    return split_arena_bytes(h, batch) + (int64_t)first_wgrad_partial_bytes((int)batch) + (int64_t)h->out_part_bytes + kCounterBytes +
+           (int64_t)output_loss_partial_bytes((int)batch, (int)h->plan.T_out) + dvar_part_bytes(h, batch);
 }
 // the output layer's per-CTA weight-gradient sums, behind the first layer's
 static float* out_part_ptr(const WunHandle* h) {
     return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum + split_arena_bytes(h, h->batch) +
                                     first_wgrad_partial_bytes(h->batch));
+}
+// the counters (zeroed at the start of every training step's output layer), behind the output layer's gradient sums
+static unsigned* counters_ptr(const WunHandle* h) {
+    return reinterpret_cast<unsigned*>(reinterpret_cast<uint8_t*>(out_part_ptr(h)) + h->out_part_bytes);
+}
+// the per-CTA loss sums, behind the counters (counters and sums are used on the caller's stream only)
+static float* loss_part_ptr(const WunHandle* h) {
+    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(counters_ptr(h)) + kCounterBytes);
+}
+// the per-CTA interp-gradient sums, behind the loss sums (used on the caller's stream only)
+static float* dvar_part_ptr(const WunHandle* h) {
+    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(loss_part_ptr(h)) + output_loss_partial_bytes(h->batch, (int)h->plan.T_out));
 }
 
 static int begin_call(WunHandle* h, const float* params, const float* mix, int64_t batch, bool training, void* ws,
@@ -1035,6 +1103,7 @@ static int begin_call(WunHandle* h, const float* params, const float* mix, int64
     if (batch < 1 || batch > (1 << 20)) return set_err(WUN_E_INVALID, "batch out of range");
     h->lay = make_layout(h->plan, batch, training);
     h->dry = dry;
+    h->train_call = training;
     h->launches = 0;
     h->batch = (int)batch;
     h->bw_grads = nullptr; h->bw_scale = 1.f; h->fuse_out = nullptr; h->out_fused = false; h->par_used = 0; h->wg_index = 0; h->first_pending = false;
@@ -1348,6 +1417,7 @@ int64_t wun_debug_launches(const WunHandle* hc, int64_t batch, char* buf, int64_
     h->mix = reinterpret_cast<const float*>((uintptr_t)1 << 42);
     run_forward(h, nullptr, nullptr, nullptr, 1);
     run_backward(h, nullptr, nullptr, 1.f);
+    lines.push_back("adam n=" + std::to_string((long long)h->plan.param_numel));     // wun_adam_step(_device) over the flat buffer
     h->export_launches = nullptr; h->ws = nullptr; h->params = nullptr; h->mix = nullptr;
     h->arena_sum = keep_sum; h->arena_bytes = keep_max; h->kernel_used = keep_used;
     std::string s;

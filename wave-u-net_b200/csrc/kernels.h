@@ -19,6 +19,8 @@ struct OutputLaunch {
     float* outputs;          // [K][B, T_out, C] or null
     float* dpre;             // [B, T_out, nconv*C] (written when targets != null)
     float* loss;             // device scalar accumulator (pre-zeroed) or null
+    float* loss_part;        // with loss: per-CTA loss sums (output_loss_partial_bytes); the last CTA adds them into *loss in a fixed order
+    unsigned* loss_count;    // with loss: CTAs done; 0 before the launch, 0 again after it
     int batch, T_in, Tf, T_out, C, F;
     int nconv, K;            // number of output convs, number of sources
     int ofs, pad_left;
@@ -37,6 +39,8 @@ struct UpsampleBwdLaunch {
     float* gx;               // [B, N, C]   out: gradient wrt the producer's PRE-activation
     const float* blend;      // sigmoid(var) [C] or null (linear: 0.5)
     float* dvar;             // gradient of the interp variable [C] or null
+    float* part;             // with dvar: per-CTA sums (upsample_dvar_partial_bytes); the last CTA adds them into dvar in a fixed order
+    unsigned* count;         // with dvar: CTAs done; 0 before the launch, 0 again after it
     int batch, N, nmid, C;
     int mid_mode;
     float scale;
@@ -73,12 +77,17 @@ void launch_first_wgrad(FirstWgrad P, int C, int N, cudaStream_t stream);
 size_t first_wgrad_partial_bytes(int batch);
 void launch_plane_wgrad_simt(WgradLaunch L, cudaStream_t stream);
 void launch_colsum(const PlaneView& V, int batch, float scale, float* out, cudaStream_t stream);
+// with targets and loss: the last CTA adds the per-CTA sums at L.loss_part into *loss in a fixed order (L.loss_count == 0)
 void launch_output_fwd(const OutputLaunch& L, cudaStream_t stream);
+size_t output_loss_partial_bytes(int batch, int T_out);
 void launch_output_dgrad(const OutputLaunch& L, float* gfeat, cudaStream_t stream);
 // part: the per-CTA sums (output_wgrad_partial_bytes), added into grads in a fixed order by a second kernel
 void launch_output_wgrad(const OutputLaunch& L, float* grads, float* part, float scale, cudaStream_t stream);
 size_t output_wgrad_partial_bytes(const OutputLaunch& L);
+// with dvar: the last CTA adds the per-CTA sums at L.part into dvar in a fixed order (L.count == 0)
 void launch_upsample_bwd(UpsampleBwdLaunch L, cudaStream_t stream);
+// bytes of UpsampleBwdLaunch::part for C channels at `batch` (any N)
+size_t upsample_dvar_partial_bytes(int batch, int C);
 void launch_sigmoid(const float* x, float* y, int n, cudaStream_t stream);
 void launch_adam(float* p, const float* g, float* m, float* v, long long n, float lr_t, float b1, float b2,
                  float eps, float* state, cudaStream_t stream);

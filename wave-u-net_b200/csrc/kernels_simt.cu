@@ -469,13 +469,44 @@ __global__ void __launch_bounds__(128) output_fwd_kernel(const __grid_constant__
                 }
             }
     }
-    if (L.targets) {
-        __shared__ float red[4];
+    if (L.targets && L.loss) {
+        // every CTA stores its sum; the CTA that finishes last adds all of them in a fixed order (thread t: sums t, t + 128, ...,
+        // then a fixed tree) with one += into *loss - the same bits on every run, unlike float atomics from the CTAs
+        __shared__ float red[128];
+        __shared__ bool last;
         for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
         if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = lsum;
         __syncthreads();
-        if (threadIdx.x == 0) atomicAdd(L.loss, (red[0] + red[1] + red[2] + red[3]) * L.inv_count);
+        if (threadIdx.x == 0) {
+            L.loss_part[blockIdx.x] = (red[0] + red[1] + red[2] + red[3]) * L.inv_count;
+            __threadfence();
+            last = atomicAdd(L.loss_count, 1u) == gridDim.x - 1;
+        }
+        __syncthreads();
+        if (last) {
+            float s = 0.f;
+            for (unsigned i0 = threadIdx.x; i0 < gridDim.x; i0 += 512) {           // 4 loads in flight, added in order
+                float v[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) v[u] = (i0 + 128 * u < gridDim.x) ? __ldcg(L.loss_part + i0 + 128 * u) : 0.f;
+#pragma unroll
+                for (int u = 0; u < 4; ++u) s += v[u];
+            }
+            red[threadIdx.x] = s;
+            for (int h = 64; h > 0; h >>= 1) {
+                __syncthreads();
+                if (threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+            }
+            if (threadIdx.x == 0) {
+                *L.loss += red[0];
+                *L.loss_count = 0u;                  // ready for the next launch
+            }
+        }
     }
+}
+
+size_t output_loss_partial_bytes(int batch, int T_out) {
+    return (size_t)(((long long)batch * T_out + 127) / 128) * sizeof(float) + 256;
 }
 
 void launch_output_fwd(const OutputLaunch& L, cudaStream_t stream) {
@@ -628,22 +659,66 @@ __global__ void __launch_bounds__(256) upsample_bwd_kernel(const __grid_constant
         }
     }
     if (L.dvar) {
+        // every CTA stores its sums at slot (item, row chunk) = blockIdx.y; the CTA that finishes last adds the slots of every
+        // channel in a fixed order (thread row ty: slots ty, ty + 8, ..., then the 8 rows in order), applies w(1-w) * scale once
+        // and does one += into dvar - the same bits on every run, unlike float atomics from the CTAs
+        __shared__ bool last;
         red[threadIdx.y][threadIdx.x] = dv;
         __syncthreads();
-        if (threadIdx.y == 0 && c < L.C) {
-            float tot = 0.f;
-            for (int i = 0; i < 8; ++i) tot += red[i][threadIdx.x];
-            const float w = __ldg(L.blend + c);
-            atomicAdd(L.dvar + c, tot * w * (1.f - w) * L.scale);
+        if (threadIdx.y == 0) {
+            if (c < L.C) {
+                float tot = 0.f;
+                for (int i = 0; i < 8; ++i) tot += red[i][threadIdx.x];
+                L.part[(long long)blockIdx.y * L.C + c] = tot;
+            }
+            __threadfence();                     // the slot is visible before this CTA is counted
         }
+        __syncthreads();
+        if (threadIdx.x == 0 && threadIdx.y == 0) last = atomicAdd(L.count, 1u) == gridDim.x * gridDim.y - 1;
+        __syncthreads();
+        if (!last) return;
+        for (int cb = 0; cb < L.C; cb += 32) {
+            const int cc = cb + threadIdx.x;
+            float s = 0.f;
+            if (cc < L.C)
+                for (unsigned y0 = threadIdx.y; y0 < gridDim.y; y0 += 64) {      // 8 loads in flight, added in slot order
+                    float v[8];
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        const unsigned y = y0 + 8 * u;
+                        v[u] = (y < gridDim.y) ? __ldcg(L.part + (long long)y * L.C + cc) : 0.f;
+                    }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) s += v[u];
+                }
+            __syncthreads();
+            red[threadIdx.y][threadIdx.x] = s;
+            __syncthreads();
+            if (threadIdx.y == 0 && cc < L.C) {
+                float tot = 0.f;
+                for (int i = 0; i < 8; ++i) tot += red[i][threadIdx.x];
+                const float w = __ldg(L.blend + cc);
+                L.dvar[cc] += tot * w * (1.f - w) * L.scale;
+            }
+        }
+        if (threadIdx.x == 0 && threadIdx.y == 0) *L.count = 0u;     // ready for the next launch
     }
 }
 
-void launch_upsample_bwd(UpsampleBwdLaunch L, cudaStream_t stream) {
-    long long per = ((long long)L.N * L.batch + 132 * 4 - 1) / (132 * 4);
+static int upsample_rows_per_cta(int N, int batch) {
+    long long per = ((long long)N * batch + 132 * 4 - 1) / (132 * 4);
     if (per < 32) per = 32;
-    if (per > L.N) per = L.N;
-    L.rows_per_cta = (int)per;
+    if (per > N) per = N;
+    return (int)per;
+}
+
+size_t upsample_dvar_partial_bytes(int batch, int C) {
+    // rows_per_cta >= N * batch / 528 or >= 32 > N * batch / 528 or = N: at most 528 + batch CTAs along y
+    return (size_t)(132 * 4 + batch) * C * sizeof(float) + 256;
+}
+
+void launch_upsample_bwd(UpsampleBwdLaunch L, cudaStream_t stream) {
+    L.rows_per_cta = upsample_rows_per_cta(L.N, L.batch);
     const int chunks = (L.N + L.rows_per_cta - 1) / L.rows_per_cta;
     dim3 grid((L.C + 31) / 32, chunks * L.batch), block(32, 8);
     upsample_bwd_kernel<<<grid, block, 0, stream>>>(L);

@@ -396,17 +396,21 @@ class Engine(object):
 
     def launch_descriptions(self, batch):
         """Every plane-convolution launch of a training step at `batch` as a list of dicts {"launch": {...}, "planes": [...],
-        "cls": [...], "terms": [...]} (wun_debug_launches; host only)."""
+        "cls": [...], "terms": [...]} (wun_debug_launches; host only).  The same dry run also leaves the weight-gradient groups in
+        self.wgrad_groups and the step's other launches in self.step_launches: [(kind, {...})] with kind "first" (first layer,
+        forward and weight gradient), "output" (output layer), "upsample" (one per up level) or "adam"."""
         n = lib.wun_debug_launches(self._h, int(batch), None, 0)
         if n < 0:
             raise RuntimeError("wun_debug_launches failed: %s" % lib.wun_last_error().decode())
         buf = ctypes.create_string_buffer(int(n))
         lib.wun_debug_launches(self._h, int(batch), buf, n)
-        out, wg = [], []
+        out, wg, step = [], [], []
         for line in buf.value.decode().splitlines():
             parts = line.split()
             d = {k: int(v) for k, v in (kv.split("=", 1) for kv in parts[1:])}
-            if parts[0] == "launch":
+            if parts[0] in ("first", "output", "upsample", "adam"):
+                step.append((parts[0], d))
+            elif parts[0] == "launch":
                 out.append({"launch": d, "planes": [], "cls": [], "terms": []})
             elif parts[0] == "wgrad":
                 wg.append({"wgrad": d, "plane": None, "dpre": None, "terms": []})
@@ -417,6 +421,7 @@ class Engine(object):
             else:
                 out[-1][{"plane": "planes", "cls": "cls", "term": "terms"}[parts[0]]].append(d)
         self.wgrad_groups = wg          # the weight-gradient (class, plane) groups of the same dry run
+        self.step_launches = step
         return out
 
     def layer_kernel(self, layer, pass_):
