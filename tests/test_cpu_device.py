@@ -63,12 +63,18 @@ def run_steps(named, overrides, batch, nf, env=None, grad_scale=1.0):
 def assert_matches_oracle(res):
     assert res["unknown"] == []
     assert res["footprint_miss"] == [], res["footprint_miss"][:3]     # (only populated under HOSTSIM_POISON=1, see below)
+    assert_steps_match_oracle(res)
+
+
+def assert_steps_match_oracle(res, loss_tol=1e-5, grad_tol=1e-4, out_tol=1e-5):
+    """The bars of two training steps with Adam and the inference calls.  tests/test_configurations_gpu.py holds the GPU to the
+    same checks with the wider loss / gradient / output bars of the fp32 tensor-core arithmetic."""
     for step in ("step1", "step2"):
         r = res[step]
-        assert r["loss_rel"] < 1e-5, (step, r)
+        assert r["loss_rel"] < loss_tol, (step, r)
         ex = r.get("grad_explained")           # None, or the LeakyReLU-slope-flip proof for a gradient that is off (run_cpu_step.py)
-        assert r["grad_worst_rel"] < 1e-4 or (ex and ex["flips"] is not None and ex["worst_after"] < 1e-4), (step, r)
-        assert r["outputs_rel"] < 1e-5, (step, r)
+        assert r["grad_worst_rel"] < grad_tol or (ex and ex["flips"] is not None and ex["worst_after"] < grad_tol), (step, r)
+        assert r["outputs_rel"] < out_tol, (step, r)
         assert r["params_rel"] < 1e-5 and r["adam_slots_rel"] < 1e-4, (step, r)
     assert res["infer_outputs_rel"] < 1e-4, res["infer_outputs_rel"]
     assert res["train_mode_outputs_rel"] < 1e-4, res["train_mode_outputs_rel"]

@@ -761,15 +761,24 @@ FULL = [("M1_full", ["baseline"], {}, 1, None, {}), ("M4_full", ["baseline_stere
 REPLAYS = MID + FORCED + FULL
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("name,named,ov,batch,nf,env", REPLAYS, ids=[r[0] for r in REPLAYS])
-def test_replayed_launches_match_float64(name, named, ov, batch, nf, env, monkeypatch):
-    import torch
-    _gpu_lib()
+def set_env(monkeypatch, env):
+    """Only the WUN_ switches of `env` are set for the test."""
     for k in [k for k in os.environ if k.startswith("WUN_")]:
         monkeypatch.delenv(k)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
+
+
+# Device bytes a replay holds per workspace word at its peak: the float32 workspace, its copy from before the launch, the
+# expected-bits copy, two float64 copies (reference and ref_abs) and the output index list.
+REPLAY_BYTES_PER_WORD = 4 + 4 + 4 + 8 + 8 + 8
+
+
+def replay_conv_and_wgrad(name, named, ov, batch, nf, prefix="replay "):
+    """Runs every conv / dgrad launch and every layer's weight gradient the engine emits for one configuration at `batch` alone,
+    on random workspace contents, against the float64 interpreter (bound TAU, every word outside the views unchanged).  The
+    kernel families are reported as `prefix` + family.  Returns the number of launches replayed."""
+    import torch
     cfg = Config.build_config(named, ov, experiment_id=0)["model_config"]
     t_in, _ = O.get_padding(cfg, nf or cfg["num_frames"])
     eng = wun.Engine(wun.config_from_model_config(cfg), input_frames=t_in)
@@ -779,6 +788,9 @@ def test_replayed_launches_match_float64(name, named, ov, batch, nf, env, monkey
         layers[G["wgrad"]["layer"]].append(G)
     margin = 1 << 16
     n_ws = eng.workspace_bytes(batch, True) // 4 + 2 * margin
+    need = REPLAY_BYTES_PER_WORD * n_ws
+    free = torch.cuda.mem_get_info()[0]
+    assert need < 0.9 * free, "%s: the replay needs %.1f GB of device memory, %.1f GB are free" % (name, need / 1e9, free / 1e9)
     gen = torch.Generator(device="cuda").manual_seed(7)
     ws_full = torch.randn(n_ws, device="cuda", generator=gen)
     ws = ws_full[margin:]
@@ -811,7 +823,7 @@ def test_replayed_launches_match_float64(name, named, ov, batch, nf, env, monkey
         rabs = mem["ws"][out_t]
         bad = ~(err <= TAU * rabs)
         assert not bad.any(), (name, D["launch"]["layer"], D["launch"]["pass"], int(bad.sum()))
-        fam = "replay " + ("wgmma " if kernel == 0 else "simt ") + ("dgrad" if D["launch"]["pass"] else "fwd")
+        fam = prefix + ("wgmma " if kernel == 0 else "simt ") + ("dgrad" if D["launch"]["pass"] else "fwd")
         nz = rabs > 0
         if nz.any():
             WORST[fam] = max(WORST[fam], float((err[nz] / rabs[nz]).max()))
@@ -840,13 +852,22 @@ def test_replayed_launches_match_float64(name, named, ov, batch, nf, env, monkey
         err = (grads[out].double() - ref[out]).abs()
         bad = ~(err <= TAU * rabs[out])
         assert not bad.any(), (name, layer, "wgrad", int(bad.sum()))
-        fam = "replay wgrad"
+        fam = prefix + ("wgrad" if mode != 3 else "simt wgrad")
         nz = rabs[out] > 0
         if nz.any():
             WORST[fam] = max(WORST[fam], float((err[nz] / rabs[out][nz]).max()))
         COUNTS[fam] += 1
         ran += 1
     assert ran > 0
+    return ran
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,named,ov,batch,nf,env", REPLAYS, ids=[r[0] for r in REPLAYS])
+def test_replayed_launches_match_float64(name, named, ov, batch, nf, env, monkeypatch):
+    _gpu_lib()
+    set_env(monkeypatch, env)
+    replay_conv_and_wgrad(name, named, ov, batch, nf)
 
 
 @pytest.mark.gpu

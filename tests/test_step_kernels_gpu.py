@@ -880,38 +880,43 @@ def _engine(named, ov, batch, nf):
     return eng
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("name,named,ov,batch,nf,env", REPLAYS, ids=[r[0] for r in REPLAYS])
-def test_replayed_step_launches_match_float64(name, named, ov, batch, nf, env, monkeypatch):
+def replay_step_launches(name, named, ov, batch, nf, adam=True, prefix="replay "):
+    """Runs every first-layer, output-layer, upsampling-backward and (with `adam`) Adam launch the engine emits for one
+    configuration at `batch` on random buffers of the exported geometry, against float64.  The kernel families are reported as
+    `prefix` + family.  Returns the exported step launches."""
     torch = _torch()
-    _gpu_lib()
-    for k in [k for k in os.environ if k.startswith("WUN_")]:
-        monkeypatch.delenv(k)
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
     eng = _engine(named, ov, batch, nf)
     kinds = [k for k, _ in eng.step_launches]
     assert kinds.count("output") == 1 and kinds.count("adam") == 1
     for i, (kind, d) in enumerate(eng.step_launches):
         if kind == "first":
             G = dict(d, name="%s_first" % name)
-            run_first_fwd(G, "float", 20 + i, family="replay first fwd")
-            run_first_wgrad(G, "float", 40 + i, scale=1.0, family="replay first wgrad")
+            run_first_fwd(G, "float", 20 + i, family=prefix + "first fwd")
+            run_first_wgrad(G, "float", 40 + i, scale=1.0, family=prefix + "first wgrad")
         elif kind == "output":
             G = dict(d, name="%s_output" % name, training=1)
             n = 16
             for s in range(8):
                 n = max(n, d["w_off%d" % s] + d["ofs"] * (d["C"] + d["F"]) * d["C"] + 8, d["b_off%d" % s] + d["C"] + 8)
             G["n_params"] = n
-            run_output_fwd(G, "float", 60, family="replay output fwd")
-            run_output_dgrad(G, "float", 61, family="replay output dgrad")
-            run_output_wgrad(G, "float", 62, scale=1.0, family="replay output wgrad")
+            run_output_fwd(G, "float", 60, family=prefix + "output fwd")
+            run_output_dgrad(G, "float", 61, family=prefix + "output dgrad")
+            run_output_wgrad(G, "float", 62, scale=1.0, family=prefix + "output wgrad")
         elif kind == "upsample":
             G = dict(d, name="%s_up%d" % (name, d["level"]))
-            run_upsample(G, "float", 80 + i, d["dvar"] >= 0, scale=1.0, family="replay upsample bwd")
-        elif kind == "adam" and batch == 1 and name.startswith("M"):
-            run_adam(d["n"], 99, True, family="replay adam")
+            run_upsample(G, "float", 80 + i, d["dvar"] >= 0, scale=1.0, family=prefix + "upsample bwd")
+        elif kind == "adam" and adam:
+            run_adam(d["n"], 99, True, family=prefix + "adam")
     torch.cuda.synchronize()
+    return eng.step_launches
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,named,ov,batch,nf,env", REPLAYS, ids=[r[0] for r in REPLAYS])
+def test_replayed_step_launches_match_float64(name, named, ov, batch, nf, env, monkeypatch):
+    _gpu_lib()
+    K.set_env(monkeypatch, env)
+    replay_step_launches(name, named, ov, batch, nf, adam=batch == 1 and name.startswith("M"))
 
 
 # ------------------------------------------------------------------------------------------------
