@@ -5,6 +5,7 @@
 // (the reference has no backward source; the derivation is in DESIGN.md "Backward").
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stdarg.h>
 #include <stdlib.h>
 #include <stdio.h>
 #include <string.h>
@@ -51,28 +52,61 @@ struct Layout {
 
 }  // namespace
 
+// The streams a launch record goes to: the caller's; ST_SIDE: weight-gradient kernels (and a training step's weight packs) run
+// on an internal side stream, concurrently with the dgrad chain on the caller's stream; ST_SPLIT: the split passes (see
+// WunHandle::split_ahead); ST_HELPER: a dgrad with two launches (the up blocks: skip pair and upsampled pair have different
+// widths) runs the second one on this helper stream, concurrently with the first: both read the same gradient planes and write
+// different tensors, and in the deep layers neither fills the GPU (WUN_DGRAD_PAR=0 disables)
+enum StreamRole : uint8_t { ST_CALLER, ST_SIDE, ST_SPLIT, ST_HELPER };
+// Event pools.  EV_PAR: fork / join pairs, one pair per use inside a call (graph capture needs distinct events); EV_PACK: one
+// event per FORWARD weight pack, so that forward conv i waits for pack i only instead of for all ~60 packs of the step (the
+// backward convs still wait for the single EV_PACKS event; WUN_PACK_EVENTS=0 disables); EV_FIRST_DONE: first-layer weight
+// gradient on the split stream; EV_BUCKET: bucket k is recorded once every gradient of the bucket is final
+enum EventPool : uint8_t { EV_NONE, EV_FORK, EV_PAR, EV_SPLIT_DONE, EV_WG_DONE, EV_PACK, EV_JOIN, EV_PACKS, EV_FIRST_DONE, EV_BUCKET,
+                           kEventPools };
+
+enum OpKind : uint8_t {
+    OP_SIGMOID, OP_FIRST_FWD, OP_CONV, OP_PACK, OP_UMMA_CONV, OP_COUNTERS, OP_OUTPUT_FWD, OP_OUTPUT_WGRAD, OP_OUTPUT_DGRAD,
+    OP_UPSAMPLE_BWD, OP_FIRST_WGRAD, OP_COLSUM, OP_WGRAD, OP_WGRAD_UMMA, OP_SPLIT, OP_WGRAD_BULK, OP_WGRAD_REDUCE,   // kernels + memset
+    OP_RECORD, OP_WAIT,          // event record / stream wait
+    OP_MAKE                      // create a stream (+ the side stream's join / packs events) or pool events, if missing
+};
+
+// One runtime operation of an engine call, with the by-value block its launcher takes.
+struct Op {
+    OpKind kind;
+    StreamRole stream;
+    EventPool pool;
+    bool early;                  // a training step's weight packs and their events: issued before everything else
+    int index;                   // RECORD / WAIT: event in the pool; MAKE: events the pool must hold; WGRAD: group of the layer
+    int layer, pass;             // pass 0 forward, 1 dgrad, 2 wgrad
+    union {
+        struct { const float* x; float* y; int n; } sig;
+        FirstLayer first;
+        ConvLaunch conv;
+        UmmaPackLaunch pack;
+        struct { UmmaLaunch U; ConvLaunch L; UmmaChoice ch; OutputFuse fuse; bool fused; } umma;
+        unsigned* counters;
+        struct { OutputLaunch O; float* grads; float* part; float scale; float* gfeat; } out;
+        UpsampleBwdLaunch up;
+        FirstWgrad fw;
+        struct { PlaneView V; int batch; float scale; float* out; } colsum;
+        WgradLaunch wg;
+        struct { UmmaWgradLaunch U; WgSplit S; SplitJobs J; } wgu;   // WGRAD_UMMA: U; SPLIT: J; WGRAD_BULK: U, S; WGRAD_REDUCE: U, J
+    };
+    Op() {}
+};
+
 struct WunHandle {
     Plan plan;
     std::vector<OpBackward> bwd_down, bwd_up;
     OpBackward bwd_bottleneck;
     bool umma_enabled = true;            // tensor-core path on (WUN_DISABLE_UMMA=1 turns it off, for A/B tests)
     bool umma_pass[3] = {true, true, true};   // per pass (fwd, dgrad, wgrad): WUN_UMMA_FWD=0 / WUN_UMMA_DGRAD=0 / WUN_UMMA_WGRAD=0
-    size_t arena_bytes = 0;              // scratch for packed bf16 weights (max over launches)
-    std::vector<std::string> kernel_used;   // [layer*3 + pass] -> "simt" | "umma" (filled by dry runs)
-    int cur_layer = 0, cur_pass = 0;
-    int debug_iters = 0;                 // > 0: wun_debug_run_conv - pack once, enqueue the conv kernel this many times
-    // weight-gradient kernels run on an internal side stream, concurrently with the dgrad chain on the caller's stream
-    cudaStream_t side = nullptr;
-    // A dgrad with two launches (the up blocks: skip pair and upsampled pair have different widths) runs the second one on this
-    // helper stream, concurrently with the first: both read the same gradient planes and write different tensors, and in the deep
-    // layers neither fills the GPU (WUN_DGRAD_PAR=0 disables)
-    cudaStream_t side2 = nullptr;
-    std::vector<cudaEvent_t> par_events;      // fork / join pairs, one pair per use inside a call (graph capture needs distinct events)
-    int par_used = 0;
+    std::vector<std::string> kernel_used;   // [layer*3 + pass] -> "simt" | "umma" (from the launch list built at create time)
+    cudaStream_t streams[4] = {};        // by StreamRole, created where a call first needs them (ST_CALLER: unused)
+    std::vector<cudaEvent_t> events[kEventPools];   // by EventPool, created where a call first needs them
     bool dgrad_par = true;
-    std::vector<cudaEvent_t> fork_events;
-    cudaEvent_t join_event = nullptr;
-    int fork_used = 0;
     bool use_side = true;                // WUN_SIDE_STREAM=0 disables
     bool first_fast = true;              // dedicated first-layer kernels (kernels_first.cu); WUN_FIRST_LAYER=0 = generic path
     bool bulk_wgrad = true;              // split pass + bulk-copy-fed tensor-core wgrad; WUN_BULK_WGRAD=0 = converter-fed kernel
@@ -81,51 +115,26 @@ struct WunHandle {
     // the wgrad stream (off the critical path), 2 = the weight gradient in the epilogue too (measured slower: it serialises
     // ~650 shuffle-reduction instructions per row tile on the four epilogue warps)
     int out_fuse_mode = 1;
-    const OutputFuse* fuse_out = nullptr;   // set by run_forward around the last up block's forward conv
-    bool out_fused = false;              // that conv carried the output layer: no output_fwd / output_dgrad / output_wgrad launches
-    float* bw_grads = nullptr;           // wun_forward_backward: gradient buffer / scale, known to the forward pass for the fused epilogue
-    float bw_scale = 1.f;
     int pair_min_ctas = 120;             // WUN_PAIR_MIN_CTAS
     bool pair_fwd = true;                // the same for the forward classes of the up blocks; WUN_PAIR_FWD=0 disables
     int pair_dgrad = 4;                  // pair-merged dgrad classes (launch.h OutView::pairC); WUN_PAIR_DGRAD=0 off, 1 all, 2 down blocks only,
                                          // 3 up blocks only, 4 (default) down blocks whose merged width still takes the fused-N MMAs (2C <= 64)
-    size_t split_item_bytes = 0;         // per batch item: largest split arena any layer's wgrad needs (dry run)
-    size_t wg_partial_bytes = 0;         // largest partial-tile scratch of a layer's wgrad (any batch; dry run)
-    size_t out_part_bytes = 0;           // the output layer's per-CTA weight-gradient sums (any batch; dry run)
-    cudaStream_t wstream = nullptr;      // stream the wgrad-side launches go to (side or main)
+    // sizes from the batch-1 training launch list built at create time
+    size_t split_item_bytes = 0;         // per batch item: largest split arena any layer's wgrad needs
+    size_t wg_partial_bytes = 0;         // largest partial-tile scratch of a layer's wgrad (any batch)
+    size_t out_part_bytes = 0;           // the output layer's per-CTA weight-gradient sums (any batch)
+    size_t arena_sum = 0;                // total pack bytes of one forward+backward
     // split passes run one layer AHEAD of the wgrad kernels, on their own stream, into a double-buffered arena: the split pass is
     // DRAM-bound, the wgrad kernel L2 / tensor bound, so they overlap well (WUN_SPLIT_AHEAD=0: same stream, one arena half)
-    cudaStream_t split_stream = nullptr;
-    std::vector<cudaEvent_t> split_done, wg_done;
-    int wg_index = 0;
     bool split_ahead = true;
-    cudaEvent_t first_done = nullptr;     // first-layer weight gradient on the split stream
-    bool first_pending = false;
-    // weight packs are hoisted off the critical path: phase 1 enqueues every pack kernel of the step on the side stream
-    // (they only depend on the parameters), phase 2 enqueues everything else; phase 0 = inline (inference, debug hook)
-    int phase = 0;
-    size_t arena_cur = 0;                // bump pointer into the pack arena (same sequence in phase 1 and 2)
-    size_t pack_floor = 0;               // launch_conv reserves at least this much: the pair-merge decision depends on the batch
-                                         // (folded or not) but the arena is sized by a batch-1 dry run, so both forms' bytes count
-    size_t arena_sum = 0;                // total pack bytes of one forward+backward (dry run)
-    cudaEvent_t packs_event = nullptr;
-    bool packs_pending = false;          // main stream has not yet waited for the hoisted packs
-    // one event per FORWARD weight pack, so that forward conv i waits for pack i only instead of for all ~60 packs of the
-    // step (the backward convs still wait for the single packs_event); WUN_PACK_EVENTS=0 disables
+    // weight packs are hoisted off the critical path: a training step enqueues every pack kernel on the side stream first (they
+    // only depend on the parameters), then everything else; inference and the debug hooks pack inline
     bool pack_events_on = true;
-    std::vector<cudaEvent_t> pack_events;
-    int pack_idx = 0;                    // forward tensor-core conv counter of the current phase
-    std::vector<std::string>* audit = nullptr;   // dry runs: one line per tensor-core launch (wun_debug_plan)
-    std::vector<std::string>* export_launches = nullptr;   // dry runs: the full description of every plane-convolution launch (wun_debug_launches)
     // data-parallel overlap: gradient buckets in PRODUCTION order (output layer first, down0 last); bucket k = flat offsets
-    // >= bucket_first[k] (and below bucket k-1's).  bucket_events[k] is recorded once every gradient of the bucket is final.
+    // >= bucket_first[k] (and below bucket k-1's)
     std::vector<int64_t> bucket_first;
-    std::vector<cudaEvent_t> bucket_events;
-    int bucket_next = 0;
     // per-call state
-    bool dry = false;
-    bool train_call = false;             // a training step (or its dry run): the CTA counters of the loss sums are zeroed
-    int64_t launches = 0;
+    std::vector<Op> ops;                 // the call's launch list (its storage is kept from call to call: no allocation per call)
     cudaStream_t stream = nullptr;
     const float* params = nullptr;
     const float* mix = nullptr;
@@ -260,111 +269,66 @@ static long long view_bstride(const WunHandle* h, const ViewSpec& v) {
     return rows * C;
 }
 
-// wun_debug_launches: one plane-convolution launch as text (addresses are raw integers relative to the fake bases the dry run
-// installs: workspace 1 << 40, parameters 1 << 41, mix 1 << 42 - nothing is dereferenced).  tests/test_launch_semantics.py
-// interprets these descriptions in numpy: the pair-merged form of a launch must compute exactly what its two-class form does.
-static void export_launch(WunHandle* h, const ConvLaunch& L) {
-    char line[768];
-    auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
-    snprintf(line, sizeof(line), "launch layer=%d pass=%d N=%d pairC=%d w_sk=%d w_sn=%d W=%lld bias=%lld epilogue=%d batch=%d nplanes=%d ncls=%d",
-             h->cur_layer, h->cur_pass, L.N, L.pairC, L.w_sk, L.w_sn, addr(L.W), L.bias ? addr(L.bias) : -1LL, L.epilogue, L.batch, L.nplanes, L.ncls);
-    h->export_launches->push_back(line);
-    for (int p = 0; p < L.nplanes; ++p) {
-        const PlaneView& P = L.planes[p];
-        snprintf(line, sizeof(line), "plane i=%d base=%lld bstride=%lld rstride=%d r_lo=%d r_hi=%d C=%d kind=%d mid_mode=%d xrows=%d blend=%lld",
-                 p, addr(P.base), P.bstride, P.rstride, P.r_lo, P.r_hi, P.C, P.kind, P.mid_mode, P.xrows, P.blend ? addr(P.blend) : -1LL);
-        h->export_launches->push_back(line);
-    }
-    int nterm = 0;
-    for (int q = 0; q < L.ncls; ++q) {
-        const OutView& O = L.cls[q];
-        nterm = std::max(nterm, O.term_end);
-        snprintf(line, sizeof(line), "cls i=%d base=%lld bstride=%lld rstride=%d m_lo=%d m_hi=%d saved=%lld acc_lo=%d acc_hi=%d term_begin=%d term_end=%d "
-                 "pairC=%d base2=%lld bstride2=%lld rstride2=%d saved2=%lld acc_lo2=%d acc_hi2=%d lo0=%d hi0=%d lo1=%d hi1=%d",
-                 q, addr(O.base), O.bstride, O.rstride, O.m_lo, O.m_hi, O.saved ? addr(O.saved) : -1LL, O.acc_lo, O.acc_hi, O.term_begin, O.term_end,
-                 O.pairC, O.pairC ? addr(O.base2) : -1LL, O.bstride2, O.rstride2, (O.pairC && O.saved2) ? addr(O.saved2) : -1LL, O.acc_lo2, O.acc_hi2,
-                 O.lo_h[0], O.hi_h[0], O.lo_h[1], O.hi_h[1]);
-        h->export_launches->push_back(line);
-    }
-    for (int t = 0; t < nterm; ++t) {
-        snprintf(line, sizeof(line), "term i=%d plane=%d d=%d woff=%d woff2=%d", t, L.terms[t].plane, L.terms[t].d, L.terms[t].woff, L.pairC ? L.terms[t].woff2 : -1);
-        h->export_launches->push_back(line);
-    }
+// ------------------------------------------------------------------------------------------------
+// launch list: build_* turn one engine call into records without any CUDA call, issue() makes the runtime calls
+// ------------------------------------------------------------------------------------------------
+struct Build {                   // the walk over the plan that appends one call's records
+    const WunHandle* h;
+    std::vector<Op>& ops;
+    bool train = false;          // a training step: the CTA counters of the loss sums are zeroed
+    bool hoist = false;          // weight packs on the side stream ahead of the step (training, side stream, tensor cores)
+    bool dgrad_fork = false;     // a dgrad's second launch may go to the helper stream
+    StreamRole ws = ST_CALLER;   // stream of the weight-gradient launches
+    float* grads = nullptr;      // training: gradient buffer / scale, known to the forward pass for the fused epilogue
+    float scale = 1.f;
+    const OutputFuse* fuse = nullptr;   // around the last up block's forward conv
+    bool out_fused = false;      // that conv carried the output layer: no output_fwd / output_dgrad / output_wgrad launches
+    int layer = -1, pass = -1;
+    size_t arena_cur = 0;        // bump pointer into the pack arena
+    int pack_idx = 0, fork_used = 0, par_used = 0, wg_index = 0, bucket_next = 0;
+    bool packs_pending = false;  // the caller's stream has not yet waited for the hoisted packs
+    bool first_pending = false;  // the first-layer weight gradient runs on the split stream
+    // sizes the workspace needs for these launches
+    size_t pack_sum = 0, split_item = 0, wg_partial = 0, out_part = 0;
+};
+
+static Op& add(Build& b, OpKind kind, StreamRole stream = ST_CALLER, EventPool pool = EV_NONE, int index = 0) {
+    b.ops.emplace_back();
+    Op& o = b.ops.back();
+    o.kind = kind; o.stream = stream; o.pool = pool; o.early = false; o.index = index; o.layer = b.layer; o.pass = b.pass;
+    return o;
 }
 
 // Every plane convolution goes through here: tensor cores (wgmma) when the launch is eligible, CUDA cores otherwise.
-static int launch_conv(WunHandle* h, const ConvLaunch& L) {
-    if (h->dry && h->export_launches) export_launch(h, L);
+// It reserves at least `pack_floor` pack bytes: the pair-merge decision depends on the batch (folded or not) but the arena is
+// sized by a batch-1 list, so both forms' bytes count.
+static int add_conv(Build& b, const ConvLaunch& L, StreamRole s, size_t pack_floor) {
+    const WunHandle* h = b.h;
     UmmaChoice ch;
-    const bool use_umma = h->umma_enabled && h->umma_pass[h->cur_pass] && umma_plan_from_conv(L, &ch);
-    const size_t slot = (size_t)h->cur_layer * 3 + h->cur_pass;
-    if (h->dry && slot < h->kernel_used.size()) h->kernel_used[slot] = use_umma ? "umma" : "simt";
-    if (use_umma) {
-        if (h->fuse_out && h->debug_iters == 0 && umma_output_fusable(L, ch, h->fuse_out->O)) h->out_fused = true;
-        if (h->phase != 1) h->launches += 2;    // weight pack + conv (counted once)
-        if (h->dry) {
-            h->arena_bytes = std::max(h->arena_bytes, std::max(ch.pack_bytes, h->pack_floor)); h->arena_sum += std::max(ch.pack_bytes, h->pack_floor);
-            if (h->audit) {
-                long long tiles = 0, mmas = 0; int max_rows = 0, span = 0;
-                for (int q = 0; q < L.ncls; ++q) {
-                    const int rows = L.cls[q].m_hi - L.cls[q].m_lo;
-                    const long long tq = (long long)((rows + ch.MT * 128 - 1) / (ch.MT * 128)) * ch.nsplit * L.batch;
-                    tiles += tq;
-                    max_rows = std::max(max_rows, rows);
-                    int t = L.cls[q].term_begin;
-                    long long ksteps = 0;                       // (16-channel chunk, tap) pairs of one tile of this class
-                    while (t < L.cls[q].term_end) {
-                        int t1 = t, dmin = L.terms[t].d, dmax = dmin;
-                        while (t1 < L.cls[q].term_end && L.terms[t1].plane == L.terms[t].plane) {
-                            dmin = std::min(dmin, L.terms[t1].d); dmax = std::max(dmax, L.terms[t1].d); ++t1; }
-                        span = std::max(span, dmax - dmin);
-                        ksteps += (long long)((L.planes[L.terms[t].plane].C + 15) / 16) * (t1 - t);
-                        t = t1;
-                    }
-                    mmas += tq * ch.MT * ksteps * 3;
-                }
-                char line[512];
-                snprintf(line, sizeof(line), "conv layer=%d pass=%d kernel=wgmma N=%d NPAD=%d nsplit=%d MT=%d rows_alloc=%d span=%d "
-                         "TB=%d nbs=%d tiles=%lld mmas=%lld max_rows=%d smem=%zu pack_bytes=%zu pair=%d outfuse=%d",
-                         h->cur_layer, h->cur_pass, L.N, ch.NPAD, ch.nsplit, ch.MT, ch.rows_alloc, span, ch.TB, ch.nbs, tiles, mmas,
-                         max_rows, umma_choice_smem_bytes(ch), ch.pack_bytes, L.pairC,
-                         (h->fuse_out && umma_output_fusable(L, ch, h->fuse_out->O)) ? 1 : 0);
-                h->audit->push_back(line);
-            }
-            return WUN_OK;
-        }
-        uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_cur;
-        h->arena_cur += std::max(ch.pack_bytes, h->pack_floor);
-        UmmaLaunch U; UmmaPackLaunch PL;
-        cudaError_t e = umma_build(L, ch, arena, &U, &PL);
-        if (e == cudaSuccess && h->phase != 2) e = launch_umma_pack(PL, (h->phase == 1) ? h->side : h->stream);
-        const bool per_pack = h->pack_events_on && h->cur_pass == 0 && h->phase != 0;
-        if (per_pack) {
-            const int idx = h->pack_idx++;
-            while ((int)h->pack_events.size() <= idx && e == cudaSuccess) {
-                cudaEvent_t ev;
-                e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-                if (e == cudaSuccess) h->pack_events.push_back(ev);
-            }
-            if (e == cudaSuccess && h->phase == 1) e = cudaEventRecord(h->pack_events[idx], h->side);
-            if (e == cudaSuccess && h->phase == 2) e = cudaStreamWaitEvent(h->stream, h->pack_events[idx], 0);
-        }
-        if (e == cudaSuccess && h->phase != 1) {
-            if (h->packs_pending && !per_pack) {   // first conv that needs ALL hoisted packs (with per-pack events: the first dgrad)
-                e = cudaStreamWaitEvent(h->stream, h->packs_event, 0);
-                h->packs_pending = false;
-            }
-            const int iters = (h->debug_iters > 0) ? h->debug_iters : 1;
-            const OutputFuse* fuse = (h->fuse_out && h->debug_iters == 0 && umma_output_fusable(L, ch, h->fuse_out->O)) ? h->fuse_out : nullptr;
-            if (fuse) h->out_fused = true;
-            for (int i = 0; i < iters && e == cudaSuccess; ++i) e = launch_plane_conv_umma(U, h->stream, fuse);
-        }
-        if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tensor-core conv launch: ") + cudaGetErrorString(e));
+    if (!(h->umma_enabled && h->umma_pass[b.pass] && umma_plan_from_conv(L, &ch))) {
+        add(b, OP_CONV, s).conv = L;
         return WUN_OK;
     }
-    if (h->phase == 1) return WUN_OK;
-    ++h->launches;
-    if (!h->dry) launch_plane_conv_simt(L, h->stream);
+    const size_t bytes = std::max(ch.pack_bytes, pack_floor);
+    uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + b.arena_cur;
+    b.arena_cur += bytes; b.pack_sum += bytes;
+    UmmaLaunch U;
+    Op& pk = add(b, OP_PACK, b.hoist ? ST_SIDE : s);
+    pk.early = b.hoist;
+    if (umma_build(L, ch, arena, &U, &pk.pack) != cudaSuccess) return set_err(WUN_E_CUDA, "tensor-core conv launch: too many pack jobs");
+    if (h->pack_events_on && b.pass == 0 && b.hoist) {     // forward conv i waits for pack i only
+        const int idx = b.pack_idx++;
+        add(b, OP_MAKE, ST_SIDE, EV_PACK, idx + 1).early = true;
+        add(b, OP_RECORD, ST_SIDE, EV_PACK, idx).early = true;
+        add(b, OP_WAIT, s, EV_PACK, idx);
+    } else if (b.packs_pending) {   // first conv that needs ALL hoisted packs (with per-pack events: the first dgrad)
+        add(b, OP_WAIT, s, EV_PACKS);
+        b.packs_pending = false;
+    }
+    Op& o = add(b, OP_UMMA_CONV, s);
+    o.umma.U = U; o.umma.L = L; o.umma.ch = ch;
+    o.umma.fused = b.fuse && umma_output_fusable(L, ch, b.fuse->O);
+    if (o.umma.fused) { o.umma.fuse = *b.fuse; b.out_fused = true; }
     return WUN_OK;
 }
 
@@ -451,26 +415,13 @@ static bool pair_worthwhile(const WunHandle* h, const ConvLaunch& M, const UmmaC
     return ctas >= h->pair_min_ctas;
 }
 
-static int conv_forward(WunHandle* h, const ConvOp& op, int layer_index) {
-    h->cur_layer = layer_index; h->cur_pass = 0;
+static int build_conv_forward(Build& b, const ConvOp& op, int layer_index) {
+    const WunHandle* h = b.h;
+    b.layer = layer_index; b.pass = 0;
     if (layer_index == 0) {
         FirstLayer F;
         if (first_layer_desc(h, op, &F)) {
-            if (h->phase == 1) return WUN_OK;
-            if (h->dry && h->export_launches) {   // wun_debug_launches: the first layer (its weight gradient has the same geometry;
-                char line[768];                   // gdec / godd = the gradient tensors it reads, dW / db = flat parameter offsets)
-                auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
-                const Plan& P = h->plan;
-                snprintf(line, sizeof(line), "first C=%d N=%d k=%d pad_left=%d batch=%d x=%lld x_bstride=%lld T=%d dec=%lld dec_bstride=%lld Td=%d "
-                         "odd=%lld odd_bstride=%lld mo_lo=%d mo_hi=%d gdec=%lld godd=%lld dW=%lld db=%lld",
-                         P.cfg.num_channels, op.cout, F.k, F.pad_left, F.batch, addr(F.x), F.x_bstride, F.T, addr(F.dec), F.dec_bstride, F.Td,
-                         addr(F.odd), F.odd_bstride, F.mo_lo, F.mo_hi, addr(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor])),
-                         addr(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor])), (long long)P.params[op.w_param].offset,
-                         (long long)P.params[op.b_param].offset);
-                h->export_launches->push_back(line);
-            }
-            ++h->launches;
-            if (!h->dry) launch_first_fwd(F, h->plan.cfg.num_channels, op.cout, h->stream);
+            add(b, OP_FIRST_FWD).first = F;
             return WUN_OK;
         }
     }
@@ -501,25 +452,24 @@ static int conv_forward(WunHandle* h, const ConvOp& op, int layer_index) {
     // the even / odd output rows of an up block (and of the bottleneck) read the same planes at the same shifts: one
     // pair-merged class of 2*cout columns (out tensor viewed as [B, rows/2, 2*cout]) - 6+6 taps instead of 2 x (5+5)
     ConvLaunch M;
-    h->pack_floor = 0;
+    size_t pack_floor = 0;
     if (h->pair_fwd && L.ncls == 2 && h->umma_enabled && h->umma_pass[0] && merge_pair(L, &M)) {
         UmmaChoice ch0, ch;
         const bool ok0 = umma_plan_from_conv(L, &ch0), ok1 = umma_plan_from_conv(M, &ch);
         if (ok0 && ok1) {
-            h->pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
+            pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
             if (pair_worthwhile(h, M, ch)) L = M;
         }
     }
-    const int rc = launch_conv(h, L);
-    h->pack_floor = 0;
-    return rc;
+    return add_conv(b, L, ST_CALLER, pack_floor);
 }
 
 // dgrad: one class per forward input plane that needs a gradient; the forward classes' gradient
 // tensors become the input planes.
-static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int layer_index) {
+static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int layer_index) {
     if (ob.dgrad.empty()) return WUN_OK;
-    h->cur_layer = layer_index; h->cur_pass = 1;
+    const WunHandle* h = b.h;
+    b.layer = layer_index; b.pass = 1;
     const Plan& P = h->plan;
     ConvLaunch L;
     memset(&L, 0, sizeof(L));
@@ -561,15 +511,12 @@ static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int 
     // classes may differ in channel count (skip vs upsampled planes): launch per distinct N
     std::vector<int> done(L.ncls, 0);
     int n_launched = 0;
-    cudaEvent_t ev_fork = nullptr;          // recorded on the caller's stream before the first launch (see `par` below)
-    if (h->dgrad_par && !h->dry && h->phase != 1 && h->use_side && h->side != nullptr && h->debug_iters == 0 && !h->packs_pending && L.ncls > 2) {
-        while ((int)h->par_events.size() < h->par_used + 2) {
-            cudaEvent_t e;
-            WUN_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            h->par_events.push_back(e);
-        }
-        ev_fork = h->par_events[h->par_used];
-        WUN_CUDA_OK(cudaEventRecord(ev_fork, h->stream));
+    // recorded on the caller's stream before the first launch (see `par` below)
+    const bool fork = b.dgrad_fork && !b.packs_pending && L.ncls > 2;
+    const int ev_fork = b.par_used;
+    if (fork) {
+        add(b, OP_MAKE, ST_CALLER, EV_PAR, b.par_used + 2);
+        add(b, OP_RECORD, ST_CALLER, EV_PAR, ev_fork);
     }
     for (int k = 0; k < L.ncls; ++k) {
         if (done[k]) continue;
@@ -599,42 +546,29 @@ static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int 
         // epilogue's slope / accumulate read-backs, not by slab fills or MMAs.
         const bool pair_on = h->pair_dgrad == 1 || (h->pair_dgrad == 2 && op.planes.size() == 2) || (h->pair_dgrad == 3 && op.planes.size() == 4) ||
                              (h->pair_dgrad == 4 && op.planes.size() == 2 && 2 * S.N <= 64);
-        h->pack_floor = 0;
+        size_t pack_floor = 0;
         if (h->pair_dgrad != 0 && S.ncls == 2 && h->umma_enabled && h->umma_pass[1] && merge_pair(S, &M)) {
             UmmaChoice ch0, ch;
             const bool ok0 = umma_plan_from_conv(S, &ch0), ok1 = umma_plan_from_conv(M, &ch);
             if (ok0 && ok1) {
-                h->pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
+                pack_floor = std::max(ch0.pack_bytes, ch.pack_bytes);
                 if (pair_on && pair_worthwhile(h, M, ch)) S = M;
             }
         }
         // second (third ...) launch of this dgrad: on the helper stream, forked from the point the first launch was enqueued at
-        const bool par = ev_fork != nullptr && n_launched > 0 && !h->dry && h->phase != 1 && h->use_side && h->side != nullptr &&
-                         h->debug_iters == 0 && !h->packs_pending;
-        cudaStream_t main_stream = h->stream;
-        cudaEvent_t ev_join = nullptr;
+        const bool par = fork && n_launched > 0;
         if (par) {
-            if (!h->side2) WUN_CUDA_OK(cudaStreamCreateWithFlags(&h->side2, cudaStreamNonBlocking));
-            while ((int)h->par_events.size() < h->par_used + 2) {
-                cudaEvent_t e;
-                WUN_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-                h->par_events.push_back(e);
-            }
-            ev_join = h->par_events[h->par_used + 1];
-            WUN_CUDA_OK(cudaStreamWaitEvent(h->side2, ev_fork, 0));
-            h->stream = h->side2;
+            add(b, OP_MAKE, ST_HELPER);
+            add(b, OP_MAKE, ST_HELPER, EV_PAR, b.par_used + 2);
+            add(b, OP_WAIT, ST_HELPER, EV_PAR, ev_fork);
         }
-        int rc = launch_conv(h, S);
-        h->pack_floor = 0;
-        if (par) {
-            h->stream = main_stream;
-            if (rc == WUN_OK) {
-                WUN_CUDA_OK(cudaEventRecord(ev_join, h->side2));
-                WUN_CUDA_OK(cudaStreamWaitEvent(main_stream, ev_join, 0));
-            }
-            h->par_used += 2;
-        }
+        const int rc = add_conv(b, S, par ? ST_HELPER : ST_CALLER, pack_floor);
         if (rc != WUN_OK) return rc;
+        if (par) {
+            add(b, OP_RECORD, ST_HELPER, EV_PAR, b.par_used + 1);
+            add(b, OP_WAIT, ST_CALLER, EV_PAR, b.par_used + 1);
+            b.par_used += 2;
+        }
         ++n_launched;
     }
     return WUN_OK;
@@ -642,422 +576,6 @@ static int conv_dgrad(WunHandle* h, const ConvOp& op, const OpBackward& ob, int 
 
 static int64_t split_arena_half_bytes(const WunHandle* h, int64_t batch) {
     return (int64_t)h->split_item_bytes * batch + 256 * (kSplitMaxJobs + 1) + (int64_t)h->wg_partial_bytes + 256;
-}
-
-static int64_t split_arena_bytes(const WunHandle* h, int64_t batch);
-static float* out_part_ptr(const WunHandle* h);
-static unsigned* counters_ptr(const WunHandle* h);
-static float* loss_part_ptr(const WunHandle* h);
-static float* dvar_part_ptr(const WunHandle* h);
-
-static int conv_wgrad(WunHandle* h, const ConvOp& op, float* grads, float scale, int layer_index) {
-    const Plan& P = h->plan;
-    h->cur_layer = layer_index;
-    if (layer_index == 0) {
-        FirstWgrad FW;
-        if (first_layer_desc(h, op, &FW.L)) {          // one launch: dW and db of both classes
-            if (h->phase == 1) return WUN_OK;
-            h->launches += 2;                             // per-CTA sums + their fixed-order total
-            if (!h->dry) {
-                FW.part = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum +
-                                                   split_arena_bytes(h, h->batch));
-                FW.L.dec = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor]));
-                FW.L.odd = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor]));
-                FW.dW = grads + P.params[op.w_param].offset;
-                FW.db = grads + P.params[op.b_param].offset;
-                FW.scale = scale; FW.rows_per_cta = 0;
-                // the CUDA-core first-layer gradient is the tail of the step: on the split stream it runs next to the second
-                // block's tensor-core wgrad instead of behind it (joined at the end of run_backward)
-                static const bool tail_on = [] { const char* e = getenv("WUN_FIRST_TAIL"); return !(e && e[0] == '0'); }();
-                const bool tail_par = tail_on && h->split_ahead && h->split_stream != nullptr && h->wstream != h->stream;
-                launch_first_wgrad(FW, P.cfg.num_channels, op.cout, tail_par ? h->split_stream : h->wstream);
-                if (tail_par) {
-                    if (!h->first_done) WUN_CUDA_OK(cudaEventCreateWithFlags(&h->first_done, cudaEventDisableTiming));
-                    WUN_CUDA_OK(cudaEventRecord(h->first_done, h->split_stream));
-                    h->first_pending = true;
-                }
-            }
-            return WUN_OK;
-        }
-    }
-    // collect (class, plane) groups
-    std::vector<WgradLaunch> groups;
-    std::vector<PlaneView> class_dpre;
-    for (const auto& c : op.classes) {
-        if (c.m_hi <= c.m_lo) continue;
-        PlaneView dpre = make_plane_on(h, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
-        class_dpre.push_back(dpre);                            // bias gradient = its column sums (fused into the split pass below)
-        size_t i = 0;
-        while (i < c.terms.size()) {
-            WgradLaunch W;
-            memset(&W, 0, sizeof(W));
-            const int p = c.terms[i].plane;
-            int dmin = c.terms[i].d;
-            while (i < c.terms.size() && c.terms[i].plane == p && W.nterms < 8 && c.terms[i].d - dmin <= 15) {
-                W.d[W.nterms] = c.terms[i].d;
-                W.woff[W.nterms] = (c.terms[i].tap * op.cin_tot + c.terms[i].coff) * op.cout;
-                ++W.nterms; ++i;
-            }
-            W.plane = make_plane(h, op.planes[p]);
-            W.dpre = dpre;
-            W.m_lo = c.m_lo; W.m_hi = c.m_hi;
-            W.N = op.cout; W.w_sk = op.cout; W.w_sn = 1;
-            W.dW = grads + P.params[op.w_param].offset;
-            W.scale = scale; W.batch = h->batch;
-            groups.push_back(W);
-        }
-    }
-    if (h->dry && h->export_launches) {      // wun_debug_launches: the (class, plane) groups of this layer's weight gradient
-        char line[512];
-        auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
-        for (size_t g = 0; g < groups.size(); ++g) {
-            const WgradLaunch& W = groups[g];
-            snprintf(line, sizeof(line), "wgrad layer=%d group=%d N=%d w_sk=%d w_sn=%d dW=%lld db=%lld m_lo=%d m_hi=%d nterms=%d batch=%d",
-                     layer_index, (int)g, W.N, W.w_sk, W.w_sn, (long long)P.params[op.w_param].offset, (long long)P.params[op.b_param].offset,
-                     W.m_lo, W.m_hi, W.nterms, W.batch);
-            h->export_launches->push_back(line);
-            const PlaneView* V[2] = {&W.plane, &W.dpre};
-            for (int k = 0; k < 2; ++k) {
-                snprintf(line, sizeof(line), "%s base=%lld bstride=%lld rstride=%d r_lo=%d r_hi=%d C=%d kind=%d mid_mode=%d xrows=%d blend=%lld",
-                         k == 0 ? "wplane" : "wdpre", addr(V[k]->base), V[k]->bstride, V[k]->rstride, V[k]->r_lo, V[k]->r_hi, V[k]->C, V[k]->kind,
-                         V[k]->mid_mode, V[k]->xrows, V[k]->blend ? addr(V[k]->blend) : -1LL);
-                h->export_launches->push_back(line);
-            }
-            for (int t = 0; t < W.nterms; ++t) {
-                snprintf(line, sizeof(line), "wterm i=%d d=%d woff=%d", t, W.d[t], W.woff[t]);
-                h->export_launches->push_back(line);
-            }
-        }
-    }
-    // tensor cores: all groups of the layer in ONE launch
-    bool use_umma = h->umma_enabled && h->umma_pass[2] && !groups.empty() && groups.size() <= (size_t)kWgMaxGroups;
-    UmmaWgradLaunch U;
-    if (use_umma) {
-        memset(&U, 0, sizeof(U));
-        U.ngroups = (int)groups.size(); U.batch = h->batch; U.dW = groups[0].dW;
-        U.w_sp = op.cout; U.w_sg = 1; U.scale = scale;
-        for (size_t g = 0; g < groups.size(); ++g) {
-            WgGroup& G = U.grp[g];
-            G.P = groups[g].plane; G.G = groups[g].dpre; G.m_lo = groups[g].m_lo; G.m_hi = groups[g].m_hi;
-            G.ntaps = groups[g].nterms;
-            for (int t = 0; t < G.ntaps; ++t) { G.d[t] = groups[g].d[t]; G.woff[t] = groups[g].woff[t]; }
-        }
-        use_umma = umma_plan_wgrad(&U);
-    }
-    const size_t slot = (size_t)h->cur_layer * 3 + 2;
-    if (h->dry && slot < h->kernel_used.size()) h->kernel_used[slot] = use_umma ? "umma" : "simt";
-    if (h->dry && h->audit && use_umma) {
-        for (int g = 0; g < U.ngroups; ++g) {
-            const WgGroup& G = U.grp[g];
-            char line[512];
-            snprintf(line, sizeof(line), "wgrad layer=%d group=%d Cp=%d Cg=%d swap=%d NT=%d mtiles=%d ntiles=%d ntaps=%d taps_per_cta=%d "
-                     "tapsets=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu issued_macs=%lld useful_macs=%lld",
-                     h->cur_layer, g, G.P.C, G.G.C, G.swap, G.NT, G.n_mtiles, G.n_ntiles, G.ntaps, G.taps_per_cta, G.n_tapsets,
-                     G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages, umma_wgrad_smem_bytes(U),
-                     umma_wgrad_issued_macs(G, U.batch), (long long)U.batch * G.chunks_per_batch * 64 * G.ntaps * G.P.C * G.G.C);
-            h->audit->push_back(line);
-        }
-    }
-    if (h->phase == 1) return WUN_OK;
-    float* bias_grad = grads ? grads + P.params[op.b_param].offset : nullptr;
-    auto colsum_launches = [&]() {                        // bias gradient by its own kernel (paths without a split pass)
-        for (const auto& dp : class_dpre) {
-            ++h->launches;
-            if (!h->dry) launch_colsum(dp, h->batch, scale, bias_grad, h->wstream);
-        }
-    };
-    if (use_umma) {
-        ++h->launches;
-        const size_t split_need = h->bulk_wgrad ? umma_plan_wgrad_split(U, 1, nullptr, nullptr, nullptr) : 0;
-        const bool bulk = split_need > 0;                 // 0: too many distinct views for one split pass -> converter-fed kernel
-        // Bias column sums inside the split pass instead of their own launches (WUN_SPLIT_COLSUM: 1 = default, 0 = separate colsum
-        // launches, 2 = fused only for the layers with few rows).  History: while the dgrad chain was the critical path the separate
-        // launches were 0.05 ms faster per step (they fill SMs the big-shared-memory kernels leave thread slots on); since the epilogue
-        // work of round 2 the wgrad stream is the critical path and the fused form wins (5.45 -> 5.39 ms, wgrad family 2.52 -> 2.24 ms).
-        static const int colsum_mode = [] { const char* e = getenv("WUN_SPLIT_COLSUM"); return e ? atoi(e) : 1; }();
-        int max_rows_g = 0;
-        for (const auto& dp : class_dpre) max_rows_g = std::max(max_rows_g, dp.r_hi - dp.r_lo);
-        const bool fused_colsum = colsum_mode == 1 || (colsum_mode == 2 && max_rows_g <= 4096);
-        if (bulk) {      // + the split pass and the fixed-order reduction of the partial tiles / column sums
-            h->launches += 2;
-            if (h->dry) {
-                h->split_item_bytes = std::max(h->split_item_bytes, split_need);
-                h->wg_partial_bytes = std::max(h->wg_partial_bytes, umma_wgrad_partial_bytes(U));
-            }
-        }
-        if (!bulk || !fused_colsum) colsum_launches();
-        if (!h->dry) {
-            cudaError_t e;
-            if (bulk) {
-                const bool ahead = h->split_ahead && h->split_stream != nullptr && h->wstream != h->stream;
-                uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum;
-                if (ahead && (h->wg_index & 1)) arena += split_arena_half_bytes(h, h->batch);
-                arena += (256 - (reinterpret_cast<uintptr_t>(arena) & 255)) & 255;
-                // split arrays, then the partial tiles, in this half; the class-gradient views among the jobs also produce the
-                // bias gradient (their column sums)
-                WgSplit S; SplitJobs J;
-                if (!umma_wgrad_bulk_setup(&U, h->batch, arena, class_dpre.data(), (int)class_dpre.size(), fused_colsum ? bias_grad : nullptr,
-                                           scale, &S, &J))
-                    return set_err(WUN_E_INVALID, "wgrad split pass: class gradient view not among the split jobs");
-                if (ahead) {
-                    const int k = h->wg_index++;
-                    while ((int)h->split_done.size() <= k) {
-                        cudaEvent_t e1, e2;
-                        WUN_CUDA_OK(cudaEventCreateWithFlags(&e1, cudaEventDisableTiming));
-                        WUN_CUDA_OK(cudaEventCreateWithFlags(&e2, cudaEventDisableTiming));
-                        h->split_done.push_back(e1); h->wg_done.push_back(e2);
-                    }
-                    if (k >= 2) WUN_CUDA_OK(cudaStreamWaitEvent(h->split_stream, h->wg_done[k - 2], 0));     // its arena half is free again
-                    e = launch_split_views(J, h->split_stream);
-                    if (e == cudaSuccess) e = cudaEventRecord(h->split_done[k], h->split_stream);
-                    if (e == cudaSuccess) e = cudaStreamWaitEvent(h->wstream, h->split_done[k], 0);
-                    if (e == cudaSuccess) e = launch_wgrad_umma_bulk(U, S, h->wstream);
-                    if (e == cudaSuccess) e = launch_wgrad_reduce(U, J, h->wstream);
-                    if (e == cudaSuccess) e = cudaEventRecord(h->wg_done[k], h->wstream);
-                } else {
-                    e = launch_split_views(J, h->wstream);      // same stream as the wgrad: the arena is reused layer after layer
-                    if (e == cudaSuccess) e = launch_wgrad_umma_bulk(U, S, h->wstream);
-                    if (e == cudaSuccess) e = launch_wgrad_reduce(U, J, h->wstream);
-                }
-            } else {
-                e = launch_wgrad_umma(U, h->wstream);
-            }
-            if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string("tensor-core wgrad launch: ") + cudaGetErrorString(e));
-        }
-        return WUN_OK;
-    }
-    colsum_launches();
-    for (const auto& W : groups) {
-        ++h->launches;
-        if (!h->dry) launch_plane_wgrad_simt(W, h->wstream);
-    }
-    return WUN_OK;
-}
-
-static int ensure_side(WunHandle* h) {
-    if (!h->side) {
-        WUN_CUDA_OK(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-        WUN_CUDA_OK(cudaEventCreateWithFlags(&h->join_event, cudaEventDisableTiming));
-        WUN_CUDA_OK(cudaEventCreateWithFlags(&h->packs_event, cudaEventDisableTiming));
-    }
-    return WUN_OK;
-}
-
-// fork: everything enqueued on the main stream so far is visible to the side stream
-static int fork_side(WunHandle* h) {
-    if (h->dry || h->phase == 1 || h->wstream == h->stream) return WUN_OK;
-    if (h->fork_used >= (int)h->fork_events.size()) {
-        cudaEvent_t e;
-        WUN_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        h->fork_events.push_back(e);
-    }
-    cudaEvent_t ev = h->fork_events[h->fork_used++];
-    WUN_CUDA_OK(cudaEventRecord(ev, h->stream));
-    WUN_CUDA_OK(cudaStreamWaitEvent(h->side, ev, 0));
-    if (h->split_ahead) {
-        if (!h->split_stream) WUN_CUDA_OK(cudaStreamCreateWithFlags(&h->split_stream, cudaStreamNonBlocking));
-        WUN_CUDA_OK(cudaStreamWaitEvent(h->split_stream, ev, 0));
-    }
-    return WUN_OK;
-}
-
-// Every gradient at a flat offset >= `ready_from` has been enqueued (side-stream work in order, main-stream work up to the
-// last fork): record the events of the buckets this completes.  Called right after a fork (side waits for main) or at the end.
-static int mark_grads_ready(WunHandle* h, int64_t ready_from, cudaStream_t on) {
-    if (h->dry || h->phase == 1) return WUN_OK;
-    while (h->bucket_next < (int)h->bucket_first.size() && h->bucket_first[h->bucket_next] >= ready_from) {
-        WUN_CUDA_OK(cudaEventRecord(h->bucket_events[h->bucket_next], on));
-        ++h->bucket_next;
-    }
-    return WUN_OK;
-}
-
-static int64_t op_first_offset(const Plan& P, const ConvOp& op, const UpsampleSpec* us) {
-    int64_t o = std::min(P.params[op.w_param].offset, P.params[op.b_param].offset);
-    if (us && us->interp_param >= 0) o = std::min<int64_t>(o, P.params[us->interp_param].offset);
-    return o;
-}
-
-static void fill_output_launch(const WunHandle* h, OutputLaunch* O, const float* targets, float* outputs, float* loss,
-                               int training) {
-    const Plan& P = h->plan;
-    memset(O, 0, sizeof(*O));
-    O->params = h->params;
-    for (int s = 0; s < P.nconv; ++s) {
-        O->w_off[s] = P.params[P.out_w_param[s]].offset;
-        O->b_off[s] = P.params[P.out_b_param[s]].offset;
-    }
-    O->mix = h->mix;
-    O->feat = tensor_ptr(h, P.t_feat);
-    O->targets = targets;
-    O->outputs = outputs;
-    O->dpre = (h->lay.off[P.t_dpre_out] >= 0) ? const_cast<float*>(tensor_ptr(h, P.t_dpre_out)) : nullptr;
-    O->loss = loss;
-    O->loss_part = (loss && !h->dry) ? loss_part_ptr(h) : nullptr;
-    O->loss_count = (loss && !h->dry) ? counters_ptr(h) : nullptr;
-    O->batch = h->batch; O->T_in = (int)P.T_in; O->Tf = (int)P.Tf; O->T_out = (int)P.T_out;
-    O->C = P.cfg.num_channels; O->F = P.cfg.num_initial_filters;
-    O->nconv = P.nconv; O->K = P.cfg.num_sources;
-    O->ofs = P.cfg.output_filter_size; O->pad_left = P.out_pad_left;
-    O->crop_feat = P.crop_feat; O->crop_out = P.crop_out;
-    O->output_type = P.cfg.output_type; O->activation = P.cfg.output_activation; O->training = training;
-    O->inv_count = 1.0f / (float)((double)h->batch * P.T_out * P.cfg.num_channels * P.cfg.num_sources);
-}
-
-static int run_forward(WunHandle* h, const float* targets, float* outputs, float* loss, int training) {
-    const Plan& P = h->plan;
-    const int L = P.cfg.num_layers;
-    for (int i = 0; i < L; ++i) {
-        const UpsampleSpec& us = P.ups[i];
-        if (us.interp_param >= 0) {
-            if (h->phase != 1) ++h->launches;
-            if (!h->dry && h->phase != 1)
-                launch_sigmoid(h->params + P.params[us.interp_param].offset,
-                               const_cast<float*>(tensor_ptr(h, us.wsig_tensor)), us.C, h->stream);
-        }
-    }
-    int rc;
-    for (int i = 0; i < L; ++i)
-        if ((rc = conv_forward(h, P.down[i], i)) != WUN_OK) return rc;
-    if ((rc = conv_forward(h, P.bottleneck, L)) != WUN_OK) return rc;
-    OutputLaunch O;
-    fill_output_launch(h, &O, targets, outputs, loss, training);
-    OutputFuse OF;
-    memset(&OF, 0, sizeof(OF));
-    h->out_fused = false;
-    for (int i = 0; i < L; ++i) {
-        if (i == L - 1 && h->out_fuse_mode != 0 && P.cfg.output_filter_size == 1) {
-            // the output layer rides in this conv's epilogue when the planner picks the persistent kernel for it
-            OF.O = O;
-            const bool bw = targets != nullptr && h->bw_grads != nullptr;
-            OF.gfeat = bw ? const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat])) : nullptr;
-            OF.grads = (bw && h->out_fuse_mode == 2) ? h->bw_grads : nullptr;
-            OF.grad_scale = h->bw_scale;
-            const ConvOp& op = P.up[i];
-            bool geom = op.classes.size() >= 1 && op.classes.size() <= (size_t)kMaxClasses;
-            OF.t_step = geom ? op.classes[0].out.row_step : 0;
-            for (size_t q = 0; geom && q < op.classes.size(); ++q) {
-                const ViewSpec& v = op.classes[q].out;
-                if (v.tensor != P.t_feat || v.row_step != OF.t_step || v.kind != PLANE_DIRECT) geom = false;
-                OF.t0[q] = v.row_offset;
-            }
-            // a pair-merged launch has ONE class whose second half is the next frame: classes (even, odd rows) = offsets (0, 1)
-            if (geom && op.classes.size() == 2 && !(OF.t0[0] == 0 && OF.t0[1] == 1 && OF.t_step == 2)) geom = false;
-            if (geom && (targets == nullptr || bw)) h->fuse_out = &OF;       // (loss without gradients: the separate kernel)
-        }
-        rc = conv_forward(h, P.up[i], L + 1 + i);
-        h->fuse_out = nullptr;
-        if (rc != WUN_OK) return rc;
-    }
-    if (h->out_fused) return WUN_OK;
-    if (h->dry && h->export_launches) {      // wun_debug_launches: the output layer's geometry (caller buffers: include/wun.h layouts)
-        char line[768];
-        auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
-        int n = snprintf(line, sizeof(line), "output batch=%d T_in=%d Tf=%d T_out=%d C=%d F=%d nconv=%d K=%d ofs=%d pad_left=%d crop_feat=%d "
-                         "crop_out=%d output_type=%d activation=%d feat=%lld dpre=%lld gfeat=%lld",
-                         O.batch, O.T_in, O.Tf, O.T_out, O.C, O.F, O.nconv, O.K, O.ofs, O.pad_left, O.crop_feat, O.crop_out, O.output_type,
-                         O.activation, addr(O.feat), addr(O.dpre), addr(tensor_ptr(h, P.grad_twin[P.t_feat])));
-        for (int s = 0; s < 8; ++s)
-            n += snprintf(line + n, sizeof(line) - n, " w_off%d=%lld b_off%d=%lld", s, s < O.nconv ? O.w_off[s] : -1LL, s,
-                          s < O.nconv ? O.b_off[s] : -1LL);
-        h->export_launches->push_back(line);
-    }
-    if (h->phase != 1) h->launches += h->train_call ? 2 : 1;       // + a training step's memset of the CTA counters
-    if (!h->dry && h->phase != 1) {
-        // the loss and interp-gradient sums count their CTAs here; each sum's last CTA sets its counter back to 0, this makes
-        // sure they start from 0 whatever the workspace held before
-        if (h->train_call) WUN_CUDA_OK(cudaMemsetAsync(counters_ptr(h), 0, 2 * sizeof(unsigned), h->stream));
-        launch_output_fwd(O, h->stream);
-    }
-    return WUN_OK;
-}
-
-static int run_backward(WunHandle* h, const float* targets, float* grads, float scale) {
-    const Plan& P = h->plan;
-    const int L = P.cfg.num_layers;
-    int rc;
-    h->wstream = h->stream;
-    if (h->phase != 1) h->fork_used = (h->phase == 2) ? 1 : 0;
-    if (!h->dry && h->use_side) {
-        int rcs = ensure_side(h);
-        if (rcs != WUN_OK) return rcs;
-        h->wstream = h->side;
-    }
-    OutputLaunch O;
-    fill_output_launch(h, &O, targets, nullptr, nullptr, 1);
-    // fused forward (run_forward): dL/dpre and the feature gradient already exist; only the output convs' weight gradient is left
-    // (mode 1), and it goes to the wgrad stream right after the first fork below
-    const bool out_wgrad_late = h->out_fused && h->out_fuse_mode != 2;
-    if (h->dry) h->out_part_bytes = std::max(h->out_part_bytes, output_wgrad_partial_bytes(O));
-    if (h->phase != 1 && !h->out_fused) h->launches += 3;
-    if (h->phase != 1 && out_wgrad_late) h->launches += 2;
-    if (!h->dry && h->phase != 1 && !h->out_fused) {
-        launch_output_wgrad(O, grads, out_part_ptr(h), scale, h->stream);
-        launch_output_dgrad(O, const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat])), h->stream);
-    }
-    if (h->phase != 1) h->bucket_next = 0;
-    int64_t ready_from = h->plan.param_numel;      // lowest flat offset whose gradient is complete once the next fork is passed
-    if (P.nconv > 0) ready_from = std::min<int64_t>(P.params[P.out_w_param[0]].offset, P.params[P.out_b_param[0]].offset);
-    for (int i = L - 1; i >= 0; --i) {
-        const ConvOp& op = P.up[i];
-        if ((rc = fork_side(h)) != WUN_OK) return rc;
-        if (i == L - 1 && out_wgrad_late && !h->dry && h->phase != 1) launch_output_wgrad(O, grads, out_part_ptr(h), scale, h->wstream);
-        if ((rc = mark_grads_ready(h, ready_from, h->wstream)) != WUN_OK) return rc;
-        ready_from = std::min(ready_from, op_first_offset(P, op, &P.ups[i]));
-        if ((rc = conv_wgrad(h, op, grads, scale, L + 1 + i)) != WUN_OK) return rc;
-        if ((rc = conv_dgrad(h, op, h->bwd_up[i], L + 1 + i)) != WUN_OK) return rc;
-        const UpsampleSpec& us = P.ups[i];
-        UpsampleBwdLaunch U;
-        memset(&U, 0, sizeof(U));
-        U.due = tensor_ptr(h, P.t_gue);
-        U.dmid = tensor_ptr(h, P.t_gmid);
-        U.x = tensor_ptr(h, us.src_tensor);
-        U.gx = const_cast<float*>(tensor_ptr(h, P.grad_twin[us.src_tensor]));
-        U.blend = (us.wsig_tensor >= 0) ? tensor_ptr(h, us.wsig_tensor) : nullptr;
-        U.dvar = (us.interp_param >= 0) ? grads + P.params[us.interp_param].offset : nullptr;
-        U.part = U.dvar ? dvar_part_ptr(h) : nullptr;
-        U.count = U.dvar ? counters_ptr(h) + 1 : nullptr;
-        U.batch = h->batch; U.N = us.N; U.nmid = us.nmid; U.C = us.C; U.mid_mode = us.mid_mode; U.scale = scale;
-        if (h->dry && h->export_launches) {  // wun_debug_launches: dvar = the interp parameter's flat offset (gradient buffer) or -1
-            char line[512];
-            auto addr = [](const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); };
-            snprintf(line, sizeof(line), "upsample level=%d batch=%d N=%d nmid=%d C=%d mid_mode=%d due=%lld dmid=%lld x=%lld gx=%lld blend=%lld dvar=%lld",
-                     i, U.batch, U.N, U.nmid, U.C, U.mid_mode, addr(U.due), addr(U.dmid), addr(U.x), addr(U.gx), U.blend ? addr(U.blend) : -1LL,
-                     us.interp_param >= 0 ? (long long)P.params[us.interp_param].offset : -1LL);
-            h->export_launches->push_back(line);
-        }
-        if (h->phase != 1) ++h->launches;
-        if (!h->dry && h->phase != 1) launch_upsample_bwd(U, h->stream);
-    }
-    if ((rc = fork_side(h)) != WUN_OK) return rc;
-    if ((rc = mark_grads_ready(h, ready_from, h->wstream)) != WUN_OK) return rc;
-    ready_from = std::min(ready_from, op_first_offset(P, P.bottleneck, nullptr));
-    if ((rc = conv_wgrad(h, P.bottleneck, grads, scale, L)) != WUN_OK) return rc;
-    if ((rc = conv_dgrad(h, P.bottleneck, h->bwd_bottleneck, L)) != WUN_OK) return rc;
-    for (int i = L - 1; i >= 0; --i) {
-        if ((rc = fork_side(h)) != WUN_OK) return rc;
-        if ((rc = mark_grads_ready(h, ready_from, h->wstream)) != WUN_OK) return rc;
-        ready_from = std::min(ready_from, op_first_offset(P, P.down[i], nullptr));
-        if ((rc = conv_wgrad(h, P.down[i], grads, scale, i)) != WUN_OK) return rc;
-        if ((rc = conv_dgrad(h, P.down[i], h->bwd_down[i], i)) != WUN_OK) return rc;
-    }
-    if (!h->dry && h->phase != 1 && h->wstream != h->stream) {       // join: the caller's stream continues only after all wgrads
-        WUN_CUDA_OK(cudaEventRecord(h->join_event, h->side));
-        WUN_CUDA_OK(cudaStreamWaitEvent(h->stream, h->join_event, 0));
-        if (h->first_pending) { WUN_CUDA_OK(cudaStreamWaitEvent(h->stream, h->first_done, 0)); h->first_pending = false; }
-    }
-    if ((rc = mark_grads_ready(h, 0, h->stream)) != WUN_OK) return rc;    // whatever is left: final after the join
-    return WUN_OK;
-}
-
-static int check_device() {
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0) {
-        cudaGetLastError();
-        return set_err(WUN_E_NOGPU, "no CUDA device: the engine has no CPU fallback");
-    }
-    return WUN_OK;
 }
 
 // bytes of the split arena behind the weight packs (bulk-fed wgrad only; per-item size from the dry run at create time)
@@ -1097,16 +615,407 @@ static float* dvar_part_ptr(const WunHandle* h) {
     return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(loss_part_ptr(h)) + output_loss_partial_bytes(h->batch, (int)h->plan.T_out));
 }
 
+static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, int layer_index) {
+    const WunHandle* h = b.h;
+    const Plan& P = h->plan;
+    b.layer = layer_index; b.pass = 2;
+    // split passes ahead on their own stream (see WunHandle::split_ahead)
+    const bool ahead = h->split_ahead && b.ws != ST_CALLER;
+    if (layer_index == 0) {
+        FirstWgrad FW;
+        if (first_layer_desc(h, op, &FW.L)) {          // one launcher call: dW and db of both classes (per-CTA sums + their total)
+            FW.part = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum +
+                                               split_arena_bytes(h, h->batch));
+            FW.L.dec = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor]));
+            FW.L.odd = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor]));
+            FW.dW = grads + P.params[op.w_param].offset;
+            FW.db = grads + P.params[op.b_param].offset;
+            FW.scale = scale; FW.rows_per_cta = 0;
+            // the CUDA-core first-layer gradient is the tail of the step: on the split stream it runs next to the second
+            // block's tensor-core wgrad instead of behind it (joined at the end of build_backward)
+            static const bool tail_on = [] { const char* e = getenv("WUN_FIRST_TAIL"); return !(e && e[0] == '0'); }();
+            const bool tail_par = tail_on && ahead;
+            add(b, OP_FIRST_WGRAD, tail_par ? ST_SPLIT : b.ws).fw = FW;
+            if (tail_par) {
+                add(b, OP_MAKE, ST_SPLIT, EV_FIRST_DONE, 1);
+                add(b, OP_RECORD, ST_SPLIT, EV_FIRST_DONE);
+                b.first_pending = true;
+            }
+            return WUN_OK;
+        }
+    }
+    // collect (class, plane) groups
+    std::vector<WgradLaunch> groups;
+    std::vector<PlaneView> class_dpre;
+    for (const auto& c : op.classes) {
+        if (c.m_hi <= c.m_lo) continue;
+        PlaneView dpre = make_plane_on(h, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
+        class_dpre.push_back(dpre);                            // bias gradient = its column sums (fused into the split pass below)
+        size_t i = 0;
+        while (i < c.terms.size()) {
+            WgradLaunch W;
+            memset(&W, 0, sizeof(W));
+            const int p = c.terms[i].plane;
+            int dmin = c.terms[i].d;
+            while (i < c.terms.size() && c.terms[i].plane == p && W.nterms < 8 && c.terms[i].d - dmin <= 15) {
+                W.d[W.nterms] = c.terms[i].d;
+                W.woff[W.nterms] = (c.terms[i].tap * op.cin_tot + c.terms[i].coff) * op.cout;
+                ++W.nterms; ++i;
+            }
+            W.plane = make_plane(h, op.planes[p]);
+            W.dpre = dpre;
+            W.m_lo = c.m_lo; W.m_hi = c.m_hi;
+            W.N = op.cout; W.w_sk = op.cout; W.w_sn = 1;
+            W.dW = grads + P.params[op.w_param].offset;
+            W.scale = scale; W.batch = h->batch;
+            groups.push_back(W);
+        }
+    }
+    // tensor cores: all groups of the layer in ONE launch
+    bool use_umma = h->umma_enabled && h->umma_pass[2] && !groups.empty() && groups.size() <= (size_t)kWgMaxGroups;
+    UmmaWgradLaunch U;
+    if (use_umma) {
+        memset(&U, 0, sizeof(U));
+        U.ngroups = (int)groups.size(); U.batch = h->batch; U.dW = groups[0].dW;
+        U.w_sp = op.cout; U.w_sg = 1; U.scale = scale;
+        for (size_t g = 0; g < groups.size(); ++g) {
+            WgGroup& G = U.grp[g];
+            G.P = groups[g].plane; G.G = groups[g].dpre; G.m_lo = groups[g].m_lo; G.m_hi = groups[g].m_hi;
+            G.ntaps = groups[g].nterms;
+            for (int t = 0; t < G.ntaps; ++t) { G.d[t] = groups[g].d[t]; G.woff[t] = groups[g].woff[t]; }
+        }
+        use_umma = umma_plan_wgrad(&U);
+    }
+    float* bias_grad = grads ? grads + P.params[op.b_param].offset : nullptr;
+    auto colsum_launches = [&]() {                        // bias gradient by its own kernel (paths without a split pass)
+        for (const auto& dp : class_dpre) {
+            Op& o = add(b, OP_COLSUM, b.ws);
+            o.colsum.V = dp; o.colsum.batch = h->batch; o.colsum.scale = scale; o.colsum.out = bias_grad;
+        }
+    };
+    if (use_umma) {
+        const size_t split_need = h->bulk_wgrad ? umma_plan_wgrad_split(U, 1, nullptr, nullptr, nullptr) : 0;
+        const bool bulk = split_need > 0;                 // 0: too many distinct views for one split pass -> converter-fed kernel
+        // Bias column sums inside the split pass instead of their own launches (WUN_SPLIT_COLSUM: 1 = default, 0 = separate colsum
+        // launches, 2 = fused only for the layers with few rows).  History: while the dgrad chain was the critical path the separate
+        // launches were 0.05 ms faster per step (they fill SMs the big-shared-memory kernels leave thread slots on); since the epilogue
+        // work of round 2 the wgrad stream is the critical path and the fused form wins (5.45 -> 5.39 ms, wgrad family 2.52 -> 2.24 ms).
+        static const int colsum_mode = [] { const char* e = getenv("WUN_SPLIT_COLSUM"); return e ? atoi(e) : 1; }();
+        int max_rows_g = 0;
+        for (const auto& dp : class_dpre) max_rows_g = std::max(max_rows_g, dp.r_hi - dp.r_lo);
+        const bool fused_colsum = colsum_mode == 1 || (colsum_mode == 2 && max_rows_g <= 4096);
+        if (bulk) {      // + the split pass and the fixed-order reduction of the partial tiles / column sums
+            b.split_item = std::max(b.split_item, split_need);
+            b.wg_partial = std::max(b.wg_partial, umma_wgrad_partial_bytes(U));
+        }
+        if (!bulk || !fused_colsum) colsum_launches();
+        if (!bulk) {
+            add(b, OP_WGRAD_UMMA, b.ws).wgu.U = U;
+            return WUN_OK;
+        }
+        uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum;
+        if (ahead && (b.wg_index & 1)) arena += split_arena_half_bytes(h, h->batch);
+        arena += (256 - (reinterpret_cast<uintptr_t>(arena) & 255)) & 255;
+        // split arrays, then the partial tiles, in this half; the class-gradient views among the jobs also produce the
+        // bias gradient (their column sums)
+        decltype(Op::wgu) W;     // shared by the split pass, the wgrad and its reduction
+        if (!umma_wgrad_bulk_setup(&U, h->batch, arena, class_dpre.data(), (int)class_dpre.size(), fused_colsum ? bias_grad : nullptr,
+                                   scale, &W.S, &W.J))
+            return set_err(WUN_E_INVALID, "wgrad split pass: class gradient view not among the split jobs");
+        W.U = U;
+        const StreamRole ss = ahead ? ST_SPLIT : b.ws;   // else the same stream as the wgrad: the arena is reused layer after layer
+        const int k = ahead ? b.wg_index++ : 0;
+        if (ahead) {
+            add(b, OP_MAKE, ST_SPLIT, EV_SPLIT_DONE, k + 1);
+            add(b, OP_MAKE, ST_SPLIT, EV_WG_DONE, k + 1);
+            if (k >= 2) add(b, OP_WAIT, ST_SPLIT, EV_WG_DONE, k - 2);     // its arena half is free again
+        }
+        add(b, OP_SPLIT, ss).wgu = W;
+        if (ahead) {
+            add(b, OP_RECORD, ST_SPLIT, EV_SPLIT_DONE, k);
+            add(b, OP_WAIT, b.ws, EV_SPLIT_DONE, k);
+        }
+        add(b, OP_WGRAD_BULK, b.ws).wgu = W;
+        add(b, OP_WGRAD_REDUCE, b.ws).wgu = W;
+        if (ahead) add(b, OP_RECORD, b.ws, EV_WG_DONE, k);
+        return WUN_OK;
+    }
+    colsum_launches();
+    for (size_t g = 0; g < groups.size(); ++g) add(b, OP_WGRAD, b.ws, EV_NONE, (int)g).wg = groups[g];
+    return WUN_OK;
+}
+
+// fork: everything enqueued on the main stream so far is visible to the side stream
+static void fork_side(Build& b) {
+    if (b.ws == ST_CALLER) return;
+    add(b, OP_MAKE, ST_CALLER, EV_FORK, b.fork_used + 1);
+    add(b, OP_RECORD, ST_CALLER, EV_FORK, b.fork_used);
+    add(b, OP_WAIT, ST_SIDE, EV_FORK, b.fork_used);
+    if (b.h->split_ahead) {
+        add(b, OP_MAKE, ST_SPLIT);
+        add(b, OP_WAIT, ST_SPLIT, EV_FORK, b.fork_used);
+    }
+    ++b.fork_used;
+}
+
+// Every gradient at a flat offset >= `ready_from` has been enqueued (side-stream work in order, main-stream work up to the
+// last fork): record the events of the buckets this completes.  Called right after a fork (side waits for main) or at the end.
+static void mark_grads_ready(Build& b, int64_t ready_from, StreamRole on) {
+    const WunHandle* h = b.h;
+    while (b.bucket_next < (int)h->bucket_first.size() && h->bucket_first[b.bucket_next] >= ready_from) {
+        add(b, OP_RECORD, on, EV_BUCKET, b.bucket_next);
+        ++b.bucket_next;
+    }
+}
+
+static int64_t op_first_offset(const Plan& P, const ConvOp& op, const UpsampleSpec* us) {
+    int64_t o = std::min(P.params[op.w_param].offset, P.params[op.b_param].offset);
+    if (us && us->interp_param >= 0) o = std::min<int64_t>(o, P.params[us->interp_param].offset);
+    return o;
+}
+
+static void fill_output_launch(const WunHandle* h, OutputLaunch* O, const float* targets, float* outputs, float* loss,
+                               int training) {
+    const Plan& P = h->plan;
+    memset(O, 0, sizeof(*O));
+    O->params = h->params;
+    for (int s = 0; s < P.nconv; ++s) {
+        O->w_off[s] = P.params[P.out_w_param[s]].offset;
+        O->b_off[s] = P.params[P.out_b_param[s]].offset;
+    }
+    O->mix = h->mix;
+    O->feat = tensor_ptr(h, P.t_feat);
+    O->targets = targets;
+    O->outputs = outputs;
+    O->dpre = (h->lay.off[P.t_dpre_out] >= 0) ? const_cast<float*>(tensor_ptr(h, P.t_dpre_out)) : nullptr;
+    O->loss = loss;
+    O->loss_part = loss ? loss_part_ptr(h) : nullptr;
+    O->loss_count = loss ? counters_ptr(h) : nullptr;
+    O->batch = h->batch; O->T_in = (int)P.T_in; O->Tf = (int)P.Tf; O->T_out = (int)P.T_out;
+    O->C = P.cfg.num_channels; O->F = P.cfg.num_initial_filters;
+    O->nconv = P.nconv; O->K = P.cfg.num_sources;
+    O->ofs = P.cfg.output_filter_size; O->pad_left = P.out_pad_left;
+    O->crop_feat = P.crop_feat; O->crop_out = P.crop_out;
+    O->output_type = P.cfg.output_type; O->activation = P.cfg.output_activation; O->training = training;
+    O->inv_count = 1.0f / (float)((double)h->batch * P.T_out * P.cfg.num_channels * P.cfg.num_sources);
+}
+
+static int build_forward(Build& b, const float* targets, float* outputs, float* loss, int training) {
+    const WunHandle* h = b.h;
+    const Plan& P = h->plan;
+    const int L = P.cfg.num_layers;
+    for (int i = 0; i < L; ++i) {
+        const UpsampleSpec& us = P.ups[i];
+        if (us.interp_param >= 0) {
+            Op& o = add(b, OP_SIGMOID);
+            o.sig.x = h->params + P.params[us.interp_param].offset;
+            o.sig.y = const_cast<float*>(tensor_ptr(h, us.wsig_tensor)); o.sig.n = us.C;
+        }
+    }
+    int rc;
+    for (int i = 0; i < L; ++i)
+        if ((rc = build_conv_forward(b, P.down[i], i)) != WUN_OK) return rc;
+    if ((rc = build_conv_forward(b, P.bottleneck, L)) != WUN_OK) return rc;
+    OutputLaunch O;
+    fill_output_launch(h, &O, targets, outputs, loss, training);
+    OutputFuse OF;
+    memset(&OF, 0, sizeof(OF));
+    b.out_fused = false;
+    for (int i = 0; i < L; ++i) {
+        if (i == L - 1 && h->out_fuse_mode != 0 && P.cfg.output_filter_size == 1) {
+            // the output layer rides in this conv's epilogue when the planner picks the persistent kernel for it
+            OF.O = O;
+            const bool bw = targets != nullptr && b.grads != nullptr;
+            OF.gfeat = bw ? const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat])) : nullptr;
+            OF.grads = (bw && h->out_fuse_mode == 2) ? b.grads : nullptr;
+            OF.grad_scale = b.scale;
+            const ConvOp& op = P.up[i];
+            bool geom = op.classes.size() >= 1 && op.classes.size() <= (size_t)kMaxClasses;
+            OF.t_step = geom ? op.classes[0].out.row_step : 0;
+            for (size_t q = 0; geom && q < op.classes.size(); ++q) {
+                const ViewSpec& v = op.classes[q].out;
+                if (v.tensor != P.t_feat || v.row_step != OF.t_step || v.kind != PLANE_DIRECT) geom = false;
+                OF.t0[q] = v.row_offset;
+            }
+            // a pair-merged launch has ONE class whose second half is the next frame: classes (even, odd rows) = offsets (0, 1)
+            if (geom && op.classes.size() == 2 && !(OF.t0[0] == 0 && OF.t0[1] == 1 && OF.t_step == 2)) geom = false;
+            if (geom && (targets == nullptr || bw)) b.fuse = &OF;       // (loss without gradients: the separate kernel)
+        }
+        rc = build_conv_forward(b, P.up[i], L + 1 + i);
+        b.fuse = nullptr;
+        if (rc != WUN_OK) return rc;
+    }
+    if (b.out_fused) return WUN_OK;
+    // the loss and interp-gradient sums count their CTAs here; each sum's last CTA sets its counter back to 0, this makes
+    // sure they start from 0 whatever the workspace held before
+    if (b.train) add(b, OP_COUNTERS).counters = counters_ptr(h);
+    add(b, OP_OUTPUT_FWD).out.O = O;
+    return WUN_OK;
+}
+
+static int build_backward(Build& b, const float* targets, float* grads, float scale) {
+    const WunHandle* h = b.h;
+    const Plan& P = h->plan;
+    const int L = P.cfg.num_layers;
+    int rc;
+    b.ws = h->use_side ? ST_SIDE : ST_CALLER;
+    b.fork_used = b.hoist ? 1 : 0;
+    if (h->use_side) add(b, OP_MAKE, ST_SIDE);
+    OutputLaunch O;
+    fill_output_launch(h, &O, targets, nullptr, nullptr, 1);
+    // fused forward (build_forward): dL/dpre and the feature gradient already exist; only the output convs' weight gradient is left
+    // (mode 1), and it goes to the wgrad stream right after the first fork below
+    const bool out_wgrad_late = b.out_fused && h->out_fuse_mode != 2;
+    b.out_part = std::max(b.out_part, output_wgrad_partial_bytes(O));
+    decltype(Op::out) out;         // the output layer's weight gradient (either form) and the gradient w.r.t. the features
+    out.O = O; out.grads = grads; out.part = out_part_ptr(h); out.scale = scale;
+    out.gfeat = const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat]));
+    if (!b.out_fused) {
+        add(b, OP_OUTPUT_WGRAD).out = out;
+        add(b, OP_OUTPUT_DGRAD).out = out;
+    }
+    int64_t ready_from = h->plan.param_numel;      // lowest flat offset whose gradient is complete once the next fork is passed
+    if (P.nconv > 0) ready_from = std::min<int64_t>(P.params[P.out_w_param[0]].offset, P.params[P.out_b_param[0]].offset);
+    for (int i = L - 1; i >= 0; --i) {
+        const ConvOp& op = P.up[i];
+        fork_side(b);
+        if (i == L - 1 && out_wgrad_late) add(b, OP_OUTPUT_WGRAD, b.ws).out = out;
+        mark_grads_ready(b, ready_from, b.ws);
+        ready_from = std::min(ready_from, op_first_offset(P, op, &P.ups[i]));
+        if ((rc = build_wgrad(b, op, grads, scale, L + 1 + i)) != WUN_OK) return rc;
+        if ((rc = build_dgrad(b, op, h->bwd_up[i], L + 1 + i)) != WUN_OK) return rc;
+        const UpsampleSpec& us = P.ups[i];
+        UpsampleBwdLaunch U;
+        memset(&U, 0, sizeof(U));
+        U.due = tensor_ptr(h, P.t_gue);
+        U.dmid = tensor_ptr(h, P.t_gmid);
+        U.x = tensor_ptr(h, us.src_tensor);
+        U.gx = const_cast<float*>(tensor_ptr(h, P.grad_twin[us.src_tensor]));
+        U.blend = (us.wsig_tensor >= 0) ? tensor_ptr(h, us.wsig_tensor) : nullptr;
+        U.dvar = (us.interp_param >= 0) ? grads + P.params[us.interp_param].offset : nullptr;
+        U.part = U.dvar ? dvar_part_ptr(h) : nullptr;
+        U.count = U.dvar ? counters_ptr(h) + 1 : nullptr;
+        U.batch = h->batch; U.N = us.N; U.nmid = us.nmid; U.C = us.C; U.mid_mode = us.mid_mode; U.scale = scale;
+        Op& o = add(b, OP_UPSAMPLE_BWD);
+        o.up = U; o.layer = L + 1 + i;
+    }
+    fork_side(b);
+    mark_grads_ready(b, ready_from, b.ws);
+    ready_from = std::min(ready_from, op_first_offset(P, P.bottleneck, nullptr));
+    if ((rc = build_wgrad(b, P.bottleneck, grads, scale, L)) != WUN_OK) return rc;
+    if ((rc = build_dgrad(b, P.bottleneck, h->bwd_bottleneck, L)) != WUN_OK) return rc;
+    for (int i = L - 1; i >= 0; --i) {
+        fork_side(b);
+        mark_grads_ready(b, ready_from, b.ws);
+        ready_from = std::min(ready_from, op_first_offset(P, P.down[i], nullptr));
+        if ((rc = build_wgrad(b, P.down[i], grads, scale, i)) != WUN_OK) return rc;
+        if ((rc = build_dgrad(b, P.down[i], h->bwd_down[i], i)) != WUN_OK) return rc;
+    }
+    if (b.ws != ST_CALLER) {       // join: the caller's stream continues only after all wgrads
+        add(b, OP_RECORD, ST_SIDE, EV_JOIN);
+        add(b, OP_WAIT, ST_CALLER, EV_JOIN);
+        if (b.first_pending) { add(b, OP_WAIT, ST_CALLER, EV_FIRST_DONE); b.first_pending = false; }
+    }
+    mark_grads_ready(b, 0, ST_CALLER);    // whatever is left: final after the join
+    return WUN_OK;
+}
+
+// A training step: forward + backward, the weight packs hoisted onto the side stream when there is one.
+static int build_step(Build& b, const float* targets, float* outputs, float* loss, float* grads, float scale) {
+    const WunHandle* h = b.h;
+    b.hoist = h->use_side && h->umma_enabled;
+    b.dgrad_fork = h->dgrad_par && h->use_side;
+    b.grads = grads; b.scale = scale; b.train = true;
+    if (b.hoist) {             // the packs go to the side stream behind the work already enqueued on the caller's stream
+        add(b, OP_MAKE, ST_SIDE).early = true;
+        add(b, OP_MAKE, ST_CALLER, EV_FORK, 1).early = true;
+        add(b, OP_RECORD, ST_CALLER, EV_FORK).early = true;
+        add(b, OP_WAIT, ST_SIDE, EV_FORK).early = true;
+        b.packs_pending = true;
+    }
+    int rc = build_forward(b, targets, outputs, loss, 1);
+    if (rc == WUN_OK) rc = build_backward(b, targets, grads, scale);
+    if (rc != WUN_OK || !b.hoist) return rc;
+    add(b, OP_RECORD, ST_SIDE, EV_PACKS).early = true;
+    if (b.packs_pending) add(b, OP_WAIT, ST_CALLER, EV_PACKS);   // no tensor-core conv consumed the packs: still join the side stream
+    return WUN_OK;
+}
+
+static cudaError_t make_events(std::vector<cudaEvent_t>& v, size_t n) {
+    while (v.size() < n) {
+        cudaEvent_t e;
+        const cudaError_t r = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+        if (r != cudaSuccess) return r;
+        v.push_back(e);
+    }
+    return cudaSuccess;
+}
+
+static cudaError_t make(WunHandle* h, const Op& o) {
+    if (o.pool != EV_NONE) return make_events(h->events[o.pool], o.index);
+    cudaStream_t& s = h->streams[o.stream];
+    if (s) return cudaSuccess;
+    cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
+    if (e == cudaSuccess && o.stream == ST_SIDE) e = make_events(h->events[EV_JOIN], 1);
+    if (e == cudaSuccess && o.stream == ST_SIDE) e = make_events(h->events[EV_PACKS], 1);
+    return e;
+}
+
+static int issue_op(WunHandle* h, const Op& o) {
+    const cudaStream_t s = o.stream == ST_CALLER ? h->stream : h->streams[o.stream];
+    cudaError_t e = cudaSuccess;
+    switch (o.kind) {
+        case OP_SIGMOID: launch_sigmoid(o.sig.x, o.sig.y, o.sig.n, s); break;
+        case OP_FIRST_FWD: launch_first_fwd(o.first, h->plan.cfg.num_channels, h->plan.down[0].cout, s); break;
+        case OP_CONV: launch_plane_conv_simt(o.conv, s); break;
+        case OP_PACK: e = launch_umma_pack(o.pack, s); break;
+        case OP_UMMA_CONV: e = launch_plane_conv_umma(o.umma.U, s, o.umma.fused ? &o.umma.fuse : nullptr); break;
+        case OP_COUNTERS: e = cudaMemsetAsync(o.counters, 0, 2 * sizeof(unsigned), s); break;
+        case OP_OUTPUT_FWD: launch_output_fwd(o.out.O, s); break;
+        case OP_OUTPUT_WGRAD: launch_output_wgrad(o.out.O, o.out.grads, o.out.part, o.out.scale, s); break;
+        case OP_OUTPUT_DGRAD: launch_output_dgrad(o.out.O, o.out.gfeat, s); break;
+        case OP_UPSAMPLE_BWD: launch_upsample_bwd(o.up, s); break;
+        case OP_FIRST_WGRAD: launch_first_wgrad(o.fw, h->plan.cfg.num_channels, h->plan.down[0].cout, s); break;
+        case OP_COLSUM: launch_colsum(o.colsum.V, o.colsum.batch, o.colsum.scale, o.colsum.out, s); break;
+        case OP_WGRAD: launch_plane_wgrad_simt(o.wg, s); break;
+        case OP_WGRAD_UMMA: e = launch_wgrad_umma(o.wgu.U, s); break;
+        case OP_SPLIT: e = launch_split_views(o.wgu.J, s); break;
+        case OP_WGRAD_BULK: e = launch_wgrad_umma_bulk(o.wgu.U, o.wgu.S, s); break;
+        case OP_WGRAD_REDUCE: e = launch_wgrad_reduce(o.wgu.U, o.wgu.J, s); break;
+        case OP_RECORD: e = cudaEventRecord(h->events[o.pool][o.index], s); break;
+        case OP_WAIT: e = cudaStreamWaitEvent(s, h->events[o.pool][o.index], 0); break;
+        case OP_MAKE: e = make(h, o); break;
+    }
+    if (e != cudaSuccess) return set_err(WUN_E_CUDA, std::string(o.kind < OP_RECORD ? "launch: " : "stream / event call: ") + cudaGetErrorString(e));
+    return WUN_OK;
+}
+
+// The records in order; with hoisted weight packs, the `early` ones (the packs and their events on the side stream) first.
+static int issue(WunHandle* h, const std::vector<Op>& ops) {
+    int rc = WUN_OK;
+    for (int early = 1; early >= 0; --early)
+        for (size_t i = 0; i < ops.size() && rc == WUN_OK; ++i)
+            if (ops[i].early == (early == 1)) rc = issue_op(h, ops[i]);
+    return rc;
+}
+
+static int check_device() {
+    int n = 0;
+    cudaError_t e = cudaGetDeviceCount(&n);
+    if (e != cudaSuccess || n == 0) {
+        cudaGetLastError();
+        return set_err(WUN_E_NOGPU, "no CUDA device: the engine has no CPU fallback");
+    }
+    return WUN_OK;
+}
+
 static int begin_call(WunHandle* h, const float* params, const float* mix, int64_t batch, bool training, void* ws,
                       int64_t ws_bytes, void* stream, bool dry) {
     if (!h) return set_err(WUN_E_INVALID, "null handle");
     if (batch < 1 || batch > (1 << 20)) return set_err(WUN_E_INVALID, "batch out of range");
     h->lay = make_layout(h->plan, batch, training);
-    h->dry = dry;
-    h->train_call = training;
-    h->launches = 0;
     h->batch = (int)batch;
-    h->bw_grads = nullptr; h->bw_scale = 1.f; h->fuse_out = nullptr; h->out_fused = false; h->par_used = 0; h->wg_index = 0; h->first_pending = false;
+    h->ops.clear();
     if (dry) return WUN_OK;
     { int rc0 = check_device(); if (rc0 != WUN_OK) return rc0; }
     if (!params || !mix || !ws) return set_err(WUN_E_INVALID, "null device pointer");
@@ -1115,6 +1024,170 @@ static int begin_call(WunHandle* h, const float* params, const float* mix, int64
     if (reinterpret_cast<uintptr_t>(ws) % 256 != 0) return set_err(WUN_E_INVALID, "workspace must be 256-byte aligned");
     h->params = params; h->mix = mix; h->ws = (float*)ws; h->stream = (cudaStream_t)stream;
     return WUN_OK;
+}
+
+// The launch list of a training step (`training` false: an inference forward) at `batch` for the entry points that describe or
+// count launches: built without a device, never issued.
+static Build build_dry(WunHandle* h, int64_t batch, bool training) {
+    begin_call(h, nullptr, nullptr, batch, training, nullptr, 0, nullptr, true);
+    Build b{h, h->ops};
+    if (training) build_step(b, nullptr, nullptr, nullptr, nullptr, 1.f);
+    else build_forward(b, nullptr, nullptr, nullptr, 0);
+    return b;
+}
+
+static const ConvOp& layer_op(const WunHandle* h, int layer) {
+    const int L = h->plan.cfg.num_layers;
+    return (layer < L) ? h->plan.down[layer] : (layer == L ? h->plan.bottleneck : h->plan.up[layer - L - 1]);
+}
+
+// kernel records, counted as launches: the output and first-layer weight gradients are two kernels each (per-CTA sums + their
+// fixed-order total), the counter memset counts as one
+static int64_t kernel_launches(const std::vector<Op>& ops) {
+    int64_t n = 0;
+    for (const Op& o : ops)
+        if (o.kind < OP_RECORD) n += (o.kind == OP_OUTPUT_WGRAD || o.kind == OP_FIRST_WGRAD) ? 2 : 1;
+    return n;
+}
+
+// ------------------------------------------------------------------------------------------------
+// launch descriptions (wun_debug_plan, wun_debug_launches)
+// ------------------------------------------------------------------------------------------------
+static long long addr(const void* p) { return (long long)reinterpret_cast<uintptr_t>(p); }
+
+static void appendf(std::string& s, const char* fmt, ...) {
+    char line[1024];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(line, sizeof(line), fmt, ap);
+    va_end(ap);
+    s += line;
+}
+
+static int64_t copy_out(const std::string& s, char* buf, int64_t capacity) {
+    if (buf && capacity > 0) {
+        int64_t n = std::min<int64_t>(capacity - 1, (int64_t)s.size());
+        memcpy(buf, s.data(), n);
+        buf[n] = 0;
+    }
+    return (int64_t)s.size() + 1;
+}
+
+// wun_debug_plan: one line per tensor-core conv, one per group of a tensor-core weight gradient
+static void audit_op(std::string& s, const Op& o) {
+    if (o.kind == OP_UMMA_CONV) {
+        const ConvLaunch& L = o.umma.L;
+        const UmmaChoice& ch = o.umma.ch;
+        long long tiles = 0, mmas = 0; int max_rows = 0, span = 0;
+        for (int q = 0; q < L.ncls; ++q) {
+            const int rows = L.cls[q].m_hi - L.cls[q].m_lo;
+            const long long tq = (long long)((rows + ch.MT * 128 - 1) / (ch.MT * 128)) * ch.nsplit * L.batch;
+            tiles += tq;
+            max_rows = std::max(max_rows, rows);
+            int t = L.cls[q].term_begin;
+            long long ksteps = 0;                       // (16-channel chunk, tap) pairs of one tile of this class
+            while (t < L.cls[q].term_end) {
+                int t1 = t, dmin = L.terms[t].d, dmax = dmin;
+                while (t1 < L.cls[q].term_end && L.terms[t1].plane == L.terms[t].plane) {
+                    dmin = std::min(dmin, L.terms[t1].d); dmax = std::max(dmax, L.terms[t1].d); ++t1; }
+                span = std::max(span, dmax - dmin);
+                ksteps += (long long)((L.planes[L.terms[t].plane].C + 15) / 16) * (t1 - t);
+                t = t1;
+            }
+            mmas += tq * ch.MT * ksteps * 3;
+        }
+        appendf(s, "conv layer=%d pass=%d kernel=wgmma N=%d NPAD=%d nsplit=%d MT=%d rows_alloc=%d span=%d "
+                "TB=%d nbs=%d tiles=%lld mmas=%lld max_rows=%d smem=%zu pack_bytes=%zu pair=%d outfuse=%d\n",
+                o.layer, o.pass, L.N, ch.NPAD, ch.nsplit, ch.MT, ch.rows_alloc, span, ch.TB, ch.nbs, tiles, mmas,
+                max_rows, umma_choice_smem_bytes(ch), ch.pack_bytes, L.pairC, o.umma.fused ? 1 : 0);
+    } else if (o.kind == OP_WGRAD_UMMA || o.kind == OP_WGRAD_BULK) {
+        const UmmaWgradLaunch& U = o.wgu.U;
+        for (int g = 0; g < U.ngroups; ++g) {
+            const WgGroup& G = U.grp[g];
+            appendf(s, "wgrad layer=%d group=%d Cp=%d Cg=%d swap=%d NT=%d mtiles=%d ntiles=%d ntaps=%d taps_per_cta=%d "
+                    "tapsets=%d chunks_per_cta=%d n_ctas_x=%d chunks=%lld grid=%dx%dx%d nstages=%d smem=%zu issued_macs=%lld useful_macs=%lld\n",
+                    o.layer, g, G.P.C, G.G.C, G.swap, G.NT, G.n_mtiles, G.n_ntiles, G.ntaps, G.taps_per_cta, G.n_tapsets,
+                    G.chunks_per_cta, G.n_ctas_x, (long long)U.batch * G.chunks_per_batch, U.grid_x, U.grid_y, U.grid_z, U.nstages,
+                    umma_wgrad_smem_bytes(U), umma_wgrad_issued_macs(G, U.batch),
+                    (long long)U.batch * G.chunks_per_batch * 64 * G.ntaps * G.P.C * G.G.C);
+        }
+    }
+}
+
+static void describe_view(std::string& s, const char* tag, const PlaneView& P) {
+    appendf(s, "%s base=%lld bstride=%lld rstride=%d r_lo=%d r_hi=%d C=%d kind=%d mid_mode=%d xrows=%d blend=%lld\n",
+            tag, addr(P.base), P.bstride, P.rstride, P.r_lo, P.r_hi, P.C, P.kind, P.mid_mode, P.xrows, P.blend ? addr(P.blend) : -1LL);
+}
+
+// one plane-convolution launch; tests/test_launch_semantics.py interprets these descriptions in numpy: the pair-merged form of
+// a launch must compute exactly what its two-class form does
+static void describe_conv(std::string& s, const ConvLaunch& L, int layer, int pass) {
+    appendf(s, "launch layer=%d pass=%d N=%d pairC=%d w_sk=%d w_sn=%d W=%lld bias=%lld epilogue=%d batch=%d nplanes=%d ncls=%d\n",
+            layer, pass, L.N, L.pairC, L.w_sk, L.w_sn, addr(L.W), L.bias ? addr(L.bias) : -1LL, L.epilogue, L.batch, L.nplanes, L.ncls);
+    for (int p = 0; p < L.nplanes; ++p) describe_view(s, ("plane i=" + std::to_string(p)).c_str(), L.planes[p]);
+    int nterm = 0;
+    for (int q = 0; q < L.ncls; ++q) {
+        const OutView& O = L.cls[q];
+        nterm = std::max(nterm, O.term_end);
+        appendf(s, "cls i=%d base=%lld bstride=%lld rstride=%d m_lo=%d m_hi=%d saved=%lld acc_lo=%d acc_hi=%d term_begin=%d term_end=%d "
+                "pairC=%d base2=%lld bstride2=%lld rstride2=%d saved2=%lld acc_lo2=%d acc_hi2=%d lo0=%d hi0=%d lo1=%d hi1=%d\n",
+                q, addr(O.base), O.bstride, O.rstride, O.m_lo, O.m_hi, O.saved ? addr(O.saved) : -1LL, O.acc_lo, O.acc_hi, O.term_begin, O.term_end,
+                O.pairC, O.pairC ? addr(O.base2) : -1LL, O.bstride2, O.rstride2, (O.pairC && O.saved2) ? addr(O.saved2) : -1LL, O.acc_lo2, O.acc_hi2,
+                O.lo_h[0], O.hi_h[0], O.lo_h[1], O.hi_h[1]);
+    }
+    for (int t = 0; t < nterm; ++t)
+        appendf(s, "term i=%d plane=%d d=%d woff=%d woff2=%d\n", t, L.terms[t].plane, L.terms[t].d, L.terms[t].woff, L.pairC ? L.terms[t].woff2 : -1);
+}
+
+// one (class, plane) group of a layer's weight gradient (dW[woff + c*cout + n], any form); dW / db = flat parameter offsets
+static void describe_wgrad(std::string& s, const WunHandle* h, const WgGroup& G, int layer, int g) {
+    const ConvOp& op = layer_op(h, layer);
+    appendf(s, "wgrad layer=%d group=%d N=%d w_sk=%d w_sn=%d dW=%lld db=%lld m_lo=%d m_hi=%d nterms=%d batch=%d\n",
+            layer, g, op.cout, op.cout, 1, (long long)h->plan.params[op.w_param].offset, (long long)h->plan.params[op.b_param].offset,
+            G.m_lo, G.m_hi, G.ntaps, h->batch);
+    describe_view(s, "wplane", G.P);
+    describe_view(s, "wdpre", G.G);
+    for (int t = 0; t < G.ntaps; ++t) appendf(s, "wterm i=%d d=%d woff=%d\n", t, G.d[t], G.woff[t]);
+}
+
+// wun_debug_launches: every launch of the step as text (addresses are raw integers relative to the fake bases installed by the
+// caller - nothing is dereferenced)
+static void describe_op(std::string& s, const WunHandle* h, const Op& o) {
+    const Plan& P = h->plan;
+    if (o.kind == OP_FIRST_FWD) {        // its weight gradient has the same geometry; gdec / godd = the gradient tensors it reads
+        const FirstLayer& F = o.first;
+        const ConvOp& op = P.down[0];
+        appendf(s, "first C=%d N=%d k=%d pad_left=%d batch=%d x=%lld x_bstride=%lld T=%d dec=%lld dec_bstride=%lld Td=%d "
+                "odd=%lld odd_bstride=%lld mo_lo=%d mo_hi=%d gdec=%lld godd=%lld dW=%lld db=%lld\n",
+                P.cfg.num_channels, op.cout, F.k, F.pad_left, F.batch, addr(F.x), F.x_bstride, F.T, addr(F.dec), F.dec_bstride, F.Td,
+                addr(F.odd), F.odd_bstride, F.mo_lo, F.mo_hi, addr(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor])),
+                addr(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor])), (long long)P.params[op.w_param].offset,
+                (long long)P.params[op.b_param].offset);
+    } else if (o.kind == OP_CONV || o.kind == OP_UMMA_CONV) {
+        describe_conv(s, o.kind == OP_CONV ? o.conv : o.umma.L, o.layer, o.pass);
+    } else if (o.kind == OP_OUTPUT_FWD) {    // caller buffers: include/wun.h layouts
+        const OutputLaunch& O = o.out.O;
+        appendf(s, "output batch=%d T_in=%d Tf=%d T_out=%d C=%d F=%d nconv=%d K=%d ofs=%d pad_left=%d crop_feat=%d "
+                "crop_out=%d output_type=%d activation=%d feat=%lld dpre=%lld gfeat=%lld",
+                O.batch, O.T_in, O.Tf, O.T_out, O.C, O.F, O.nconv, O.K, O.ofs, O.pad_left, O.crop_feat, O.crop_out, O.output_type,
+                O.activation, addr(O.feat), addr(O.dpre), addr(tensor_ptr(h, P.grad_twin[P.t_feat])));
+        for (int k = 0; k < 8; ++k)
+            appendf(s, " w_off%d=%lld b_off%d=%lld", k, k < O.nconv ? O.w_off[k] : -1LL, k, k < O.nconv ? O.b_off[k] : -1LL);
+        s += "\n";
+    } else if (o.kind == OP_UPSAMPLE_BWD) {  // dvar = the interp parameter's flat offset (gradient buffer) or -1
+        const UpsampleBwdLaunch& U = o.up;
+        const int i = o.layer - P.cfg.num_layers - 1;
+        appendf(s, "upsample level=%d batch=%d N=%d nmid=%d C=%d mid_mode=%d due=%lld dmid=%lld x=%lld gx=%lld blend=%lld dvar=%lld\n",
+                i, U.batch, U.N, U.nmid, U.C, U.mid_mode, addr(U.due), addr(U.dmid), addr(U.x), addr(U.gx), U.blend ? addr(U.blend) : -1LL,
+                P.ups[i].interp_param >= 0 ? (long long)P.params[P.ups[i].interp_param].offset : -1LL);
+    } else if (o.kind == OP_WGRAD) {         // one group per CUDA-core launch
+        WgGroup G;
+        G.P = o.wg.plane; G.G = o.wg.dpre; G.m_lo = o.wg.m_lo; G.m_hi = o.wg.m_hi; G.ntaps = o.wg.nterms;
+        for (int t = 0; t < G.ntaps; ++t) { G.d[t] = o.wg.d[t]; G.woff[t] = o.wg.woff[t]; }
+        describe_wgrad(s, h, G, o.layer, o.index);
+    } else if (o.kind == OP_WGRAD_UMMA || o.kind == OP_WGRAD_BULK) {    // all groups of the layer in one launch
+        for (int g = 0; g < o.wgu.U.ngroups; ++g) describe_wgrad(s, h, o.wgu.U.grp[g], o.layer, g);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1155,9 +1228,13 @@ int wun_create_for_input(const WunConfig* cfg, int64_t input_frames, WunHandle**
     { const char* v = getenv("WUN_PAIR_MIN_CTAS"); h->pair_min_ctas = v ? atoi(v) : 120; }
     { const char* v = getenv("WUN_OUT_FUSE"); h->out_fuse_mode = v ? atoi(v) : 1; }
     { const char* v = getenv("WUN_PAIR_FWD"); h->pair_fwd = !(v && v[0] == '0'); }
+    // the launch list of a batch-1 training step: which kernel each layer uses and how much scratch the launches need
+    const Build b = build_dry(h, 1, true);
+    h->arena_sum = b.pack_sum; h->split_item_bytes = b.split_item; h->wg_partial_bytes = b.wg_partial; h->out_part_bytes = b.out_part;
     h->kernel_used.assign((size_t)(2 * h->plan.cfg.num_layers + 1) * 3, "simt");
-    // dry run: which kernel each layer uses and how much pack scratch the tensor-core launches need
-    wun_launches_forward_backward(h);
+    for (const Op& o : b.ops)      // a layer pass runs on the kernel of its last plane convolution / weight gradient
+        if (o.kind == OP_CONV || o.kind == OP_WGRAD) h->kernel_used[o.layer * 3 + o.pass] = "simt";
+        else if (o.kind == OP_UMMA_CONV || o.kind == OP_WGRAD_UMMA || o.kind == OP_WGRAD_BULK) h->kernel_used[o.layer * 3 + o.pass] = "umma";
     *out = h;
     return WUN_OK;
 }
@@ -1173,18 +1250,10 @@ int wun_create(const WunConfig* cfg, int64_t num_frames, WunHandle** out) {
 
 int wun_destroy(WunHandle* h) {
     if (h) {
-        for (auto e : h->fork_events) cudaEventDestroy(e);
-        if (h->join_event) cudaEventDestroy(h->join_event);
-        if (h->packs_event) cudaEventDestroy(h->packs_event);
-        for (auto e : h->pack_events) cudaEventDestroy(e);
-        for (auto e : h->bucket_events) cudaEventDestroy(e);
-        if (h->side) cudaStreamDestroy(h->side);
-        if (h->side2) cudaStreamDestroy(h->side2);
-        if (h->split_stream) cudaStreamDestroy(h->split_stream);
-        for (auto e : h->split_done) cudaEventDestroy(e);
-        for (auto e : h->wg_done) cudaEventDestroy(e);
-        if (h->first_done) cudaEventDestroy(h->first_done);
-        for (auto e : h->par_events) cudaEventDestroy(e);
+        for (const auto& pool : h->events)
+            for (auto e : pool) cudaEventDestroy(e);
+        for (auto st : h->streams)
+            if (st) cudaStreamDestroy(st);
         delete h;
     }
     return WUN_OK;
@@ -1213,23 +1282,12 @@ double wun_forward_backward_flops(const WunHandle* h, int64_t batch) {
     return h ? (3.0 * h->plan.fwd_flops_per_item - h->plan.dgrad0_flops_per_item) * batch : 0;
 }
 
-int64_t wun_launches_forward(const WunHandle* hc) {
-    WunHandle* h = const_cast<WunHandle*>(hc);
-    if (begin_call(h, nullptr, nullptr, 1, false, nullptr, 0, nullptr, true) != WUN_OK) return -1;
-    const size_t keep = h->arena_sum;
-    h->phase = 0;
-    run_forward(h, nullptr, nullptr, nullptr, 0);
-    h->arena_sum = keep;
-    return h->launches;
+int64_t wun_launches_forward(const WunHandle* h) {
+    return h ? kernel_launches(build_dry(const_cast<WunHandle*>(h), 1, false).ops) : -1;
 }
 
-int64_t wun_launches_forward_backward(const WunHandle* hc) {
-    WunHandle* h = const_cast<WunHandle*>(hc);
-    if (begin_call(h, nullptr, nullptr, 1, true, nullptr, 0, nullptr, true) != WUN_OK) return -1;
-    h->arena_sum = 0; h->phase = 0;
-    run_forward(h, nullptr, nullptr, nullptr, 1);
-    run_backward(h, nullptr, nullptr, 1.f);
-    return h->launches;
+int64_t wun_launches_forward_backward(const WunHandle* h) {
+    return h ? kernel_launches(build_dry(const_cast<WunHandle*>(h), 1, true).ops) : -1;
 }
 
 int wun_forward(WunHandle* h, const float* params, const float* mix, int64_t batch, int training, float* outputs,
@@ -1237,8 +1295,9 @@ int wun_forward(WunHandle* h, const float* params, const float* mix, int64_t bat
     int rc = begin_call(h, params, mix, batch, false, workspace, workspace_bytes, stream, false);
     if (rc != WUN_OK) return rc;
     if (!outputs) return set_err(WUN_E_INVALID, "outputs is null");
-    h->phase = 0; h->arena_cur = 0;
-    rc = run_forward(h, nullptr, outputs, nullptr, training);
+    Build b{h, h->ops};
+    rc = build_forward(b, nullptr, outputs, nullptr, training);
+    if (rc == WUN_OK) rc = issue(h, b.ops);
     if (rc != WUN_OK) return rc;
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
@@ -1252,32 +1311,10 @@ int wun_forward_backward(WunHandle* h, const float* params, const float* mix, co
     if (!targets || !loss || !grads) return set_err(WUN_E_INVALID, "targets/loss/grads must not be null");
     WUN_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), h->stream));
     WUN_CUDA_OK(cudaMemsetAsync(grads, 0, sizeof(float) * h->plan.param_numel, h->stream));
-    h->bw_grads = grads; h->bw_scale = grad_scale;
-    if (h->use_side && h->umma_enabled) {
-        // phase 1: every weight pack of the step on the side stream, behind the work already enqueued on `stream`
-        rc = ensure_side(h);
-        if (rc != WUN_OK) return rc;
-        if (h->fork_events.empty()) { cudaEvent_t e; WUN_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); h->fork_events.push_back(e); }
-        WUN_CUDA_OK(cudaEventRecord(h->fork_events[0], h->stream));
-        WUN_CUDA_OK(cudaStreamWaitEvent(h->side, h->fork_events[0], 0));
-        h->phase = 1; h->arena_cur = 0; h->pack_idx = 0;
-        rc = run_forward(h, targets, outputs, loss, 1);
-        if (rc == WUN_OK) rc = run_backward(h, targets, grads, grad_scale);
-        h->phase = 0;
-        if (rc != WUN_OK) return rc;
-        WUN_CUDA_OK(cudaEventRecord(h->packs_event, h->side));
-        h->packs_pending = true;
-        h->phase = 2;
-    }
-    h->arena_cur = 0; h->pack_idx = 0;
-    rc = run_forward(h, targets, outputs, loss, 1);
-    if (rc == WUN_OK) rc = run_backward(h, targets, grads, grad_scale);
-    h->phase = 0;
+    Build b{h, h->ops};
+    rc = build_step(b, targets, outputs, loss, grads, grad_scale);
+    if (rc == WUN_OK) rc = issue(h, b.ops);
     if (rc != WUN_OK) return rc;
-    if (h->packs_pending) {                     // no tensor-core conv consumed the packs: still join the side stream
-        WUN_CUDA_OK(cudaStreamWaitEvent(h->stream, h->packs_event, 0));
-        h->packs_pending = false;
-    }
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
 }
@@ -1312,19 +1349,14 @@ int wun_set_grad_buckets(WunHandle* h, int n, const int64_t* first_offset) {
     }
     if (n > 0 && first_offset[n - 1] != 0) return set_err(WUN_E_INVALID, "the last bucket must start at offset 0");
     if (n > 0) { int rc = check_device(); if (rc != WUN_OK) return rc; }
-    while ((int)h->bucket_events.size() < n) {
-        cudaEvent_t e;
-        WUN_CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        h->bucket_events.push_back(e);
-    }
+    WUN_CUDA_OK(make_events(h->events[EV_BUCKET], n));
     h->bucket_first.assign(first_offset, first_offset + n);
-    h->bucket_next = 0;
     return WUN_OK;
 }
 
 int wun_stream_wait_grad_bucket(WunHandle* h, int k, void* stream) {
     if (!h || k < 0 || k >= (int)h->bucket_first.size()) return set_err(WUN_E_INVALID, "no such gradient bucket");
-    WUN_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, h->bucket_events[k], 0));
+    WUN_CUDA_OK(cudaStreamWaitEvent((cudaStream_t)stream, h->events[EV_BUCKET][k], 0));
     return WUN_OK;
 }
 
@@ -1374,60 +1406,28 @@ int64_t wun_describe(const WunHandle* h, char* buf, int64_t capacity) {
     for (size_t i = 0; i + 2 < h->kernel_used.size(); i += 3)
         s += h->kernel_used[i] + "/" + h->kernel_used[i + 1] + "/" + h->kernel_used[i + 2] + " ";
     s += "\n";
-    if (buf && capacity > 0) {
-        int64_t n = std::min<int64_t>(capacity - 1, (int64_t)s.size());
-        memcpy(buf, s.data(), n);
-        buf[n] = 0;
-    }
-    return (int64_t)s.size() + 1;
+    return copy_out(s, buf, capacity);
 }
 
 int64_t wun_debug_plan(const WunHandle* hc, int64_t batch, char* buf, int64_t capacity) {
     WunHandle* h = const_cast<WunHandle*>(hc);
     if (!h || batch < 1) return -1;
-    std::vector<std::string> lines;
-    const size_t keep_sum = h->arena_sum, keep_max = h->arena_bytes;
-    const std::vector<std::string> keep_used = h->kernel_used;
-    if (begin_call(h, nullptr, nullptr, batch, true, nullptr, 0, nullptr, true) != WUN_OK) return -1;
-    h->audit = &lines; h->phase = 0;
-    run_forward(h, nullptr, nullptr, nullptr, 1);
-    run_backward(h, nullptr, nullptr, 1.f);
-    h->audit = nullptr;
-    h->arena_sum = keep_sum; h->arena_bytes = keep_max; h->kernel_used = keep_used;
     std::string s;
-    for (const auto& l : lines) { s += l; s += "\n"; }
-    if (buf && capacity > 0) {
-        int64_t n = std::min<int64_t>(capacity - 1, (int64_t)s.size());
-        memcpy(buf, s.data(), n);
-        buf[n] = 0;
-    }
-    return (int64_t)s.size() + 1;
+    for (const Op& o : build_dry(h, batch, true).ops) audit_op(s, o);
+    return copy_out(s, buf, capacity);
 }
 
 int64_t wun_debug_launches(const WunHandle* hc, int64_t batch, char* buf, int64_t capacity) {
     WunHandle* h = const_cast<WunHandle*>(hc);
     if (!h || batch < 1) return -1;
-    std::vector<std::string> lines;
-    const size_t keep_sum = h->arena_sum, keep_max = h->arena_bytes;
-    const std::vector<std::string> keep_used = h->kernel_used;
-    if (begin_call(h, nullptr, nullptr, batch, true, nullptr, 0, nullptr, true) != WUN_OK) return -1;
-    h->export_launches = &lines; h->phase = 0;
-    // fake, far-apart bases (never dereferenced in a dry run): every exported address identifies its buffer
+    // fake, far-apart bases (never dereferenced): every described address identifies its buffer
     h->ws = reinterpret_cast<float*>((uintptr_t)1 << 40); h->params = reinterpret_cast<const float*>((uintptr_t)1 << 41);
     h->mix = reinterpret_cast<const float*>((uintptr_t)1 << 42);
-    run_forward(h, nullptr, nullptr, nullptr, 1);
-    run_backward(h, nullptr, nullptr, 1.f);
-    lines.push_back("adam n=" + std::to_string((long long)h->plan.param_numel));     // wun_adam_step(_device) over the flat buffer
-    h->export_launches = nullptr; h->ws = nullptr; h->params = nullptr; h->mix = nullptr;
-    h->arena_sum = keep_sum; h->arena_bytes = keep_max; h->kernel_used = keep_used;
     std::string s;
-    for (const auto& l : lines) { s += l; s += "\n"; }
-    if (buf && capacity > 0) {
-        int64_t n = std::min<int64_t>(capacity - 1, (int64_t)s.size());
-        memcpy(buf, s.data(), n);
-        buf[n] = 0;
-    }
-    return (int64_t)s.size() + 1;
+    for (const Op& o : build_dry(h, batch, true).ops) describe_op(s, h, o);
+    s += "adam n=" + std::to_string((long long)h->plan.param_numel) + "\n";     // wun_adam_step(_device) over the flat buffer
+    h->ws = nullptr; h->params = nullptr; h->mix = nullptr;
+    return copy_out(s, buf, capacity);
 }
 
 static double op_forward_flops(const ConvOp& op, int64_t batch) {
@@ -1448,7 +1448,7 @@ int wun_debug_run_layer(WunHandle* h, int layer, int pass, int iters, const floa
     if (pass == 2 && !grads_scratch) return set_err(WUN_E_INVALID, "wgrad pass needs a gradient scratch buffer");
     int rc = begin_call(h, params, mix, batch, true, workspace, workspace_bytes, stream, false);
     if (rc != WUN_OK) return rc;
-    const ConvOp& op = (layer < L) ? h->plan.down[layer] : (layer == L ? h->plan.bottleneck : h->plan.up[layer - L - 1]);
+    const ConvOp& op = layer_op(h, layer);
     const OpBackward& ob = (layer < L) ? h->bwd_down[layer] : (layer == L ? h->bwd_bottleneck : h->bwd_up[layer - L - 1]);
     if (flops_per_launch) {
         // algorithmic (live-position) FLOPs: dgrad = the forward MACs of the planes that need a gradient, wgrad = all of them
@@ -1465,17 +1465,15 @@ int wun_debug_run_layer(WunHandle* h, int layer, int pass, int iters, const floa
         }
         *flops_per_launch = f;
     }
-    h->phase = 0; h->arena_cur = 0; h->wstream = h->stream;
-    if (pass == 0) {
-        h->debug_iters = iters;
-        rc = conv_forward(h, op, layer);
-        h->debug_iters = 0;
-    } else {
-        for (int i = 0; i < iters && rc == WUN_OK; ++i) {
-            h->arena_cur = 0;
-            rc = (pass == 1) ? conv_dgrad(h, op, ob, layer) : conv_wgrad(h, op, grads_scratch, 1.f, layer);
-        }
-    }
+    // the layer pass as in a step, on the caller's stream (a dgrad's second launch on the helper stream once a step made it)
+    Build b{h, h->ops};
+    b.dgrad_fork = h->dgrad_par && h->use_side && h->streams[ST_SIDE] != nullptr;
+    rc = (pass == 0) ? build_conv_forward(b, op, layer) : (pass == 1) ? build_dgrad(b, op, ob, layer) : build_wgrad(b, op, grads_scratch, 1.f, layer);
+    if (rc == WUN_OK) rc = issue(h, b.ops);
+    // forward: packed once, the tensor-core conv enqueued `iters` times; dgrad / wgrad: the whole pass again
+    for (int i = 1; i < iters && rc == WUN_OK; ++i)
+        for (size_t k = 0; k < b.ops.size() && rc == WUN_OK; ++k)
+            if (pass != 0 || b.ops[k].kind == OP_UMMA_CONV) rc = issue_op(h, b.ops[k]);
     if (rc != WUN_OK) return rc;
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
