@@ -120,6 +120,24 @@ def test_workspace_and_describe():
     assert e.launches(False) > 20 and e.launches(True) > e.launches(False)
 
 
+def test_every_switch_is_read_when_a_handle_is_created(monkeypatch):
+    """The A/B switches (DESIGN.md section 9) belong to the handle, not to the process: WUN_SPLIT_COLSUM=0 set after a default
+    handle exists gives the next handle one bias column-sum launch per class of each tensor-core weight gradient, and a handle
+    created after the switch is unset is back to the default launch count."""
+    cfg = wun.config_from_model_config(mc(["baseline_stereo"], num_layers=4))
+    monkeypatch.delenv("WUN_SPLIT_COLSUM", raising=False)
+    default = wun.Engine(cfg, num_frames=16384)
+    n = default.launches(True)
+    default.launch_descriptions(1)
+    classes = {(g["wgrad"]["layer"], g["dpre"]["base"]) for g in default.wgrad_groups
+               if default.layer_kernel(g["wgrad"]["layer"], 2) == "umma"}
+    assert classes
+    monkeypatch.setenv("WUN_SPLIT_COLSUM", "0")
+    assert wun.Engine(cfg, num_frames=16384).launches(True) == n + len(classes)
+    monkeypatch.delenv("WUN_SPLIT_COLSUM")
+    assert wun.Engine(cfg, num_frames=16384).launches(True) == n
+
+
 def test_compute_entry_points_fail_loudly_without_gpu():
     import torch
     if torch.cuda.is_available():

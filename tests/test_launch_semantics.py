@@ -26,7 +26,7 @@ def test_pair_merged_launches_compute_what_the_two_class_launches_do(name, named
     cfg = Config.build_config(named, ov, experiment_id=0)["model_config"]
     t_in, _ = O.get_padding(cfg, nf)
     wcfg = wun.config_from_model_config(cfg)
-    for k, v in (("WUN_FOLD", "0"), ("WUN_PAIR_FWD", "0"), ("WUN_PAIR_DGRAD", "0")):
+    for k, v in (("WUN_PAIR_FWD", "0"), ("WUN_PAIR_DGRAD", "0")):
         monkeypatch.setenv(k, v)
     plain = wun.Engine(wcfg, input_frames=t_in)
     LA = plain.launch_descriptions(batch)
@@ -114,7 +114,7 @@ def test_exported_forward_launches_reproduce_the_oracle(name, named, ov, batch, 
     up_i at their live rows, tests/helpers.py) of the oracle's get_output (UnetAudioSeparator.py:97-125) in float64."""
     import torch
     from helpers import live_rows
-    for k, v in (("WUN_FIRST_LAYER", "0"), ("WUN_FOLD", "0"), ("WUN_PAIR_FWD", str(pairs)), ("WUN_PAIR_MIN_CTAS", "1")):
+    for k, v in (("WUN_FIRST_LAYER", "0"), ("WUN_PAIR_FWD", str(pairs)), ("WUN_PAIR_MIN_CTAS", "1")):
         monkeypatch.setenv(k, v)
     cfg = Config.build_config(named, ov, experiment_id=0)["model_config"]
     t_in, t_out = O.get_padding(cfg, nf)
@@ -200,8 +200,7 @@ def _host_backward(named, ov, batch, nf, pairs, monkeypatch):
     """Forward launches, then the dgrad chain seeded with the oracle's gradient at the last up block, all on the host.
     Returns (cfg, eng, mem, dpre, param_grads, keys, t_in): dpre / param_grads are torch autograd through the oracle in float64."""
     import torch
-    for k, v in (("WUN_FIRST_LAYER", "0"), ("WUN_FOLD", "0"), ("WUN_PAIR_FWD", str(pairs)), ("WUN_PAIR_DGRAD", str(pairs)),
-                 ("WUN_PAIR_MIN_CTAS", "1")):
+    for k, v in (("WUN_FIRST_LAYER", "0"), ("WUN_PAIR_FWD", str(pairs)), ("WUN_PAIR_DGRAD", str(pairs)), ("WUN_PAIR_MIN_CTAS", "1")):
         monkeypatch.setenv(k, v)
     cfg = Config.build_config(named, ov, experiment_id=0)["model_config"]
     t_in, t_out = O.get_padding(cfg, nf)

@@ -45,16 +45,82 @@ struct OpBackward {
     std::vector<DgradClass> dgrad;   // empty: no input gradient needed (down0)
 };
 
-struct Layout {
-    std::vector<int64_t> off;   // float offsets per tensor; -1 = not allocated
-    int64_t total = 0;
+// The A/B switches (DESIGN.md section 9), read from the environment once per handle, when it is created (read_options)
+struct Options {
+    bool umma_enabled = true;            // tensor-core path on (WUN_DISABLE_UMMA=1 turns it off, for A/B tests)
+    bool umma_pass[3] = {true, true, true};   // per pass (fwd, dgrad, wgrad): WUN_UMMA_FWD=0 / WUN_UMMA_DGRAD=0 / WUN_UMMA_WGRAD=0
+    bool use_side = true;                // WUN_SIDE_STREAM=0 disables
+    bool first_fast = true;              // dedicated first-layer kernels (kernels_first.cu); WUN_FIRST_LAYER=0 = generic path
+    bool bulk_wgrad = true;              // split pass + bulk-copy-fed tensor-core wgrad; WUN_BULK_WGRAD=0 = converter-fed kernel
+    bool dgrad_par = true;               // WUN_DGRAD_PAR=0: a dgrad's second launch stays on the caller's stream
+    // split passes run one layer AHEAD of the wgrad kernels, on their own stream, into a double-buffered arena: the split pass is
+    // DRAM-bound, the wgrad kernel L2 / tensor bound, so they overlap well (WUN_SPLIT_AHEAD=0: same stream, one arena half)
+    bool split_ahead = true;
+    bool first_tail = true;              // first-layer weight gradient on the split stream (build_wgrad); WUN_FIRST_TAIL=0 disables
+    // weight packs are hoisted off the critical path: a training step enqueues every pack kernel on the side stream first (they
+    // only depend on the parameters), then everything else; inference and the debug hooks pack inline.  WUN_PACK_EVENTS=0: the
+    // forward convs wait for all packs instead of each for its own
+    bool pack_events_on = true;
+    bool pair_fwd = true;                // pair-merged forward classes of the up blocks; WUN_PAIR_FWD=0 disables
+    int pair_dgrad = 4;                  // pair-merged dgrad classes (launch.h OutView::pairC); WUN_PAIR_DGRAD=0 off, 1 all, 2 down blocks only,
+                                         // 3 up blocks only, 4 (default) down blocks whose merged width still takes the fused-N MMAs (2C <= 64)
+    int pair_min_ctas = 120;             // WUN_PAIR_MIN_CTAS
+    // output layer in the last up block's conv epilogue (kernels_umma.h OutputFuse).  WUN_OUT_FUSE: 0 = separate kernels, 1 (default) =
+    // estimates + loss + dL/dpre + the gradient w.r.t. the features fused, the output convs' weight gradient as its own launch on
+    // the wgrad stream (off the critical path), 2 = the weight gradient in the epilogue too (measured slower: it serialises
+    // ~650 shuffle-reduction instructions per row tile on the four epilogue warps)
+    int out_fuse_mode = 1;
+    int split_colsum = 1;                // bias column sums in the split pass (build_wgrad); WUN_SPLIT_COLSUM=0 separate launches, 2 few-row layers only
+};
+
+static Options read_options() {
+    auto on = [](const char* name) { const char* v = getenv(name); return !(v && v[0] == '0'); };   // off only for "0..."
+    auto num = [](const char* name, int def) { const char* v = getenv(name); return v ? atoi(v) : def; };
+    Options o;
+    const char* dis = getenv("WUN_DISABLE_UMMA");
+    o.umma_enabled = !(dis && dis[0] == '1');
+    o.umma_pass[0] = on("WUN_UMMA_FWD"); o.umma_pass[1] = on("WUN_UMMA_DGRAD"); o.umma_pass[2] = on("WUN_UMMA_WGRAD");
+    o.use_side = on("WUN_SIDE_STREAM");
+    o.first_fast = on("WUN_FIRST_LAYER");
+    o.bulk_wgrad = on("WUN_BULK_WGRAD");
+    o.dgrad_par = on("WUN_DGRAD_PAR");
+    o.split_ahead = on("WUN_SPLIT_AHEAD");
+    o.first_tail = on("WUN_FIRST_TAIL");
+    o.pack_events_on = on("WUN_PACK_EVENTS");
+    o.pair_fwd = on("WUN_PAIR_FWD");
+    o.pair_dgrad = num("WUN_PAIR_DGRAD", 4);
+    o.pair_min_ctas = num("WUN_PAIR_MIN_CTAS", 120);
+    o.out_fuse_mode = num("WUN_OUT_FUSE", 1);
+    o.split_colsum = num("WUN_SPLIT_COLSUM", 1);
+    return o;
+}
+
+// Where one call's regions lie in its workspace, in this order: the activations (float offsets per tensor from the base; -1 = not
+// allocated in this kind of call), the weight packs, then the training scratch: the split arena (two halves; bulk-fed wgrad only),
+// the per-CTA sums of the first layer's and of the output layer's weight gradients, the CTA counters of the loss and interp-gradient
+// sums ([0] loss, [1] interp; zeroed at the start of every training step's output layer), the per-CTA loss sums and the per-CTA
+// interp-gradient sums (each added up in a fixed order).  Byte offsets from the base; `end` = the bytes a call needs.
+struct WsMap {
+    std::vector<int64_t> act;
+    int64_t packs = 0, split[2] = {0, 0}, first_part = 0, out_part = 0, counters = 0, loss_part = 0, dvar_part = 0, end = 0;
+};
+
+// One engine call's inputs: the caller's buffers and stream, the batch and the workspace map.  The calls that only build a launch
+// list (counts, descriptions, the create-time sizes) have null or fake buffers and no stream.
+struct Call {
+    const float* params = nullptr;
+    const float* mix = nullptr;
+    float* ws = nullptr;
+    cudaStream_t stream = nullptr;
+    int batch = 0;
+    WsMap map;
 };
 
 }  // namespace
 
 // The streams a launch record goes to: the caller's; ST_SIDE: weight-gradient kernels (and a training step's weight packs) run
 // on an internal side stream, concurrently with the dgrad chain on the caller's stream; ST_SPLIT: the split passes (see
-// WunHandle::split_ahead); ST_HELPER: a dgrad with two launches (the up blocks: skip pair and upsampled pair have different
+// Options::split_ahead); ST_HELPER: a dgrad with two launches (the up blocks: skip pair and upsampled pair have different
 // widths) runs the second one on this helper stream, concurrently with the first: both read the same gradient planes and write
 // different tensors, and in the deep layers neither fills the GPU (WUN_DGRAD_PAR=0 disables)
 enum StreamRole : uint8_t { ST_CALLER, ST_SIDE, ST_SPLIT, ST_HELPER };
@@ -101,46 +167,19 @@ struct WunHandle {
     Plan plan;
     std::vector<OpBackward> bwd_down, bwd_up;
     OpBackward bwd_bottleneck;
-    bool umma_enabled = true;            // tensor-core path on (WUN_DISABLE_UMMA=1 turns it off, for A/B tests)
-    bool umma_pass[3] = {true, true, true};   // per pass (fwd, dgrad, wgrad): WUN_UMMA_FWD=0 / WUN_UMMA_DGRAD=0 / WUN_UMMA_WGRAD=0
+    Options opt;
     std::vector<std::string> kernel_used;   // [layer*3 + pass] -> "simt" | "umma" (from the launch list built at create time)
     cudaStream_t streams[4] = {};        // by StreamRole, created where a call first needs them (ST_CALLER: unused)
     std::vector<cudaEvent_t> events[kEventPools];   // by EventPool, created where a call first needs them
-    bool dgrad_par = true;
-    bool use_side = true;                // WUN_SIDE_STREAM=0 disables
-    bool first_fast = true;              // dedicated first-layer kernels (kernels_first.cu); WUN_FIRST_LAYER=0 = generic path
-    bool bulk_wgrad = true;              // split pass + bulk-copy-fed tensor-core wgrad; WUN_BULK_WGRAD=0 = converter-fed kernel
-    // output layer in the last up block's conv epilogue (kernels_umma.h OutputFuse).  WUN_OUT_FUSE: 0 = separate kernels, 1 (default) =
-    // estimates + loss + dL/dpre + the gradient w.r.t. the features fused, the output convs' weight gradient as its own launch on
-    // the wgrad stream (off the critical path), 2 = the weight gradient in the epilogue too (measured slower: it serialises
-    // ~650 shuffle-reduction instructions per row tile on the four epilogue warps)
-    int out_fuse_mode = 1;
-    int pair_min_ctas = 120;             // WUN_PAIR_MIN_CTAS
-    bool pair_fwd = true;                // the same for the forward classes of the up blocks; WUN_PAIR_FWD=0 disables
-    int pair_dgrad = 4;                  // pair-merged dgrad classes (launch.h OutView::pairC); WUN_PAIR_DGRAD=0 off, 1 all, 2 down blocks only,
-                                         // 3 up blocks only, 4 (default) down blocks whose merged width still takes the fused-N MMAs (2C <= 64)
     // sizes from the batch-1 training launch list built at create time
     size_t split_item_bytes = 0;         // per batch item: largest split arena any layer's wgrad needs
     size_t wg_partial_bytes = 0;         // largest partial-tile scratch of a layer's wgrad (any batch)
     size_t out_part_bytes = 0;           // the output layer's per-CTA weight-gradient sums (any batch)
     size_t arena_sum = 0;                // total pack bytes of one forward+backward
-    // split passes run one layer AHEAD of the wgrad kernels, on their own stream, into a double-buffered arena: the split pass is
-    // DRAM-bound, the wgrad kernel L2 / tensor bound, so they overlap well (WUN_SPLIT_AHEAD=0: same stream, one arena half)
-    bool split_ahead = true;
-    // weight packs are hoisted off the critical path: a training step enqueues every pack kernel on the side stream first (they
-    // only depend on the parameters), then everything else; inference and the debug hooks pack inline
-    bool pack_events_on = true;
     // data-parallel overlap: gradient buckets in PRODUCTION order (output layer first, down0 last); bucket k = flat offsets
     // >= bucket_first[k] (and below bucket k-1's)
     std::vector<int64_t> bucket_first;
-    // per-call state
-    std::vector<Op> ops;                 // the call's launch list (its storage is kept from call to call: no allocation per call)
-    cudaStream_t stream = nullptr;
-    const float* params = nullptr;
-    const float* mix = nullptr;
-    float* ws = nullptr;
-    Layout lay;
-    int batch = 0;
+    std::vector<Op> ops;                 // storage of the calls' launch lists, kept from call to call: no allocation per call
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -208,28 +247,48 @@ static void plan_backward(WunHandle* h) {
     for (int i = L - 1; i >= 0; --i) plan_op(P.down[i], &h->bwd_down[i], false);
 }
 
-static Layout make_layout(const Plan& P, int64_t B, bool training) {
-    Layout l;
-    l.off.assign(P.tensors.size(), -1);
+constexpr int64_t kCounterBytes = 256;     // the CTA counters of the loss and interp-gradient sums
+
+static WsMap ws_map(const WunHandle* h, int64_t B, bool training) {
+    const Plan& P = h->plan;
+    WsMap m;
+    m.act.assign(P.tensors.size(), -1);
     int64_t cur = 0;
     for (size_t i = 0; i < P.tensors.size(); ++i) {
         const TensorSpec& t = P.tensors[i];
         if (t.training_only && !training) continue;
         int64_t n = t.rows * t.C * (t.per_batch ? B : 1);
-        l.off[i] = cur;
+        m.act[i] = cur;
         cur += (n + 63) / 64 * 64;
     }
-    l.total = cur + 64;
-    return l;
+    m.packs = (cur + 64) * (int64_t)sizeof(float);
+    m.end = m.packs + (int64_t)h->arena_sum;
+    auto region = [&](int64_t bytes) { const int64_t at = m.end; if (training) m.end += bytes; return at; };   // inference: none
+    // split arena: each half holds the split arrays of one layer's wgrad, then its partial tiles, from a 256-byte boundary
+    const int64_t half = (int64_t)h->split_item_bytes * B + 256 * (kSplitMaxJobs + 1) + (int64_t)h->wg_partial_bytes + 256;
+    const int64_t split = region((h->opt.bulk_wgrad && h->split_item_bytes) ? 2 * half : 0);
+    m.split[0] = (split + 255) / 256 * 256;
+    m.split[1] = (split + half + 255) / 256 * 256;
+    m.first_part = region((int64_t)first_wgrad_partial_bytes((int)B));
+    m.out_part = region((int64_t)h->out_part_bytes);
+    m.counters = region(kCounterBytes);
+    m.loss_part = region((int64_t)output_loss_partial_bytes((int)B, (int)P.T_out));
+    int C = 0;      // interp gradients: one level at a time, all on the caller's stream (none without learned upsampling)
+    for (int i = 0; i < P.cfg.num_layers; ++i)
+        if (P.ups[i].interp_param >= 0) C = std::max(C, P.ups[i].C);
+    m.dvar_part = region(C ? (int64_t)upsample_dvar_partial_bytes((int)B, C) : 0);
+    return m;
 }
 
 // ------------------------------------------------------------------------------------------------
 // materialisation of launch blocks
 // ------------------------------------------------------------------------------------------------
-static const float* tensor_ptr(const WunHandle* h, int tensor) {
-    if (tensor == TENSOR_MIX) return h->mix;
-    return h->ws + h->lay.off[tensor];
+static const float* tensor_ptr(const Call& call, int tensor) {
+    if (tensor == TENSOR_MIX) return call.mix;
+    return call.ws + call.map.act[tensor];
 }
+
+static uint8_t* ws_at(const Call& call, int64_t offset) { return reinterpret_cast<uint8_t*>(call.ws) + offset; }
 
 static void tensor_geom(const WunHandle* h, int tensor, int64_t* rows, int* C, bool* per_batch) {
     if (tensor == TENSOR_MIX) { *rows = h->plan.T_in; *C = h->plan.cfg.num_channels; *per_batch = true; return; }
@@ -237,25 +296,25 @@ static void tensor_geom(const WunHandle* h, int tensor, int64_t* rows, int* C, b
     *rows = t.rows; *C = t.C; *per_batch = t.per_batch;
 }
 
-static PlaneView make_plane(const WunHandle* h, const ViewSpec& v) {
+static PlaneView make_plane(const WunHandle* h, const Call& call, const ViewSpec& v) {
     PlaneView p;
     memset(&p, 0, sizeof(p));
     int64_t rows; int C; bool pb;
     tensor_geom(h, v.tensor, &rows, &C, &pb);
-    p.base = tensor_ptr(h, v.tensor) + (long long)v.row_offset * C;
+    p.base = tensor_ptr(call, v.tensor) + (long long)v.row_offset * C;
     p.bstride = pb ? rows * C : 0;
     p.rstride = v.row_step * C;
     p.r_lo = v.r_lo; p.r_hi = v.r_hi; p.C = v.C;
     p.kind = v.kind; p.mid_mode = v.mid_mode; p.xrows = v.xrows;
-    p.blend = (v.blend_tensor >= 0) ? tensor_ptr(h, v.blend_tensor) : nullptr;
+    p.blend = (v.blend_tensor >= 0) ? tensor_ptr(call, v.blend_tensor) : nullptr;
     return p;
 }
 
 // the same geometry as `v`, but on another tensor (gradient twin / scratch) with explicit batch stride
-static PlaneView make_plane_on(const WunHandle* h, const ViewSpec& v, int tensor, long long bstride, int r_lo, int r_hi) {
+static PlaneView make_plane_on(const Call& call, const ViewSpec& v, int tensor, long long bstride, int r_lo, int r_hi) {
     PlaneView p;
     memset(&p, 0, sizeof(p));
-    p.base = tensor_ptr(h, tensor) + (long long)v.row_offset * v.C;
+    p.base = tensor_ptr(call, tensor) + (long long)v.row_offset * v.C;
     p.bstride = bstride;
     p.rstride = v.row_step * v.C;
     p.r_lo = r_lo; p.r_hi = r_hi; p.C = v.C;
@@ -274,6 +333,7 @@ static long long view_bstride(const WunHandle* h, const ViewSpec& v) {
 // ------------------------------------------------------------------------------------------------
 struct Build {                   // the walk over the plan that appends one call's records
     const WunHandle* h;
+    const Call& call;
     std::vector<Op>& ops;
     bool train = false;          // a training step: the CTA counters of the loss sums are zeroed
     bool hoist = false;          // weight packs on the side stream ahead of the step (training, side stream, tensor cores)
@@ -284,11 +344,10 @@ struct Build {                   // the walk over the plan that appends one call
     const OutputFuse* fuse = nullptr;   // around the last up block's forward conv
     bool out_fused = false;      // that conv carried the output layer: no output_fwd / output_dgrad / output_wgrad launches
     int layer = -1, pass = -1;
-    size_t arena_cur = 0;        // bump pointer into the pack arena
     int pack_idx = 0, fork_used = 0, par_used = 0, wg_index = 0, bucket_next = 0;
     bool packs_pending = false;  // the caller's stream has not yet waited for the hoisted packs
     bool first_pending = false;  // the first-layer weight gradient runs on the split stream
-    // sizes the workspace needs for these launches
+    // sizes the workspace needs for these launches (pack_sum: also the bump pointer into the pack arena)
     size_t pack_sum = 0, split_item = 0, wg_partial = 0, out_part = 0;
 };
 
@@ -305,18 +364,18 @@ static Op& add(Build& b, OpKind kind, StreamRole stream = ST_CALLER, EventPool p
 static int add_conv(Build& b, const ConvLaunch& L, StreamRole s, size_t pack_floor) {
     const WunHandle* h = b.h;
     UmmaChoice ch;
-    if (!(h->umma_enabled && h->umma_pass[b.pass] && umma_plan_from_conv(L, &ch))) {
+    if (!(h->opt.umma_enabled && h->opt.umma_pass[b.pass] && umma_plan_from_conv(L, &ch))) {
         add(b, OP_CONV, s).conv = L;
         return WUN_OK;
     }
     const size_t bytes = std::max(ch.pack_bytes, pack_floor);
-    uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + b.arena_cur;
-    b.arena_cur += bytes; b.pack_sum += bytes;
+    uint8_t* arena = ws_at(b.call, b.call.map.packs + b.pack_sum);
+    b.pack_sum += bytes;
     UmmaLaunch U;
     Op& pk = add(b, OP_PACK, b.hoist ? ST_SIDE : s);
     pk.early = b.hoist;
     if (umma_build(L, ch, arena, &U, &pk.pack) != cudaSuccess) return set_err(WUN_E_CUDA, "tensor-core conv launch: too many pack jobs");
-    if (h->pack_events_on && b.pass == 0 && b.hoist) {     // forward conv i waits for pack i only
+    if (h->opt.pack_events_on && b.pass == 0 && b.hoist) {     // forward conv i waits for pack i only
         const int idx = b.pack_idx++;
         add(b, OP_MAKE, ST_SIDE, EV_PACK, idx + 1).early = true;
         add(b, OP_RECORD, ST_SIDE, EV_PACK, idx).early = true;
@@ -334,8 +393,8 @@ static int add_conv(Build& b, const ConvLaunch& L, StreamRole s, size_t pack_flo
 
 // The first down block in the form kernels_first.cu wants, if the op has exactly the shape plan.cpp builds for it: input =
 // the caller's mix in two parity planes, class 0 = even full-rate rows -> dec0, class 1 = odd rows of the skip window -> odd0.
-static bool first_layer_desc(const WunHandle* h, const ConvOp& op, FirstLayer* F) {
-    if (!h->first_fast || op.planes.size() != 2 || op.classes.size() != 2) return false;
+static bool first_layer_desc(const WunHandle* h, const Call& call, const ConvOp& op, FirstLayer* F) {
+    if (!h->opt.first_fast || op.planes.size() != 2 || op.classes.size() != 2) return false;
     const ViewSpec& p0 = op.planes[0];
     const ViewSpec& p1 = op.planes[1];
     if (p0.tensor != TENSOR_MIX || p1.tensor != TENSOR_MIX || p0.row_step != 2 || p1.row_step != 2 || p0.row_offset != 0 ||
@@ -353,14 +412,14 @@ static bool first_layer_desc(const WunHandle* h, const ConvOp& op, FirstLayer* F
         for (const auto& t : op.classes[q].terms)
             if (2 * t.d + t.plane != q + t.tap - pad || t.coff != 0) return false;
     memset(F, 0, sizeof(*F));
-    F->x = h->mix; F->x_bstride = (long long)h->plan.T_in * C; F->T = (int)h->plan.T_in;
+    F->x = call.mix; F->x_bstride = (long long)h->plan.T_in * C; F->T = (int)h->plan.T_in;
     F->k = op.k; F->pad_left = pad;
-    F->dec = const_cast<float*>(tensor_ptr(h, c0.out.tensor)); F->dec_bstride = view_bstride(h, c0.out); F->Td = c0.m_hi;
-    F->odd = const_cast<float*>(tensor_ptr(h, c1.out.tensor)); F->odd_bstride = view_bstride(h, c1.out);
+    F->dec = const_cast<float*>(tensor_ptr(call, c0.out.tensor)); F->dec_bstride = view_bstride(h, c0.out); F->Td = c0.m_hi;
+    F->odd = const_cast<float*>(tensor_ptr(call, c1.out.tensor)); F->odd_bstride = view_bstride(h, c1.out);
     F->mo_lo = c1.m_lo; F->mo_hi = c1.m_hi;
-    F->W = h->params + h->plan.params[op.w_param].offset;
-    F->bias = h->params + h->plan.params[op.b_param].offset;
-    F->batch = h->batch;
+    F->W = call.params + h->plan.params[op.w_param].offset;
+    F->bias = call.params + h->plan.params[op.b_param].offset;
+    F->batch = call.batch;
     return true;
 }
 
@@ -412,15 +471,16 @@ static bool pair_worthwhile(const WunHandle* h, const ConvLaunch& M, const UmmaC
     long long ctas = 0;
     for (int q = 0; q < M.ncls; ++q)
         ctas += (long long)((M.cls[q].m_hi - M.cls[q].m_lo + ch.MT * 128 - 1) / (ch.MT * 128)) * ch.nsplit * M.batch;
-    return ctas >= h->pair_min_ctas;
+    return ctas >= h->opt.pair_min_ctas;
 }
 
 static int build_conv_forward(Build& b, const ConvOp& op, int layer_index) {
     const WunHandle* h = b.h;
+    const Call& call = b.call;
     b.layer = layer_index; b.pass = 0;
     if (layer_index == 0) {
         FirstLayer F;
-        if (first_layer_desc(h, op, &F)) {
+        if (first_layer_desc(h, call, op, &F)) {
             add(b, OP_FIRST_FWD).first = F;
             return WUN_OK;
         }
@@ -428,13 +488,13 @@ static int build_conv_forward(Build& b, const ConvOp& op, int layer_index) {
     ConvLaunch L;
     memset(&L, 0, sizeof(L));
     L.nplanes = (int)op.planes.size();
-    for (int p = 0; p < L.nplanes; ++p) L.planes[p] = make_plane(h, op.planes[p]);
+    for (int p = 0; p < L.nplanes; ++p) L.planes[p] = make_plane(h, call, op.planes[p]);
     L.ncls = (int)op.classes.size();
     int nt = 0, max_rows = 0;
     for (int q = 0; q < L.ncls; ++q) {
         const ClassSpec& c = op.classes[q];
         OutView& o = L.cls[q];
-        PlaneView ov = make_plane(h, c.out);
+        PlaneView ov = make_plane(h, call, c.out);
         o.base = const_cast<float*>(ov.base); o.bstride = ov.bstride; o.rstride = ov.rstride;
         o.m_lo = c.m_lo; o.m_hi = c.m_hi; o.saved = nullptr; o.acc_lo = o.acc_hi = 0;
         o.term_begin = nt;
@@ -446,14 +506,14 @@ static int build_conv_forward(Build& b, const ConvOp& op, int layer_index) {
         max_rows = std::max(max_rows, c.m_hi - c.m_lo);
     }
     L.N = op.cout; L.w_sk = op.cout; L.w_sn = 1;
-    L.W = h->params + h->plan.params[op.w_param].offset;
-    L.bias = h->params + h->plan.params[op.b_param].offset;
-    L.epilogue = EPI_BIAS_LRELU; L.batch = h->batch; L.max_rows = max_rows;
+    L.W = call.params + h->plan.params[op.w_param].offset;
+    L.bias = call.params + h->plan.params[op.b_param].offset;
+    L.epilogue = EPI_BIAS_LRELU; L.batch = call.batch; L.max_rows = max_rows;
     // the even / odd output rows of an up block (and of the bottleneck) read the same planes at the same shifts: one
     // pair-merged class of 2*cout columns (out tensor viewed as [B, rows/2, 2*cout]) - 6+6 taps instead of 2 x (5+5)
     ConvLaunch M;
     size_t pack_floor = 0;
-    if (h->pair_fwd && L.ncls == 2 && h->umma_enabled && h->umma_pass[0] && merge_pair(L, &M)) {
+    if (h->opt.pair_fwd && L.ncls == 2 && h->opt.umma_enabled && h->opt.umma_pass[0] && merge_pair(L, &M)) {
         UmmaChoice ch0, ch;
         const bool ok0 = umma_plan_from_conv(L, &ch0), ok1 = umma_plan_from_conv(M, &ch);
         if (ok0 && ok1) {
@@ -469,6 +529,7 @@ static int build_conv_forward(Build& b, const ConvOp& op, int layer_index) {
 static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int layer_index) {
     if (ob.dgrad.empty()) return WUN_OK;
     const WunHandle* h = b.h;
+    const Call& call = b.call;
     b.layer = layer_index; b.pass = 1;
     const Plan& P = h->plan;
     ConvLaunch L;
@@ -476,7 +537,7 @@ static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int lay
     L.nplanes = (int)op.classes.size();
     for (int q = 0; q < L.nplanes; ++q) {
         const ClassSpec& c = op.classes[q];
-        L.planes[q] = make_plane_on(h, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
+        L.planes[q] = make_plane_on(call, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
     }
     L.ncls = (int)ob.dgrad.size();
     int nt = 0, max_rows = 0;
@@ -486,11 +547,11 @@ static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int lay
         const int gt = op.plane_grad_tensor[dc.plane];
         long long bs = view_bstride(h, v);
         if (gt == P.t_gmid) bs = (long long)(v.r_hi - v.r_lo) * v.C;   // [B, nmid, C]
-        PlaneView ov = make_plane_on(h, v, gt, bs, dc.r_lo, dc.r_hi);
+        PlaneView ov = make_plane_on(call, v, gt, bs, dc.r_lo, dc.r_hi);
         OutView& o = L.cls[k];
         o.base = const_cast<float*>(ov.base); o.bstride = ov.bstride; o.rstride = ov.rstride;
         o.m_lo = dc.r_lo; o.m_hi = dc.r_hi;
-        o.saved = op.plane_slope[dc.plane] ? make_plane(h, v).base : nullptr;
+        o.saved = op.plane_slope[dc.plane] ? make_plane(h, call, v).base : nullptr;
         o.acc_lo = dc.acc_lo; o.acc_hi = dc.acc_hi;
         o.term_begin = nt;
         for (int q = 0; q < (int)op.classes.size(); ++q)
@@ -530,11 +591,11 @@ static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int lay
                 done[k2] = 1;
             }
         S.N = N; S.w_sk = 1; S.w_sn = op.cout;
-        S.W = h->params + P.params[op.w_param].offset;
+        S.W = call.params + P.params[op.w_param].offset;
         S.bias = nullptr;
         // slope is per class (saved != null); classes without saved use EPI_PLAIN semantics via null check
         S.epilogue = EPI_SLOPE;
-        S.batch = h->batch;
+        S.batch = call.batch;
         if (S.max_rows <= 0) continue;
         // Pair merge: two classes of the same width (the even / odd input rows of a down block; the skip-even / skip-odd or
         // the copied / interpolated inputs of an up block) read the same gradient planes with the same row shifts.  As ONE
@@ -544,10 +605,10 @@ static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int lay
         // Measured (M4 batch 16, same-box A/B): down1 (2C = 48, fused-N MMAs) 368 -> 332 us; wider pairs lose the fused-N form and
         // got slower (down2 276 -> 317, down3 216 -> 250, down4 156 -> 183, up11 194 -> 215 us): their dgrad is bound by the
         // epilogue's slope / accumulate read-backs, not by slab fills or MMAs.
-        const bool pair_on = h->pair_dgrad == 1 || (h->pair_dgrad == 2 && op.planes.size() == 2) || (h->pair_dgrad == 3 && op.planes.size() == 4) ||
-                             (h->pair_dgrad == 4 && op.planes.size() == 2 && 2 * S.N <= 64);
+        const bool pair_on = h->opt.pair_dgrad == 1 || (h->opt.pair_dgrad == 2 && op.planes.size() == 2) || (h->opt.pair_dgrad == 3 && op.planes.size() == 4) ||
+                             (h->opt.pair_dgrad == 4 && op.planes.size() == 2 && 2 * S.N <= 64);
         size_t pack_floor = 0;
-        if (h->pair_dgrad != 0 && S.ncls == 2 && h->umma_enabled && h->umma_pass[1] && merge_pair(S, &M)) {
+        if (h->opt.pair_dgrad != 0 && S.ncls == 2 && h->opt.umma_enabled && h->opt.umma_pass[1] && merge_pair(S, &M)) {
             UmmaChoice ch0, ch;
             const bool ok0 = umma_plan_from_conv(S, &ch0), ok1 = umma_plan_from_conv(M, &ch);
             if (ok0 && ok1) {
@@ -574,67 +635,25 @@ static int build_dgrad(Build& b, const ConvOp& op, const OpBackward& ob, int lay
     return WUN_OK;
 }
 
-static int64_t split_arena_half_bytes(const WunHandle* h, int64_t batch) {
-    return (int64_t)h->split_item_bytes * batch + 256 * (kSplitMaxJobs + 1) + (int64_t)h->wg_partial_bytes + 256;
-}
-
-// bytes of the split arena behind the weight packs (bulk-fed wgrad only; per-item size from the dry run at create time)
-static int64_t split_arena_bytes(const WunHandle* h, int64_t batch) {
-    return (h && h->bulk_wgrad && h->split_item_bytes) ? 2 * split_arena_half_bytes(h, batch) : 0;     // two halves
-}
-// bytes of the per-CTA sums of the interp gradients: one level at a time, all on the caller's stream (0 without learned upsampling)
-static int64_t dvar_part_bytes(const WunHandle* h, int64_t batch) {
-    int C = 0;
-    for (int i = 0; i < h->plan.cfg.num_layers; ++i)
-        if (h->plan.ups[i].interp_param >= 0) C = std::max(C, h->plan.ups[i].C);
-    return C ? (int64_t)upsample_dvar_partial_bytes((int)batch, C) : 0;
-}
-constexpr int64_t kCounterBytes = 256;     // the CTA counters of the loss and interp-gradient sums: [0] loss, [1] interp
-// training scratch behind the activations, the weight packs and the split arena: the per-CTA sums of the first layer's and the
-// output layer's weight gradients, then the counters and the per-CTA sums of the loss and of the interp gradients (each added up
-// in a fixed order)
-static int64_t train_scratch_bytes(const WunHandle* h, int64_t batch) {
-    return split_arena_bytes(h, batch) + (int64_t)first_wgrad_partial_bytes((int)batch) + (int64_t)h->out_part_bytes + kCounterBytes +
-           (int64_t)output_loss_partial_bytes((int)batch, (int)h->plan.T_out) + dvar_part_bytes(h, batch);
-}
-// the output layer's per-CTA weight-gradient sums, behind the first layer's
-static float* out_part_ptr(const WunHandle* h) {
-    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum + split_arena_bytes(h, h->batch) +
-                                    first_wgrad_partial_bytes(h->batch));
-}
-// the counters (zeroed at the start of every training step's output layer), behind the output layer's gradient sums
-static unsigned* counters_ptr(const WunHandle* h) {
-    return reinterpret_cast<unsigned*>(reinterpret_cast<uint8_t*>(out_part_ptr(h)) + h->out_part_bytes);
-}
-// the per-CTA loss sums, behind the counters (counters and sums are used on the caller's stream only)
-static float* loss_part_ptr(const WunHandle* h) {
-    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(counters_ptr(h)) + kCounterBytes);
-}
-// the per-CTA interp-gradient sums, behind the loss sums (used on the caller's stream only)
-static float* dvar_part_ptr(const WunHandle* h) {
-    return reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(loss_part_ptr(h)) + output_loss_partial_bytes(h->batch, (int)h->plan.T_out));
-}
-
 static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, int layer_index) {
     const WunHandle* h = b.h;
+    const Call& call = b.call;
     const Plan& P = h->plan;
     b.layer = layer_index; b.pass = 2;
-    // split passes ahead on their own stream (see WunHandle::split_ahead)
-    const bool ahead = h->split_ahead && b.ws != ST_CALLER;
+    // split passes ahead on their own stream (see Options::split_ahead)
+    const bool ahead = h->opt.split_ahead && b.ws != ST_CALLER;
     if (layer_index == 0) {
         FirstWgrad FW;
-        if (first_layer_desc(h, op, &FW.L)) {          // one launcher call: dW and db of both classes (per-CTA sums + their total)
-            FW.part = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum +
-                                               split_arena_bytes(h, h->batch));
-            FW.L.dec = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor]));
-            FW.L.odd = const_cast<float*>(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor]));
+        if (first_layer_desc(h, call, op, &FW.L)) {    // one launcher call: dW and db of both classes (per-CTA sums + their total)
+            FW.part = reinterpret_cast<float*>(ws_at(call, call.map.first_part));
+            FW.L.dec = const_cast<float*>(tensor_ptr(call, P.grad_twin[op.classes[0].out.tensor]));
+            FW.L.odd = const_cast<float*>(tensor_ptr(call, P.grad_twin[op.classes[1].out.tensor]));
             FW.dW = grads + P.params[op.w_param].offset;
             FW.db = grads + P.params[op.b_param].offset;
             FW.scale = scale; FW.rows_per_cta = 0;
             // the CUDA-core first-layer gradient is the tail of the step: on the split stream it runs next to the second
             // block's tensor-core wgrad instead of behind it (joined at the end of build_backward)
-            static const bool tail_on = [] { const char* e = getenv("WUN_FIRST_TAIL"); return !(e && e[0] == '0'); }();
-            const bool tail_par = tail_on && ahead;
+            const bool tail_par = h->opt.first_tail && ahead;
             add(b, OP_FIRST_WGRAD, tail_par ? ST_SPLIT : b.ws).fw = FW;
             if (tail_par) {
                 add(b, OP_MAKE, ST_SPLIT, EV_FIRST_DONE, 1);
@@ -649,7 +668,7 @@ static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, in
     std::vector<PlaneView> class_dpre;
     for (const auto& c : op.classes) {
         if (c.m_hi <= c.m_lo) continue;
-        PlaneView dpre = make_plane_on(h, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
+        PlaneView dpre = make_plane_on(call, c.out, P.grad_twin[c.out.tensor], view_bstride(h, c.out), c.m_lo, c.m_hi);
         class_dpre.push_back(dpre);                            // bias gradient = its column sums (fused into the split pass below)
         size_t i = 0;
         while (i < c.terms.size()) {
@@ -662,21 +681,21 @@ static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, in
                 W.woff[W.nterms] = (c.terms[i].tap * op.cin_tot + c.terms[i].coff) * op.cout;
                 ++W.nterms; ++i;
             }
-            W.plane = make_plane(h, op.planes[p]);
+            W.plane = make_plane(h, call, op.planes[p]);
             W.dpre = dpre;
             W.m_lo = c.m_lo; W.m_hi = c.m_hi;
             W.N = op.cout; W.w_sk = op.cout; W.w_sn = 1;
             W.dW = grads + P.params[op.w_param].offset;
-            W.scale = scale; W.batch = h->batch;
+            W.scale = scale; W.batch = call.batch;
             groups.push_back(W);
         }
     }
     // tensor cores: all groups of the layer in ONE launch
-    bool use_umma = h->umma_enabled && h->umma_pass[2] && !groups.empty() && groups.size() <= (size_t)kWgMaxGroups;
+    bool use_umma = h->opt.umma_enabled && h->opt.umma_pass[2] && !groups.empty() && groups.size() <= (size_t)kWgMaxGroups;
     UmmaWgradLaunch U;
     if (use_umma) {
         memset(&U, 0, sizeof(U));
-        U.ngroups = (int)groups.size(); U.batch = h->batch; U.dW = groups[0].dW;
+        U.ngroups = (int)groups.size(); U.batch = call.batch; U.dW = groups[0].dW;
         U.w_sp = op.cout; U.w_sg = 1; U.scale = scale;
         for (size_t g = 0; g < groups.size(); ++g) {
             WgGroup& G = U.grp[g];
@@ -690,20 +709,19 @@ static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, in
     auto colsum_launches = [&]() {                        // bias gradient by its own kernel (paths without a split pass)
         for (const auto& dp : class_dpre) {
             Op& o = add(b, OP_COLSUM, b.ws);
-            o.colsum.V = dp; o.colsum.batch = h->batch; o.colsum.scale = scale; o.colsum.out = bias_grad;
+            o.colsum.V = dp; o.colsum.batch = call.batch; o.colsum.scale = scale; o.colsum.out = bias_grad;
         }
     };
     if (use_umma) {
-        const size_t split_need = h->bulk_wgrad ? umma_plan_wgrad_split(U, 1, nullptr, nullptr, nullptr) : 0;
+        const size_t split_need = h->opt.bulk_wgrad ? umma_plan_wgrad_split(U, 1, nullptr, nullptr, nullptr) : 0;
         const bool bulk = split_need > 0;                 // 0: too many distinct views for one split pass -> converter-fed kernel
         // Bias column sums inside the split pass instead of their own launches (WUN_SPLIT_COLSUM: 1 = default, 0 = separate colsum
         // launches, 2 = fused only for the layers with few rows).  History: while the dgrad chain was the critical path the separate
         // launches were 0.05 ms faster per step (they fill SMs the big-shared-memory kernels leave thread slots on); since the epilogue
         // work of round 2 the wgrad stream is the critical path and the fused form wins (5.45 -> 5.39 ms, wgrad family 2.52 -> 2.24 ms).
-        static const int colsum_mode = [] { const char* e = getenv("WUN_SPLIT_COLSUM"); return e ? atoi(e) : 1; }();
         int max_rows_g = 0;
         for (const auto& dp : class_dpre) max_rows_g = std::max(max_rows_g, dp.r_hi - dp.r_lo);
-        const bool fused_colsum = colsum_mode == 1 || (colsum_mode == 2 && max_rows_g <= 4096);
+        const bool fused_colsum = h->opt.split_colsum == 1 || (h->opt.split_colsum == 2 && max_rows_g <= 4096);
         if (bulk) {      // + the split pass and the fixed-order reduction of the partial tiles / column sums
             b.split_item = std::max(b.split_item, split_need);
             b.wg_partial = std::max(b.wg_partial, umma_wgrad_partial_bytes(U));
@@ -713,13 +731,11 @@ static int build_wgrad(Build& b, const ConvOp& op, float* grads, float scale, in
             add(b, OP_WGRAD_UMMA, b.ws).wgu.U = U;
             return WUN_OK;
         }
-        uint8_t* arena = reinterpret_cast<uint8_t*>(h->ws + h->lay.total) + h->arena_sum;
-        if (ahead && (b.wg_index & 1)) arena += split_arena_half_bytes(h, h->batch);
-        arena += (256 - (reinterpret_cast<uintptr_t>(arena) & 255)) & 255;
+        uint8_t* arena = ws_at(call, call.map.split[ahead ? b.wg_index & 1 : 0]);
         // split arrays, then the partial tiles, in this half; the class-gradient views among the jobs also produce the
         // bias gradient (their column sums)
         decltype(Op::wgu) W;     // shared by the split pass, the wgrad and its reduction
-        if (!umma_wgrad_bulk_setup(&U, h->batch, arena, class_dpre.data(), (int)class_dpre.size(), fused_colsum ? bias_grad : nullptr,
+        if (!umma_wgrad_bulk_setup(&U, call.batch, arena, class_dpre.data(), (int)class_dpre.size(), fused_colsum ? bias_grad : nullptr,
                                    scale, &W.S, &W.J))
             return set_err(WUN_E_INVALID, "wgrad split pass: class gradient view not among the split jobs");
         W.U = U;
@@ -751,7 +767,7 @@ static void fork_side(Build& b) {
     add(b, OP_MAKE, ST_CALLER, EV_FORK, b.fork_used + 1);
     add(b, OP_RECORD, ST_CALLER, EV_FORK, b.fork_used);
     add(b, OP_WAIT, ST_SIDE, EV_FORK, b.fork_used);
-    if (b.h->split_ahead) {
+    if (b.h->opt.split_ahead) {
         add(b, OP_MAKE, ST_SPLIT);
         add(b, OP_WAIT, ST_SPLIT, EV_FORK, b.fork_used);
     }
@@ -774,42 +790,43 @@ static int64_t op_first_offset(const Plan& P, const ConvOp& op, const UpsampleSp
     return o;
 }
 
-static void fill_output_launch(const WunHandle* h, OutputLaunch* O, const float* targets, float* outputs, float* loss,
-                               int training) {
+static void fill_output_launch(const WunHandle* h, const Call& call, OutputLaunch* O, const float* targets, float* outputs,
+                               float* loss, int training) {
     const Plan& P = h->plan;
     memset(O, 0, sizeof(*O));
-    O->params = h->params;
+    O->params = call.params;
     for (int s = 0; s < P.nconv; ++s) {
         O->w_off[s] = P.params[P.out_w_param[s]].offset;
         O->b_off[s] = P.params[P.out_b_param[s]].offset;
     }
-    O->mix = h->mix;
-    O->feat = tensor_ptr(h, P.t_feat);
+    O->mix = call.mix;
+    O->feat = tensor_ptr(call, P.t_feat);
     O->targets = targets;
     O->outputs = outputs;
-    O->dpre = (h->lay.off[P.t_dpre_out] >= 0) ? const_cast<float*>(tensor_ptr(h, P.t_dpre_out)) : nullptr;
+    O->dpre = (call.map.act[P.t_dpre_out] >= 0) ? const_cast<float*>(tensor_ptr(call, P.t_dpre_out)) : nullptr;
     O->loss = loss;
-    O->loss_part = loss ? loss_part_ptr(h) : nullptr;
-    O->loss_count = loss ? counters_ptr(h) : nullptr;
-    O->batch = h->batch; O->T_in = (int)P.T_in; O->Tf = (int)P.Tf; O->T_out = (int)P.T_out;
+    O->loss_part = loss ? reinterpret_cast<float*>(ws_at(call, call.map.loss_part)) : nullptr;
+    O->loss_count = loss ? reinterpret_cast<unsigned*>(ws_at(call, call.map.counters)) : nullptr;
+    O->batch = call.batch; O->T_in = (int)P.T_in; O->Tf = (int)P.Tf; O->T_out = (int)P.T_out;
     O->C = P.cfg.num_channels; O->F = P.cfg.num_initial_filters;
     O->nconv = P.nconv; O->K = P.cfg.num_sources;
     O->ofs = P.cfg.output_filter_size; O->pad_left = P.out_pad_left;
     O->crop_feat = P.crop_feat; O->crop_out = P.crop_out;
     O->output_type = P.cfg.output_type; O->activation = P.cfg.output_activation; O->training = training;
-    O->inv_count = 1.0f / (float)((double)h->batch * P.T_out * P.cfg.num_channels * P.cfg.num_sources);
+    O->inv_count = 1.0f / (float)((double)call.batch * P.T_out * P.cfg.num_channels * P.cfg.num_sources);
 }
 
 static int build_forward(Build& b, const float* targets, float* outputs, float* loss, int training) {
     const WunHandle* h = b.h;
+    const Call& call = b.call;
     const Plan& P = h->plan;
     const int L = P.cfg.num_layers;
     for (int i = 0; i < L; ++i) {
         const UpsampleSpec& us = P.ups[i];
         if (us.interp_param >= 0) {
             Op& o = add(b, OP_SIGMOID);
-            o.sig.x = h->params + P.params[us.interp_param].offset;
-            o.sig.y = const_cast<float*>(tensor_ptr(h, us.wsig_tensor)); o.sig.n = us.C;
+            o.sig.x = call.params + P.params[us.interp_param].offset;
+            o.sig.y = const_cast<float*>(tensor_ptr(call, us.wsig_tensor)); o.sig.n = us.C;
         }
     }
     int rc;
@@ -817,17 +834,17 @@ static int build_forward(Build& b, const float* targets, float* outputs, float* 
         if ((rc = build_conv_forward(b, P.down[i], i)) != WUN_OK) return rc;
     if ((rc = build_conv_forward(b, P.bottleneck, L)) != WUN_OK) return rc;
     OutputLaunch O;
-    fill_output_launch(h, &O, targets, outputs, loss, training);
+    fill_output_launch(h, call, &O, targets, outputs, loss, training);
     OutputFuse OF;
     memset(&OF, 0, sizeof(OF));
     b.out_fused = false;
     for (int i = 0; i < L; ++i) {
-        if (i == L - 1 && h->out_fuse_mode != 0 && P.cfg.output_filter_size == 1) {
+        if (i == L - 1 && h->opt.out_fuse_mode != 0 && P.cfg.output_filter_size == 1) {
             // the output layer rides in this conv's epilogue when the planner picks the persistent kernel for it
             OF.O = O;
             const bool bw = targets != nullptr && b.grads != nullptr;
-            OF.gfeat = bw ? const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat])) : nullptr;
-            OF.grads = (bw && h->out_fuse_mode == 2) ? b.grads : nullptr;
+            OF.gfeat = bw ? const_cast<float*>(tensor_ptr(call, P.grad_twin[P.t_feat])) : nullptr;
+            OF.grads = (bw && h->opt.out_fuse_mode == 2) ? b.grads : nullptr;
             OF.grad_scale = b.scale;
             const ConvOp& op = P.up[i];
             bool geom = op.classes.size() >= 1 && op.classes.size() <= (size_t)kMaxClasses;
@@ -848,28 +865,29 @@ static int build_forward(Build& b, const float* targets, float* outputs, float* 
     if (b.out_fused) return WUN_OK;
     // the loss and interp-gradient sums count their CTAs here; each sum's last CTA sets its counter back to 0, this makes
     // sure they start from 0 whatever the workspace held before
-    if (b.train) add(b, OP_COUNTERS).counters = counters_ptr(h);
+    if (b.train) add(b, OP_COUNTERS).counters = reinterpret_cast<unsigned*>(ws_at(call, call.map.counters));
     add(b, OP_OUTPUT_FWD).out.O = O;
     return WUN_OK;
 }
 
 static int build_backward(Build& b, const float* targets, float* grads, float scale) {
     const WunHandle* h = b.h;
+    const Call& call = b.call;
     const Plan& P = h->plan;
     const int L = P.cfg.num_layers;
     int rc;
-    b.ws = h->use_side ? ST_SIDE : ST_CALLER;
+    b.ws = h->opt.use_side ? ST_SIDE : ST_CALLER;
     b.fork_used = b.hoist ? 1 : 0;
-    if (h->use_side) add(b, OP_MAKE, ST_SIDE);
+    if (h->opt.use_side) add(b, OP_MAKE, ST_SIDE);
     OutputLaunch O;
-    fill_output_launch(h, &O, targets, nullptr, nullptr, 1);
+    fill_output_launch(h, call, &O, targets, nullptr, nullptr, 1);
     // fused forward (build_forward): dL/dpre and the feature gradient already exist; only the output convs' weight gradient is left
     // (mode 1), and it goes to the wgrad stream right after the first fork below
-    const bool out_wgrad_late = b.out_fused && h->out_fuse_mode != 2;
+    const bool out_wgrad_late = b.out_fused && h->opt.out_fuse_mode != 2;
     b.out_part = std::max(b.out_part, output_wgrad_partial_bytes(O));
     decltype(Op::out) out;         // the output layer's weight gradient (either form) and the gradient w.r.t. the features
-    out.O = O; out.grads = grads; out.part = out_part_ptr(h); out.scale = scale;
-    out.gfeat = const_cast<float*>(tensor_ptr(h, P.grad_twin[P.t_feat]));
+    out.O = O; out.grads = grads; out.part = reinterpret_cast<float*>(ws_at(call, call.map.out_part)); out.scale = scale;
+    out.gfeat = const_cast<float*>(tensor_ptr(call, P.grad_twin[P.t_feat]));
     if (!b.out_fused) {
         add(b, OP_OUTPUT_WGRAD).out = out;
         add(b, OP_OUTPUT_DGRAD).out = out;
@@ -887,15 +905,15 @@ static int build_backward(Build& b, const float* targets, float* grads, float sc
         const UpsampleSpec& us = P.ups[i];
         UpsampleBwdLaunch U;
         memset(&U, 0, sizeof(U));
-        U.due = tensor_ptr(h, P.t_gue);
-        U.dmid = tensor_ptr(h, P.t_gmid);
-        U.x = tensor_ptr(h, us.src_tensor);
-        U.gx = const_cast<float*>(tensor_ptr(h, P.grad_twin[us.src_tensor]));
-        U.blend = (us.wsig_tensor >= 0) ? tensor_ptr(h, us.wsig_tensor) : nullptr;
+        U.due = tensor_ptr(call, P.t_gue);
+        U.dmid = tensor_ptr(call, P.t_gmid);
+        U.x = tensor_ptr(call, us.src_tensor);
+        U.gx = const_cast<float*>(tensor_ptr(call, P.grad_twin[us.src_tensor]));
+        U.blend = (us.wsig_tensor >= 0) ? tensor_ptr(call, us.wsig_tensor) : nullptr;
         U.dvar = (us.interp_param >= 0) ? grads + P.params[us.interp_param].offset : nullptr;
-        U.part = U.dvar ? dvar_part_ptr(h) : nullptr;
-        U.count = U.dvar ? counters_ptr(h) + 1 : nullptr;
-        U.batch = h->batch; U.N = us.N; U.nmid = us.nmid; U.C = us.C; U.mid_mode = us.mid_mode; U.scale = scale;
+        U.part = U.dvar ? reinterpret_cast<float*>(ws_at(call, call.map.dvar_part)) : nullptr;
+        U.count = U.dvar ? reinterpret_cast<unsigned*>(ws_at(call, call.map.counters)) + 1 : nullptr;
+        U.batch = call.batch; U.N = us.N; U.nmid = us.nmid; U.C = us.C; U.mid_mode = us.mid_mode; U.scale = scale;
         Op& o = add(b, OP_UPSAMPLE_BWD);
         o.up = U; o.layer = L + 1 + i;
     }
@@ -923,8 +941,8 @@ static int build_backward(Build& b, const float* targets, float* grads, float sc
 // A training step: forward + backward, the weight packs hoisted onto the side stream when there is one.
 static int build_step(Build& b, const float* targets, float* outputs, float* loss, float* grads, float scale) {
     const WunHandle* h = b.h;
-    b.hoist = h->use_side && h->umma_enabled;
-    b.dgrad_fork = h->dgrad_par && h->use_side;
+    b.hoist = h->opt.use_side && h->opt.umma_enabled;
+    b.dgrad_fork = h->opt.dgrad_par && h->opt.use_side;
     b.grads = grads; b.scale = scale; b.train = true;
     if (b.hoist) {             // the packs go to the side stream behind the work already enqueued on the caller's stream
         add(b, OP_MAKE, ST_SIDE).early = true;
@@ -961,8 +979,8 @@ static cudaError_t make(WunHandle* h, const Op& o) {
     return e;
 }
 
-static int issue_op(WunHandle* h, const Op& o) {
-    const cudaStream_t s = o.stream == ST_CALLER ? h->stream : h->streams[o.stream];
+static int issue_op(WunHandle* h, cudaStream_t caller, const Op& o) {
+    const cudaStream_t s = o.stream == ST_CALLER ? caller : h->streams[o.stream];
     cudaError_t e = cudaSuccess;
     switch (o.kind) {
         case OP_SIGMOID: launch_sigmoid(o.sig.x, o.sig.y, o.sig.n, s); break;
@@ -991,11 +1009,11 @@ static int issue_op(WunHandle* h, const Op& o) {
 }
 
 // The records in order; with hoisted weight packs, the `early` ones (the packs and their events on the side stream) first.
-static int issue(WunHandle* h, const std::vector<Op>& ops) {
+static int issue(WunHandle* h, const Call& call, const std::vector<Op>& ops) {
     int rc = WUN_OK;
     for (int early = 1; early >= 0; --early)
         for (size_t i = 0; i < ops.size() && rc == WUN_OK; ++i)
-            if (ops[i].early == (early == 1)) rc = issue_op(h, ops[i]);
+            if (ops[i].early == (early == 1)) rc = issue_op(h, call.stream, ops[i]);
     return rc;
 }
 
@@ -1009,28 +1027,33 @@ static int check_device() {
     return WUN_OK;
 }
 
-static int begin_call(WunHandle* h, const float* params, const float* mix, int64_t batch, bool training, void* ws,
-                      int64_t ws_bytes, void* stream, bool dry) {
+// Checks a call's arguments and makes its context; the handle's launch-list storage is emptied for the call's records.
+static int begin_call(WunHandle* h, Call* call, const float* params, const float* mix, int64_t batch, bool training, void* ws,
+                      int64_t ws_bytes, void* stream) {
     if (!h) return set_err(WUN_E_INVALID, "null handle");
     if (batch < 1 || batch > (1 << 20)) return set_err(WUN_E_INVALID, "batch out of range");
-    h->lay = make_layout(h->plan, batch, training);
-    h->batch = (int)batch;
-    h->ops.clear();
-    if (dry) return WUN_OK;
     { int rc0 = check_device(); if (rc0 != WUN_OK) return rc0; }
     if (!params || !mix || !ws) return set_err(WUN_E_INVALID, "null device pointer");
-    if (ws_bytes < h->lay.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + (training ? train_scratch_bytes(h, batch) : 0))
-        return set_err(WUN_E_INVALID, "workspace too small");
+    call->map = ws_map(h, batch, training);
+    if (ws_bytes < call->map.end) return set_err(WUN_E_INVALID, "workspace too small");
     if (reinterpret_cast<uintptr_t>(ws) % 256 != 0) return set_err(WUN_E_INVALID, "workspace must be 256-byte aligned");
-    h->params = params; h->mix = mix; h->ws = (float*)ws; h->stream = (cudaStream_t)stream;
+    call->params = params; call->mix = mix; call->ws = (float*)ws; call->stream = (cudaStream_t)stream; call->batch = (int)batch;
+    h->ops.clear();
     return WUN_OK;
 }
 
-// The launch list of a training step (`training` false: an inference forward) at `batch` for the entry points that describe or
-// count launches: built without a device, never issued.
-static Build build_dry(WunHandle* h, int64_t batch, bool training) {
-    begin_call(h, nullptr, nullptr, batch, training, nullptr, 0, nullptr, true);
-    Build b{h, h->ops};
+// A call that is only built, never issued (launch counts, descriptions, the create-time sizes): no buffers unless the caller
+// sets fake ones, no stream.
+static Call dry_call(const WunHandle* h, int64_t batch, bool training) {
+    Call call;
+    call.batch = (int)batch;
+    call.map = ws_map(h, batch, training);
+    return call;
+}
+
+// The launch list of a training step (`training` false: an inference forward) of a dry call, appended to `ops`.
+static Build build_dry(const WunHandle* h, const Call& call, std::vector<Op>& ops, bool training) {
+    Build b{h, call, ops};
     if (training) build_step(b, nullptr, nullptr, nullptr, nullptr, 1.f);
     else build_forward(b, nullptr, nullptr, nullptr, 0);
     return b;
@@ -1140,19 +1163,19 @@ static void describe_conv(std::string& s, const ConvLaunch& L, int layer, int pa
 }
 
 // one (class, plane) group of a layer's weight gradient (dW[woff + c*cout + n], any form); dW / db = flat parameter offsets
-static void describe_wgrad(std::string& s, const WunHandle* h, const WgGroup& G, int layer, int g) {
+static void describe_wgrad(std::string& s, const WunHandle* h, const WgGroup& G, int layer, int g, int batch) {
     const ConvOp& op = layer_op(h, layer);
     appendf(s, "wgrad layer=%d group=%d N=%d w_sk=%d w_sn=%d dW=%lld db=%lld m_lo=%d m_hi=%d nterms=%d batch=%d\n",
             layer, g, op.cout, op.cout, 1, (long long)h->plan.params[op.w_param].offset, (long long)h->plan.params[op.b_param].offset,
-            G.m_lo, G.m_hi, G.ntaps, h->batch);
+            G.m_lo, G.m_hi, G.ntaps, batch);
     describe_view(s, "wplane", G.P);
     describe_view(s, "wdpre", G.G);
     for (int t = 0; t < G.ntaps; ++t) appendf(s, "wterm i=%d d=%d woff=%d\n", t, G.d[t], G.woff[t]);
 }
 
-// wun_debug_launches: every launch of the step as text (addresses are raw integers relative to the fake bases installed by the
-// caller - nothing is dereferenced)
-static void describe_op(std::string& s, const WunHandle* h, const Op& o) {
+// wun_debug_launches: every launch of the step as text (addresses are raw integers relative to the call's fake bases - nothing
+// is dereferenced)
+static void describe_op(std::string& s, const WunHandle* h, const Call& call, const Op& o) {
     const Plan& P = h->plan;
     if (o.kind == OP_FIRST_FWD) {        // its weight gradient has the same geometry; gdec / godd = the gradient tensors it reads
         const FirstLayer& F = o.first;
@@ -1160,8 +1183,8 @@ static void describe_op(std::string& s, const WunHandle* h, const Op& o) {
         appendf(s, "first C=%d N=%d k=%d pad_left=%d batch=%d x=%lld x_bstride=%lld T=%d dec=%lld dec_bstride=%lld Td=%d "
                 "odd=%lld odd_bstride=%lld mo_lo=%d mo_hi=%d gdec=%lld godd=%lld dW=%lld db=%lld\n",
                 P.cfg.num_channels, op.cout, F.k, F.pad_left, F.batch, addr(F.x), F.x_bstride, F.T, addr(F.dec), F.dec_bstride, F.Td,
-                addr(F.odd), F.odd_bstride, F.mo_lo, F.mo_hi, addr(tensor_ptr(h, P.grad_twin[op.classes[0].out.tensor])),
-                addr(tensor_ptr(h, P.grad_twin[op.classes[1].out.tensor])), (long long)P.params[op.w_param].offset,
+                addr(F.odd), F.odd_bstride, F.mo_lo, F.mo_hi, addr(tensor_ptr(call, P.grad_twin[op.classes[0].out.tensor])),
+                addr(tensor_ptr(call, P.grad_twin[op.classes[1].out.tensor])), (long long)P.params[op.w_param].offset,
                 (long long)P.params[op.b_param].offset);
     } else if (o.kind == OP_CONV || o.kind == OP_UMMA_CONV) {
         describe_conv(s, o.kind == OP_CONV ? o.conv : o.umma.L, o.layer, o.pass);
@@ -1170,7 +1193,7 @@ static void describe_op(std::string& s, const WunHandle* h, const Op& o) {
         appendf(s, "output batch=%d T_in=%d Tf=%d T_out=%d C=%d F=%d nconv=%d K=%d ofs=%d pad_left=%d crop_feat=%d "
                 "crop_out=%d output_type=%d activation=%d feat=%lld dpre=%lld gfeat=%lld",
                 O.batch, O.T_in, O.Tf, O.T_out, O.C, O.F, O.nconv, O.K, O.ofs, O.pad_left, O.crop_feat, O.crop_out, O.output_type,
-                O.activation, addr(O.feat), addr(O.dpre), addr(tensor_ptr(h, P.grad_twin[P.t_feat])));
+                O.activation, addr(O.feat), addr(O.dpre), addr(tensor_ptr(call, P.grad_twin[P.t_feat])));
         for (int k = 0; k < 8; ++k)
             appendf(s, " w_off%d=%lld b_off%d=%lld", k, k < O.nconv ? O.w_off[k] : -1LL, k, k < O.nconv ? O.b_off[k] : -1LL);
         s += "\n";
@@ -1184,9 +1207,9 @@ static void describe_op(std::string& s, const WunHandle* h, const Op& o) {
         WgGroup G;
         G.P = o.wg.plane; G.G = o.wg.dpre; G.m_lo = o.wg.m_lo; G.m_hi = o.wg.m_hi; G.ntaps = o.wg.nterms;
         for (int t = 0; t < G.ntaps; ++t) { G.d[t] = o.wg.d[t]; G.woff[t] = o.wg.woff[t]; }
-        describe_wgrad(s, h, G, o.layer, o.index);
+        describe_wgrad(s, h, G, o.layer, o.index, call.batch);
     } else if (o.kind == OP_WGRAD_UMMA || o.kind == OP_WGRAD_BULK) {    // all groups of the layer in one launch
-        for (int g = 0; g < o.wgu.U.ngroups; ++g) describe_wgrad(s, h, o.wgu.U.grp[g], o.layer, g);
+        for (int g = 0; g < o.wgu.U.ngroups; ++g) describe_wgrad(s, h, o.wgu.U.grp[g], o.layer, g, call.batch);
     }
 }
 
@@ -1213,23 +1236,10 @@ int wun_create_for_input(const WunConfig* cfg, int64_t input_frames, WunHandle**
     int rc = build_plan(*cfg, input_frames, &h->plan, &msg);
     if (rc != WUN_OK) { delete h; return set_err(rc, msg); }
     plan_backward(h);
-    const char* dis = getenv("WUN_DISABLE_UMMA");
-    h->umma_enabled = !(dis && dis[0] == '1');
-    { const char* names[3] = {"WUN_UMMA_FWD", "WUN_UMMA_DGRAD", "WUN_UMMA_WGRAD"};
-      for (int i = 0; i < 3; ++i) { const char* v = getenv(names[i]); h->umma_pass[i] = !(v && v[0] == '0'); } }
-    { const char* v = getenv("WUN_SIDE_STREAM"); h->use_side = !(v && v[0] == '0'); }
-    // "=0" selects the generic path for A/B runs
-    { const char* v = getenv("WUN_FIRST_LAYER"); h->first_fast = !(v && v[0] == '0'); }
-    { const char* v = getenv("WUN_PACK_EVENTS"); h->pack_events_on = !(v && v[0] == '0'); }
-    { const char* v = getenv("WUN_BULK_WGRAD"); h->bulk_wgrad = !(v && v[0] == '0'); }
-    { const char* v = getenv("WUN_PAIR_DGRAD"); h->pair_dgrad = v ? atoi(v) : 4; }
-    { const char* v = getenv("WUN_DGRAD_PAR"); h->dgrad_par = !(v && v[0] == '0'); }
-    { const char* v = getenv("WUN_SPLIT_AHEAD"); h->split_ahead = !(v && v[0] == '0'); }
-    { const char* v = getenv("WUN_PAIR_MIN_CTAS"); h->pair_min_ctas = v ? atoi(v) : 120; }
-    { const char* v = getenv("WUN_OUT_FUSE"); h->out_fuse_mode = v ? atoi(v) : 1; }
-    { const char* v = getenv("WUN_PAIR_FWD"); h->pair_fwd = !(v && v[0] == '0'); }
+    h->opt = read_options();
     // the launch list of a batch-1 training step: which kernel each layer uses and how much scratch the launches need
-    const Build b = build_dry(h, 1, true);
+    const Call call = dry_call(h, 1, true);
+    const Build b = build_dry(h, call, h->ops, true);
     h->arena_sum = b.pack_sum; h->split_item_bytes = b.split_item; h->wg_partial_bytes = b.wg_partial; h->out_part_bytes = b.out_part;
     h->kernel_used.assign((size_t)(2 * h->plan.cfg.num_layers + 1) * 3, "simt");
     for (const Op& o : b.ops)      // a layer pass runs on the kernel of its last plane convolution / weight gradient
@@ -1273,8 +1283,7 @@ int wun_param_table(const WunHandle* h, WunParamInfo* out, int64_t capacity) {
 
 int64_t wun_workspace_bytes(const WunHandle* h, int64_t batch, int training) {
     if (!h || batch < 1) return -1;
-    Layout l = make_layout(h->plan, batch, training != 0);
-    return l.total * (int64_t)sizeof(float) + (int64_t)h->arena_sum + 256 + (training ? train_scratch_bytes(h, batch) : 0);
+    return ws_map(h, batch, training != 0).end + 256;
 }
 
 double wun_forward_flops(const WunHandle* h, int64_t batch) { return h ? h->plan.fwd_flops_per_item * batch : 0; }
@@ -1282,22 +1291,25 @@ double wun_forward_backward_flops(const WunHandle* h, int64_t batch) {
     return h ? (3.0 * h->plan.fwd_flops_per_item - h->plan.dgrad0_flops_per_item) * batch : 0;
 }
 
-int64_t wun_launches_forward(const WunHandle* h) {
-    return h ? kernel_launches(build_dry(const_cast<WunHandle*>(h), 1, false).ops) : -1;
+static int64_t dry_launches(const WunHandle* h, bool training) {
+    if (!h) return -1;
+    std::vector<Op> ops;
+    build_dry(h, dry_call(h, 1, training), ops, training);
+    return kernel_launches(ops);
 }
 
-int64_t wun_launches_forward_backward(const WunHandle* h) {
-    return h ? kernel_launches(build_dry(const_cast<WunHandle*>(h), 1, true).ops) : -1;
-}
+int64_t wun_launches_forward(const WunHandle* h) { return dry_launches(h, false); }
+int64_t wun_launches_forward_backward(const WunHandle* h) { return dry_launches(h, true); }
 
 int wun_forward(WunHandle* h, const float* params, const float* mix, int64_t batch, int training, float* outputs,
                 void* workspace, int64_t workspace_bytes, void* stream) {
-    int rc = begin_call(h, params, mix, batch, false, workspace, workspace_bytes, stream, false);
+    Call call;
+    int rc = begin_call(h, &call, params, mix, batch, false, workspace, workspace_bytes, stream);
     if (rc != WUN_OK) return rc;
     if (!outputs) return set_err(WUN_E_INVALID, "outputs is null");
-    Build b{h, h->ops};
+    Build b{h, call, h->ops};
     rc = build_forward(b, nullptr, outputs, nullptr, training);
-    if (rc == WUN_OK) rc = issue(h, b.ops);
+    if (rc == WUN_OK) rc = issue(h, call, b.ops);
     if (rc != WUN_OK) return rc;
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
@@ -1306,14 +1318,15 @@ int wun_forward(WunHandle* h, const float* params, const float* mix, int64_t bat
 int wun_forward_backward(WunHandle* h, const float* params, const float* mix, const float* targets, int64_t batch,
                          float* outputs, float* loss, float* grads, float grad_scale, void* workspace,
                          int64_t workspace_bytes, void* stream) {
-    int rc = begin_call(h, params, mix, batch, true, workspace, workspace_bytes, stream, false);
+    Call call;
+    int rc = begin_call(h, &call, params, mix, batch, true, workspace, workspace_bytes, stream);
     if (rc != WUN_OK) return rc;
     if (!targets || !loss || !grads) return set_err(WUN_E_INVALID, "targets/loss/grads must not be null");
-    WUN_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), h->stream));
-    WUN_CUDA_OK(cudaMemsetAsync(grads, 0, sizeof(float) * h->plan.param_numel, h->stream));
-    Build b{h, h->ops};
+    WUN_CUDA_OK(cudaMemsetAsync(loss, 0, sizeof(float), call.stream));
+    WUN_CUDA_OK(cudaMemsetAsync(grads, 0, sizeof(float) * h->plan.param_numel, call.stream));
+    Build b{h, call, h->ops};
     rc = build_step(b, targets, outputs, loss, grads, grad_scale);
-    if (rc == WUN_OK) rc = issue(h, b.ops);
+    if (rc == WUN_OK) rc = issue(h, call, b.ops);
     if (rc != WUN_OK) return rc;
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
@@ -1409,24 +1422,26 @@ int64_t wun_describe(const WunHandle* h, char* buf, int64_t capacity) {
     return copy_out(s, buf, capacity);
 }
 
-int64_t wun_debug_plan(const WunHandle* hc, int64_t batch, char* buf, int64_t capacity) {
-    WunHandle* h = const_cast<WunHandle*>(hc);
+int64_t wun_debug_plan(const WunHandle* h, int64_t batch, char* buf, int64_t capacity) {
     if (!h || batch < 1) return -1;
+    std::vector<Op> ops;
+    build_dry(h, dry_call(h, batch, true), ops, true);
     std::string s;
-    for (const Op& o : build_dry(h, batch, true).ops) audit_op(s, o);
+    for (const Op& o : ops) audit_op(s, o);
     return copy_out(s, buf, capacity);
 }
 
-int64_t wun_debug_launches(const WunHandle* hc, int64_t batch, char* buf, int64_t capacity) {
-    WunHandle* h = const_cast<WunHandle*>(hc);
+int64_t wun_debug_launches(const WunHandle* h, int64_t batch, char* buf, int64_t capacity) {
     if (!h || batch < 1) return -1;
     // fake, far-apart bases (never dereferenced): every described address identifies its buffer
-    h->ws = reinterpret_cast<float*>((uintptr_t)1 << 40); h->params = reinterpret_cast<const float*>((uintptr_t)1 << 41);
-    h->mix = reinterpret_cast<const float*>((uintptr_t)1 << 42);
+    Call call = dry_call(h, batch, true);
+    call.ws = reinterpret_cast<float*>((uintptr_t)1 << 40); call.params = reinterpret_cast<const float*>((uintptr_t)1 << 41);
+    call.mix = reinterpret_cast<const float*>((uintptr_t)1 << 42);
+    std::vector<Op> ops;
+    build_dry(h, call, ops, true);
     std::string s;
-    for (const Op& o : build_dry(h, batch, true).ops) describe_op(s, h, o);
+    for (const Op& o : ops) describe_op(s, h, call, o);
     s += "adam n=" + std::to_string((long long)h->plan.param_numel) + "\n";     // wun_adam_step(_device) over the flat buffer
-    h->ws = nullptr; h->params = nullptr; h->mix = nullptr;
     return copy_out(s, buf, capacity);
 }
 
@@ -1446,7 +1461,8 @@ int wun_debug_run_layer(WunHandle* h, int layer, int pass, int iters, const floa
     const int L = h->plan.cfg.num_layers;
     if (layer < 0 || layer > 2 * L) return set_err(WUN_E_INVALID, "layer out of range");
     if (pass == 2 && !grads_scratch) return set_err(WUN_E_INVALID, "wgrad pass needs a gradient scratch buffer");
-    int rc = begin_call(h, params, mix, batch, true, workspace, workspace_bytes, stream, false);
+    Call call;
+    int rc = begin_call(h, &call, params, mix, batch, true, workspace, workspace_bytes, stream);
     if (rc != WUN_OK) return rc;
     const ConvOp& op = layer_op(h, layer);
     const OpBackward& ob = (layer < L) ? h->bwd_down[layer] : (layer == L ? h->bwd_bottleneck : h->bwd_up[layer - L - 1]);
@@ -1466,14 +1482,14 @@ int wun_debug_run_layer(WunHandle* h, int layer, int pass, int iters, const floa
         *flops_per_launch = f;
     }
     // the layer pass as in a step, on the caller's stream (a dgrad's second launch on the helper stream once a step made it)
-    Build b{h, h->ops};
-    b.dgrad_fork = h->dgrad_par && h->use_side && h->streams[ST_SIDE] != nullptr;
+    Build b{h, call, h->ops};
+    b.dgrad_fork = h->opt.dgrad_par && h->opt.use_side && h->streams[ST_SIDE] != nullptr;
     rc = (pass == 0) ? build_conv_forward(b, op, layer) : (pass == 1) ? build_dgrad(b, op, ob, layer) : build_wgrad(b, op, grads_scratch, 1.f, layer);
-    if (rc == WUN_OK) rc = issue(h, b.ops);
+    if (rc == WUN_OK) rc = issue(h, call, b.ops);
     // forward: packed once, the tensor-core conv enqueued `iters` times; dgrad / wgrad: the whole pass again
     for (int i = 1; i < iters && rc == WUN_OK; ++i)
         for (size_t k = 0; k < b.ops.size() && rc == WUN_OK; ++k)
-            if (pass != 0 || b.ops[k].kind == OP_UMMA_CONV) rc = issue_op(h, b.ops[k]);
+            if (pass != 0 || b.ops[k].kind == OP_UMMA_CONV) rc = issue_op(h, call.stream, b.ops[k]);
     if (rc != WUN_OK) return rc;
     WUN_CUDA_OK(cudaGetLastError());
     return WUN_OK;
@@ -1487,11 +1503,11 @@ int wun_debug_run_conv(WunHandle* h, int layer, int iters, const float* params, 
 int wun_debug_tensor(const WunHandle* h, const char* name, int64_t batch, int training, int64_t* offset_floats,
                      int64_t* rows, int32_t* channels) {
     if (!h || !name || !offset_floats || !rows || !channels) return set_err(WUN_E_INVALID, "null argument");
-    Layout l = make_layout(h->plan, batch, training != 0);
+    const WsMap m = ws_map(h, batch, training != 0);
     for (size_t i = 0; i < h->plan.tensors.size(); ++i)
         if (h->plan.tensors[i].name == name) {
-            if (l.off[i] < 0) return set_err(WUN_E_INVALID, "tensor exists only in training workspaces");
-            *offset_floats = l.off[i]; *rows = h->plan.tensors[i].rows; *channels = h->plan.tensors[i].C;
+            if (m.act[i] < 0) return set_err(WUN_E_INVALID, "tensor exists only in training workspaces");
+            *offset_floats = m.act[i]; *rows = h->plan.tensors[i].rows; *channels = h->plan.tensors[i].C;
             return WUN_OK;
         }
     return set_err(WUN_E_INVALID, std::string("no workspace tensor named ") + name);
