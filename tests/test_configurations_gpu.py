@@ -6,12 +6,12 @@ fallback for channel counts that are not multiples of 8, the dedicated first lay
 emit are not the ones the smaller replay and parity tests reach.  Four checks:
   A  every conv / dgrad / wgrad / first / output / upsample / Adam launch of each configuration, alone, against the float64
      interpreter, with the bounds, sentinels and "outside the views" checks of tests/test_kernels_gpu.py and
-     tests/test_step_kernels_gpu.py;
+     tests/test_step_kernels_gpu.py (the replays of tests/conv_launches.py and tests/step_launches.py);
   B  whole training steps against the oracle with the bars of tests/test_gpu_parity.py (outputs 1e-4, gradients 1e-3 or proven
      LeakyReLU slope flips), grads(B) == sum of per-example grads, and windowed prediction over two forward batch sizes;
   C  the random sweep of tests/test_cpu_device.py (same draws) on the device: two training steps with Adam plus inference against
      the oracle with that file's bars, and the launch replays of A;
-  D  every switch of tests/test_cpu_device.SWITCHES against the oracle and against the default path's gradients.
+  D  every switch of SWITCHES (tests/configurations.py) against the oracle and against the default path's gradients.
 A host-only test (E) asserts from the dry runs that the configurations still reach the paths A-D are meant to cover.
 
 Run with -s for the per-configuration table: launches replayed per kernel family, worst err / ref_abs against its bound, the
@@ -22,13 +22,16 @@ from collections import OrderedDict, defaultdict
 
 import numpy as np
 import pytest
+import torch
 
 import Config
 import wun
+from configurations import (FORCED, GRAD_TOL, OUT_TOL, SWITCHES, assert_steps_match_oracle, check_outputs, engine_masks, make_sep,
+                            random_model_configs, random_problem, rel_l2, rel_max)
+from conv_launches import replay_conv_and_wgrad
+from launch_checks import engine, gpu_lib, lib_or_skip, print_report, set_env
 from oracle import wave_unet_oracle as O
-import test_kernels_gpu as K
-import test_step_kernels_gpu as S
-from test_cpu_device import FORCED, SWITCHES, assert_steps_match_oracle, random_model_configs
+from step_launches import replay_step_launches
 
 START = time.time()
 REPORT = OrderedDict()               # configuration -> (peak device GB, seconds)
@@ -50,27 +53,10 @@ DRAWS = random_model_configs(16, seed=2026)
 # residual shrinks: after one Adam step of the L=5 switch net the loss sits 1.1e-5 from float64 (1.0e-6 before it), and one
 # learned-upsampling draw's interp gradient 1.3e-4.  These are the bars of tests/test_gpu_parity.py for outputs and gradients.
 GPU_BARS = dict(loss_tol=1e-4, grad_tol=1e-3, out_tol=1e-4)
-# the bound each family's float regime is held to (tests/test_kernels_gpu.py, tests/test_step_kernels_gpu.py)
-BOUNDS = {"fwd": K.TAU, "dgrad": K.TAU, "wgrad": K.TAU, "first fwd": S.TAU_FIRST, "first wgrad": S.TAU_RED, "output fwd": S.TAU_OUT,
-          "output dgrad": S.TAU_OUT, "output wgrad": S.TAU_RED, "upsample bwd": S.TAU_UP}
-
-
-def _torch():
-    import torch
-    return torch
 
 
 def model_config(named, ov):
     return Config.build_config(named, ov, experiment_id=0)["model_config"]
-
-
-def dry_run(named, ov, batch, nf):
-    """-> (cfg, engine, conv launch descriptions, plan audit) of a training step at `batch` (host only)."""
-    cfg = model_config(named, ov)
-    t_in, _ = O.get_padding(cfg, nf or cfg["num_frames"])
-    eng = wun.Engine(wun.config_from_model_config(cfg), input_frames=t_in)
-    descs = eng.launch_descriptions(batch)
-    return cfg, eng, descs, eng.plan_audit(batch)
 
 
 def tensor_core_expected(D):
@@ -79,25 +65,16 @@ def tensor_core_expected(D):
     return D["launch"]["N"] >= 16 and all(P["C"] % 8 == 0 for P in D["planes"])
 
 
-def print_report(prefix):
-    print("\n%-44s %6s %12s %10s" % (prefix + " kernel family", "cases", "worst", "bound"))
-    for fam in sorted(f for f in K.COUNTS if f.startswith(prefix)):
-        short = fam[len(prefix):]
-        w = K.WORST.get(fam, K.WORST.get(fam + " (err/bound)"))
-        bound = next((b for k, b in BOUNDS.items() if short.endswith(k)), None)
-        print("%-44s %6d %12s %10s" % (fam, K.COUNTS[fam], "-" if w is None else "%.2e" % w,
-                                       "ulp" if bound is None else "%.2e" % bound))
-
-
 # ------------------------------------------------------------------------------------------------
 # E: host only - the dry runs still reach what the GPU tests rely on
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name,named,ov,batch,nf,env", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_configurations_reach_the_paths_their_gpu_tests_cover(name, named, ov, batch, nf, env, monkeypatch):
     """Host only: a planner change cannot quietly drop a path from the GPU tests of this file."""
-    lib = K._lib_or_skip()
-    K.set_env(monkeypatch, env)
-    cfg, eng, descs, audit = dry_run(named, ov, batch, nf)
+    lib = lib_or_skip()
+    set_env(monkeypatch, env)
+    cfg, _, eng, descs = engine(named, ov, batch, nf)
+    audit = eng.plan_audit(batch)
     wgmma = {(d["layer"], d["pass"]) for d in audit if d["op"] == "conv"}
     kinds = [k for k, _ in eng.step_launches]
     for D in descs:                                  # tensor cores exactly on the multiple-of-8 launches
@@ -129,8 +106,8 @@ def test_configurations_reach_the_paths_their_gpu_tests_cover(name, named, ov, b
 def test_random_draws_and_switch_nets_reach_their_paths_host_only(monkeypatch):
     """Host only: the random sweep keeps drawing CUDA-core launches and learned upsampling (never with MID_CLAMP), and every switch
     of SWITCHES changes the launch set it is meant to change."""
-    K._lib_or_skip()
-    K.set_env(monkeypatch, {})
+    lib_or_skip()
+    set_env(monkeypatch, {})
     seen = defaultdict(int)
     for label, named, ov, batch, nf, _, _ in DRAWS:
         cfg = model_config(named, ov)
@@ -147,12 +124,13 @@ def test_random_draws_and_switch_nets_reach_their_paths_host_only(monkeypatch):
             seen["learned"] += 1
             assert all(d["mid_mode"] != 1 for k, d in eng.step_launches if k == "upsample"), label
     assert seen["feasible"] >= 10 and seen["simt"] > 0 and seen["wgmma"] > 0 and seen["learned"] > 0, dict(seen)
-    base = _switch_nets()[0]
-    K.set_env(monkeypatch, FORCED)
-    _, _, _, audit0 = dry_run(base[1], base[2], base[3], base[4])
+    _, named, ov, batch, nf, _ = _switch_nets()[0]
+    set_env(monkeypatch, FORCED)
+    audit0 = engine(named, ov, batch, nf)[2].plan_audit(batch)
     for sw in SWITCHES:
-        K.set_env(monkeypatch, dict(FORCED, **sw))
-        _, eng, _, audit = dry_run(base[1], base[2], base[3], base[4])
+        set_env(monkeypatch, dict(FORCED, **sw))
+        eng = engine(named, ov, batch, nf)[2]
+        audit = eng.plan_audit(batch)
         if sw.get("WUN_DISABLE_UMMA") == "1":
             assert not any(d["op"] == "conv" for d in audit)
         if sw.get("WUN_FIRST_LAYER") == "0":
@@ -168,17 +146,15 @@ def test_random_draws_and_switch_nets_reach_their_paths_host_only(monkeypatch):
 # A: launch-by-launch replays
 # ------------------------------------------------------------------------------------------------
 def replay_all(name, named, ov, batch, nf):
-    torch = _torch()
-    K._gpu_lib()
-    S._gpu_lib()
+    gpu_lib()
     torch.cuda.synchronize()
     torch.cuda.reset_peak_memory_stats()
     t0 = time.time()
     prefix = name + ": "
-    n_conv = K.replay_conv_and_wgrad(name, named, ov, batch, nf, prefix=prefix)
-    steps = S.replay_step_launches(name, named, ov, batch, nf, adam=True, prefix=prefix)
+    n_conv = replay_conv_and_wgrad(name, named, ov, batch, nf, prefix=prefix)
+    steps = replay_step_launches(name, named, ov, batch, nf, adam=True, prefix=prefix)
     REPORT[name] = (torch.cuda.max_memory_allocated() / 1e9, time.time() - t0)
-    print_report(prefix)
+    print_report(prefix + " kernel family", prefix)
     print("%s: %d conv / wgrad and %d step launches replayed, peak %.1f GB, %.0f s" % (name, n_conv, len(steps), REPORT[name][0],
                                                                                        REPORT[name][1]))
     return n_conv, steps
@@ -187,7 +163,7 @@ def replay_all(name, named, ov, batch, nf):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,named,ov,batch,nf,env", CONFIGS, ids=[c[0] for c in CONFIGS])
 def test_replayed_launches_of_the_configuration_match_float64(name, named, ov, batch, nf, env, monkeypatch):
-    K.set_env(monkeypatch, env)
+    set_env(monkeypatch, env)
     replay_all(name, named, ov, batch, nf)
 
 
@@ -197,11 +173,9 @@ def test_replayed_launches_of_the_configuration_match_float64(name, named, ov, b
 def step_vs_oracle(cfg, B, seed, per_example=True, oracle=True):
     """Estimates (test and train mode), loss and every gradient of one training step at batch B against the oracle, and with
     `per_example` grads(B) == the sum of the B per-example gradients at grad_scale = 1/B.  Returns the separator."""
-    import test_gpu_parity as P
-    torch = _torch()
-    t_in, t_out, params, mix, targets = P.random_problem(cfg, B, cfg["num_frames"], seed)
+    t_in, t_out, params, mix, targets = random_problem(cfg, B, cfg["num_frames"], seed)
     names = cfg["source_names"]
-    sep = P.make_sep(cfg, params, t_in)
+    sep = make_sep(cfg, params, t_in)
     mix_d = torch.from_numpy(mix).cuda()
     t_oracle = 0.0
     if oracle:
@@ -209,14 +183,14 @@ def step_vs_oracle(cfg, B, seed, per_example=True, oracle=True):
             t = time.time()
             want = O.forward_np(cfg, params, mix, training)
             t_oracle += time.time() - t
-            P.check_outputs(sep.get_output(mix_d, training, False, reuse=True), want, names)
+            check_outputs(sep.get_output(mix_d, training, False, reuse=True), want, names)
     tg = sep.stack_targets({k: torch.from_numpy(v).cuda() for k, v in targets.items()})
     outs = torch.empty((len(names), B, t_out, O.num_channels(cfg)), device="cuda")
     loss_b = float(sep.loss_and_gradients(mix_d, tg, outputs=outs).item())
     g_b = sep.grads.clone()
     named_b = {n: g.cpu().numpy().copy() for n, g in sep.gradients().items()}
     outs = outs.cpu().numpy()
-    masks = P.engine_masks(sep, cfg, B, t_in)
+    masks = engine_masks(sep, cfg, B, t_in)
     tab = sep.engine(input_frames=t_in).param_table
     per = {}
     if per_example:
@@ -227,7 +201,7 @@ def step_vs_oracle(cfg, B, seed, per_example=True, oracle=True):
                                                        grad_scale=1.0 / B).item()))
             acc += sep.grads
         assert abs(np.mean(losses) - loss_b) <= 1e-5 * loss_b, (np.mean(losses), loss_b)
-        per = {n: P.rel_l2(g_b[o:o + c].cpu().numpy(), acc[o:o + c].cpu().numpy()) for n, _, o, c in tab}
+        per = {n: rel_l2(g_b[o:o + c].cpu().numpy(), acc[o:o + c].cpu().numpy()) for n, _, o, c in tab}
         print("B=%d vs the sum of B=1 gradients: worst tensor %.2e" % (B, max(per.values())))
     per_o = {}
     if oracle:
@@ -236,16 +210,16 @@ def step_vs_oracle(cfg, B, seed, per_example=True, oracle=True):
         t_oracle += time.time() - t
         assert abs(loss_b - loss_o) <= 1e-5 * abs(loss_o), (loss_b, loss_o)
         for k, s in enumerate(names):
-            assert P.rel_l2(outs[k], outs_o[s]) <= P.OUT_TOL and P.rel_max(outs[k], outs_o[s]) <= P.OUT_TOL, s
-        per_o = {n: P.rel_l2(named_b[n], grads_o[n]) for n in params}
+            assert rel_l2(outs[k], outs_o[s]) <= OUT_TOL and rel_max(outs[k], outs_o[s]) <= OUT_TOL, s
+        per_o = {n: rel_l2(named_b[n], grads_o[n]) for n in params}
         print("B=%d vs oracle: worst tensor %.2e (oracle CPU time %.0f s)" % (B, max(per_o.values()), t_oracle))
-    if max(list(per_o.values()) + [0.0]) > P.GRAD_TOL or max(list(per.values()) + [0.0]) > 1e-4:
+    if max(list(per_o.values()) + [0.0]) > GRAD_TOL or max(list(per.values()) + [0.0]) > 1e-4:
         # LeakyReLU slope flips (test_gpu_parity.check_grads): the oracle with the engine's own slopes of the batch-B step
         _, _, grads_m, report = O.forward_backward_with_masks(cfg, params, mix, targets, masks)
-        per_m = {n: P.rel_l2(named_b[n], grads_m[n]) for n in params}
-        assert max(per_m.values()) <= P.GRAD_TOL, sorted(per_m.items(), key=lambda kv: -kv[1])[:3]
+        per_m = {n: rel_l2(named_b[n], grads_m[n]) for n in params}
+        assert max(per_m.values()) <= GRAD_TOL, sorted(per_m.items(), key=lambda kv: -kv[1])[:3]
         assert max(r[2] for r in report) <= 1e-4, report
-        assert max(list(per.values()) + [0.0]) <= P.GRAD_TOL, max(per.values())
+        assert max(list(per.values()) + [0.0]) <= GRAD_TOL, max(per.values())
     return sep, t_in
 
 
@@ -254,7 +228,7 @@ def step_vs_oracle(cfg, B, seed, per_example=True, oracle=True):
 def test_benchmarked_batches_match_the_oracle(preset, B, monkeypatch):
     """M5 `full` at batch 16 (bench.py's M5 workload) and M6 at 4 per GPU (its 8-GPU split): the planner really takes output-channel
     splits here, and estimates, loss and every gradient match the oracle and the per-example sum."""
-    K.set_env(monkeypatch, {})
+    set_env(monkeypatch, {})
     cfg = model_config([preset], {})
     sep, t_in = step_vs_oracle(cfg, B, 4243)
     audit = sep.engine(input_frames=t_in).plan_audit(B)
@@ -264,11 +238,11 @@ def test_benchmarked_batches_match_the_oracle(preset, B, monkeypatch):
 @pytest.mark.gpu
 def test_m6_batch32_matches_the_per_example_sum_and_the_oracle(monkeypatch):
     """bench.py's one-GPU M6 workload (batch 32): grads(32) == the sum of the 32 per-example gradients, and the oracle."""
-    K.set_env(monkeypatch, {})
-    _torch().cuda.reset_peak_memory_stats()
+    set_env(monkeypatch, {})
+    torch.cuda.reset_peak_memory_stats()
     t = time.time()
     step_vs_oracle(model_config(["full_multi_instrument"], {}), 32, 4244)
-    REPORT["M6_full_b32 parity"] = (_torch().cuda.max_memory_allocated() / 1e9, time.time() - t)
+    REPORT["M6_full_b32 parity"] = (torch.cuda.max_memory_allocated() / 1e9, time.time() - t)
 
 
 @pytest.mark.gpu
@@ -276,7 +250,7 @@ def test_m6_batch32_matches_the_per_example_sum_and_the_oracle(monkeypatch):
 def test_unrun_presets_match_the_oracle(preset, B, monkeypatch):
     """The two reference presets no other test builds, at their full window: 14 levels of single-tap merge convs down to a few
     rows, and 34 * k channels, mostly on the CUDA-core kernels with the first layer through the generic plane kernels."""
-    K.set_env(monkeypatch, {})
+    set_env(monkeypatch, {})
     cfg = model_config([preset], {})
     sep, t_in = step_vs_oracle(cfg, B, 4245, per_example=False)
     eng = sep.engine(input_frames=t_in)
@@ -296,35 +270,28 @@ def test_unrun_presets_match_the_oracle(preset, B, monkeypatch):
 def test_predict_track_at_two_forward_batch_sizes_matches_the_oracle(monkeypatch):
     """Evaluate.predict_track with full_44KHz on a stereo track of 18 windows, 16 windows per forward: one handle runs a batch of
     16 and a batch of 2, against the oracle's window-by-window loop."""
-    import test_gpu_parity as P
     import Evaluate
-    K.set_env(monkeypatch, {})
+    set_env(monkeypatch, {})
     cfg = model_config(["full_44KHz"], {})
-    t_in, t_out, params, _, _ = P.random_problem(cfg, 1, cfg["num_frames"], 4246)
+    t_in, t_out, params, _, _ = random_problem(cfg, 1, cfg["num_frames"], 4246)
     n = 17 * t_out + t_out // 3
     assert len(Evaluate.window_starts(n, t_out)) == 18
     audio = (np.random.default_rng(4247).uniform(-1.0, 1.0, size=(n, 2)) * 0.5).astype(np.float32)
-    sep = P.make_sep(cfg, params, t_in)
+    sep = make_sep(cfg, params, t_in)
     got = Evaluate.predict_track(cfg, sep, audio, batch_windows=16)
     want = O.predict_track(cfg, params, audio, t_in, t_out)
     for s in cfg["source_names"]:
         assert got[s].shape == want[s].shape
-        assert P.rel_l2(got[s], want[s]) <= P.OUT_TOL and P.rel_max(got[s], want[s]) <= P.OUT_TOL, (s, P.rel_l2(got[s], want[s]))
+        assert rel_l2(got[s], want[s]) <= OUT_TOL and rel_max(got[s], want[s]) <= OUT_TOL, (s, rel_l2(got[s], want[s]))
 
 
 # ------------------------------------------------------------------------------------------------
 # C / D: two training steps with Adam and inference on the device (the problem of tests/hostsim/run_cpu_step.py)
 # ------------------------------------------------------------------------------------------------
-def _rel(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30))
-
-
 def device_steps(cfg, batch, nf, grad_scale=1.0):
     """Two training steps with TF-form Adam and the inference calls on the GPU, each against the oracle at the parameters the
     engine holds, in the result form of tests/hostsim/run_cpu_step.py; plus "grads1" (the first step's flat gradient) and
     "repro1" (the first step run twice from the same state gives the same bits)."""
-    torch = _torch()
     from Models.UnetAudioSeparator import UnetAudioSeparator
     t_in, t_out = O.get_padding(cfg, nf)
     params = O.init_params(cfg, seed=11)
@@ -357,7 +324,7 @@ def device_steps(cfg, batch, nf, grad_scale=1.0):
         l64 = O.mse_loss(cfg, outs64, {k: torch.as_tensor(v).to(torch.float64) for k, v in targets.items()})
         grads_o = {k: gg.numpy() for k, gg in zip(tp, torch.autograd.grad(l64, list(tp.values())))}
         got = {n: v.cpu().numpy().copy() / np.float32(grad_scale) for n, v in sep.gradients().items()}
-        per = {n: _rel(got[n], grads_o[n]) for n in got}
+        per = {n: rel_l2(got[n], grads_o[n]) for n in got}
         which = max(per, key=per.get)
         explained = None
         if per[which] >= GPU_BARS["grad_tol"]:
@@ -365,19 +332,19 @@ def device_steps(cfg, batch, nf, grad_scale=1.0):
             explained = {"flips": None if flips is None else len(flips), "worst_after": float(w_after)}
         o = out.cpu().numpy()
         res["step%d" % step] = {"loss_rel": abs(loss - loss_o) / abs(loss_o), "grad_worst_rel": per[which], "grad_worst_tensor": which,
-                                "grad_explained": explained, "outputs_rel": max(_rel(o[k], outs_o[s]) for k, s in enumerate(names))}
+                                "grad_explained": explained, "outputs_rel": max(rel_l2(o[k], outs_o[s]) for k, s in enumerate(names))}
         p_prev, g_now = sep.params.cpu().numpy().copy(), sep.grads.cpu().numpy().copy()
         m_prev, v_prev = sep.adam_m.cpu().numpy().copy(), sep.adam_v.cpu().numpy().copy()
         sep.adam_step(1e-3)
         p_want, m_want, v_want = O.adam_update(p_prev, g_now, m_prev, v_prev, step, 1e-3)
-        res["step%d" % step]["params_rel"] = _rel(sep.params.cpu().numpy(), p_want)
-        res["step%d" % step]["adam_slots_rel"] = max(_rel(sep.adam_m.cpu().numpy(), m_want), _rel(sep.adam_v.cpu().numpy(), v_want))
+        res["step%d" % step]["params_rel"] = rel_l2(sep.params.cpu().numpy(), p_want)
+        res["step%d" % step]["adam_slots_rel"] = max(rel_l2(sep.adam_m.cpu().numpy(), m_want), rel_l2(sep.adam_v.cpu().numpy(), v_want))
     res["adam_state"] = [float(x) for x in sep._adam_state.cpu()]
     o_par = OrderedDict((n, v.cpu().numpy().copy()) for n, v in sep.variables().items())
     for training, key in ((False, "infer_outputs_rel"), (True, "train_mode_outputs_rel")):
         got_o = sep.get_output(mix_d, training, False, reuse=True)
         want = O.forward_np(cfg, o_par, mix, training)
-        res[key] = max(_rel(got_o[s].cpu().numpy(), want[s]) for s in names)
+        res[key] = max(rel_l2(got_o[s].cpu().numpy(), want[s]) for s in names)
     # the window gather / scatter of predict_track (the last window shifted back, plain overwrite)
     eng = sep.engine(input_frames=t_in)
     n_frames = 3 * t_out - 7
@@ -423,7 +390,7 @@ def feasibility(cfg, nf):
 def test_random_configuration_on_the_device(label, named, ov, batch, nf, env, grad_scale, monkeypatch):
     """The seeded sweep of tests/test_cpu_device.py (the same 16 draws) on the GPU: two training steps with Adam and inference
     against the oracle, and every launch of the draw replayed against float64."""
-    K.set_env(monkeypatch, {})
+    set_env(monkeypatch, {})
     cfg = model_config(named, ov)
     outcome = feasibility(cfg, nf)
     if outcome is not None:
@@ -458,15 +425,15 @@ def test_every_switch_position_gives_the_same_step_on_the_device(net, sw, monkey
     and reproducible bit for bit wherever the path is free of float atomics."""
     _, named, ov, batch, nf, env = next(n for n in _switch_nets() if n[0] == net)
     if net not in _DEFAULT:
-        K.set_env(monkeypatch, env)
+        set_env(monkeypatch, env)
         _DEFAULT[net] = device_steps(model_config(named, ov), batch, nf)
         assert_steps_match_oracle(_DEFAULT[net], **GPU_BARS)
         assert _DEFAULT[net]["repro1"], "two identical steps of the default path differ"
-    K.set_env(monkeypatch, dict(env, **sw))
+    set_env(monkeypatch, dict(env, **sw))
     res = device_steps(model_config(named, ov), batch, nf)
     assert_steps_match_oracle(res, **GPU_BARS)
     g, g0 = res["grads1"], _DEFAULT[net]["grads1"]
-    assert _rel(g, g0) <= 1e-4, _rel(g, g0)
+    assert rel_l2(g, g0) <= 1e-4, rel_l2(g, g0)
     if sw in SAME_KERNELS:
         assert np.array_equal(g.view(np.uint32), g0.view(np.uint32))
     if sw not in ATOMIC:

@@ -19,6 +19,8 @@ import sys
 
 import pytest
 
+from configurations import FORCED, SWITCHES, assert_steps_match_oracle, random_model_configs
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "hostsim"))
 import schedule  # noqa: E402
@@ -44,9 +46,6 @@ def _need_simulation(_build_once):
         pytest.skip("host simulation of the engine not built (needs nvcc and g++)")
 
 
-FORCED = {"WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}
-
-
 def run_steps(named, overrides, batch, nf, env=None, grad_scale=1.0):
     e = dict(os.environ)
     for k in [k for k in e if k.startswith("WUN_")]:
@@ -64,22 +63,6 @@ def assert_matches_oracle(res):
     assert res["unknown"] == []
     assert res["footprint_miss"] == [], res["footprint_miss"][:3]     # (only populated under HOSTSIM_POISON=1, see below)
     assert_steps_match_oracle(res)
-
-
-def assert_steps_match_oracle(res, loss_tol=1e-5, grad_tol=1e-4, out_tol=1e-5):
-    """The bars of two training steps with Adam and the inference calls.  tests/test_configurations_gpu.py holds the GPU to the
-    same checks with the wider loss / gradient / output bars of the fp32 tensor-core arithmetic."""
-    for step in ("step1", "step2"):
-        r = res[step]
-        assert r["loss_rel"] < loss_tol, (step, r)
-        ex = r.get("grad_explained")           # None, or the LeakyReLU-slope-flip proof for a gradient that is off (run_cpu_step.py)
-        assert r["grad_worst_rel"] < grad_tol or (ex and ex["flips"] is not None and ex["worst_after"] < grad_tol), (step, r)
-        assert r["outputs_rel"] < out_tol, (step, r)
-        assert r["params_rel"] < 1e-5 and r["adam_slots_rel"] < 1e-4, (step, r)
-    assert res["infer_outputs_rel"] < 1e-4, res["infer_outputs_rel"]
-    assert res["train_mode_outputs_rel"] < 1e-4, res["train_mode_outputs_rel"]
-    assert res["gather_exact"] and res["scatter_exact"]          # predict_track's window tiling (Evaluate.py:125-139)
-    assert abs(res["adam_state"][0] - 0.9 ** 3) < 1e-6 and abs(res["adam_state"][1] - 0.999 ** 3) < 1e-6 and res["adam_state"][2] == 2.0
 
 
 FAMILIES = [
@@ -118,19 +101,6 @@ def test_two_training_steps_and_inference_on_the_cpu_device_match_the_oracle(var
             assert "output_fwd_kernel" in ks, sorted(ks)
         except AssertionError as ex:
             raise AssertionError("%s: %s" % (name, ex))
-
-
-SWITCHES = [
-    {"WUN_OUT_FUSE": "2"},                       # output-layer switch in its other positions (the output layer runs in its own
-    {"WUN_OUT_FUSE": "0"},                       #   kernels either way: the step must not change)
-    {"WUN_BULK_WGRAD": "0"},                     # converter-fed tensor-core wgrad, bias sums by colsum_kernel
-    {"WUN_SPLIT_COLSUM": "0"},
-    {"WUN_FIRST_LAYER": "0"},                    # first layer through the generic plane kernels
-    {"WUN_DISABLE_UMMA": "1"},                   # the exact-fp32 CUDA-core path for everything
-    {"WUN_UMMA_DGRAD": "0"},
-    {"WUN_PAIR_FWD": "0", "WUN_PAIR_DGRAD": "0"},
-    {"WUN_SIDE_STREAM": "0"},
-]
 
 
 def test_every_structural_switch_gives_the_same_step():
@@ -207,27 +177,6 @@ def test_predict_track_pipeline_through_the_c_abi_matches_the_oracle():
                     ("same_mono_learned", ["baseline"], dict(num_layers=3, upsampling="learned"), 1, 256, dict(HOSTSIM_PREDICT="1"), 1.0)])
     for label, r in res.items():
         assert r["predict_windows"] == 3 and r["predict_rel"] < 1e-4, (label, r["predict_rel"])
-
-
-def random_model_configs(n, seed):
-    """n reproducible draws from the space of shapes the reference allows (Config.py:9-39 keys the separator reads)."""
-    import numpy as np
-    rng = np.random.default_rng(seed)
-    out = []
-    for i in range(n):
-        L = int(rng.integers(1, 5))
-        context = bool(rng.integers(0, 2))
-        # (even filter widths only with 'same' padding: with context they make T_in - T_out odd, which the reference's callers
-        #  assert against - Test.py:25)
-        fs = int(rng.choice([3, 5, 7, 9, 15] if context else [3, 5, 7, 9, 15, 4, 6]))
-        ov = dict(num_layers=L, num_initial_filters=int(rng.choice([4, 8, 12, 16, 24, 40])), filter_size=fs, input_filter_size=fs,
-                  merge_filter_size=int(rng.choice([1, 3, 5] if context else [1, 3, 5, 2])), output_filter_size=int(rng.choice([1, 1, 1, 3])), context=context,
-                  upsampling=str(rng.choice(["linear", "learned"])), output_type=str(rng.choice(["direct", "difference"])),
-                  output_activation=str(rng.choice(["tanh", "linear"])), mono_downmix=bool(rng.integers(0, 2)),
-                  task=str(rng.choice(["voice", "multi_instrument"])))
-        nf = int(rng.integers(40, 200)) if context else int((2 ** L) * rng.integers(4, 24))
-        out.append(("draw%02d" % i, ["baseline"], ov, int(rng.integers(1, 4)), nf, None, 1.0))
-    return out
 
 
 def test_random_model_configurations_on_the_cpu_device():

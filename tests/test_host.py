@@ -11,6 +11,7 @@ import pytest
 import Config
 import wun
 from Models.UnetAudioSeparator import UnetAudioSeparator
+from configurations import plan_audit
 from oracle import wave_unet_oracle as O
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -157,18 +158,11 @@ SMEM_LIMIT = 200 * 1024      # cudaFuncSetAttribute value of the conv and wgrad 
 SMEM_PER_SM = 228 * 1024     # H100: shared memory of one SM (1 KB of it reserved per resident CTA)
 
 
-def _audit(preset, batch, overrides=None):
-    from Models.UnetAudioSeparator import UnetAudioSeparator
-    mc = Config.build_config([preset], overrides or {}, experiment_id=0)["model_config"]
-    sep = UnetAudioSeparator(mc)
-    return sep.engine(num_frames=mc["num_frames"]).plan_audit(batch)
-
-
 @pytest.mark.parametrize("preset", ["baseline", "baseline_context", "baseline_stereo", "full", "full_multi_instrument", "full_44KHz"])
 @pytest.mark.parametrize("batch", [1, 2, 4, 8, 16, 32])
 def test_planned_tcgen05_launches_respect_hardware_limits(preset, batch):
     """Every tensor-core (wgmma) launch the planner would issue, against the H100 limits."""
-    lines = _audit(preset, batch)
+    lines = plan_audit(preset, batch)
     convs = [d for d in lines if d["op"] == "conv"]
     wgs = [d for d in lines if d["op"] == "wgrad"]
     assert convs and wgs
@@ -196,7 +190,7 @@ def test_planned_tcgen05_launches_respect_hardware_limits(preset, batch):
 def test_plan_audit_matches_the_measured_configuration():
     """The tiling of the benchmark (M4, batch 16): every conv but the first layer's on the tensor cores, the wide layers split
     over output channels, one wgrad launch per layer."""
-    lines = _audit("baseline_stereo", 16)
+    lines = plan_audit("baseline_stereo", 16)
     fwd = {d["layer"]: d for d in lines if d["op"] == "conv" and d["pass"] == 0}
     assert all(d["kernel"] == "wgmma" for d in fwd.values())
     assert fwd[3]["NPAD"] == 96 and fwd[3]["nsplit"] == 1
@@ -210,13 +204,13 @@ def test_round2_planner_decisions_for_the_benchmark():
     """What bench.py times at M4 batch 16 (DESIGN.md 2 / 4.1): pair-merged forward classes for the up blocks that still fill the GPU,
     the pair-merged dgrad only where the merged width stays narrow (down1) - and no forward merge at batch 1, where those
     launches do not fill the GPU."""
-    lines = [d for d in _audit("baseline_stereo", 16) if d["op"] == "conv"]
+    lines = [d for d in plan_audit("baseline_stereo", 16) if d["op"] == "conv"]
     fwd = {d["layer"]: d for d in lines if d["pass"] == 0}
     dg = [d for d in lines if d["pass"] == 1]
     assert sorted(l for l, d in fwd.items() if d["pair"]) == [20, 21, 22, 23, 24]        # up7 .. up11
     assert all(fwd[l]["N"] == 2 * fwd[l]["pair"] for l in (20, 21, 22, 23, 24))
     assert [(d["layer"], d["N"]) for d in dg if d["pair"]] == [(1, 48)]                    # down1: 2 x 24 columns
-    small = [d for d in _audit("baseline_stereo", 1) if d["op"] == "conv"]
+    small = [d for d in plan_audit("baseline_stereo", 1) if d["op"] == "conv"]
     assert not any(d["pair"] and d["pass"] == 0 for d in small)
 
 

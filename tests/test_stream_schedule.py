@@ -17,10 +17,11 @@ import sys
 
 import pytest
 
+from configurations import FORCED, random_model_configs
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "hostsim"))
 import schedule  # noqa: E402
-
 
 
 _SIM, _WHY = None, "not built yet"
@@ -50,7 +51,6 @@ def test_the_simulation_library_builds_where_the_tool_chain_exists():
     assert _SIM is not None and os.path.exists(_SIM), _WHY
 
 
-FORCED = {"WUN_PAIR_MIN_CTAS": "1", "WUN_PAIR_DGRAD": "1"}      # as tests/test_gpu_parity.py
 FAMILIES = [
     ("m4_like_L5", ["baseline_stereo"], dict(num_layers=5), 3, 2000),
     ("m5_like_L4", ["full"], dict(num_layers=4, num_initial_filters=16), 2, 1500),
@@ -211,11 +211,10 @@ def test_the_limit_check_notices_an_oversized_launch():
 
 
 def test_random_model_configurations_are_race_free_and_within_the_launch_limits():
-    """A seeded sweep over the configuration space (the draws of tests/test_cpu_device.py: layer counts, filter widths, channel
+    """A seeded sweep over the configuration space (the draws of random_model_configs: layer counts, filter widths, channel
     counts that fall back to the CUDA-core kernels, both paddings / upsamplers / output types, batch 1-3) with the bucketed
     all-reduce: whatever mix of launches and streams the planner produces, no race, no out-of-bounds or uninitialised access,
     every stream joined, every launch within the hardware limits.  (One-off campaigns: 96 draws, none bad.)"""
-    from test_cpu_device import random_model_configs
     for i, (label, named, ov, batch, nf, _, _) in enumerate(random_model_configs(6, seed=77)):
         meta, ops = schedule.trace("train_dp", named, ov, batch, nf, FORCED if i % 2 else None)
         stats = assert_race_free(meta, ops)

@@ -8,14 +8,15 @@ counts included), a 144-channel M side of 3 blocks, and split and unsplit tiles 
 bulk-fed and the converter-fed forms (tests/test_kernels_gpu.py runs them the same way)."""
 import pytest
 
-from test_kernels_gpu import H, _gpu_lib, _lib_or_skip, p, run_wgrad_case, wgrad_layer
-from test_host import _audit
+from configurations import plan_audit
+from conv_launches import p, run_wgrad_case, wgrad_layer
+from launch_checks import H, gpu_lib, lib_or_skip
 
 OLD_ISSUED_GMAC = 223.9        # 128-channel M tiles, same swap / NT rules: the same audit at the parent's tiling
 
 
 def _wgrad_lines():
-    return [d for d in _audit("baseline_stereo", 16) if d["op"] == "wgrad"]
+    return [d for d in plan_audit("baseline_stereo", 16) if d["op"] == "wgrad"]
 
 
 def test_issued_macs_of_the_benchmark_step():
@@ -57,7 +58,7 @@ def tile_cases():
 
 
 def test_tile_cases_plan_the_variants_they_are_for():
-    _lib_or_skip()
+    lib_or_skip()
     plans = {W["name"]: H.plan_wgrad(H.wgrad_text(W["groups"])) for W in tile_cases()}
     for name, pw in plans.items():
         assert pw["eligible"] and pw["bulk"], name
@@ -74,6 +75,6 @@ def test_tile_cases_plan_the_variants_they_are_for():
 @pytest.mark.parametrize("regime", ["exact", "float"])
 @pytest.mark.parametrize("mode", [0, 1, 2], ids=["bulk_fused", "bulk_colsum", "converter"])
 def test_tile_variants_match_float64(mode, regime):
-    _gpu_lib()
+    gpu_lib()
     for k, W in enumerate(tile_cases()):
         run_wgrad_case(W, mode, regime, 3000 + k, 0.5 if k % 2 else 2.0)
