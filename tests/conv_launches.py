@@ -150,8 +150,24 @@ def plane_reads(P, B):
     return np.concatenate(idx)
 
 
-def data(rng, n, regime, kind="act"):
-    if regime == "exact":
+# The exact regimes with non-zero lo halves: one side of every product carries up to 12 significant bits (j / 2^10, |j| <= 2^12;
+# its bf16 lo half is mostly non-zero), the other is exact in bf16, so hi*hi + hi*lo + lo*hi is the product itself.  exact_lo_x:
+# activations / the wgrad's plane side carry the 12 bits, weights / the gradient side are integers in [-3, 3].  exact_lo_w: the
+# reverse, against activations / plane rows k/4 in [-1, 1].  The exact side is zero with probability 1 - rho, rho chosen per
+# case (lo_density) so that every sum stays within 2^23 units of the product grid.
+LO_REGIMES = ("exact_lo_x", "exact_lo_w")
+LO_BITS = 2.0 ** -10
+LO_MEAN = 2048.0                       # mean |j| of the 12-bit side, in units of LO_BITS
+SUM_UNITS = 2.0 ** 23                  # |partial sums| below 2^23 grid units: exact in fp32 in any order
+
+
+def data(rng, n, regime, kind="act", rho=1.0):
+    if regime in LO_REGIMES and kind != "blend":
+        if (kind == "act") == (regime == "exact_lo_x"):
+            return (rng.integers(-4096, 4097, n) * LO_BITS).astype(np.float32)
+        v = rng.integers(-3, 4, n) if kind == "w" else rng.integers(-4, 5, n) / 4.0
+        return (v * (rng.random(n) < rho)).astype(np.float32)
+    if regime.startswith("exact"):
         if kind == "w":
             return rng.integers(-3, 4, n).astype(np.float32)
         if kind == "blend":
@@ -162,24 +178,61 @@ def data(rng, n, regime, kind="act"):
     return (rng.standard_normal(n) * 2.0 ** rng.uniform(-6, 6, n)).astype(np.float32)
 
 
+def lo_unit(regime, planes):
+    """The grid of the products of a lo regime: the plane side's grid refined by MID blends (weights in quarters) or midpoints."""
+    refine = max([4 if P["kind"] == 1 and P["blend"] >= 0 else 2 if P["kind"] == 1 else 1 for P in planes])
+    return (LO_BITS if regime == "exact_lo_x" else 0.25 * LO_BITS) / refine, refine
+
+
+def lo_density(regime, planes, nterms):
+    """rho of the exact side: nterms products of mean LO_MEAN x (mean exact-side units) stay near SUM_UNITS / 2."""
+    mean = 12.0 / 7.0 if regime == "exact_lo_x" else 20.0 / 9.0
+    return min(1.0, SUM_UNITS / 2 / (nterms * LO_MEAN * mean * lo_unit(regime, planes)[1]))
+
+
+def lo_fraction(x):
+    """The fraction of x whose bf16 lo half is non-zero: split_hi_lo's hi = round to nearest even of the top 16 bits."""
+    b = np.ascontiguousarray(x, np.float32).view(np.uint32).astype(np.uint64)
+    hi = ((b + 0x7FFF + ((b >> 16) & 1)) & 0xFFFF0000).astype(np.uint32).view(np.float32)
+    return float(np.mean(x.astype(np.float32) - hi != 0))
+
+
+def assert_lo_regime(name, regime, side, ref_abs, unit):
+    """The lo regime is not vacuous (most of the 12-bit side has lo != 0) and its sums are exact in any order."""
+    frac = lo_fraction(side)
+    assert frac > 0.5, "%s (%s): only %.2f of the 12-bit side has a non-zero lo half" % (name, regime, frac)
+    worst = float(np.max(ref_abs)) / unit
+    assert worst < SUM_UNITS, "%s (%s): sum |terms| reaches %.3g grid units - shrink the case" % (name, regime, worst)
+
+
 def fill_conv(D, rng, regime):
     S, L, B = D["synth"], D["launch"], D["launch"]["batch"]
     ws = np.full(S.n["ws"] + GUARD, np.nan, np.float32)
     par = np.full(S.n["par"] + GUARD, np.nan, np.float32)
+    rho = 1.0
+    if regime in LO_REGIMES:                             # products per output: the channels of every term of a class
+        nterms = max(sum(D["planes"][t["plane"]]["C"] for t in D["terms"][q["term_begin"]:q["term_end"]]) for q in D["cls"])
+        rho = lo_density(regime, D["planes"], nterms)
+    side = []                                            # the 12-bit side of a lo regime
     for P in D["planes"]:
         idx = plane_reads(P, B)
-        ws[idx] = data(rng, idx.size, regime)
+        ws[idx] = data(rng, idx.size, regime, rho=rho)
+        side.append(ws[idx])
         if P["blend"] >= 0:
             b0 = (P["blend"] - WS_BASE) // 4
             ws[b0:b0 + P["C"]] = data(rng, P["C"], regime, "blend")
     W0 = (L["W"] - PAR_BASE) // 4
     Nh = L["pairC"] or L["N"]
+    wside = []
     for t in D["terms"]:
         C = D["planes"][t["plane"]]["C"]
         for wo in (t["woff"], t["woff2"] if L["pairC"] else -1):
             if wo >= 0:
                 idx = (W0 + wo + np.arange(C)[:, None] * L["w_sk"] + np.arange(Nh)[None, :] * L["w_sn"]).reshape(-1)
-                par[idx] = data(rng, idx.size, regime, "w")
+                par[idx] = data(rng, idx.size, regime, "w", rho)
+                wside.append(par[idx])
+    if regime == "exact_lo_w":
+        side = wside
     if L["bias"] >= 0:
         b0 = (L["bias"] - PAR_BASE) // 4
         par[b0:b0 + Nh] = data(rng, Nh, regime)
@@ -191,7 +244,7 @@ def fill_conv(D, rng, regime):
         s = data(rng, saved.size, regime)
         s[rng.random(saved.size) < 0.1] = 0.0            # slope 0.2 at exactly 0 (MaximumGrad)
         ws[saved] = s
-    return {"ws": ws, "par": par, "mix": np.zeros(64, np.float32)}
+    return {"ws": ws, "par": par, "mix": np.zeros(64, np.float32)}, np.concatenate(side)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -236,24 +289,41 @@ def wgrad_outputs(groups):
     return np.unique(np.concatenate(idx))
 
 
+def wgrad_rows(W):
+    """The longest reduction of a wgrad case: batch x the rows of all its classes (a dW element receives <= 2 class sums)."""
+    ranges = {(G["wgrad"]["m_lo"], G["wgrad"]["m_hi"]) for G in W["groups"]}
+    return W["batch"] * sum(hi - lo for lo, hi in ranges)
+
+
+def lo_fits(W):
+    """Whether a wgrad case can take the lo regimes: the bias sums of 12-bit gradient rows stay within SUM_UNITS / 2."""
+    return wgrad_rows(W) * LO_MEAN <= SUM_UNITS / 2
+
+
 def fill_wgrad(W, rng, regime):
+    """-> (memory, pre-filled gradient buffer, the 12-bit side of a lo regime).  The lo regimes put the plane side in place of
+    the activations and the gradient side in place of the weights."""
     S, B = W["synth"], W["batch"]
     ws = np.full(S.n["ws"] + GUARD, np.nan, np.float32)
+    rho = lo_density(regime, [G["plane"] for G in W["groups"]], wgrad_rows(W)) if regime in LO_REGIMES else 1.0
     seen = set()
+    side = []
     for G in W["groups"]:
-        for P in (G["plane"], G["dpre"]):
+        for P, kind in ((G["plane"], "act"), (G["dpre"], "w" if regime in LO_REGIMES else "act")):
             if P["base"] in seen:
                 continue
             seen.add(P["base"])
             idx = plane_reads(P, B)
-            ws[idx] = data(rng, idx.size, regime)
+            ws[idx] = data(rng, idx.size, regime, kind, rho)
+            if (kind == "act") == (regime == "exact_lo_x"):
+                side.append(ws[idx])
             if P["blend"] >= 0:
                 b0 = (P["blend"] - WS_BASE) // 4
                 ws[b0:b0 + P["C"]] = data(rng, P["C"], regime, "blend")
     grads = np.full(W["grads_n"], SENTINEL, np.float32)
     out = wgrad_outputs(W["groups"])
-    grads[out] = data(rng, out.size, "exact") if regime == "exact" else 0.0
-    return {"ws": ws, "par": np.zeros(64, np.float32), "mix": np.zeros(64, np.float32)}, grads
+    grads[out] = data(rng, out.size, "exact") if regime.startswith("exact") else 0.0
+    return {"ws": ws, "par": np.zeros(64, np.float32), "mix": np.zeros(64, np.float32)}, grads, np.concatenate(side or [np.zeros(0)])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -270,8 +340,10 @@ def _arena(nbytes):
 def run_conv_case(D, kernel, regime, seed):
     """Runs one conv description on the GPU and checks every output element and the bits of everything else."""
     family = ("simt " if kernel else "wgmma ") + ("dgrad" if D["launch"]["pass"] else "fwd")
+    if regime in LO_REGIMES:
+        family += " " + regime
     rng = np.random.default_rng(seed)
-    mem = fill_conv(D, rng, regime)
+    mem, side = fill_conv(D, rng, regime)
     text = H.conv_text(D)
     plan = H.plan_conv(text)
     ws_d, par_d, mix_d = _dev(mem["ws"]), _dev(mem["par"]), _dev(mem["mix"])
@@ -285,7 +357,11 @@ def run_conv_case(D, kernel, regime, seed):
     assert np.array_equal(got.view(np.uint32)[keep], mem["ws"].view(np.uint32)[keep]), \
         "%s: %d elements outside the output views changed" % (D["name"], int((got.view(np.uint32)[keep] != mem["ws"].view(np.uint32)[keep]).sum()))
     m64 = {k: v.astype(np.float64) for k, v in mem.items()}
-    if regime == "exact":
+    if regime in LO_REGIMES:
+        mabs = {k: v.astype(np.float64) for k, v in mem.items()}
+        run_launch(mabs, D, "abs")
+        assert_lo_regime(D["name"], regime, side, mabs["ws"][out], lo_unit(regime, D["planes"])[0])
+    if regime.startswith("exact"):
         fma = np.zeros(got.size, bool)
         run_launch(m64, D, "f32", fma)
         g, r = got[out], m64["ws"][out].astype(np.float32)
@@ -330,8 +406,10 @@ def conv_power_check(D, mem, ref_abs):
 
 def run_wgrad_case(W, mode, regime, seed, scale):
     family = ["wgrad bulk+fused colsum", "wgrad bulk+colsum", "wgrad converter-fed", "wgrad simt"][mode]
+    if regime in LO_REGIMES:
+        family += " " + regime
     rng = np.random.default_rng(seed)
-    mem, grads = fill_wgrad(W, rng, regime)
+    mem, grads, side = fill_wgrad(W, rng, regime)
     text = H.wgrad_text(W["groups"])
     plan = H.plan_wgrad(text)
     ws_d = _dev(mem["ws"])
@@ -359,7 +437,17 @@ def run_wgrad_case(W, mode, regime, seed, scale):
     m64 = {k: v.astype(np.float64) for k, v in mem.items()}
     ref = grads.astype(np.float64)
     run_wgrad_layer(m64, W["groups"], ref, "f64", scale)
-    if regime == "exact":
+    if regime in LO_REGIMES:
+        rabs = np.zeros_like(ref)
+        run_wgrad_layer(m64, W["groups"], rabs, "abs", scale)
+        unit, _ = lo_unit(regime, [G["plane"] for G in W["groups"]])
+        db = np.zeros(rabs.size, bool)
+        for G in W["groups"]:
+            db[G["wgrad"]["db"] + np.arange(G["wgrad"]["N"])] = True
+        # dW: products of the plane and gradient grids; db: sums of the gradient side alone (LO_BITS or integers)
+        units = np.where(db, rabs / (abs(scale) * (LO_BITS if regime == "exact_lo_w" else 1.0)), rabs / (abs(scale) * unit))
+        assert_lo_regime(W["name"], regime, side, units[out], 1.0)
+    if regime.startswith("exact"):
         g, r = got[out], ref[out]
         ok = g.astype(np.float64) == r
         assert ok.all(), "%s (%s): %d of %d gradient elements differ; first: got %r want %r" % (

@@ -209,6 +209,41 @@ int wkh_plan_conv(const char* desc, long long* out) {
     } catch (const std::string& e) { g_err = e; return -1; } catch (const std::exception& e) { g_err = e.what(); return -1; }
 }
 
+// The K-loop steps the tensor-core conv walks (kernels_umma.h next_step) for every (class, row tile) of a launch, from the
+// product's planner and umma_build (on a fake pack arena: only block indices are used).  out: TB, nbs, ncls; per class:
+// ngroups, ntiles; per tile: nsteps, then (g, c, t0, nt, blk) per step.  Returns the number of values written, or -1 (malformed,
+// not eligible, or more than cap values).
+int wkh_conv_steps(const char* desc, long long* out, long long cap) {
+    try {
+        ConvLaunch L;
+        if (!conv_from(desc, kFake, &L)) { g_err = "malformed conv description"; return -1; }
+        UmmaChoice ch;
+        if (!umma_plan_from_conv(L, &ch)) { g_err = "launch not eligible for the tensor-core conv"; return -1; }
+        UmmaLaunch U;
+        UmmaPackLaunch PL;
+        if (umma_build(L, ch, reinterpret_cast<uint8_t*>((uintptr_t)256), &U, &PL) != cudaSuccess) { g_err = "umma_build failed"; return -1; }
+        std::vector<long long> v = {U.TB, U.nbs, U.ncls};
+        for (int q = 0; q < U.ncls; ++q) {
+            const UmmaClass& K = U.cls[q];
+            const int ntiles = std::max(0, (K.out.m_hi - K.out.m_lo + 127) / 128);
+            v.push_back(K.ngroups);
+            v.push_back(ntiles);
+            for (int x = 0; x < ntiles; ++x) {
+                const size_t at = v.size();
+                v.push_back(0);
+                ConvStep s = {-1, 0, 0, 0, 0};
+                while (next_step(U, K, K.out.m_lo + 128 * x, s)) {
+                    v.insert(v.end(), {s.g, s.c, s.t0, s.nt, s.blk});
+                    ++v[at];
+                }
+            }
+        }
+        if ((long long)v.size() > cap) { g_err = "output too small"; return -1; }
+        std::copy(v.begin(), v.end(), out);
+        return (int)v.size();
+    } catch (const std::string& e) { g_err = e; return -1; } catch (const std::exception& e) { g_err = e.what(); return -1; }
+}
+
 // out[0..10): eligible, bulk split fits (umma_plan_wgrad_split > 0), split bytes, partial bytes, ngroups, grid x/y/z, nstages,
 // arena bytes wkh_run_wgrad needs for the bulk modes; then per group 10 values: swap, NT, n_mtiles, n_ntiles, taps_per_cta,
 // n_tapsets, chunks_per_batch, chunks_per_cta, n_ctas_x, slot0.

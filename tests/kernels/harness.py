@@ -70,7 +70,8 @@ def _bind(lib):
     lib.wkh_plan_wgrad.argtypes = [S, ctypes.POINTER(I64), ctypes.c_int]
     lib.wkh_run_conv.argtypes = [S, P, P, P, ctypes.c_int, P, I64, P]
     lib.wkh_run_wgrad.argtypes = [S, P, P, P, P, ctypes.c_float, ctypes.c_int, P, I64, P]
-    for f in (lib.wkh_plan_conv, lib.wkh_plan_wgrad, lib.wkh_run_conv, lib.wkh_run_wgrad):
+    lib.wkh_conv_steps.argtypes = [S, ctypes.POINTER(I64), I64]
+    for f in (lib.wkh_plan_conv, lib.wkh_plan_wgrad, lib.wkh_run_conv, lib.wkh_run_wgrad, lib.wkh_conv_steps):
         f.restype = ctypes.c_int
     G, F, I = ctypes.POINTER(I64), ctypes.c_float, ctypes.c_int
     sig = {
@@ -170,6 +171,28 @@ def plan_conv(text):
     out = (ctypes.c_longlong * 8)()
     _check(load().wkh_plan_conv(text.encode(), out), "wkh_plan_conv")
     return dict(zip(["eligible", "NPAD", "nsplit", "MT", "rows_alloc", "TB", "nbs", "pack_bytes"], list(out)))
+
+
+def conv_steps(text):
+    """-> dict(TB, nbs, cls=[dict(ngroups, tiles=[[(g, c, t0, nt, blk) per K step] per row tile])]): the steps the tensor-core
+    conv walks, from the product's own next_step (host only)."""
+    cap = 1 << 20
+    out = (ctypes.c_longlong * cap)()
+    n = load().wkh_conv_steps(text.encode(), out, cap)
+    _check(0 if n >= 0 else -1, "wkh_conv_steps")
+    v = list(out[:n])
+    r = dict(TB=v[0], nbs=v[1], cls=[])
+    i = 3
+    for _ in range(v[2]):
+        q = dict(ngroups=v[i], tiles=[])
+        ntiles = v[i + 1]
+        i += 2
+        for _ in range(ntiles):
+            k = v[i]
+            q["tiles"].append([tuple(v[i + 1 + 5 * j:i + 6 + 5 * j]) for j in range(k)])
+            i += 1 + 5 * k
+        r["cls"].append(q)
+    return r
 
 
 GROUP_KEYS = ["swap", "NT", "n_mtiles", "n_ntiles", "taps_per_cta", "n_tapsets", "chunks_per_batch", "chunks_per_cta", "n_ctas_x", "slot0"]

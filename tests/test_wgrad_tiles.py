@@ -72,7 +72,7 @@ def test_tile_cases_plan_the_variants_they_are_for():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("regime", ["exact", "float"])
+@pytest.mark.parametrize("regime", ["exact", "exact_lo_x", "exact_lo_w", "float"])
 @pytest.mark.parametrize("mode", [0, 1, 2], ids=["bulk_fused", "bulk_colsum", "converter"])
 def test_tile_variants_match_float64(mode, regime):
     gpu_lib()

@@ -229,15 +229,6 @@ __device__ __forceinline__ void load_row16(const PlaneView& P, int b, int r, int
     }
 }
 
-// A (plane, tile) pair whose slab would hold nothing but zero rows - the tile's rows plus the group's tap span lie
-// entirely outside the plane's valid rows - contributes nothing: the K loop skips the group and its packed weights.  This
-// is what the dgrad of a down block looks like outside the skip window: the gradient of the odd rows (g_odd) is zero there.
-__device__ __forceinline__ bool group_is_empty(const UmmaLaunch& L, const UmmaGroup& G, int m_base) {
-    const PlaneView& P = L.planes[G.plane];
-    const int lo = m_base + G.dmin;
-    return lo + L.rows_alloc <= P.r_lo || lo >= P.r_hi;
-}
-
 // ------------------------------------------------------------------------------------------------
 // conv epilogue: staged rows -> global memory
 // ------------------------------------------------------------------------------------------------
@@ -339,39 +330,6 @@ __device__ __forceinline__ void epi_write_rows_vec(const float* __restrict__ sta
 // ------------------------------------------------------------------------------------------------
 constexpr int kConvThreads = 256;      // two warpgroups: rows [0, 64) and [64, 128) of the tile
 constexpr int kBStagesMax = 6;         // weight ring: L.nbs stages of up to L.TB taps
-
-// One step of a CTA's K loop = one weight-ring stage: taps [t0, t0 + nt) (relative to the group) of 16-channel chunk c of
-// group g; blk = index of its first packed weight block (pack order: group, chunk, term).
-struct ConvStep {
-    int g, c, t0, nt, blk;
-};
-// Moves s to the next step (from g = -1: to the first one), skipping groups whose slab would be all zeros together with
-// their packed blocks.  false = the K loop is done.
-__device__ __forceinline__ bool next_step(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
-    if (s.g >= 0) {
-        const UmmaGroup& G = K.groups[s.g];
-        const int nterm = G.term_end - G.term_begin;
-        s.blk += s.nt;
-        s.t0 += s.nt;
-        if (s.t0 < nterm) { s.nt = min(L.TB, nterm - s.t0); return true; }
-        s.t0 = 0;
-        if (++s.c < ((L.planes[G.plane].C + 15) >> 4)) { s.nt = min(L.TB, nterm); return true; }
-    }
-    for (++s.g; s.g < K.ngroups; ++s.g) {
-        const UmmaGroup& G = K.groups[s.g];
-        const int nterm = G.term_end - G.term_begin;
-        if (!group_is_empty(L, G, m_base)) { s.c = 0; s.t0 = 0; s.nt = min(L.TB, nterm); return true; }
-        s.blk += ((L.planes[G.plane].C + 15) >> 4) * nterm;
-    }
-    return false;
-}
-
-// Moves s from any step of its (group, chunk) to the first step of the next non-empty (group, chunk).  false = none left.
-__device__ __forceinline__ bool next_chunk(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
-    const UmmaGroup& G = K.groups[s.g];
-    s.nt = (G.term_end - G.term_begin) - s.t0;      // as if this step ran to the chunk's last tap
-    return next_step(L, K, m_base, s);
-}
 
 // The slab of (group, chunk) holds plane rows m_base + dmin + [0, rows_alloc), 16 channels, as hi / lo atom planes.  Each thread
 // owns one slab row (rows_alloc <= 152 < kConvThreads; threads past the slab redo its last row: the same bits to the same

@@ -41,6 +41,54 @@ struct UmmaLaunch {
     int pairC;              // > 0: pair-merged classes (launch.h OutView::pairC); the bias repeats with this period
 };
 
+#ifndef __CUDACC__
+inline int min(int a, int b) { return a < b ? a : b; }      // host compilers lack CUDA's min(int, int)
+#endif
+
+// The conv kernel's K-loop walk, here so that host code (the kernel test harness) walks the very same steps.
+//
+// A (plane, tile) pair whose slab would hold nothing but zero rows - the tile's rows plus the group's tap span lie
+// entirely outside the plane's valid rows - contributes nothing: the K loop skips the group and its packed weights.  This
+// is what the dgrad of a down block looks like outside the skip window: the gradient of the odd rows (g_odd) is zero there.
+__host__ __device__ __forceinline__ bool group_is_empty(const UmmaLaunch& L, const UmmaGroup& G, int m_base) {
+    const PlaneView& P = L.planes[G.plane];
+    const int lo = m_base + G.dmin;
+    return lo + L.rows_alloc <= P.r_lo || lo >= P.r_hi;
+}
+
+// One step of a CTA's K loop = one weight-ring stage: taps [t0, t0 + nt) (relative to the group) of 16-channel chunk c of
+// group g; blk = index of its first packed weight block (pack order: group, chunk, term).
+struct ConvStep {
+    int g, c, t0, nt, blk;
+};
+// Moves s to the next step (from g = -1: to the first one), skipping groups whose slab would be all zeros together with
+// their packed blocks.  false = the K loop is done.
+__host__ __device__ __forceinline__ bool next_step(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
+    if (s.g >= 0) {
+        const UmmaGroup& G = K.groups[s.g];
+        const int nterm = G.term_end - G.term_begin;
+        s.blk += s.nt;
+        s.t0 += s.nt;
+        if (s.t0 < nterm) { s.nt = min(L.TB, nterm - s.t0); return true; }
+        s.t0 = 0;
+        if (++s.c < ((L.planes[G.plane].C + 15) >> 4)) { s.nt = min(L.TB, nterm); return true; }
+    }
+    for (++s.g; s.g < K.ngroups; ++s.g) {
+        const UmmaGroup& G = K.groups[s.g];
+        const int nterm = G.term_end - G.term_begin;
+        if (!group_is_empty(L, G, m_base)) { s.c = 0; s.t0 = 0; s.nt = min(L.TB, nterm); return true; }
+        s.blk += ((L.planes[G.plane].C + 15) >> 4) * nterm;
+    }
+    return false;
+}
+
+// Moves s from any step of its (group, chunk) to the first step of the next non-empty (group, chunk).  false = none left.
+__host__ __device__ __forceinline__ bool next_chunk(const UmmaLaunch& L, const UmmaClass& K, int m_base, ConvStep& s) {
+    const UmmaGroup& G = K.groups[s.g];
+    s.nt = (G.term_end - G.term_begin) - s.t0;      // as if this step ran to the chunk's last tap
+    return next_step(L, K, m_base, s);
+}
+
 constexpr int kUmmaMaxPackJobs = kMaxClasses * kUmmaMaxSplit;
 
 struct UmmaPackJob {        // one (class, split) weight pack
