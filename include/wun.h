@@ -236,6 +236,74 @@ int wun_snippet_batch(const float* pool, int64_t total_frames, int64_t num_sourc
 int wun_eval_batch_loss(const float* outputs, const float* targets, int64_t num_sources, int64_t n, double* state,
                         double* batch_loss, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* --- spectrogram U-Net, inference ------------------------------------------------------------------
+ * The Jansson et al. baselines of the reference's Models/UnetSpectrogramSeparator.py (presets unet_spectrogram / U7 and
+ * unet_spectrogram_l1 / U7a), the graph get_output(mix, training=False, return_spectrogram) builds:
+ *   STFT (frame 1024, hop 768, fft 1024, periodic Hann, no end padding): n = 1 + (T - 1024) / 768 frames of 513 bins;
+ *   per source, in source_names order, one U-Net on log1p(|X|) without the last bin, NHWC [B, n, 512, 1]:
+ *     L down layers: conv2d 5x5 stride 2 'same' (F * 2^i filters) + batch norm + LeakyReLU(0.2);
+ *     L - 1 up layers: conv2d_transpose 5x5 stride 2 'same' (F * 2^(L-i-2) filters) + batch norm + ReLU, then
+ *       concat([skip, up]) on channels;
+ *     mask: conv2d_transpose to 1 channel + sigmoid, bin 512 = 0.5;
+ *   magnitude output mask * |X| [K][B, n, 513], or audio output inverse_stft(mask * X) with
+ *   inverse_stft_window_fn(768, hann): [K][B, T, 1].
+ * Batch norm is the inference form (x - moving_mean) / sqrt(moving_variance + 1e-3) + beta (center, no scale).
+ * Parameters: one flat float32 buffer in TF creation order under "separator" - per source and layer conv2d_<i>/kernel
+ * [5, 5, C_in, C_out] (conv2d_transpose_<i>/kernel: [5, 5, C_out, C_in]), its bias, then BatchNorm_<j>/beta,
+ * moving_mean, moving_variance; the suffixes continue across the two U-Nets as TF's name uniquification does.
+ * Every reduction has a fixed order: a window's estimate has the same bits whatever batch holds it.  No allocation,
+ * synchronisation or copy inside wun_spec_forward / wun_spec_l1_batch_loss: both can be captured in a CUDA graph.
+ * Errors: WUN_E_SHAPE (the reference's AssertionError) for a stereo model, num_sources != 2, (T - 1024) % 768 != 0, or an
+ * n or a bin count (512) not divisible by 2^num_layers; WUN_E_INVALID for other bad arguments. */
+typedef struct WunSpecConfig {
+    int32_t num_layers;
+    int32_t num_initial_filters;
+    int32_t num_channels;     /* must be 1 (mono_downmix) */
+    int32_t num_sources;      /* must be 2 */
+} WunSpecConfig;
+
+typedef struct WunSpecParamInfo {
+    char     name[64];        /* e.g. "separator/conv2d_6/kernel", "separator/BatchNorm_11/moving_variance" */
+    int32_t  ndim;
+    int32_t  shape[4];
+    int64_t  offset;          /* element offset into the flat parameter buffer */
+    int64_t  numel;
+} WunSpecParamInfo;
+
+typedef struct WunSpecHandle WunSpecHandle;
+
+#define WUN_SPEC_BINS 513
+
+/* pure host (usable without a GPU) */
+int wun_spec_create(const WunSpecConfig* cfg, int64_t num_frames, WunSpecHandle** out);
+int wun_spec_destroy(WunSpecHandle* h);
+int64_t wun_spec_input_frames(const WunSpecHandle* h);      /* T (= num_frames) */
+int64_t wun_spec_output_frames(const WunSpecHandle* h);     /* T */
+int64_t wun_spec_stft_frames(const WunSpecHandle* h);       /* n */
+int64_t wun_spec_param_count(const WunSpecHandle* h);
+int64_t wun_spec_param_numel(const WunSpecHandle* h);
+int wun_spec_param_table(const WunSpecHandle* h, WunSpecParamInfo* out, int64_t capacity);
+/* scratch of wun_spec_forward and wun_spec_l1_batch_loss at `batch` (one workspace serves both) */
+int64_t wun_spec_workspace_bytes(const WunSpecHandle* h, int64_t batch);
+/* 2 FLOP per convolution MAC over all 25 taps (down: output positions, transposed: input positions) */
+double wun_spec_forward_flops(const WunSpecHandle* h, int64_t batch);
+int64_t wun_spec_launches_forward(const WunSpecHandle* h, int return_spectrogram);
+
+/* get_output(mix, training=False, return_spectrogram): mix [B, T, 1] -> outputs [K][B, T, 1], or with return_spectrogram
+ * [K][B, n, 513] magnitudes.  Workspace 256-byte aligned, at least wun_spec_workspace_bytes(h, batch). */
+int wun_spec_forward(WunSpecHandle* h, const float* params, const float* mix, int64_t batch, int return_spectrogram,
+                     float* outputs, void* workspace, int64_t workspace_bytes, void* stream);
+/* Test.test's U7a loss (Test.py:57-71): curr = sum_k mean|STFTmag(targets[k]) - est_mags[k]| / K over [B, n, 513] in float64,
+ * then the running mean of wun_eval_batch_loss on state = {total, n}.  est_mags [K][B, n, 513] (wun_spec_forward with
+ * return_spectrogram), targets [K][B, T, 1]; batch_loss optional.  Same fixed-order reduction as wun_eval_batch_loss. */
+int wun_spec_l1_batch_loss(WunSpecHandle* h, const float* est_mags, const float* targets, int64_t batch, double* state,
+                           double* batch_loss, void* workspace, int64_t workspace_bytes, void* stream);
+/* wun_gather_windows / wun_scatter_windows for this handle's window (T_in = T_out = T, one channel, K sources) */
+int wun_spec_gather_windows(WunSpecHandle* h, const float* padded, int64_t n_padded, const int64_t* starts,
+                            int64_t n_windows, float* mix_batch, void* stream);
+int wun_spec_scatter_windows(WunSpecHandle* h, const float* outputs, const int64_t* starts, int64_t n_windows,
+                             float* preds, int64_t n_frames, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

@@ -37,7 +37,8 @@ def window_starts(n_frames, t_out):
 
 def predict_track(model_config, separator, mix_audio, batch_windows=16, device="cuda"):
     """mix_audio: float array [n_frames, n_channels] at expected_sr.  `separator`: a
-    Models.UnetAudioSeparator.UnetAudioSeparator holding variables.  Returns OrderedDict name -> [n_frames, C]."""
+    Models.UnetAudioSeparator.UnetAudioSeparator or Models.UnetSpectrogramSeparator.UnetSpectrogramSeparator holding
+    variables.  Returns OrderedDict name -> [n_frames, C]."""
     import torch
     assert len(mix_audio.shape) == 2
     mix_audio = _model_channels(model_config, mix_audio)
@@ -127,9 +128,16 @@ def predict(model_config, separator, audio, rate, references=None, results_dir=N
 
 def load_separator(model_config, load_model):
     """A separator holding the variables of `load_model` (a TF-V2 checkpoint prefix - written by Training.train or by the
-    reference - or a round-1 .npz; reference restore: Evaluate.py:55-57); None leaves them uninitialised."""
-    from Models.UnetAudioSeparator import UnetAudioSeparator
-    separator = UnetAudioSeparator(model_config)
+    reference - or a round-1 .npz; reference restore: Evaluate.py:55-57); None leaves them uninitialised.  The class
+    follows model_config["network"] as in the reference (Evaluate.py:27-32): a UnetAudioSeparator for "unet", a
+    UnetSpectrogramSeparator (inference only) for "unet_spectrogram"."""
+    if model_config["network"] == "unet":
+        from Models.UnetAudioSeparator import UnetAudioSeparator as Separator
+    elif model_config["network"] == "unet_spectrogram":
+        from Models.UnetSpectrogramSeparator import UnetSpectrogramSeparator as Separator
+    else:
+        raise NotImplementedError
+    separator = Separator(model_config)
     in_shape, _ = separator.get_padding(np.array([1, model_config["num_frames"], 0]))
     if load_model is not None:
         import TFCheckpoint

@@ -5,7 +5,9 @@
 Snippets start every T_out frames (take_all_snippets, Datasets.py:21-25), the mix is the recorded mixture, the targets are
 centre-cropped, batches of model_config["batch_size"] cross track boundaries and the last incomplete batch is dropped.  Per
 batch, curr = sum_k mean((target_k - estimate_k)^2) / K with the forward in test mode (output clip on), and the result is
-the running mean total += (1 / n) * (curr - total) (Test.py:57-79).
+the running mean total += (1 / n) * (curr - total) (Test.py:57-79).  The spectrogram U-Net (network "unet_spectrogram") runs
+the same way; with raw_audio_loss=False (preset unet_spectrogram_l1, U7a) curr is sum_k mean|STFTmag(target_k) -
+estimate_k| / K over the magnitudes [B, n, 513] instead.
 
 On the device: one CUDA graph of wun_snippet_batch -> wun_forward -> wun_eval_batch_loss, replayed once per batch; the
 batch counter and the fp64 running mean live on the device, so the partition costs one host synchronisation, at the end,
@@ -15,15 +17,17 @@ import numpy as np
 
 
 def test(model_config, partition, model_folder, load_model, dataset=None, separator=None):
-    """Running-mean MSE over the full batches of `partition` ("valid" or "test") of `dataset` (a Datasets.Dataset; staged
+    """Running-mean MSE (or, for U7a, L1 of magnitudes) over the full batches of `partition` ("valid" or "test") of `dataset` (a Datasets.Dataset; staged
     from model_config["musdb_path"] when None), with `separator` or else the variables of checkpoint `load_model`.
     Raises ValueError when the partition has fewer snippets than one batch."""
     import torch
     import Datasets
     import Evaluate
     import wun
-    if model_config["network"] != "unet":
+    if model_config["network"] not in ("unet", "unet_spectrogram"):
         raise NotImplementedError
+    # the spectrogram U-Net's U7a preset scores magnitudes: mean |STFTmag(target) - estimate| (Test.py:63-67)
+    magnitude_loss = model_config["network"] == "unet_spectrogram" and not model_config["raw_audio_loss"]
     if separator is None:
         separator = Evaluate.load_separator(model_config, load_model)
     B = int(model_config["batch_size"])
@@ -44,14 +48,21 @@ def test(model_config, partition, model_folder, load_model, dataset=None, separa
     counter = torch.zeros(1, dtype=torch.int64, device=dev)
     mix = torch.empty((B, t_in, C), dtype=torch.float32, device=dev)
     targets = torch.empty((K, B, t_out, C), dtype=torch.float32, device=dev)
-    outputs = torch.empty_like(targets)
     state = torch.zeros(2, dtype=torch.float64, device=dev)
-    slots = torch.empty(K * wun.EVAL_LOSS_CTAS, dtype=torch.float64, device=dev)
+    if magnitude_loss:
+        outputs = torch.empty(eng.output_shape(B, return_spectrogram=True), dtype=torch.float32, device=dev)
+    else:
+        outputs = torch.empty_like(targets)
+        slots = torch.empty(K * wun.EVAL_LOSS_CTAS, dtype=torch.float64, device=dev)
 
     def batch():
         wun.snippet_batch(pool, positions, B, counter, mix, targets)
-        eng.forward(separator.params, mix, False, out=outputs)
-        wun.eval_batch_loss(outputs, targets, state, slots)
+        if magnitude_loss:
+            eng.forward(separator.params, mix, False, out=outputs, return_spectrogram=True)
+            eng.l1_batch_loss(outputs, targets, state)
+        else:
+            eng.forward(separator.params, mix, False, out=outputs)
+            wun.eval_batch_loss(outputs, targets, state, slots)
 
     with torch.cuda.device(dev):
         cur = torch.cuda.current_stream(dev)
@@ -68,5 +79,5 @@ def test(model_config, partition, model_folder, load_model, dataset=None, separa
                     graph.replay()
         cur.wait_stream(side)
         total = float(state[0].item())
-    print("Finished testing - Mean MSE: " + str(total))
+    print("Finished testing - Mean %s: %s" % ("L1" if magnitude_loss else "MSE", total))
     return total

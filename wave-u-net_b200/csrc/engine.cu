@@ -25,6 +25,8 @@ using namespace wun;
 
 static thread_local std::string g_err;
 static int set_err(int code, const std::string& m) { g_err = m; return code; }
+// the spectrogram engine (spec.cu) reports through the same wun_last_error()
+int wun::set_last_error(int code, const char* msg) { return set_err(code, msg); }
 
 #define WUN_CUDA_OK(expr)                                                                  \
     do {                                                                                   \

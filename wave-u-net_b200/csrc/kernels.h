@@ -8,6 +8,9 @@
 
 namespace wun {
 
+// Sets the message wun_last_error() returns and returns `code` (engine.cu).
+int set_last_error(int code, const char* msg);
+
 // Output layer (OutputLayer.py:5-23) + loss (Training.py:50-63) parameter block.
 struct OutputLaunch {
     const float* params;     // flat parameter buffer
@@ -101,5 +104,37 @@ cudaError_t launch_feed_batch(const float* pool, long long total_frames, const l
                               const long long* track_length, int n_tracks, int batch, int K, int C, int T_in, int T_out,
                               int augmentation, unsigned long long seed, long long* step_state, float* mix_out,
                               float* targets_out, long long* chosen, cudaStream_t stream);
+
+// kernels_eval.cu: Test.test's per-batch loss and running mean - curr = sum_k mean(d_k) / K with d = (target - output)^2, or
+// |target - output| with l1 - over slots of K * WUN_EVAL_LOSS_CTAS doubles (include/wun.h wun_eval_batch_loss)
+void launch_eval_loss(const float* outputs, const float* targets, int K, long long n, double* state, double* batch_loss,
+                      double* slots, bool l1, cudaStream_t stream);
+
+// kernels_spec.cu: the spectrogram U-Net's inference graph (frame 1024, hop 768, 513 bins)
+struct SpecStft {
+    const float* signal;     // [signals][T]
+    long long T;
+    int n_frames;            // 1 + (T - 1024) / 768
+    float* spec;             // [signals][n_frames][513] complex (float2), or null
+    float* logmag;           // [signals][n_frames][512]: log1p(|X|) without the last bin, or null
+    float* mag;              // [signals][n_frames][513]: |X|, or null
+};
+void launch_spec_stft(const SpecStft& P, int signals, cudaStream_t stream);
+
+// A 5x5 stride-2 layer over NHWC tensors whose channels sit at a pitch: x[b][h][w][x_pitch] (channels [0, Ci)),
+// y[b][h][w][y_pitch] (channels [y_off, y_off + Co)).  W is [5][5][Ci][Co] for the down conv, [5][5][Co][Ci] transposed.
+struct SpecConv {
+    const float* x; int Hi, Wi, Ci, x_pitch;
+    float* y; int Ho, Wo, Co, y_pitch, y_off;
+    const float* W; const float* bias;
+    const float* beta; const float* mean; const float* var;      // inference batch norm (unused by the mask)
+    int batch;
+};
+void launch_spec_down(const SpecConv& A, cudaStream_t stream);      // + bias, batch norm, LeakyReLU(0.2)
+void launch_spec_up(const SpecConv& A, cudaStream_t stream);        // transposed + bias, batch norm, ReLU
+// transposed to 1 channel + sigmoid, bin 512 = 0.5; out = mask * X (complex [B][n][513]) or mask * |X| with magnitude
+void launch_spec_mask(const SpecConv& A, const float* X, float* out, int magnitude, cudaStream_t stream);
+// irfft + inverse window per frame into frames [batch][n_frames][1024], then overlap-add into out [batch][T]
+void launch_spec_istft(const float* Y, int n_frames, int batch, float* frames, float* out, long long T, cudaStream_t stream);
 
 }  // namespace wun

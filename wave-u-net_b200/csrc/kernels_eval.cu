@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "../../include/wun.h"
+#include "kernels.h"
 
 namespace {
 
@@ -70,7 +71,9 @@ __device__ __forceinline__ double block_sum(double v, double* red) {
     return v;
 }
 
-// slots[k][cta] = sum over this CTA's elements of source k of (target - estimate)^2, each thread in a fixed grid stride.
+// slots[k][cta] = sum over this CTA's elements of source k of (target - estimate)^2, or |target - estimate| with kL1 (the
+// spectrogram U-Net's magnitude loss, Test.py:63-67), each thread in a fixed grid stride.
+template <bool kL1>
 __global__ void __launch_bounds__(kThreads) eval_loss_partials(const float* __restrict__ outputs,
                                                                const float* __restrict__ targets, long long n,
                                                                double* __restrict__ slots) {
@@ -81,7 +84,7 @@ __global__ void __launch_bounds__(kThreads) eval_loss_partials(const float* __re
     double acc = 0.0;
     for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)kLossCtas * kThreads) {
         const double d = __dsub_rn((double)__ldg(t + i), (double)__ldg(o + i));
-        acc = __dadd_rn(acc, __dmul_rn(d, d));
+        acc = __dadd_rn(acc, kL1 ? fabs(d) : __dmul_rn(d, d));
     }
     acc = block_sum(acc, red);
     if (threadIdx.x == 0) slots[(long long)k * kLossCtas + blockIdx.x] = acc;
@@ -149,9 +152,16 @@ extern "C" int wun_eval_batch_loss(const float* outputs, const float* targets, i
     if (workspace_bytes < num_sources * kLossCtas * (int64_t)sizeof(double) || (reinterpret_cast<uintptr_t>(workspace) & 7))
         return WUN_E_INVALID;
     if (!have_gpu()) return WUN_E_NOGPU;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    double* slots = static_cast<double*>(workspace);
-    eval_loss_partials<<<dim3(kLossCtas, (unsigned)num_sources), kThreads, 0, st>>>(outputs, targets, n, slots);
-    eval_loss_finish<<<1, kThreads, 0, st>>>(slots, (int)num_sources, n, state, batch_loss);
+    wun::launch_eval_loss(outputs, targets, (int)num_sources, n, state, batch_loss, static_cast<double*>(workspace), false,
+                          static_cast<cudaStream_t>(stream));
     return cudaGetLastError() == cudaSuccess ? WUN_OK : WUN_E_CUDA;
+}
+
+void wun::launch_eval_loss(const float* outputs, const float* targets, int K, long long n, double* state, double* batch_loss,
+                           double* slots, bool l1, cudaStream_t stream) {
+    if (l1)
+        eval_loss_partials<true><<<dim3(kLossCtas, (unsigned)K), kThreads, 0, stream>>>(outputs, targets, n, slots);
+    else
+        eval_loss_partials<false><<<dim3(kLossCtas, (unsigned)K), kThreads, 0, stream>>>(outputs, targets, n, slots);
+    eval_loss_finish<<<1, kThreads, 0, stream>>>(slots, K, n, state, batch_loss);
 }

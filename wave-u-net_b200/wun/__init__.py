@@ -21,6 +21,10 @@ SYMBOLS = [
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
     "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_resample_frames", "wun_resample",
     "wun_snippet_batch", "wun_eval_batch_loss",
+    "wun_spec_create", "wun_spec_destroy", "wun_spec_input_frames", "wun_spec_output_frames", "wun_spec_stft_frames",
+    "wun_spec_param_count", "wun_spec_param_numel", "wun_spec_param_table", "wun_spec_workspace_bytes",
+    "wun_spec_forward_flops", "wun_spec_launches_forward", "wun_spec_forward", "wun_spec_l1_batch_loss",
+    "wun_spec_gather_windows", "wun_spec_scatter_windows",
 ]
 
 
@@ -33,6 +37,15 @@ class WunConfig(ctypes.Structure):
 
 class WunParamInfo(ctypes.Structure):
     _fields_ = [("name", ctypes.c_char * 64), ("ndim", ctypes.c_int32), ("shape", ctypes.c_int32 * 3),
+                ("offset", ctypes.c_int64), ("numel", ctypes.c_int64)]
+
+
+class WunSpecConfig(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("num_layers", "num_initial_filters", "num_channels", "num_sources")]
+
+
+class WunSpecParamInfo(ctypes.Structure):
+    _fields_ = [("name", ctypes.c_char * 64), ("ndim", ctypes.c_int32), ("shape", ctypes.c_int32 * 4),
                 ("offset", ctypes.c_int64), ("numel", ctypes.c_int64)]
 
 
@@ -100,6 +113,24 @@ def _load():
     if hasattr(lib, "wun_snippet_batch"):   # likewise the validation-loss kernels
         lib.wun_snippet_batch.argtypes = [VP, I64, I64, I64, I64, I64, VP, I64, I64, VP, VP, VP, VP]
         lib.wun_eval_batch_loss.argtypes = [VP, VP, I64, I64, VP, VP, VP, I64, VP]
+    if hasattr(lib, "wun_spec_create"):     # likewise the spectrogram U-Net
+        lib.wun_spec_create.argtypes = [P(WunSpecConfig), I64, P(H)]
+        lib.wun_spec_destroy.argtypes = [H]
+        for n in ("wun_spec_input_frames", "wun_spec_output_frames", "wun_spec_stft_frames", "wun_spec_param_count",
+                  "wun_spec_param_numel"):
+            getattr(lib, n).argtypes = [H]
+            getattr(lib, n).restype = I64
+        lib.wun_spec_param_table.argtypes = [H, P(WunSpecParamInfo), I64]
+        lib.wun_spec_workspace_bytes.argtypes = [H, I64]
+        lib.wun_spec_workspace_bytes.restype = I64
+        lib.wun_spec_forward_flops.argtypes = [H, I64]
+        lib.wun_spec_forward_flops.restype = ctypes.c_double
+        lib.wun_spec_launches_forward.argtypes = [H, ctypes.c_int]
+        lib.wun_spec_launches_forward.restype = I64
+        lib.wun_spec_forward.argtypes = [H, VP, VP, I64, ctypes.c_int, VP, VP, I64, VP]
+        lib.wun_spec_l1_batch_loss.argtypes = [H, VP, VP, I64, VP, VP, VP, I64, VP]
+        lib.wun_spec_gather_windows.argtypes = [H, VP, I64, VP, I64, VP, VP]
+        lib.wun_spec_scatter_windows.argtypes = [H, VP, VP, I64, VP, I64, VP]
     return lib
 
 
@@ -571,3 +602,112 @@ class Engine(object):
     def scatter_windows(self, outputs, starts, preds):
         check(lib.wun_scatter_windows(self._h, outputs.data_ptr(), starts.data_ptr(), starts.numel(),
                                       preds.data_ptr(), preds.shape[1], self._stream(preds.device)))
+
+
+SPEC_BINS = 513             # include/wun.h WUN_SPEC_BINS
+
+
+def spec_config_from_model_config(mc):
+    """model_config dict (Config.py) -> WunSpecConfig: the keys UnetSpectrogramSeparator.__init__ reads."""
+    c = WunSpecConfig()
+    c.num_layers = int(mc["num_layers"])
+    c.num_initial_filters = int(mc["num_initial_filters"])
+    c.num_channels = 1 if mc["mono_downmix"] else 2
+    c.num_sources = len(mc["source_names"])
+    return c
+
+
+class SpecEngine(object):
+    """The spectrogram U-Net's inference graph for one window length (include/wun.h wun_spec_*).  Mirrors the parts of
+    Engine that Evaluate._separate_on_device and Test.test use; T_in == T_out == the window length."""
+
+    def __init__(self, cfg, num_frames=None, input_frames=None):
+        self._h = ctypes.c_void_p()
+        self.cfg = cfg
+        check(lib.wun_spec_create(ctypes.byref(cfg), int(input_frames if input_frames is not None else num_frames),
+                                  ctypes.byref(self._h)))
+        self.T_in = lib.wun_spec_input_frames(self._h)
+        self.T_out = lib.wun_spec_output_frames(self._h)
+        self.stft_frames = lib.wun_spec_stft_frames(self._h)
+        n = lib.wun_spec_param_count(self._h)
+        arr = (WunSpecParamInfo * n)()
+        check(lib.wun_spec_param_table(self._h, arr, n))
+        self.param_table = [(a.name.decode(), tuple(a.shape[:a.ndim]), int(a.offset), int(a.numel)) for a in arr]
+        self.param_numel = lib.wun_spec_param_numel(self._h)
+        self._ws = {}
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib.wun_spec_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+    def workspace_bytes(self, batch):
+        return lib.wun_spec_workspace_bytes(self._h, int(batch))
+
+    def forward_flops(self, batch):
+        return lib.wun_spec_forward_flops(self._h, int(batch))
+
+    def launches(self, return_spectrogram=False):
+        return lib.wun_spec_launches_forward(self._h, 1 if return_spectrogram else 0)
+
+    def output_shape(self, batch, return_spectrogram=False):
+        K = self.cfg.num_sources
+        return (K, batch, self.stft_frames, SPEC_BINS) if return_spectrogram else (K, batch, self.T_out, 1)
+
+    def _workspace(self, batch, device):
+        import torch
+        # kept while the engine lives: a captured CUDA graph (Test.test) bakes the pointer in
+        key = (int(batch), str(device))
+        ws = self._ws.get(key)
+        if ws is None:
+            ws = torch.empty((self.workspace_bytes(batch) + 3) // 4, dtype=torch.float32, device=device)
+            self._ws[key] = ws
+        return ws
+
+    def forward(self, params, mix, training, out=None, return_spectrogram=False):
+        """mix [B, T, 1] -> [K, B, T, 1] audio, or [K, B, n, 513] magnitudes with return_spectrogram.  Inference only."""
+        import torch
+        if training:
+            raise NotImplementedError("the spectrogram U-Net runs in inference mode only (training=False)")
+        B = int(mix.shape[0])
+        assert mix.is_cuda and mix.dtype == torch.float32 and mix.is_contiguous(), "mix must be a contiguous float32 CUDA tensor"
+        assert tuple(mix.shape[1:]) == (self.T_in, 1), ("mix shape", tuple(mix.shape), "expected [B, %d, 1]" % self.T_in)
+        shape = self.output_shape(B, return_spectrogram)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.float32, device=mix.device)
+        assert out.is_cuda and out.device == mix.device and out.dtype == torch.float32 and out.is_contiguous()
+        assert tuple(out.shape) == shape, ("outputs", tuple(out.shape), "expected", shape)
+        assert params.is_cuda and params.device == mix.device and params.dtype == torch.float32 and params.is_contiguous()
+        assert params.numel() >= self.param_numel, ("flat buffer too small", params.numel(), self.param_numel)
+        ws = self._workspace(B, mix.device)
+        with torch.cuda.device(mix.device):
+            check(lib.wun_spec_forward(self._h, params.data_ptr(), mix.data_ptr(), B, 1 if return_spectrogram else 0,
+                                       out.data_ptr(), ws.data_ptr(), ws.numel() * 4, Engine._stream(mix.device)))
+        return out
+
+    def l1_batch_loss(self, est_mags, targets, state, batch_loss=None):
+        """Test.test's U7a loss and running mean (wun_spec_l1_batch_loss): est_mags [K, B, n, 513] from forward(...,
+        return_spectrogram=True), targets [K, B, T, 1] audio, state float64 [2] {total, n} updated in place."""
+        import torch
+        B = int(targets.shape[1])
+        assert tuple(est_mags.shape) == self.output_shape(B, True) and est_mags.is_contiguous(), "est_mags shape"
+        assert tuple(targets.shape) == self.output_shape(B, False) and targets.is_contiguous(), "targets shape"
+        assert targets.dtype == torch.float32 and est_mags.dtype == torch.float32
+        assert state.dtype == torch.float64 and state.numel() == 2 and state.is_cuda
+        assert batch_loss is None or (batch_loss.dtype == torch.float64 and batch_loss.is_cuda)
+        ws = self._workspace(B, targets.device)
+        with torch.cuda.device(targets.device):
+            check(lib.wun_spec_l1_batch_loss(self._h, est_mags.data_ptr(), targets.data_ptr(), B, state.data_ptr(),
+                                             batch_loss.data_ptr() if batch_loss is not None else None, ws.data_ptr(),
+                                             ws.numel() * 4, Engine._stream(targets.device)))
+
+    def gather_windows(self, padded, starts, mix_batch):
+        check(lib.wun_spec_gather_windows(self._h, padded.data_ptr(), padded.shape[0], starts.data_ptr(),
+                                          starts.numel(), mix_batch.data_ptr(), Engine._stream(padded.device)))
+
+    def scatter_windows(self, outputs, starts, preds):
+        check(lib.wun_spec_scatter_windows(self._h, outputs.data_ptr(), starts.data_ptr(), starts.numel(),
+                                           preds.data_ptr(), preds.shape[1], Engine._stream(preds.device)))
