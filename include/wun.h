@@ -304,6 +304,44 @@ int wun_spec_gather_windows(WunSpecHandle* h, const float* padded, int64_t n_pad
 int wun_spec_scatter_windows(WunSpecHandle* h, const float* outputs, const int64_t* starts, int64_t n_windows,
                              float* preds, int64_t n_frames, void* stream);
 
+/* --- spectrogram U-Net, training ------------------------------------------------------------------
+ * One step of the reference's Training.py (:47-77) for network="unet_spectrogram": get_output(mix, training=True,
+ * return_spectrogram=not raw_audio_loss), the loss sum_k loss_k / K and its gradients, and the batch-norm UPDATE_OPS.
+ *   U7  (raw_audio_loss = 1): loss_k = mean((target_k - audio_k)^2) over [B, T, 1], through the inverse STFT;
+ *   U7a (raw_audio_loss = 0): loss_k = mean|STFTmag(target_k) - mask_k |X|| over [B, n, 513].
+ * Training differs from inference in two layers:
+ *   batch norm: normalised with the batch mean and biased variance over B*H*W per channel; moving_mean and moving_variance
+ *     in `params` move by (moving - batch value) * (1 - 0.999), the variance Bessel-corrected (N / max(N - 1, 1));
+ *   dropout(rate 0.5) on the concatenations of up steps 0, 1, 2 (levels L-2, L-3, L-4), kept elements times 2.  The keep
+ *     bit of element i (flat NHWC index) of level d in the U-Net of source k is a splitmix64 hash of (seed, the dropout
+ *     counter *step_state, k, d, i) (oracle/spectrogram_train_oracle.py restates it); the call advances the counter by one.
+ * LeakyReLU's slope at 0 is 0.2 and ReLU's is 0, as TF's Maximum / Relu gradients have them.  The two U-Nets run one after
+ * the other on one set of activation buffers.
+ *   params  DEVICE float32 [param_numel]: read, and the moving statistics updated
+ *   mix [B, T, 1], targets [K][B, T, 1]; grads DEVICE float32 [param_numel]: every variable's gradient (0 for the moving
+ *   statistics); loss DEVICE float64[1]; step_state DEVICE int64[1].
+ * Every sum has a fixed order and there are no atomics: the same inputs give the same bits.  No allocation, host
+ * synchronisation or copy inside these calls: feed, forward_backward and Adam can be captured in one CUDA graph. */
+int64_t wun_spec_train_workspace_bytes(const WunSpecHandle* h, int64_t batch);
+/* forward + input-gradient + weight-gradient convolution FLOPs of one step (the first layer has no input gradient) */
+double wun_spec_train_flops(const WunSpecHandle* h, int64_t batch);
+int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
+                              int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
+                              void* workspace, int64_t workspace_bytes, void* stream);
+/* tf.train.AdamOptimizer step on the trainable variables (kernels, biases, betas), as wun_adam_step_device: state = DEVICE
+ * float32[3] {beta1_power, beta2_power, step}.  The moving statistics have zero gradients and zero slots, so they keep their
+ * bits; only the trainables' slots are checkpointed. */
+int wun_spec_adam_step_device(WunSpecHandle* h, float* params, const float* grads, float* m, float* v, float* state,
+                              float lr, float beta1, float beta2, float eps, void* stream);
+/* Tests: where concatenation level `level` ([B, H, W, C] NHWC: the down layer's LeakyReLU output, then the up layer's ReLU
+ * output; the bottom level has only the former) lies in the training workspace at `batch`.  After wun_spec_forward_backward
+ * it holds the last source's activations, whose signs are the slopes the backward used. */
+int wun_spec_debug_train_level(const WunSpecHandle* h, int64_t batch, int level, int64_t* offset_bytes, int64_t* elems);
+/* wun_feed_batch for this handle: T_in = T_out = T, one channel, K sources */
+int wun_spec_feed_batch(WunSpecHandle* h, const float* pool, int64_t total_frames, const int64_t* track_offset,
+                        const int64_t* track_length, int64_t n_tracks, int64_t batch, int augmentation, uint64_t seed,
+                        int64_t* step_state, float* mix_out, float* targets_out, int64_t* chosen, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

@@ -10,7 +10,13 @@ Same class name, constructor argument and method names as the reference's Models
 As with UnetAudioSeparator here, `mix` is a float32 CUDA tensor [B, T, 1] and the result an ordered dict source name ->
 float32 CUDA tensor: audio [B, T, 1], or with return_spectrogram the magnitudes [B, n, 513].  The variables (kernels,
 biases, batch-norm betas and moving statistics) live in one flat float32 CUDA buffer in TF creation order under
-"separator".  Only the inference graph exists: training=True raises NotImplementedError.
+"separator".
+
+Training is the training half of the graph Training.py builds (:47-77) and goes through loss_and_gradients() / adam_step(),
+as with UnetAudioSeparator: training-mode batch norm (batch statistics, moving averages updated on every step), dropout on
+the first three concatenations of the up path, the U7 (audio MSE) or U7a (L1 on magnitudes, raw_audio_loss=False) loss,
+every trainable variable's gradient and tf.train.AdamOptimizer on kernels, biases and betas.  A standalone
+get_output(training=True) graph does not exist and raises NotImplementedError.
 """
 from collections import OrderedDict
 import math
@@ -31,10 +37,41 @@ class UnetSpectrogramSeparator:
         self.frame_len = 1024
         self.hop = 768
         self._cfg = wun.spec_config_from_model_config(model_config)
+        self.raw_audio_loss = bool(model_config.get("raw_audio_loss", True))
         self._engines = {}                      # T -> wun.SpecEngine
         self.params = None
-        self.global_step = 0
+        self.grads = None
+        self.adam_m = None
+        self.adam_v = None
+        self._adam_state = None                 # device float32[3] {beta1_power, beta2_power, step}: TF's beta*_power
+        self._betas = (0.9, 0.999)
+        self._step0 = 0
+        self._loss = None
+        self._dropout_step = None               # device int64[1]: the dropout masks' step counter
         self.seed = 1337
+        self.last_feeder = None
+        self.last_feeder_tracks = None
+
+    # global_step lives on the device next to Adam's beta-power accumulators, so that a CUDA-graph replay of a whole
+    # training step advances it and uses the right bias correction every replay.
+    @property
+    def global_step(self):
+        if self._adam_state is None:
+            return self._step0
+        return int(round(float(self._adam_state[2].item())))
+
+    @global_step.setter
+    def global_step(self, n):
+        self._step0 = int(n)
+        if self._adam_state is not None:
+            self._write_adam_state()
+
+    def _write_adam_state(self):
+        import torch
+        b1, b2 = self._betas
+        n = self._step0
+        vals = torch.tensor([b1 ** (n + 1), b2 ** (n + 1), float(n)], dtype=torch.float32)
+        self._adam_state.copy_(vals.to(self._adam_state.device))
 
     def get_padding(self, shape):
         """The shape unchanged: input and output are [batch, frames, 1]."""
@@ -43,7 +80,8 @@ class UnetSpectrogramSeparator:
     def get_output(self, input, training, return_spectrogram=False, reuse=True):
         """Audio estimates [B, T, 1] per source, or with return_spectrogram their magnitudes [B, n, 513]."""
         if training:
-            raise NotImplementedError("training the spectrogram U-Net is not supported; use training=False")
+            raise NotImplementedError("the spectrogram U-Net trains through loss_and_gradients() / adam_step(); "
+                                      "get_output runs with training=False")
         eng = self._engine_for(int(input.shape[1]))
         self._ensure_params(eng, input.device, create=not reuse)
         out = eng.forward(self.params, input.contiguous(), False, return_spectrogram=return_spectrogram)
@@ -104,3 +142,60 @@ class UnetSpectrogramSeparator:
             assert tuple(a.shape) == tuple(shape), (name, a.shape, shape)
             flat[off:off + numel] = a.reshape(-1)
         self.params = torch.from_numpy(flat).to(device)
+        self.grads = self.adam_m = self.adam_v = None
+        if self._adam_state is not None:
+            self._step0 = self.global_step
+            self._adam_state = None
+            self._dropout_step = None
+
+    def trainable_variable_names(self):
+        """The variables AdamOptimizer trains and the checkpoint has slots for: kernels, biases, betas (not the moving
+        statistics, which only the batch-norm update moves)."""
+        eng = next(iter(self._engines.values()))
+        return [n for n, _, _ in eng.trainable_ranges]
+
+    def gradients(self):
+        eng = next(iter(self._engines.values()))
+        return OrderedDict((n, self.grads[o:o + c].view(*s)) for n, s, o, c in eng.param_table)
+
+    # ------------------------------------------------------------------------------------------
+    # the training half of the graph (Training.py:47-77)
+    # ------------------------------------------------------------------------------------------
+    def _ensure_training_state(self):
+        import torch
+        if self.grads is None:
+            dev = self.params.device
+            self.grads = torch.zeros_like(self.params)
+            self.adam_m = torch.zeros_like(self.params)
+            self.adam_v = torch.zeros_like(self.params)
+            self._loss = torch.zeros(1, dtype=torch.float64, device=dev)
+            self._adam_state = torch.zeros(3, dtype=torch.float32, device=dev)
+            self._write_adam_state()
+            # one dropout step per optimiser step: a resumed run continues the masks where the checkpoint left them
+            self._dropout_step = torch.full((1,), self._step0, dtype=torch.int64, device=dev)
+
+    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0):
+        """separator_loss (Training.py:50-63) of get_output(mix, training=True, not raw_audio_loss) and d loss / d variables;
+        the batch-norm moving statistics in self.params take their update.  targets: [K, B, T, 1] tensor or dict.
+        Returns the device float64 loss; the gradients land in self.grads (flat, 0 for the moving statistics)."""
+        import torch
+        if grad_scale != 1.0:
+            raise ValueError("the spectrogram U-Net trains on one GPU: batch statistics of a shard would change the model")
+        if isinstance(targets, dict):
+            targets = torch.stack([targets[n] for n in self.source_names])
+        eng = self._engine_for(int(mix.shape[1]))
+        self._ensure_params(eng, mix.device, create=not reuse)
+        self._ensure_training_state()
+        eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, self._loss,
+                             self.raw_audio_loss, self.seed, self._dropout_step)
+        return self._loss
+
+    def adam_step(self, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8):
+        """tf.train.AdamOptimizer(learning_rate).minimize step on the trainable separator variables (:77)."""
+        eng = next(iter(self._engines.values()))
+        if (beta1, beta2) != self._betas:
+            self._step0 = self.global_step
+            self._betas = (beta1, beta2)
+            self._write_adam_state()
+        eng.adam_step_device(self.params, self.grads, self.adam_m, self.adam_v, self._adam_state, learning_rate, beta1,
+                             beta2, epsilon)

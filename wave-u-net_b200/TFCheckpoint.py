@@ -437,12 +437,13 @@ SOLVER_SCOPE = "separator_solver"
 
 def separator_tensors(variables, adam_m=None, adam_v=None, global_step=0, beta1=0.9, beta2=0.999):
     """What Saver(tf.global_variables()) holds for the reference's training graph.
-    variables / adam_m / adam_v: ordered mappings TF-name -> numpy array (m, v optional: inference-only checkpoint)."""
+    variables / adam_m / adam_v: ordered mappings TF-name -> numpy array (m, v optional: inference-only checkpoint); the
+    slots are written for the names adam_m holds (the trainable variables)."""
     out = OrderedDict()
     for n, a in variables.items():
         out[n] = np.asarray(a, dtype=np.float32)
     if adam_m is not None:
-        for n in variables:
+        for n in adam_m:
             out["%s/%s/Adam" % (SOLVER_SCOPE, n)] = np.asarray(adam_m[n], dtype=np.float32)
             out["%s/%s/Adam_1" % (SOLVER_SCOPE, n)] = np.asarray(adam_v[n], dtype=np.float32)
         # TF's Adam initialises the power accumulators to beta and multiplies once per applied step
@@ -452,9 +453,10 @@ def separator_tensors(variables, adam_m=None, adam_v=None, global_step=0, beta1=
     return out
 
 
-def split_separator_tensors(tensors, variable_names):
+def split_separator_tensors(tensors, variable_names, slot_names=None):
     """Inverse of separator_tensors, tolerant to the optimizer's scope prefix: returns
-    (variables, adam_m or None, adam_v or None, global_step)."""
+    (variables, adam_m or None, adam_v or None, global_step).  slot_names: the variables that have Adam slots (default:
+    every variable); m / v are None unless all of them have both."""
     variables = OrderedDict()
     missing = [n for n in variable_names if n not in tensors]
     if missing:
@@ -472,7 +474,7 @@ def split_separator_tensors(tensors, variable_names):
         return tensors[hits[0]] if len(hits) == 1 else None
 
     m, v = OrderedDict(), OrderedDict()
-    for n in variable_names:
+    for n in (variable_names if slot_names is None else slot_names):
         a, b = slot(n, "Adam"), slot(n, "Adam_1")
         if a is None or b is None:
             m = v = None
@@ -490,14 +492,23 @@ def is_npz(path):
     return path.endswith(".npz") or (not os.path.exists(path + ".index") and os.path.isfile(path))
 
 
+def _slot_names(sep):
+    """The variables with Adam slots: the separator's trainables when it tells them apart (the spectrogram U-Net's moving
+    statistics are not trained), else every variable."""
+    names = getattr(sep, "trainable_variable_names", None)
+    return names() if names is not None else None
+
+
 def save_separator(path, sep):
     """Write what the reference's `saver.save(sess, path, global_step)` writes; returns the checkpoint prefix."""
     table = sep.param_table()
     flat = sep.params.detach().cpu().numpy()
+    slots = _slot_names(sep)
     per_var = lambda buf: OrderedDict((n, buf[o:o + c].reshape(s)) for n, s, o, c in table)
+    per_slot = lambda buf: OrderedDict((n, buf[o:o + c].reshape(s)) for n, s, o, c in table if slots is None or n in slots)
     m = v = None
     if sep.adam_m is not None:
-        m, v = per_var(sep.adam_m.detach().cpu().numpy()), per_var(sep.adam_v.detach().cpu().numpy())
+        m, v = per_slot(sep.adam_m.detach().cpu().numpy()), per_slot(sep.adam_v.detach().cpu().numpy())
     if path.endswith(".npz"):
         blob = dict(per_var(flat))
         if m is not None:
@@ -527,7 +538,7 @@ def restore_separator(path, sep, input_frames, with_optimizer=True):
             sep.adam_v.copy_(torch.from_numpy(tensors["separator_solver/adam_v"]))
         return sep
     tensors = read_checkpoint(path)
-    variables, m, v, step = split_separator_tensors(tensors, names)
+    variables, m, v, step = split_separator_tensors(tensors, names, _slot_names(sep))
     sep.load_variables(variables, input_frames=input_frames)          # asserts every shape against the plan
     sep.global_step = step
     if with_optimizer and m is not None:
@@ -536,6 +547,8 @@ def restore_separator(path, sep, input_frames, with_optimizer=True):
         fm = np.zeros(sep.params.numel(), np.float32)
         fv = np.zeros(sep.params.numel(), np.float32)
         for n, s, o, c in table:
+            if n not in m:
+                continue
             if tuple(m[n].shape) != tuple(s) or tuple(v[n].shape) != tuple(s):
                 raise CheckpointError("%s: Adam slot shape %s does not match the variable %s" % (n, m[n].shape, s))
             fm[o:o + c] = np.asarray(m[n], np.float32).reshape(-1)

@@ -20,6 +20,10 @@ opt-in with a top-level extra:
 
 which stages the MUSDB18 WAV dataset on the device (Datasets.py), validates with Test.test, returns the best checkpoint's
 test loss and writes its estimates and BSS Eval JSONs (Evaluate.produce_musdb_source_estimates), as the reference does.
+
+network="unet_spectrogram" (presets cfg.unet_spectrogram / U7 and cfg.unet_spectrogram_l1 / U7a) trains the spectrogram
+U-Net the same way on one GPU (Models/UnetSpectrogramSeparator.py); its batch statistics are those of the whole batch, so a
+data-parallel run, whose ranks would each normalise with their own shard's statistics, is refused.
 """
 import os
 import sys
@@ -30,7 +34,17 @@ import numpy as np
 import Config
 import TFCheckpoint
 from Models.UnetAudioSeparator import UnetAudioSeparator
+from Models.UnetSpectrogramSeparator import UnetSpectrogramSeparator
 from wun import parallel
+
+
+def separator_class(model_config):
+    """The separator model_config["network"] names (reference Training.py:30-33)."""
+    if model_config["network"] == "unet":
+        return UnetAudioSeparator
+    if model_config["network"] == "unet_spectrogram":
+        return UnetSpectrogramSeparator
+    raise NotImplementedError(model_config["network"])
 
 
 class SyntheticBatches(object):
@@ -113,10 +127,12 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
     rank, world = parallel.world()
     if device is None:
         device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    if model_config["network"] != "unet":
-        raise NotImplementedError                                   # reference :33 (unet_spectrogram is out of scope)
+    cls = separator_class(model_config)                             # reference :30-33
+    if cls is UnetSpectrogramSeparator and world > 1:
+        raise ValueError("the spectrogram U-Net trains on one GPU: with %d ranks every rank would normalise with its own "
+                         "shard's batch statistics, which changes the model" % world)
     if sep is None:
-        sep = UnetAudioSeparator(model_config)
+        sep = cls(model_config)
     disc_input_shape = [model_config["batch_size"], model_config["num_frames"], 0]
     in_shape, out_shape = sep.get_padding(np.array(disc_input_shape))                 # :35
     t_in = int(in_shape[1])
@@ -166,15 +182,25 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
 
 
 def validation_loss(model_config, sep, batches=4, seed=99):
-    """Running-mean MSE over a fixed synthetic validation set (reference Test.test, Test.py:57-71)."""
+    """Running-mean loss over a fixed synthetic validation set (reference Test.test, Test.py:57-71): MSE on audio, or for
+    the spectrogram U-Net with raw_audio_loss=False the L1 loss on STFT magnitudes (Test.py:63-67)."""
     import torch
     in_shape, out_shape = sep.get_padding(np.array([model_config["batch_size"], model_config["num_frames"], 0]))
     src = SyntheticBatches(model_config, in_shape, out_shape, seed=seed)
     names = model_config["source_names"]
+    l1 = model_config["network"] == "unet_spectrogram" and not model_config["raw_audio_loss"]
     tot, n = 0.0, 0
     for _ in range(batches):
         b = next(src)
         mix = torch.from_numpy(b["mix"]).to(sep.params.device)
+        if l1:
+            eng = sep.engine(num_frames=int(mix.shape[1]))
+            est = eng.forward(sep.params, mix, False, return_spectrogram=True)
+            tg = torch.stack([torch.from_numpy(b[k]) for k in names]).to(mix.device).contiguous()
+            state = torch.zeros(2, dtype=torch.float64, device=mix.device)
+            eng.l1_batch_loss(est, tg, state)
+            tot += float(state[0].item()); n += 1
+            continue
         out = sep.get_output(mix, training=False, reuse=True)
         loss = sum(float(torch.mean((torch.from_numpy(b[k]).to(mix.device) - out[k]) ** 2)) for k in names) / len(names)
         tot += loss; n += 1
@@ -301,7 +327,7 @@ def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks):
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
     device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    probe = UnetAudioSeparator(model_config)
+    probe = separator_class(model_config)(model_config)
     in_shape, out_shape = probe.get_padding(np.array([model_config["batch_size"], model_config["num_frames"], 0]))
     ds = Datasets.load_musdb(model_config, int(in_shape[1]), int(out_shape[1]), model_config["musdb_path"], ccmixter_xml,
                              valid_tracks, device)

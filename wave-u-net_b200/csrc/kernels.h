@@ -99,6 +99,12 @@ void launch_gather_windows(const float* padded, long long n_padded, const long l
 void launch_scatter_windows(const float* outs, const long long* starts, int n_windows, int n_sources, int T_out,
                             int C, float* preds, long long n_frames, cudaStream_t stream);
 
+__host__ __device__ __forceinline__ uint64_t feed_mix64(uint64_t z) {       // splitmix64 finaliser
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 // kernels_feed.cu: one training batch cut out of a device-resident track pool (random snippet, random_amplify, centre crop)
 cudaError_t launch_feed_batch(const float* pool, long long total_frames, const long long* track_offset,
                               const long long* track_length, int n_tracks, int batch, int K, int C, int T_in, int T_out,
@@ -136,5 +142,72 @@ void launch_spec_up(const SpecConv& A, cudaStream_t stream);        // transpose
 void launch_spec_mask(const SpecConv& A, const float* X, float* out, int magnitude, cudaStream_t stream);
 // irfft + inverse window per frame into frames [batch][n_frames][1024], then overlap-add into out [batch][T]
 void launch_spec_istft(const float* Y, int n_frames, int batch, float* frames, float* out, long long T, cudaStream_t stream);
+
+// kernels_spec_train.cu: the spectrogram U-Net's training step
+// tf.layers.dropout(rate=0.5) keep bit of element i (flat NHWC index of the concatenation) of `level` in the U-Net of
+// `source` at dropout step `step`; oracle/spectrogram_train_oracle.py restates it in numpy
+__host__ __device__ __forceinline__ bool spec_dropout_keep(uint64_t seed, uint64_t step, int source, int level, uint64_t i) {
+    const uint64_t key = (step << 16) ^ ((uint64_t)source << 8) ^ (uint64_t)level;
+    const uint64_t stream = feed_mix64(seed ^ feed_mix64(key + 0x9E3779B97F4A7C15ull));
+    return (feed_mix64(stream + i * 0x9E3779B97F4A7C15ull) >> 63) != 0;
+}
+
+// A 5x5 gather over NHWC tensors at channel pitches, in the stride-2 (output o reads input 2o + k - 1) or transposed
+// (output o gathers input (o + 1 - k) / 2, o < 2 Hi) geometry.  Weight of (tap, output channel co, input channel ci) at
+// W[tap * w_tap + co * w_co + ci * w_ci].  x_drop / y_drop: keep masks laid out like x / y (kept elements count twice).
+struct SpecTrainConv {
+    const float* x; int Hi, Wi, Ci, x_pitch; const uint8_t* x_drop;
+    float* y; int Ho, Wo, Co, y_pitch, y_off; const uint8_t* y_drop; int accumulate;
+    const float* W; long long w_tap, w_co, w_ci;
+    const float* bias;                                            // or null
+    int batch;
+};
+void launch_spec_train_conv(const SpecTrainConv& A, int up, cudaStream_t stream);
+
+// Per-channel sums over the N rows of z [N][C] in fp64, in a fixed order, then per channel:
+//   mode 0  batch mean and rstd = 1/sqrt(biased var + 1e-3) into stat; moving_mean / moving_var updated with decay 0.999
+//   mode 1  dy = g * (a > 0 ? 1 : neg_slope) (g, a at `pitch`): out = sum dy (beta's gradient), coef = (mean dy, mean dy*xhat)
+//   mode 2  out = sum z (a conv bias gradient)
+struct SpecChanSum {
+    int mode;
+    const float* z; long long N; int C;
+    const float* g; const float* a; int pitch; float neg_slope;
+    float2* stat; float2* coef; float* out;
+    float* moving_mean; float* moving_var;
+    double2* part;                                                // [spec_chan_partials(N)][C]
+};
+int spec_chan_partials(long long N);
+void launch_spec_chan_sum(const SpecChanSum& S, cudaStream_t stream);
+// (z - mean) * rstd + beta, then max(neg_slope * v, v), into y [N][y_pitch]
+void launch_spec_bn_apply(const float* z, long long N, int C, const float2* stat, const float* beta, float neg_slope,
+                          float* y, int y_pitch, cudaStream_t stream);
+// in place: z [N][C] -> dz = rstd * (dy - coef.x - xhat * coef.y)
+void launch_spec_bn_backward(float* z, long long N, int C, const float* g, const float* a, int pitch, float neg_slope,
+                             const float2* stat, const float2* coef, cudaStream_t stream);
+void launch_spec_dropout(uint8_t* keep, long long n, unsigned long long seed, const long long* step_state, int source,
+                         int level, cudaStream_t stream);
+// mask [frames][512]: logits in, sigmoid out; out = mask * X (complex [frames][513]) or mask * |X| with magnitude
+void launch_spec_mask_apply(float* mask, long long frames, const float* X, float* out, int magnitude, cudaStream_t stream);
+struct SpecMaskBwd {
+    const float* X; const float* mask; float* dlogit;             // [B][n][513] complex, [B][n][512], [B][n][512]
+    int n_frames; long long T;
+    int raw_audio;
+    const float* audio; const float* target;                      // U7: [B][T]
+    const float* tmag;                                            // U7a: [B][n][513]
+    float scale;                                                  // 1 / (B T K) or 1 / (B n 513 K)
+};
+void launch_spec_mask_backward(const SpecMaskBwd& M, int batch, cudaStream_t stream);
+// dW[tap * w_tap + c_lo * w_lo + c_hi * w_hi] = sum over low-resolution positions p = (b, h, w) of
+// lo[p][c_lo] * hi[b][2h + kh - 1][2w + kw - 1][c_hi]
+struct SpecWgrad {
+    const float* lo; int lo_pitch; const uint8_t* lo_drop; int Clo;
+    const float* hi; int hi_pitch; int Chi;
+    int Hl, Wl, batch;
+    float* dW; long long w_tap, w_lo, w_hi;
+    float* part;                                                  // [spec_wgrad_partials][25 Clo Chi] when that is > 1
+};
+int spec_wgrad_partials(const SpecWgrad& G);
+void launch_spec_wgrad(const SpecWgrad& G, cudaStream_t stream);
+void launch_spec_step_advance(long long* step_state, cudaStream_t stream);
 
 }  // namespace wun

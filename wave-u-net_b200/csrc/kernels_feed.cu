@@ -19,11 +19,6 @@
 
 namespace wun {
 
-__host__ __device__ __forceinline__ uint64_t feed_mix64(uint64_t z) {       // splitmix64 finaliser
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    return z ^ (z >> 31);
-}
 // slot 0: track, 1: start position, 2 + k: gain of source k
 __host__ __device__ __forceinline__ uint64_t feed_rand(uint64_t seed, uint64_t step, uint32_t example, uint32_t slot) {
     const uint64_t key = (step << 32) ^ ((uint64_t)example << 8) ^ (uint64_t)slot;

@@ -25,6 +25,8 @@ SYMBOLS = [
     "wun_spec_param_count", "wun_spec_param_numel", "wun_spec_param_table", "wun_spec_workspace_bytes",
     "wun_spec_forward_flops", "wun_spec_launches_forward", "wun_spec_forward", "wun_spec_l1_batch_loss",
     "wun_spec_gather_windows", "wun_spec_scatter_windows",
+    "wun_spec_train_workspace_bytes", "wun_spec_train_flops", "wun_spec_forward_backward", "wun_spec_adam_step_device",
+    "wun_spec_feed_batch", "wun_spec_debug_train_level",
 ]
 
 
@@ -131,6 +133,15 @@ def _load():
         lib.wun_spec_l1_batch_loss.argtypes = [H, VP, VP, I64, VP, VP, VP, I64, VP]
         lib.wun_spec_gather_windows.argtypes = [H, VP, I64, VP, I64, VP, VP]
         lib.wun_spec_scatter_windows.argtypes = [H, VP, VP, I64, VP, I64, VP]
+        lib.wun_spec_train_workspace_bytes.argtypes = [H, I64]
+        lib.wun_spec_train_workspace_bytes.restype = I64
+        lib.wun_spec_train_flops.argtypes = [H, I64]
+        lib.wun_spec_train_flops.restype = ctypes.c_double
+        lib.wun_spec_forward_backward.argtypes = [H, VP, VP, VP, I64, ctypes.c_int, ctypes.c_uint64, VP, VP, VP, VP, I64,
+                                                  VP]
+        lib.wun_spec_adam_step_device.argtypes = [H, VP, VP, VP, VP, VP, F, F, F, F, VP]
+        lib.wun_spec_debug_train_level.argtypes = [H, I64, ctypes.c_int, P(I64), P(I64)]
+        lib.wun_spec_feed_batch.argtypes = [H, VP, I64, VP, VP, I64, I64, ctypes.c_int, ctypes.c_uint64, VP, VP, VP, VP, VP]
     return lib
 
 
@@ -618,8 +629,9 @@ def spec_config_from_model_config(mc):
 
 
 class SpecEngine(object):
-    """The spectrogram U-Net's inference graph for one window length (include/wun.h wun_spec_*).  Mirrors the parts of
-    Engine that Evaluate._separate_on_device and Test.test use; T_in == T_out == the window length."""
+    """The spectrogram U-Net for one window length (include/wun.h wun_spec_*): the inference graph, and the training step
+    (forward_backward, adam_step_device, feed_batch).  Mirrors the parts of Engine that Evaluate._separate_on_device,
+    Test.test, Training.train and wun.feeder.DeviceFeeder use; T_in == T_out == the window length."""
 
     def __init__(self, cfg, num_frames=None, input_frames=None):
         self._h = ctypes.c_void_p()
@@ -635,6 +647,7 @@ class SpecEngine(object):
         self.param_table = [(a.name.decode(), tuple(a.shape[:a.ndim]), int(a.offset), int(a.numel)) for a in arr]
         self.param_numel = lib.wun_spec_param_numel(self._h)
         self._ws = {}
+        self._train_ws = {}
 
     def __del__(self):
         try:
@@ -649,6 +662,18 @@ class SpecEngine(object):
 
     def forward_flops(self, batch):
         return lib.wun_spec_forward_flops(self._h, int(batch))
+
+    def train_workspace_bytes(self, batch):
+        return lib.wun_spec_train_workspace_bytes(self._h, int(batch))
+
+    def train_flops(self, batch):
+        return lib.wun_spec_train_flops(self._h, int(batch))
+
+    @property
+    def trainable_ranges(self):
+        """[(name, offset, numel)] of the variables Adam trains (kernels, biases, betas), in table order; the moving
+        statistics are not among them."""
+        return [(n, o, c) for n, _, o, c in self.param_table if not n.endswith(("/moving_mean", "/moving_variance"))]
 
     def launches(self, return_spectrogram=False):
         return lib.wun_spec_launches_forward(self._h, 1 if return_spectrogram else 0)
@@ -703,6 +728,65 @@ class SpecEngine(object):
             check(lib.wun_spec_l1_batch_loss(self._h, est_mags.data_ptr(), targets.data_ptr(), B, state.data_ptr(),
                                              batch_loss.data_ptr() if batch_loss is not None else None, ws.data_ptr(),
                                              ws.numel() * 4, Engine._stream(targets.device)))
+
+    def forward_backward(self, params, mix, targets, grads, loss, raw_audio_loss, seed, step_state):
+        """One training step's loss and gradients (wun_spec_forward_backward): mix [B, T, 1], targets [K, B, T, 1], grads
+        float32 [param_numel], loss float64 [1], step_state int64 [1] (the dropout counter, advanced by one).  Updates the
+        moving statistics inside `params`."""
+        import torch
+        B = int(mix.shape[0])
+        assert mix.is_cuda and mix.dtype == torch.float32 and mix.is_contiguous(), "mix must be a contiguous float32 CUDA tensor"
+        assert tuple(mix.shape[1:]) == (self.T_in, 1), ("mix shape", tuple(mix.shape), "expected [B, %d, 1]" % self.T_in)
+        assert tuple(targets.shape) == self.output_shape(B) and targets.is_contiguous() and targets.dtype == torch.float32
+        for t in (params, grads):
+            assert t.is_cuda and t.device == mix.device and t.dtype == torch.float32 and t.is_contiguous()
+            assert t.numel() >= self.param_numel, ("flat buffer too small", t.numel(), self.param_numel)
+        assert loss.is_cuda and loss.dtype == torch.float64 and step_state.is_cuda and step_state.dtype == torch.int64
+        key = (B, str(mix.device))
+        ws = self._train_ws.get(key)        # kept while the engine lives: a captured CUDA graph bakes the pointer in
+        if ws is None:
+            ws = torch.empty((self.train_workspace_bytes(B) + 3) // 4, dtype=torch.float32, device=mix.device)
+            self._train_ws[key] = ws
+        with torch.cuda.device(mix.device):
+            check(lib.wun_spec_forward_backward(self._h, params.data_ptr(), mix.data_ptr(), targets.data_ptr(), B,
+                                                1 if raw_audio_loss else 0, int(seed) & (2 ** 64 - 1), step_state.data_ptr(),
+                                                grads.data_ptr(), loss.data_ptr(), ws.data_ptr(), ws.numel() * 4,
+                                                Engine._stream(mix.device)))
+        return loss
+
+    def debug_train_level(self, batch, level, device):
+        """Tests: view of concatenation level `level` [B, H, W, C] in the training workspace - after forward_backward the
+        last source's down (LeakyReLU) and up (ReLU) activations."""
+        off, n = ctypes.c_int64(), ctypes.c_int64()
+        check(lib.wun_spec_debug_train_level(self._h, int(batch), int(level), ctypes.byref(off), ctypes.byref(n)))
+        ws = self._train_ws[(int(batch), str(device))]
+        H, W = self.stft_frames >> (level + 1), 512 >> (level + 1)
+        return ws[off.value // 4:off.value // 4 + n.value].view(int(batch), H, W, -1)
+
+    def adam_step_device(self, params, grads, m, v, state, lr, beta1=0.9, beta2=0.999, eps=1e-8):
+        """Graph-safe Adam on the trainable variables: `state` = device float32[3] {beta1_power, beta2_power, step}."""
+        import torch
+        with torch.cuda.device(params.device):
+            check(lib.wun_spec_adam_step_device(self._h, params.data_ptr(), grads.data_ptr(), m.data_ptr(), v.data_ptr(),
+                                                state.data_ptr(), float(lr), float(beta1), float(beta2), float(eps),
+                                                Engine._stream(params.device)))
+
+    def feed_batch(self, pool, track_offset, track_length, batch, augmentation, seed, step_state, mix_out, targets_out,
+                   chosen=None):
+        """Engine.feed_batch for this window (wun_spec_feed_batch): T_in = T_out = T, one channel."""
+        import torch
+        K = targets_out.shape[0]
+        assert K == self.cfg.num_sources and pool.shape[2] == 1
+        assert pool.is_cuda and pool.dtype == torch.float32 and pool.is_contiguous() and pool.dim() == 3 and pool.shape[0] == K + 1
+        assert track_offset.dtype == torch.int64 and track_length.dtype == torch.int64 and step_state.dtype == torch.int64
+        assert tuple(mix_out.shape) == (batch, self.T_in, 1) and mix_out.is_contiguous()
+        assert tuple(targets_out.shape) == (K, batch, self.T_out, 1) and targets_out.is_contiguous()
+        with torch.cuda.device(mix_out.device):
+            check(lib.wun_spec_feed_batch(self._h, pool.data_ptr(), pool.shape[1], track_offset.data_ptr(),
+                                          track_length.data_ptr(), track_offset.numel(), int(batch), int(bool(augmentation)),
+                                          int(seed) & (2 ** 64 - 1), step_state.data_ptr(), mix_out.data_ptr(),
+                                          targets_out.data_ptr(), chosen.data_ptr() if chosen is not None else None,
+                                          Engine._stream(mix_out.device)))
 
     def gather_windows(self, padded, starts, mix_batch):
         check(lib.wun_spec_gather_windows(self._h, padded.data_ptr(), padded.shape[0], starts.data_ptr(),
