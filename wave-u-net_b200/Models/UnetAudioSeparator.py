@@ -185,18 +185,19 @@ class UnetAudioSeparator:
         import torch
         return torch.stack([batch[name] for name in self.source_names]).contiguous()
 
-    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0, outputs=None):
+    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0, outputs=None, loss=None):
         """separator_loss (Training.py:50-63) and d loss / d variables (the tf.gradients part of :77).
-        targets: [K,B,T_out,C] tensor or dict.  Returns the device scalar loss; gradients land in
-        self.grads (flat)."""
+        targets: [K,B,T_out,C] tensor or dict.  Returns the device scalar loss, written into `loss` (a float32 CUDA
+        tensor, e.g. one slot of a per-step history) when given; gradients land in self.grads (flat)."""
         if isinstance(targets, dict):
             targets = self.stack_targets(targets)
         eng = self._engine_for(int(mix.shape[1]))
         self._ensure_params(eng, mix.device, create=not reuse)
         self._ensure_training_state()
-        eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, self._loss,
+        loss = self._loss if loss is None else loss
+        eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, loss,
                              grad_scale=grad_scale, out=outputs)
-        return self._loss
+        return loss
 
     def adam_step(self, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8):
         """tf.train.AdamOptimizer(learning_rate).minimize step on the separator variables (:77)."""

@@ -174,10 +174,11 @@ class UnetSpectrogramSeparator:
             # one dropout step per optimiser step: a resumed run continues the masks where the checkpoint left them
             self._dropout_step = torch.full((1,), self._step0, dtype=torch.int64, device=dev)
 
-    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0):
+    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0, loss=None):
         """separator_loss (Training.py:50-63) of get_output(mix, training=True, not raw_audio_loss) and d loss / d variables;
         the batch-norm moving statistics in self.params take their update.  targets: [K, B, T, 1] tensor or dict.
-        Returns the device float64 loss; the gradients land in self.grads (flat, 0 for the moving statistics)."""
+        Returns the device float64 loss, written into `loss` (a float64 CUDA tensor, e.g. one slot of a per-step history)
+        when given; the gradients land in self.grads (flat, 0 for the moving statistics)."""
         import torch
         if grad_scale != 1.0:
             raise ValueError("the spectrogram U-Net trains on one GPU: batch statistics of a shard would change the model")
@@ -186,9 +187,10 @@ class UnetSpectrogramSeparator:
         eng = self._engine_for(int(mix.shape[1]))
         self._ensure_params(eng, mix.device, create=not reuse)
         self._ensure_training_state()
-        eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, self._loss,
+        loss = self._loss if loss is None else loss
+        eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, loss,
                              self.raw_audio_loss, self.seed, self._dropout_step)
-        return self._loss
+        return loss
 
     def adam_step(self, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8):
         """tf.train.AdamOptimizer(learning_rate).minimize step on the trainable separator variables (:77)."""

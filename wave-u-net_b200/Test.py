@@ -11,19 +11,26 @@ estimate_k| / K over the magnitudes [B, n, 513] instead.
 
 On the device: one CUDA graph of wun_snippet_batch -> wun_forward -> wun_eval_batch_loss, replayed once per batch; the
 batch counter and the fp64 running mean live on the device, so the partition costs one host synchronisation, at the end,
-and gives the same bits on every run.  The reference's test_loss TensorBoard summary is not written.
+and gives the same bits on every run.  With summaries=True the result is also written as the reference's `test_loss`
+TensorBoard scalar (Test.py:41,81-82), in a new events file of log_dir/<model_folder> (Summaries.py).
 """
+import os
+
 import numpy as np
 
 
-def test(model_config, partition, model_folder, load_model, dataset=None, separator=None):
+def test(model_config, partition, model_folder, load_model, dataset=None, separator=None, summaries=False):
     """Running-mean MSE (or, for U7a, L1 of magnitudes) over the full batches of `partition` ("valid" or "test") of `dataset` (a Datasets.Dataset; staged
     from model_config["musdb_path"] when None), with `separator` or else the variables of checkpoint `load_model`.
-    Raises ValueError when the partition has fewer snippets than one batch."""
+    Raises ValueError when the partition has fewer snippets than one batch.  With `summaries`, rank 0 writes the result,
+    rounded to float32, as a `test_loss` scalar at the separator's global step (both partitions use that tag, as in the
+    reference); every rank computes the same bits, so no collective is needed."""
     import torch
     import Datasets
     import Evaluate
+    import Summaries
     import wun
+    from wun import parallel
     if model_config["network"] not in ("unet", "unet_spectrogram"):
         raise NotImplementedError
     # the spectrogram U-Net's U7a preset scores magnitudes: mean |STFTmag(target) - estimate| (Test.py:63-67)
@@ -79,5 +86,7 @@ def test(model_config, partition, model_folder, load_model, dataset=None, separa
                     graph.replay()
         cur.wait_stream(side)
         total = float(state[0].item())
+    if summaries and parallel.world()[0] == 0:
+        Summaries.write_scalar(os.path.join(model_config["log_dir"], str(model_folder)), "test_loss", total, separator.global_step)
     print("Finished testing - Mean %s: %s" % ("L1" if magnitude_loss else "MSE", total))
     return total

@@ -12,6 +12,11 @@ train()    one "epoch" of model_config["epoch_it"] steps (reference :103-109): e
            "separator/..." variables, Adam slots and global_step, as the reference's Saver does (:98,113).
 optimise() early stopping on a validation loss + fine-tuning stage with doubled batch and lr 1e-5 (:123-150).
 
+run(), and so the command line, writes the reference's TensorBoard summaries (Summaries.py) into
+model_config["log_dir"]/<experiment_id>: a `sep_loss` scalar at every training step (:80-81,88,106) and a `test_loss` scalar
+after every validation and the final test (Test.py:41,81-82).  train, optimise, validation_loss and Test.test take
+summaries=False by default and write nothing.  The FileWriter's graph events are not written: there is no TensorFlow graph.
+
 By default batches come from `batch_source`, by default the synthetic generator of SURVEY 8(d) (uniform sources, random
 gains as Utils.random_amplify :26-36, centre-cropped targets as Utils.crop_sample :38-42).  Training on real music is
 opt-in with a top-level extra:
@@ -32,6 +37,7 @@ import time
 import numpy as np
 
 import Config
+import Summaries
 import TFCheckpoint
 from Models.UnetAudioSeparator import UnetAudioSeparator
 from Models.UnetSpectrogramSeparator import UnetSpectrogramSeparator
@@ -118,11 +124,14 @@ def _device_feeder(model_config, sep, eng, device, rank, world, local_batch, dat
 
 
 def train(model_config, experiment_id, load_model=None, batch_source=None, sep=None, device=None, log_every=100, feeder=None,
-          dataset=None):
+          dataset=None, summaries=False):
     """One epoch (reference train(), :24-121).  Returns (checkpoint path, separator).
     Data: `batch_source` (an iterator of host numpy batches, e.g. SyntheticBatches) if given; otherwise, on a CUDA device,
     the device-side feeder (`feeder="device"`, the default there); `feeder="host"` forces the numpy generator.  With
-    `dataset` (a Datasets.Dataset) the device-side feeder draws from its train partition."""
+    `dataset` (a Datasets.Dataset) the device-side feeder draws from its train partition.
+    With `summaries`, rank 0 writes a new TensorBoard events file into log_dir/<experiment_id> (:80-81,88,106): one
+    `sep_loss` scalar per step, the whole batch's loss of the forward pass before that step's update, at the global step
+    before it.  The losses stay on the device until the epoch ends, so logging adds no host synchronisation per step."""
     import torch
     rank, world = parallel.world()
     if device is None:
@@ -154,6 +163,12 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
         if dataset is not None:
             raise ValueError("training on a dataset needs the device-side feeder on a CUDA device")
         batch_source = SyntheticBatches(model_config, in_shape, out_shape, seed=1337 + sep.global_step)
+    history = done = None
+    if summaries:
+        # the engine writes each step's loss straight into its slot; an event after each step marks when it finished
+        step0 = sep.global_step
+        history = torch.empty(model_config["epoch_it"], dtype=sep._loss.dtype, device=sep.params.device)
+        done = [torch.cuda.Event(enable_timing=True) for _ in range(model_config["epoch_it"])]
     running, t0 = 0.0, time.time()
     # N > 1: the gradient all-reduce runs bucketed on a communication stream while backward still computes
     overlap = parallel.BucketedAllReduce(eng, sep.grads) if (world > 1 and sep.grads.is_cuda) else None
@@ -164,16 +179,23 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
             mix, tg = _to_device(next(batch_source), names, device)
             mix_l = parallel.shard_batch(mix, rank, world).contiguous()
             tg_l = parallel.shard_batch(tg, rank, world, dim=1).contiguous()
-        loss = sep.loss_and_gradients(mix_l, tg_l, grad_scale=parallel.grad_scale_for(mix_l.shape[0], global_batch))
+        loss = sep.loss_and_gradients(mix_l, tg_l, grad_scale=parallel.grad_scale_for(mix_l.shape[0], global_batch),
+                                      loss=None if history is None else history[it:it + 1])
         if overlap is not None:
             overlap.run()
         else:
             parallel.allreduce_gradients(sep.grads)
         sep.adam_step(lr)
+        if done is not None:
+            done[it].record(torch.cuda.current_stream(sep.params.device))
         if log_every and (it + 1) % log_every == 0 and rank == 0:
             running = float(loss.item())
             print("step %d  sep_loss(local shard) %.6f  %.1f steps/s" % (sep.global_step, running,
                                                                          (it + 1) / (time.time() - t0)))
+    if done:
+        lo, hi = parallel.shard_range(global_batch, rank, world)
+        _write_sep_loss(os.path.join(model_config["log_dir"], str(experiment_id)), history, done, step0, hi - lo,
+                        global_batch, rank)
     path = None
     if rank == 0:
         path = save_checkpoint(os.path.join(model_config["model_base_dir"], str(experiment_id),
@@ -181,9 +203,24 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
     return path, sep
 
 
-def validation_loss(model_config, sep, batches=4, seed=99):
+def _write_sep_loss(logdir, history, done, step0, local_batch, global_batch, rank):
+    """The epoch's sep_loss summaries from the device-side loss history and the per-step CUDA events `done`: step i's
+    wall time is the host time at the epoch's one wait for the device, less the device time from step i to the last."""
+    done[-1].synchronize()
+    t_last = time.time()
+    walls = [t_last - ev.elapsed_time(done[-1]) / 1e3 for ev in done]
+    losses = parallel.batch_loss_history(history, local_batch, global_batch).tolist()
+    if rank == 0:
+        with Summaries.EventFileWriter(logdir) as w:
+            for i, (loss, wall) in enumerate(zip(losses, walls)):
+                w.add_scalar("sep_loss", loss, step0 + i, wall)
+
+
+def validation_loss(model_config, sep, batches=4, seed=99, summaries=False, model_folder=None):
     """Running-mean loss over a fixed synthetic validation set (reference Test.test, Test.py:57-71): MSE on audio, or for
-    the spectrogram U-Net with raw_audio_loss=False the L1 loss on STFT magnitudes (Test.py:63-67)."""
+    the spectrogram U-Net with raw_audio_loss=False the L1 loss on STFT magnitudes (Test.py:63-67).  With `summaries`,
+    rank 0 writes it as Test.test does: a `test_loss` scalar at the separator's global step, in a new events file of
+    log_dir/<model_folder>."""
     import torch
     in_shape, out_shape = sep.get_padding(np.array([model_config["batch_size"], model_config["num_frames"], 0]))
     src = SyntheticBatches(model_config, in_shape, out_shape, seed=seed)
@@ -204,16 +241,22 @@ def validation_loss(model_config, sep, batches=4, seed=99):
         out = sep.get_output(mix, training=False, reuse=True)
         loss = sum(float(torch.mean((torch.from_numpy(b[k]).to(mix.device) - out[k]) ** 2)) for k in names) / len(names)
         tot += loss; n += 1
+    if summaries and parallel.world()[0] == 0:
+        if model_folder is None:
+            raise ValueError("validation_loss(summaries=True) needs the model_folder to write log_dir/<model_folder>")
+        Summaries.write_scalar(os.path.join(model_config["log_dir"], str(model_folder)), "test_loss", tot / n,
+                               sep.global_step)
     return tot / n
 
 
-def optimise(model_config, experiment_id, max_epochs=None, dataset=None):
+def optimise(model_config, experiment_id, max_epochs=None, dataset=None, summaries=False):
     """Early stopping + fine-tuning (reference optimise(), :123-150).  Without `dataset`: synthetic batches, validated by
     validation_loss, returns (best checkpoint, its validation loss).  With `dataset` (a Datasets.Dataset): trained on its
     train partition, validated by Test.test on "valid" at the current batch size, and, as the reference does, returns
-    (best checkpoint, Test.test of that checkpoint on "test")."""
+    (best checkpoint, Test.test of that checkpoint on "test").  `summaries` is passed to train and to the validation and
+    test losses: sep_loss and test_loss TensorBoard scalars in log_dir/<experiment_id>."""
     if dataset is not None:
-        return _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset)
+        return _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries)
     epoch, best_loss, model_path, best_model_path, sep = 0, 10000, None, None, None
     for i in range(2):
         worse_epochs = 0
@@ -225,8 +268,8 @@ def optimise(model_config, experiment_id, max_epochs=None, dataset=None):
             if max_epochs is not None and epoch >= max_epochs:
                 break
             print("EPOCH: " + str(epoch))
-            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep)
-            curr_loss = validation_loss(model_config, sep)
+            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, summaries=summaries)
+            curr_loss = validation_loss(model_config, sep, summaries=summaries, model_folder=str(experiment_id))
             epoch += 1
             if curr_loss < best_loss:
                 worse_epochs = 0
@@ -238,7 +281,7 @@ def optimise(model_config, experiment_id, max_epochs=None, dataset=None):
     return best_model_path, best_loss
 
 
-def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset):
+def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries):
     import Test
     rank, world = parallel.world()
     epoch, best_loss, model_path, best_model_path, best_step, sep = 0, 10000, None, None, None, None
@@ -252,10 +295,12 @@ def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset):
             if max_epochs is not None and epoch >= max_epochs:
                 break
             print("EPOCH: " + str(epoch))
-            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, dataset=dataset)
+            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, dataset=dataset,
+                                    summaries=summaries)
             # every rank evaluates the whole partition; the loss has the same bits on every rank, so they all take the
             # same early-stopping decision without a collective
-            curr_loss = Test.test(model_config, "valid", str(experiment_id), model_path, dataset=dataset, separator=sep)
+            curr_loss = Test.test(model_config, "valid", str(experiment_id), model_path, dataset=dataset, separator=sep,
+                                  summaries=summaries)
             epoch += 1
             if curr_loss < best_loss:
                 worse_epochs = 0
@@ -272,7 +317,7 @@ def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset):
         import torch.distributed as dist
         dist.barrier()
     print("TRAINING FINISHED - TESTING WITH BEST MODEL " + best_model_path)
-    test_loss = Test.test(model_config, "test", str(experiment_id), best_model_path, dataset=dataset)
+    test_loss = Test.test(model_config, "test", str(experiment_id), best_model_path, dataset=dataset, summaries=summaries)
     return best_model_path, test_loss
 
 
@@ -307,7 +352,7 @@ def run(cfg, max_epochs=None, dataset=None, ccmixter_xml=None, valid_tracks=25):
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
-    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs)
+    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, summaries=True)
     print("Supervised training finished! Saved model at " + str(sup_model_path) + ". Performance: " + str(sup_loss))
     return sup_model_path, sup_loss
 
@@ -331,7 +376,8 @@ def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks):
     in_shape, out_shape = probe.get_padding(np.array([model_config["batch_size"], model_config["num_frames"], 0]))
     ds = Datasets.load_musdb(model_config, int(in_shape[1]), int(out_shape[1]), model_config["musdb_path"], ccmixter_xml,
                              valid_tracks, device)
-    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, dataset=ds)
+    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, dataset=ds,
+                                        summaries=True)
     print("Supervised training finished! Saved model at " + str(sup_model_path) + ". Performance: " + str(sup_loss))
     Evaluate.produce_musdb_source_estimates(model_config, sup_model_path, model_config["musdb_path"],
                                             model_config["estimates_path"])

@@ -557,6 +557,7 @@ class Engine(object):
         import torch
         B = mix.shape[0]
         self._check_io(mix, targets=targets, out=out, flat=(params, grads))
+        assert loss.is_cuda and loss.device == mix.device and loss.dtype == torch.float32, "loss must be a float32 CUDA tensor"
         ws = self._workspace(B, True, mix.device)
         with torch.cuda.device(mix.device):
             check(lib.wun_forward_backward(self._h, params.data_ptr(), mix.data_ptr(), targets.data_ptr(), B,

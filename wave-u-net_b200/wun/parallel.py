@@ -36,6 +36,16 @@ def grad_scale_for(local_batch, global_batch):
     return float(local_batch) / float(global_batch)
 
 
+def batch_loss_history(history, local_batch, global_batch, group=None):
+    """Per-step mean losses of this rank's shard -> those of the whole batch, on every rank (in place): each rank weights
+    its history by B_r / B and ONE all-reduce (sum) adds the ranks' histories - one collective per epoch, none per step."""
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+        history.mul_(grad_scale_for(local_batch, global_batch))
+        dist.all_reduce(history, op=dist.ReduceOp.SUM, group=group)
+    return history
+
+
 def allreduce_gradients(flat_grads, group=None):
     """The single collective of a training step: in-place sum of the flat gradient buffer over all ranks."""
     import torch.distributed as dist
