@@ -342,6 +342,32 @@ int wun_spec_feed_batch(WunSpecHandle* h, const float* pool, int64_t total_frame
                         const int64_t* track_length, int64_t n_tracks, int64_t batch, int augmentation, uint64_t seed,
                         int64_t* step_state, float* mix_out, float* targets_out, int64_t* chosen, void* stream);
 
+/* --- FLAC decoding (csrc/kernels_flac.cu, DESIGN.md §4.10) -----------------------------------------
+ * The reference loads compressed audio through librosa 0.6 / audioread / ffmpeg (Utils.load); these decode FLAC streams on the
+ * device.  The host parses the metadata blocks and passes STREAMINFO's bits per sample (4..24), channels (1..8), sample rate
+ * and maximum block size (0: unknown); `buf` is the DEVICE copy of the frame area (everything after the metadata), `nbytes`
+ * long.  wun.read_flac (wun/flac.py) drives the two calls and chains the frames between them. */
+typedef struct {
+    int64_t offset;      /* byte offset of the frame in buf */
+    int64_t number;      /* the header's frame number (fixed block size) or first sample number (variable block size) */
+    int64_t end;         /* offset just past the frame's CRC-16, or a negative status (flac_frame.h: truncated, bad header,
+                            bad subframe, bad residual, CRC-16 mismatch) */
+    int32_t block_size;
+    int32_t variable;    /* the header's blocking-strategy bit */
+} WunFlacFrame;
+/* Every frame candidate: each byte offset with a sync code, a legal header agreeing with STREAMINFO and a matching CRC-8,
+ * parsed to its end.  Candidates go to `frames` (DEVICE, `capacity` records) in no particular order; *count (DEVICE uint64,
+ * zeroed by the call) receives how many there are, which may exceed `capacity` (then call again with more room). */
+int wun_flac_find_frames(const uint8_t* buf, int64_t nbytes, int32_t bps, int32_t channels, int32_t rate, int32_t max_block,
+                         WunFlacFrame* frames, int64_t capacity, uint64_t* count, void* stream);
+/* Decode the chained frames: frame j starts at byte offsets[j] and its samples go to rows first_samples[j] .. + block size
+ * of `out` (DEVICE int32 [total_samples][channels], samples at full depth, FLAC channel order).  status[j] (DEVICE int32)
+ * receives 0, or a negative status when the frame does not decode or does not fit the output; nothing is written outside the
+ * frame's own rows. */
+int wun_flac_decode_frames(const uint8_t* buf, int64_t nbytes, int32_t bps, int32_t channels, int32_t rate,
+                           int32_t max_block, const int64_t* offsets, const int64_t* first_samples, int64_t nframes,
+                           int32_t* out, int64_t total_samples, int32_t* status, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

@@ -9,14 +9,17 @@ input_path:
          librosa's kaiser_best, as the reference's predict() does (Evaluate.py:60-71) - and every estimate is written to
          <output_path or input_path>_<source>.wav as 32-bit float WAV at the input's rate (librosa.output.write_wav,
          Evaluate.py:193).
+  *.flac FLAC, 4 to 24 bits per sample, 1 to 8 channels, decoded on the GPU (wun.read_flac) and converted as the
+         reference's ffmpeg path loads it: each sample shifted to 16 bits (left for fewer bits, arithmetically right for
+         more) and divided by 32768.  Then as for WAV; estimates are still written as float WAV.
   *.npy  a float array [n_frames, n_channels] already at model_config["expected_sr"]; estimates are written to
          <output_path or input_path>_<source>.npy.
-Other audio formats (mp3 and friends need ffmpeg, Evaluate.py:172) are out of scope.
+Other audio formats (mp3 and friends, Evaluate.py:172) are out of scope.
 
 With references_path= and results_dir=<dir>, the predictions are also scored with BSS Eval v4 on the GPU
 (Evaluate.eval_track, the reference's museval.eval_mus_track at Evaluate.py:71) at the input's rate and written to
 <results_dir>/<input file name>.json, which Evaluate.compute_mean_metrics reads.  references_path is a directory of
-<source>.wav stems at the input's rate, or a .npz with one [n_frames, n_channels] array per source name.  Mono-model
+<source>.wav or <source>.flac stems at the input's rate, or a .npz with one [n_frames, n_channels] array per source name.  Mono-model
 estimates are tiled to the references' channel count (Evaluate.py:66-67).
 """
 import glob
@@ -43,6 +46,25 @@ def read_wav(path):
     return int(rate), np.ascontiguousarray(audio.reshape(audio.shape[0], -1))
 
 
+def read_flac(path):
+    """(rate, float32 [n_frames, n_channels]) of a FLAC file, as the reference's Utils.load gives it through librosa 0.6,
+    audioread and `ffmpeg -f s16le`: decoded on the GPU, STREAMINFO MD5 checked, then wun.flac.to_float."""
+    import wun
+    from wun import flac
+    rate, bps, samples = wun.read_flac(path)
+    return int(rate), flac.to_float(samples.cpu().numpy(), bps)
+
+
+def read_audio(path):
+    """read_wav for .wav, read_flac for .flac; anything else raises ValueError."""
+    ext = os.path.splitext(path)[1].lower()
+    if ext == ".wav":
+        return read_wav(path)
+    if ext == ".flac":
+        return read_flac(path)
+    raise ValueError("%s: only .wav and .flac audio can be read" % path)
+
+
 def write_wav(path, audio, rate):
     """32-bit float WAV of `audio` [n_frames, n_channels] at `rate`, as librosa.output.write_wav writes float32 audio."""
     audio = np.asarray(audio, np.float32)
@@ -50,14 +72,20 @@ def write_wav(path, audio, rate):
 
 
 def load_references(references_path, rate):
-    """name -> [n_frames, n_channels] from a directory of <source>.wav stems at `rate`, or from a .npz."""
+    """name -> [n_frames, n_channels] from a directory of <source>.wav / <source>.flac stems at `rate`, or from a .npz.
+    One source given in both formats raises ValueError."""
     if os.path.isdir(references_path):
         refs = {}
-        for path in sorted(glob.glob(os.path.join(references_path, "*.wav"))):
-            sr, audio = read_wav(path)
+        paths = sorted(glob.glob(os.path.join(references_path, "*.wav")) + glob.glob(os.path.join(references_path, "*.flac")))
+        names = [os.path.splitext(os.path.basename(p))[0] for p in paths]
+        twice = sorted(set(n for n in names if names.count(n) > 1))
+        if twice:
+            raise ValueError("%s: sources %s are given both as .wav and as .flac" % (references_path, twice))
+        for name, path in zip(names, paths):
+            sr, audio = read_audio(path)
             if sr != rate:
                 raise ValueError("%s is at %d Hz, the mixture at %d Hz" % (path, sr, rate))
-            refs[os.path.splitext(os.path.basename(path))[0]] = audio
+            refs[name] = audio
         return refs
     with np.load(references_path) as z:
         return {name: z[name] for name in z.files}
@@ -68,8 +96,8 @@ def main(cfg, model_path, input_path, output_path=None, references_path=None, re
     base = output_path if output_path is not None else input_path
     track = os.path.splitext(os.path.basename(input_path))[0]
     score = references_path is not None and results_dir is not None
-    if input_path.lower().endswith(".wav"):
-        rate, mix = read_wav(input_path)
+    if input_path.lower().endswith((".wav", ".flac")):
+        rate, mix = read_audio(input_path)
         refs = load_references(references_path, rate) if score else None
         preds = Evaluate.predict(model_config, Evaluate.load_separator(model_config, model_path), mix, rate,
                                  references=refs, results_dir=results_dir, track_name=track)
@@ -89,15 +117,15 @@ def main(cfg, model_path, input_path, output_path=None, references_path=None, re
     return preds
 
 
-# the reference's defaults (Predict.py:9-13); its default input is an mp3 - decoding mp3 needs ffmpeg, so input_path has to
-# be given
+# the reference's defaults (Predict.py:9-13); its default input is an mp3, which is not read here, so input_path has to be
+# given
 DEFAULT_MODEL_PATH = os.path.join("checkpoints", "full_44KHz", "full_44KHz-236118")
 
 
 if __name__ == "__main__":
     cfg, extras = Config.parse_command_line(sys.argv[1:])
     if "input_path" not in extras:
-        raise SystemExit("Predict.py: input_path=<song.wav or mix.npy> is required (the reference's default, an mp3 of "
-                         "audio_examples/, needs ffmpeg)\n" + __doc__)
+        raise SystemExit("Predict.py: input_path=<song.wav, song.flac or mix.npy> is required (the reference's default, an "
+                         "mp3 of audio_examples/, is not a format read here)\n" + __doc__)
     main(cfg, extras.get("model_path", DEFAULT_MODEL_PATH), extras["input_path"], extras.get("output_path"),
          extras.get("references_path"), extras.get("results_dir"))

@@ -27,6 +27,7 @@ SYMBOLS = [
     "wun_spec_gather_windows", "wun_spec_scatter_windows",
     "wun_spec_train_workspace_bytes", "wun_spec_train_flops", "wun_spec_forward_backward", "wun_spec_adam_step_device",
     "wun_spec_feed_batch", "wun_spec_debug_train_level",
+    "wun_flac_find_frames", "wun_flac_decode_frames",
 ]
 
 
@@ -49,6 +50,11 @@ class WunSpecConfig(ctypes.Structure):
 class WunSpecParamInfo(ctypes.Structure):
     _fields_ = [("name", ctypes.c_char * 64), ("ndim", ctypes.c_int32), ("shape", ctypes.c_int32 * 4),
                 ("offset", ctypes.c_int64), ("numel", ctypes.c_int64)]
+
+
+class WunFlacFrame(ctypes.Structure):
+    _fields_ = [("offset", ctypes.c_int64), ("number", ctypes.c_int64), ("end", ctypes.c_int64),
+                ("block_size", ctypes.c_int32), ("variable", ctypes.c_int32)]
 
 
 class WunError(RuntimeError):
@@ -112,6 +118,10 @@ def _load():
         lib.wun_resample_frames.argtypes = [I64, I64, I64]
         lib.wun_resample_frames.restype = I64
         lib.wun_resample.argtypes = [VP, I64, I64, I64, I64, VP, VP, I64, I64, VP, I64, VP]
+    if hasattr(lib, "wun_flac_find_frames"):    # likewise the FLAC decoder
+        I32 = ctypes.c_int32
+        lib.wun_flac_find_frames.argtypes = [VP, I64, I32, I32, I32, I32, VP, I64, VP, VP]
+        lib.wun_flac_decode_frames.argtypes = [VP, I64, I32, I32, I32, I32, VP, VP, I64, VP, I64, VP, VP]
     if hasattr(lib, "wun_snippet_batch"):   # likewise the validation-loss kernels
         lib.wun_snippet_batch.argtypes = [VP, I64, I64, I64, I64, I64, VP, I64, I64, VP, VP, VP, VP]
         lib.wun_eval_batch_loss.argtypes = [VP, VP, I64, I64, VP, VP, VP, I64, VP]
@@ -281,6 +291,59 @@ def resample(x, sr_in, sr_out):
     if rc != WUN_OK:
         raise WunError(rc, "wun_resample failed")
     return y
+
+
+def read_flac(source, verify_md5=True, device="cuda"):
+    """(rate, bps, samples) of a FLAC stream decoded on the GPU (include/wun.h wun_flac_find_frames / wun_flac_decode_frames,
+    DESIGN.md §4.10): `source` a path or bytes; `samples` an int32 CUDA tensor [n, channels] at full depth in FLAC's channel
+    order.  With verify_md5 (the default) the samples are checked against STREAMINFO's MD5 unless that is all zero (not
+    computed).  A stream that is not FLAC, is not 4-24 bits per sample, or whose frames do not chain raises ValueError."""
+    import numpy as np
+    import torch
+    from . import flac
+    if isinstance(source, (bytes, bytearray, memoryview)):
+        data = bytes(source)
+    else:
+        with open(source, "rb") as f:
+            data = f.read()
+    info = flac.parse_stream(data)
+    area = data[info.frames_start:]
+    nbytes = len(area)
+    dev = torch.device(device)
+    if nbytes == 0:
+        if info.total_samples:
+            raise ValueError("FLAC: STREAMINFO says %d samples, the stream has no frames" % info.total_samples)
+        return info.rate, info.bps, torch.zeros((0, info.channels), dtype=torch.int32, device=dev)
+    si = (info.bps, info.channels, info.rate, info.max_block)
+    buf = torch.frombuffer(bytearray(area), dtype=torch.uint8).to(dev)
+    count = torch.zeros(1, dtype=torch.int64, device=dev)
+    # a frame is at least ~10 bytes; most streams have far fewer candidates than this, and a second pass covers the rest
+    capacity = nbytes // 256 + 1024
+    with torch.cuda.device(dev):
+        stream = Engine._stream(dev)
+        while True:
+            rec = torch.empty((capacity, ctypes.sizeof(WunFlacFrame)), dtype=torch.uint8, device=dev)
+            check(lib.wun_flac_find_frames(buf.data_ptr(), nbytes, *si, rec.data_ptr(), capacity, count.data_ptr(), stream))
+            found = int(count.item())
+            if found <= capacity:
+                break
+            capacity = found
+        dtype = np.dtype([(n, np.int64 if t is ctypes.c_int64 else np.int32) for n, t in WunFlacFrame._fields_])
+        frames = rec[:found].cpu().numpy().view(dtype).reshape(-1)
+        offsets, firsts, n = flac.chain_frames(frames, nbytes, info)
+        out = torch.empty((n, info.channels), dtype=torch.int32, device=dev)
+        status = torch.zeros(len(offsets), dtype=torch.int32, device=dev)
+        off_d, first_d = torch.from_numpy(offsets).to(dev), torch.from_numpy(firsts).to(dev)
+        check(lib.wun_flac_decode_frames(buf.data_ptr(), nbytes, *si, off_d.data_ptr(), first_d.data_ptr(), len(offsets),
+                                         out.data_ptr(), n, status.data_ptr(), stream))
+        bad = torch.nonzero(status).reshape(-1).cpu().numpy()
+    if bad.size:
+        j = int(bad[0])
+        raise ValueError("FLAC frame %d at byte offset %d: %s" % (j, info.frames_start + int(offsets[j]),
+                                                                  flac.STATUS.get(int(status[j]), "invalid")))
+    if verify_md5 and info.md5 != bytes(16) and flac.md5_of(out, info.bps) != info.md5:
+        raise ValueError("FLAC: the decoded samples do not match the stream's MD5")
+    return info.rate, info.bps, out
 
 
 EVAL_LOSS_CTAS = 264        # include/wun.h WUN_EVAL_LOSS_CTAS
