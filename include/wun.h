@@ -328,6 +328,34 @@ double wun_spec_train_flops(const WunSpecHandle* h, int64_t batch);
 int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
                               int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
                               void* workspace, int64_t workspace_bytes, void* stream);
+/* Data parallel: one rank's shard of a batch of global_batch examples.  The step on every rank is the single-device step on
+ * the whole batch, up to the order of floating-point sums:
+ *   batch norm: each layer's per-channel fp64 sums of this shard ((z, z^2) forward, (dy, dy * xhat) backward) are gathered
+ *     from every rank into gathered [world][C][2] by `gather`, then added in rank order from 0.0 over global_batch * H * W
+ *     rows, so every rank computes the same statistics and moving averages without a broadcast.  beta's gradient stays
+ *     this shard's sum of dy, as every other gradient does;
+ *   the loss gradient is scaled by 1 / global_batch, so the SUM of the ranks' gradients is the whole batch's; the loss
+ *     written is this shard's mean;
+ *   dropout hashes element i of the shard as element sample_offset * (elements per example) + i of the batch, so a
+ *     shard's masks are those of its examples in the single-device step.
+ * `gather(ctx, local, gathered, count, stream)` must put every rank's `count` doubles at `local` into gathered[rank *
+ * count ...] and only enqueue work on `stream` (so that a step stays capturable in a CUDA graph); it returns 0 on success.
+ * `local` is overwritten by later work on `stream`.  `gathered`: DEVICE, at least world * 16 * num_initial_filters *
+ * 2^(num_layers - 1) bytes (gathered_bytes).  With world = 1 the gather may be null; then the call is
+ * wun_spec_forward_backward bit for bit.  About 2 gathers per batch-norm layer per source per step (4 L - 2 for each of the
+ * K = 2 sources), each at most 16 * C bytes per rank. */
+typedef int (*WunSpecGatherFn)(void* ctx, const double* local, double* gathered, int64_t count, void* stream);
+typedef struct WunSpecShard {
+    int32_t rank, world;
+    int64_t global_batch, sample_offset;
+    double* gathered;
+    int64_t gathered_bytes;
+    WunSpecGatherFn gather;
+    void* ctx;
+} WunSpecShard;
+int wun_spec_forward_backward_dp(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
+                                 int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
+                                 void* workspace, int64_t workspace_bytes, void* stream, const WunSpecShard* shard);
 /* tf.train.AdamOptimizer step on the trainable variables (kernels, biases, betas), as wun_adam_step_device: state = DEVICE
  * float32[3] {beta1_power, beta2_power, step}.  The moving statistics have zero gradients and zero slots, so they keep their
  * bits; only the trainables' slots are checkpointed. */
@@ -337,6 +365,11 @@ int wun_spec_adam_step_device(WunSpecHandle* h, float* params, const float* grad
  * output; the bottom level has only the former) lies in the training workspace at `batch`.  After wun_spec_forward_backward
  * it holds the last source's activations, whose signs are the slopes the backward used. */
 int wun_spec_debug_train_level(const WunSpecHandle* h, int64_t batch, int level, int64_t* offset_bytes, int64_t* elems);
+/* Tests: where a buffer of the training workspace at `batch` lies; after wun_spec_forward_backward it holds the last
+ * source's.  what = 0: the keep mask (uint8 [B, H, W, C] like the level) of dropped level `index`; 1 / 2: the batch
+ * statistics (float32 [C][2] mean, rstd) of down / up layer `index`. */
+int wun_spec_debug_train_buffer(const WunSpecHandle* h, int64_t batch, int what, int index, int64_t* offset_bytes,
+                                int64_t* elems);
 /* wun_feed_batch for this handle: T_in = T_out = T, one channel, K sources */
 int wun_spec_feed_batch(WunSpecHandle* h, const float* pool, int64_t total_frames, const int64_t* track_offset,
                         const int64_t* track_length, int64_t n_tracks, int64_t batch, int augmentation, uint64_t seed,

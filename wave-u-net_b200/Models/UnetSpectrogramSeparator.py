@@ -17,6 +17,10 @@ as with UnetAudioSeparator: training-mode batch norm (batch statistics, moving a
 the first three concatenations of the up path, the U7 (audio MSE) or U7a (L1 on magnitudes, raw_audio_loss=False) loss,
 every trainable variable's gradient and tf.train.AdamOptimizer on kernels, biases and betas.  A standalone
 get_output(training=True) graph does not exist and raises NotImplementedError.
+
+Data-parallel training is opt-in, like torch's SyncBatchNorm: loss_and_gradients(..., sync_batch_norm=shard) with a
+wun.parallel.BatchStatsGather runs this rank's shard with the whole batch's batch-norm statistics, dropout masks and 1/B
+loss scaling, so that after the gradient all-reduce every rank holds the single-device step's gradients.
 """
 from collections import OrderedDict
 import math
@@ -174,14 +178,25 @@ class UnetSpectrogramSeparator:
             # one dropout step per optimiser step: a resumed run continues the masks where the checkpoint left them
             self._dropout_step = torch.full((1,), self._step0, dtype=torch.int64, device=dev)
 
-    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0, loss=None):
+    def loss_and_gradients(self, mix, targets, reuse=True, grad_scale=1.0, loss=None, sync_batch_norm=None):
         """separator_loss (Training.py:50-63) of get_output(mix, training=True, not raw_audio_loss) and d loss / d variables;
         the batch-norm moving statistics in self.params take their update.  targets: [K, B, T, 1] tensor or dict.
         Returns the device float64 loss, written into `loss` (a float64 CUDA tensor, e.g. one slot of a per-step history)
-        when given; the gradients land in self.grads (flat, 0 for the moving statistics)."""
+        when given; the gradients land in self.grads (flat, 0 for the moving statistics).
+        sync_batch_norm (a wun.parallel.BatchStatsGather): mix and targets are this rank's shard of the batch; batch norm
+        uses the whole batch's statistics and the gradients are this shard's part of the whole batch's (grad_scale, if
+        given, must be the shard's local_batch / global_batch), to be summed over the ranks.  The loss is the shard's mean."""
         import torch
-        if grad_scale != 1.0:
-            raise ValueError("the spectrogram U-Net trains on one GPU: batch statistics of a shard would change the model")
+        if sync_batch_norm is None and grad_scale != 1.0:
+            raise ValueError("the spectrogram U-Net trains on one GPU unless sync_batch_norm is given: batch statistics of "
+                             "a shard would change the model")
+        if sync_batch_norm is not None:
+            part = float(sync_batch_norm.local_batch) / float(sync_batch_norm.global_batch)
+            if grad_scale != 1.0 and abs(grad_scale - part) > 1e-12:
+                raise ValueError("grad_scale %r: a synchronised shard's gradients are scaled by local_batch / global_batch "
+                                 "= %r" % (grad_scale, part))
+            if int(mix.shape[0]) != sync_batch_norm.local_batch:
+                raise ValueError("the shard holds %d examples, mix %d" % (sync_batch_norm.local_batch, int(mix.shape[0])))
         if isinstance(targets, dict):
             targets = torch.stack([targets[n] for n in self.source_names])
         eng = self._engine_for(int(mix.shape[1]))
@@ -189,7 +204,7 @@ class UnetSpectrogramSeparator:
         self._ensure_training_state()
         loss = self._loss if loss is None else loss
         eng.forward_backward(self.params, mix.contiguous(), targets.contiguous(), self.grads, loss,
-                             self.raw_audio_loss, self.seed, self._dropout_step)
+                             self.raw_audio_loss, self.seed, self._dropout_step, shard=sync_batch_norm)
         return loss
 
     def adam_step(self, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8):

@@ -27,8 +27,13 @@ which stages the MUSDB18 WAV dataset on the device (Datasets.py), validates with
 test loss and writes its estimates and BSS Eval JSONs (Evaluate.produce_musdb_source_estimates), as the reference does.
 
 network="unet_spectrogram" (presets cfg.unet_spectrogram / U7 and cfg.unet_spectrogram_l1 / U7a) trains the spectrogram
-U-Net the same way on one GPU (Models/UnetSpectrogramSeparator.py); its batch statistics are those of the whole batch, so a
-data-parallel run, whose ranks would each normalise with their own shard's statistics, is refused.
+U-Net the same way (Models/UnetSpectrogramSeparator.py).  Its batch norm normalises with the statistics of the whole batch,
+so data parallelism is opt-in, as torch's SyncBatchNorm is:
+
+    torchrun --nproc-per-node 8 Training.py with cfg.unet_spectrogram sync_batch_norm=1
+
+gathers every batch-norm layer's per-channel sums from all ranks at every step, so that each step is the one-GPU step on the
+whole batch up to the order of floating-point sums.  Without sync_batch_norm a data-parallel run of it is refused.
 """
 import os
 import sys
@@ -124,22 +129,25 @@ def _device_feeder(model_config, sep, eng, device, rank, world, local_batch, dat
 
 
 def train(model_config, experiment_id, load_model=None, batch_source=None, sep=None, device=None, log_every=100, feeder=None,
-          dataset=None, summaries=False):
+          dataset=None, summaries=False, sync_batch_norm=False):
     """One epoch (reference train(), :24-121).  Returns (checkpoint path, separator).
     Data: `batch_source` (an iterator of host numpy batches, e.g. SyntheticBatches) if given; otherwise, on a CUDA device,
     the device-side feeder (`feeder="device"`, the default there); `feeder="host"` forces the numpy generator.  With
     `dataset` (a Datasets.Dataset) the device-side feeder draws from its train partition.
     With `summaries`, rank 0 writes a new TensorBoard events file into log_dir/<experiment_id> (:80-81,88,106): one
     `sep_loss` scalar per step, the whole batch's loss of the forward pass before that step's update, at the global step
-    before it.  The losses stay on the device until the epoch ends, so logging adds no host synchronisation per step."""
+    before it.  The losses stay on the device until the epoch ends, so logging adds no host synchronisation per step.
+    With `sync_batch_norm`, the spectrogram U-Net trains data parallel: every rank's batch norm uses the whole batch's
+    statistics (wun.parallel.BatchStatsGather).  The Wave-U-Net has no batch norm and ignores it."""
     import torch
     rank, world = parallel.world()
     if device is None:
         device = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
     cls = separator_class(model_config)                             # reference :30-33
-    if cls is UnetSpectrogramSeparator and world > 1:
-        raise ValueError("the spectrogram U-Net trains on one GPU: with %d ranks every rank would normalise with its own "
-                         "shard's batch statistics, which changes the model" % world)
+    spectrogram = cls is UnetSpectrogramSeparator
+    if spectrogram and world > 1 and not sync_batch_norm:
+        raise ValueError("the spectrogram U-Net trains on one GPU unless sync_batch_norm=True: with %d ranks every rank would "
+                         "normalise with its own shard's batch statistics, which changes the model" % world)
     if sep is None:
         sep = cls(model_config)
     disc_input_shape = [model_config["batch_size"], model_config["num_frames"], 0]
@@ -154,6 +162,7 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
     names = model_config["source_names"]
     lr = model_config["init_sup_sep_lr"]
     global_batch = int(in_shape[0])
+    shard = parallel.BatchStatsGather(global_batch) if (spectrogram and world > 1) else None
     dev_feeder = None
     if batch_source is None and feeder != "host" and device.type == "cuda":
         lo, hi = parallel.shard_range(global_batch, rank, world)
@@ -171,7 +180,8 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
         done = [torch.cuda.Event(enable_timing=True) for _ in range(model_config["epoch_it"])]
     running, t0 = 0.0, time.time()
     # N > 1: the gradient all-reduce runs bucketed on a communication stream while backward still computes
-    overlap = parallel.BucketedAllReduce(eng, sep.grads) if (world > 1 and sep.grads.is_cuda) else None
+    # (the spectrogram engine reports no gradient buckets: its gradients are all-reduced after the call)
+    overlap = parallel.BucketedAllReduce(eng, sep.grads) if (world > 1 and sep.grads.is_cuda and not spectrogram) else None
     for it in range(model_config["epoch_it"]):                      # :103
         if dev_feeder is not None:
             mix_l, tg_l = dev_feeder.next_batch()                   # this rank's shard, built on the device
@@ -179,8 +189,9 @@ def train(model_config, experiment_id, load_model=None, batch_source=None, sep=N
             mix, tg = _to_device(next(batch_source), names, device)
             mix_l = parallel.shard_batch(mix, rank, world).contiguous()
             tg_l = parallel.shard_batch(tg, rank, world, dim=1).contiguous()
+        sync = {} if shard is None else {"sync_batch_norm": shard}
         loss = sep.loss_and_gradients(mix_l, tg_l, grad_scale=parallel.grad_scale_for(mix_l.shape[0], global_batch),
-                                      loss=None if history is None else history[it:it + 1])
+                                      loss=None if history is None else history[it:it + 1], **sync)
         if overlap is not None:
             overlap.run()
         else:
@@ -249,14 +260,15 @@ def validation_loss(model_config, sep, batches=4, seed=99, summaries=False, mode
     return tot / n
 
 
-def optimise(model_config, experiment_id, max_epochs=None, dataset=None, summaries=False):
+def optimise(model_config, experiment_id, max_epochs=None, dataset=None, summaries=False, sync_batch_norm=False):
     """Early stopping + fine-tuning (reference optimise(), :123-150).  Without `dataset`: synthetic batches, validated by
     validation_loss, returns (best checkpoint, its validation loss).  With `dataset` (a Datasets.Dataset): trained on its
     train partition, validated by Test.test on "valid" at the current batch size, and, as the reference does, returns
     (best checkpoint, Test.test of that checkpoint on "test").  `summaries` is passed to train and to the validation and
-    test losses: sep_loss and test_loss TensorBoard scalars in log_dir/<experiment_id>."""
+    test losses: sep_loss and test_loss TensorBoard scalars in log_dir/<experiment_id>.  `sync_batch_norm` is passed to
+    train."""
     if dataset is not None:
-        return _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries)
+        return _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries, sync_batch_norm)
     epoch, best_loss, model_path, best_model_path, sep = 0, 10000, None, None, None
     for i in range(2):
         worse_epochs = 0
@@ -268,7 +280,8 @@ def optimise(model_config, experiment_id, max_epochs=None, dataset=None, summari
             if max_epochs is not None and epoch >= max_epochs:
                 break
             print("EPOCH: " + str(epoch))
-            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, summaries=summaries)
+            model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, summaries=summaries,
+                                    sync_batch_norm=sync_batch_norm)
             curr_loss = validation_loss(model_config, sep, summaries=summaries, model_folder=str(experiment_id))
             epoch += 1
             if curr_loss < best_loss:
@@ -281,7 +294,7 @@ def optimise(model_config, experiment_id, max_epochs=None, dataset=None, summari
     return best_model_path, best_loss
 
 
-def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries):
+def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summaries, sync_batch_norm):
     import Test
     rank, world = parallel.world()
     epoch, best_loss, model_path, best_model_path, best_step, sep = 0, 10000, None, None, None, None
@@ -296,7 +309,7 @@ def _optimise_on_dataset(model_config, experiment_id, max_epochs, dataset, summa
                 break
             print("EPOCH: " + str(epoch))
             model_path, sep = train(model_config, experiment_id, load_model=model_path, sep=sep, dataset=dataset,
-                                    summaries=summaries)
+                                    summaries=summaries, sync_batch_norm=sync_batch_norm)
             # every rank evaluates the whole partition; the loss has the same bits on every rank, so they all take the
             # same early-stopping decision without a collective
             curr_loss = Test.test(model_config, "valid", str(experiment_id), model_path, dataset=dataset, separator=sep,
@@ -337,12 +350,13 @@ def dataset_options(extras):
     return opts
 
 
-def run(cfg, max_epochs=None, dataset=None, ccmixter_xml=None, valid_tracks=25):
+def run(cfg, max_epochs=None, dataset=None, ccmixter_xml=None, valid_tracks=25, sync_batch_norm=False):
     """The reference's run() (:152-166).  With dataset="musdb" the MUSDB18 WAV dataset at model_config["musdb_path"] (and
     CCMixter's tracks for the voice task, from `ccmixter_xml`) is staged on the device once, trained and validated on,
-    and the best checkpoint's estimates and BSS Eval JSONs are written under model_config["estimates_path"]."""
+    and the best checkpoint's estimates and BSS Eval JSONs are written under model_config["estimates_path"].
+    `sync_batch_norm` lets the spectrogram U-Net train data parallel (train)."""
     if dataset is not None:
-        return _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks)
+        return _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks, sync_batch_norm)
     model_config = cfg["model_config"]
     print("SCRIPT START")
     for d in [model_config["model_base_dir"], model_config["log_dir"]]:
@@ -352,12 +366,13 @@ def run(cfg, max_epochs=None, dataset=None, ccmixter_xml=None, valid_tracks=25):
         import torch.distributed as dist
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", "0")))
         dist.init_process_group("nccl")
-    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, summaries=True)
+    sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, summaries=True,
+                                        sync_batch_norm=sync_batch_norm)
     print("Supervised training finished! Saved model at " + str(sup_model_path) + ". Performance: " + str(sup_loss))
     return sup_model_path, sup_loss
 
 
-def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks):
+def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks, sync_batch_norm):
     import torch
     import Datasets
     import Evaluate
@@ -377,13 +392,20 @@ def _run_on_dataset(cfg, max_epochs, dataset, ccmixter_xml, valid_tracks):
     ds = Datasets.load_musdb(model_config, int(in_shape[1]), int(out_shape[1]), model_config["musdb_path"], ccmixter_xml,
                              valid_tracks, device)
     sup_model_path, sup_loss = optimise(model_config, cfg["experiment_id"], max_epochs=max_epochs, dataset=ds,
-                                        summaries=True)
+                                        summaries=True, sync_batch_norm=sync_batch_norm)
     print("Supervised training finished! Saved model at " + str(sup_model_path) + ". Performance: " + str(sup_loss))
     Evaluate.produce_musdb_source_estimates(model_config, sup_model_path, model_config["musdb_path"],
                                             model_config["estimates_path"])
     return sup_model_path, sup_loss
 
 
+def main(argv):
+    """The command line: sacred-style `with cfg.<preset> ...` (Config.parse_command_line) and the top-level extras
+    max_epochs=N, sync_batch_norm=1 and the dataset ones (dataset_options)."""
+    cfg, extras = Config.parse_command_line(argv)
+    return run(cfg, max_epochs=extras.get("max_epochs"), sync_batch_norm=bool(extras.get("sync_batch_norm", False)),
+               **dataset_options(extras))
+
+
 if __name__ == "__main__":
-    cfg, extras = Config.parse_command_line(sys.argv[1:])
-    run(cfg, max_epochs=extras.get("max_epochs"), **dataset_options(extras))
+    main(sys.argv[1:])

@@ -175,17 +175,24 @@ struct SpecChanSum {
     float2* stat; float2* coef; float* out;
     float* moving_mean; float* moving_var;
     double2* part;                                                // [spec_chan_partials(N)][C]
+    double2* local;                                               // modes 0, 1: this call's [C] (sum 1, sum 2)
+    const double2* gathered;                                      // modes 0, 1: [world][C], every rank's local
+    double n;                                                     // modes 0, 1: rows over all ranks
 };
 int spec_chan_partials(long long N);
+// sums over this call's N rows: mode 2 writes out, modes 0 and 1 write local
 void launch_spec_chan_sum(const SpecChanSum& S, cudaStream_t stream);
+// modes 0 and 1, after the ranks' local sums are gathered
+void launch_spec_chan_finish(const SpecChanSum& S, int world, cudaStream_t stream);
 // (z - mean) * rstd + beta, then max(neg_slope * v, v), into y [N][y_pitch]
 void launch_spec_bn_apply(const float* z, long long N, int C, const float2* stat, const float* beta, float neg_slope,
                           float* y, int y_pitch, cudaStream_t stream);
 // in place: z [N][C] -> dz = rstd * (dy - coef.x - xhat * coef.y)
 void launch_spec_bn_backward(float* z, long long N, int C, const float* g, const float* a, int pitch, float neg_slope,
                              const float2* stat, const float2* coef, cudaStream_t stream);
-void launch_spec_dropout(uint8_t* keep, long long n, unsigned long long seed, const long long* step_state, int source,
-                         int level, cudaStream_t stream);
+// keep[i] is the keep bit of element first + i
+void launch_spec_dropout(uint8_t* keep, long long n, long long first, unsigned long long seed, const long long* step_state,
+                         int source, int level, cudaStream_t stream);
 // mask [frames][512]: logits in, sigmoid out; out = mask * X (complex [frames][513]) or mask * |X| with magnitude
 void launch_spec_mask_apply(float* mask, long long frames, const float* X, float* out, int magnitude, cudaStream_t stream);
 struct SpecMaskBwd {

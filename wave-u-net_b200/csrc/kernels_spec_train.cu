@@ -10,11 +10,13 @@
 //                              the output (the skip gradient's second part)
 //   spec_chan_sum_kernel       per-channel fp64 sums over the rows of an [N][C] tensor, per CTA into partials:
 //                              (z, z^2) for the batch statistics, (dy, dy * xhat) for the batch-norm backward, dz for a bias
-//   spec_chan_finish_kernel    the partials summed in a fixed order per channel, then: batch mean / rstd and the moving-average
-//                              update, or beta's gradient and the backward's two means, or a conv bias gradient
+//   spec_chan_local_kernel     the partials summed in a fixed order per channel: a conv bias gradient, or the call's own sums
+//   spec_chan_finish_kernel    the ranks' gathered sums added in rank order, then: batch mean / rstd and the moving-average
+//                              update, or beta's gradient and the backward's two means
 //   spec_bn_apply_kernel       (z - mean) * rstd + beta, LeakyReLU(0.2) / ReLU, into the concatenation buffer
 //   spec_bn_backward_kernel    dz = rstd * (dy - mean(dy) - xhat * mean(dy * xhat)), dy = g * activation slope; in place over z
-//   spec_dropout_kernel        keep masks of tf.layers.dropout(rate 0.5) from a counter-based hash (spec_dropout_keep)
+//   spec_dropout_kernel        keep masks of tf.layers.dropout(rate 0.5) from a counter-based hash (spec_dropout_keep) of
+//                              the element's index in the whole batch
 //   spec_mask_apply_kernel     sigmoid of the mask conv, kept for the backward, times X (complex) or |X|, bin 512 = 0.5
 //   spec_mask_backward_kernel  d loss / d mask-logit: U7 through the adjoint of the inverse STFT (a windowed forward real DFT of
 //                              the frame-gathered audio gradient), U7a through the L1 magnitude loss; then sigmoid'
@@ -147,7 +149,8 @@ __global__ void __launch_bounds__(256) spec_chan_sum_kernel(const SpecChanSum S)
     }
 }
 
-__global__ void spec_chan_finish_kernel(const SpecChanSum S, int P) {
+// The partials summed in a fixed order per channel: a conv bias gradient (mode 2), or this call's (sum 1, sum 2) into local[c].
+__global__ void spec_chan_local_kernel(const SpecChanSum S, int P) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= S.C) return;
     double t1 = 0.0, t2 = 0.0;
@@ -156,7 +159,22 @@ __global__ void spec_chan_finish_kernel(const SpecChanSum S, int P) {
         t1 += v.x;
         t2 += v.y;
     }
-    const double n = (double)S.N;
+    if (S.mode == 2) S.out[c] = (float)t1;
+    else S.local[c] = make_double2(t1, t2);
+}
+
+// The ranks' sums gathered[r][c] added in rank order from 0.0 over n = S.n rows (the whole batch's); one rank gives the
+// single-device arithmetic bit for bit, as 0.0 + t = t.
+__global__ void spec_chan_finish_kernel(const SpecChanSum S, int world) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= S.C) return;
+    double t1 = 0.0, t2 = 0.0;
+    for (int r = 0; r < world; ++r) {
+        const double2 v = S.gathered[(long long)r * S.C + c];
+        t1 += v.x;
+        t2 += v.y;
+    }
+    const double n = S.n;
     if (S.mode == 0) {
         const double mean = t1 / n;
         const double var = fmax(t2 / n - mean * mean, 0.0);                     // biased: normalises the batch
@@ -165,11 +183,10 @@ __global__ void spec_chan_finish_kernel(const SpecChanSum S, int P) {
         const float bm = (float)mean, bv = (float)(var * n / fmax(n - 1.0, 1.0));
         S.moving_mean[c] = __fsub_rn(S.moving_mean[c], __fmul_rn(__fsub_rn(S.moving_mean[c], bm), kDecayComplement));
         S.moving_var[c] = __fsub_rn(S.moving_var[c], __fmul_rn(__fsub_rn(S.moving_var[c], bv), kDecayComplement));
-    } else if (S.mode == 1) {
-        S.out[c] = (float)t1;                                                    // d beta = sum dy
-        S.coef[c] = make_float2((float)(t1 / n), (float)(t2 / n));
     } else {
-        S.out[c] = (float)t1;
+        // d beta = this call's own sum dy: the gradient all-reduce after a data-parallel step adds the ranks'
+        S.out[c] = (float)S.local[c].x;
+        S.coef[c] = make_float2((float)(t1 / n), (float)(t2 / n));
     }
 }
 
@@ -200,11 +217,12 @@ __global__ void __launch_bounds__(256) spec_bn_backward_kernel(float* __restrict
     }
 }
 
-__global__ void __launch_bounds__(256) spec_dropout_kernel(uint8_t* __restrict__ keep, long long n, unsigned long long seed,
-                                                           const long long* __restrict__ step_state, int source, int level) {
+__global__ void __launch_bounds__(256) spec_dropout_kernel(uint8_t* __restrict__ keep, long long n, long long first,
+                                                           unsigned long long seed, const long long* __restrict__ step_state,
+                                                           int source, int level) {
     const uint64_t step = (uint64_t)step_state[0];
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-        keep[i] = (uint8_t)spec_dropout_keep(seed, step, source, level, (uint64_t)i);
+        keep[i] = (uint8_t)spec_dropout_keep(seed, step, source, level, (uint64_t)(first + i));
 }
 
 // One thread per (example, frame, bin < 512); the thread of bin 0 also writes bin 512 with the constant mask 0.5.
@@ -362,7 +380,11 @@ int spec_chan_partials(long long N) {
 void launch_spec_chan_sum(const SpecChanSum& S, cudaStream_t stream) {
     const int P = spec_chan_partials(S.N);
     spec_chan_sum_kernel<<<dim3((unsigned)((S.C + 31) / 32), (unsigned)P), dim3(32, kRedRows), 0, stream>>>(S);
-    spec_chan_finish_kernel<<<blocks_for(S.C, 128), 128, 0, stream>>>(S, P);
+    spec_chan_local_kernel<<<blocks_for(S.C, 128), 128, 0, stream>>>(S, P);
+}
+
+void launch_spec_chan_finish(const SpecChanSum& S, int world, cudaStream_t stream) {
+    spec_chan_finish_kernel<<<blocks_for(S.C, 128), 128, 0, stream>>>(S, world);
 }
 
 void launch_spec_bn_apply(const float* z, long long N, int C, const float2* stat, const float* beta, float neg_slope,
@@ -375,9 +397,9 @@ void launch_spec_bn_backward(float* z, long long N, int C, const float* g, const
     spec_bn_backward_kernel<<<grid_stride_blocks(N * C), 256, 0, stream>>>(z, N, C, g, a, pitch, neg_slope, stat, coef);
 }
 
-void launch_spec_dropout(uint8_t* keep, long long n, unsigned long long seed, const long long* step_state, int source,
-                         int level, cudaStream_t stream) {
-    spec_dropout_kernel<<<grid_stride_blocks(n), 256, 0, stream>>>(keep, n, seed, step_state, source, level);
+void launch_spec_dropout(uint8_t* keep, long long n, long long first, unsigned long long seed, const long long* step_state,
+                         int source, int level, cudaStream_t stream) {
+    spec_dropout_kernel<<<grid_stride_blocks(n), 256, 0, stream>>>(keep, n, first, seed, step_state, source, level);
 }
 
 void launch_spec_mask_apply(float* mask, long long frames, const float* X, float* out, int magnitude, cudaStream_t stream) {

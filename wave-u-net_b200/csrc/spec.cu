@@ -143,11 +143,12 @@ int level_pitch(const Layer& l, int d, int L) { return d + 1 < L ? 2 * l.Co : l.
 // Training workspace at `batch`: the inference map, then per level the gradient twin of its concatenation buffer and the
 // keep mask of a dropped level, the pre-batch-norm output of every layer (overwritten by its gradient in the backward),
 // the mask (logits, then sigmoid) and its gradient, the K outputs the loss reads, the per-channel statistics and backward
-// coefficients, the partial sums of the channel reductions and of the weight gradients, and the loss's running-mean state.
+// coefficients, the partial sums of the channel reductions, this call's per-channel sums, the partial sums of the weight
+// gradients, and the loss's running-mean state.
 struct TrainMap {
     WsMap base;
     std::vector<int64_t> glevel, drop, zdown, zup, sdown, sup;     // s*: per-channel (batch mean, rstd) of every layer
-    int64_t mask, dlogit, out, coef, red, wpart, loss_state, end;
+    int64_t mask, dlogit, out, coef, red, local, wpart, loss_state, end;
 };
 
 std::vector<SpecWgrad> wgrad_shapes(const WunSpecHandle* h, int B) {
@@ -199,6 +200,7 @@ TrainMap train_map(const WunSpecHandle* h, int64_t B) {
     m.out = take(K * std::max(bins, B * h->T) * 4);
     m.coef = take(cmax * 8);
     m.red = take((int64_t)spec_chan_partials(rows_max) * cmax * 16);
+    m.local = take(cmax * 16);
     int64_t wpart = 0;
     for (const SpecWgrad& G : wgrad_shapes(h, (int)B)) {
         const int P = spec_wgrad_partials(G);
@@ -227,7 +229,11 @@ int check_call(const WunSpecHandle* h, int64_t batch, const void* ws, int64_t ws
     return check_device();
 }
 
-// One U-Net's training forward and backward (source k), on the activation buffers every source shares.
+// The widest batch-norm layer (the bottom one): a rank's gathered statistics take world * 16 bytes per channel of it.
+int64_t widest_bn(const WunSpecHandle* h) { return h->nets[0].down.back().Co; }
+
+// One U-Net's training forward and backward (source k), on the activation buffers every source shares.  The batch-norm
+// statistics are those of the whole batch of `shard`: each layer's per-channel sums go through the shard's gather.
 struct TrainCall {
     const WunSpecHandle* h;
     float* params;
@@ -240,6 +246,20 @@ struct TrainCall {
     long long* step_state;
     const float* targets;          // [K][B][T]
     cudaStream_t st;
+    WunSpecShard shard;
+
+    // every rank's (sum 1, sum 2) of S.local (written by launch_spec_chan_sum) into S.gathered; one rank without a gather
+    // reads its own
+    int gather(SpecChanSum& S) const {
+        if (!shard.gather) {
+            S.gathered = S.local;
+            return WUN_OK;
+        }
+        S.gathered = reinterpret_cast<const double2*>(shard.gathered);
+        const int rc = shard.gather(shard.ctx, reinterpret_cast<const double*>(S.local), shard.gathered, 2LL * S.C, st);
+        return rc == 0 ? WUN_OK : fail(WUN_E_CUDA, "spectrogram training: the batch-statistics gather failed (" +
+                                                       std::to_string(rc) + ")");
+    }
 
     template <class T> T* at(int64_t off) const { return reinterpret_cast<T*>(ws + off); }
     float* level(int d) const { return at<float>(m->base.level[d]); }
@@ -247,30 +267,40 @@ struct TrainCall {
     const uint8_t* drop(int d) const { return m->drop[d] >= 0 ? at<uint8_t>(m->drop[d]) : nullptr; }
 
     // batch statistics, moving averages, normalise + beta + activation into y
-    void bn_forward(const Layer& l, const float* z, float2* stat, float* y, int y_pitch, float neg_slope) const {
+    int bn_forward(const Layer& l, const float* z, float2* stat, float* y, int y_pitch, float neg_slope) const {
         const long long N = (long long)B * l.Ho * l.Wo;
         SpecChanSum S{};
         S.mode = 0; S.z = z; S.N = N; S.C = l.Co;
         S.stat = stat;
         S.moving_mean = params + l.mean; S.moving_var = params + l.var;
         S.part = at<double2>(m->red);
+        S.local = at<double2>(m->local);
+        S.n = (double)(shard.global_batch * l.Ho * l.Wo);
         launch_spec_chan_sum(S, st);
+        if (int rc = gather(S)) return rc;
+        launch_spec_chan_finish(S, shard.world, st);
         launch_spec_bn_apply(z, N, l.Co, S.stat, params + l.beta, neg_slope, y, y_pitch, st);
+        return WUN_OK;
     }
 
     // g, a: the layer's output gradient and activation at `pitch`; z (pre-BN output) becomes dz.  Also the gradients of
     // beta and of the conv bias (the fixed-order sum of dz).
-    void bn_backward(const Layer& l, float* z, float2* stat, const float* g, const float* a, int pitch,
-                     float neg_slope) const {
+    int bn_backward(const Layer& l, float* z, float2* stat, const float* g, const float* a, int pitch,
+                    float neg_slope) const {
         const long long N = (long long)B * l.Ho * l.Wo;
         SpecChanSum S{};
         S.mode = 1; S.z = z; S.N = N; S.C = l.Co; S.stat = stat;
         S.part = at<double2>(m->red);
         S.g = g; S.a = a; S.pitch = pitch; S.neg_slope = neg_slope;
         S.coef = at<float2>(m->coef); S.out = grads + l.beta;
+        S.local = at<double2>(m->local);
+        S.n = (double)(shard.global_batch * l.Ho * l.Wo);
         launch_spec_chan_sum(S, st);
+        if (int rc = gather(S)) return rc;
+        launch_spec_chan_finish(S, shard.world, st);
         launch_spec_bn_backward(z, N, l.Co, g, a, pitch, neg_slope, S.stat, S.coef, st);
         bias_grad(l, z, N);
+        return WUN_OK;
     }
 
     void bias_grad(const Layer& l, const float* dz, long long N) const {
@@ -285,10 +315,10 @@ struct TrainCall {
         launch_spec_wgrad(G, st);
     }
 
-    void run(int k) const;
+    int run(int k) const;
 };
 
-void TrainCall::run(int k) const {
+int TrainCall::run(int k) const {
     const WunSpecHandle* H = h;
     const Net& net = H->nets[k];
     const int L = H->cfg.num_layers, K = H->cfg.num_sources;
@@ -316,14 +346,15 @@ void TrainCall::run(int k) const {
                         params + l.w, (long long)l.Ci * l.Co, 1, l.Co, params + l.b, B};
         launch_spec_train_conv(A, 0, st);
         const int y_pitch = level_pitch(l, d, L);
-        bn_forward(l, zd(d), sd(d), level(d), y_pitch, 0.2f);
+        if (int rc = bn_forward(l, zd(d), sd(d), level(d), y_pitch, 0.2f)) return rc;
         x = level(d);
         x_pitch = y_pitch;
     }
     for (int d = 0; d < L; ++d)
         if (drop(d)) {
             const Layer& l = net.down[d];
-            launch_spec_dropout(const_cast<uint8_t*>(drop(d)), (long long)B * l.Ho * l.Wo * level_pitch(l, d, L), seed,
+            const long long per_sample = (long long)l.Ho * l.Wo * level_pitch(l, d, L);
+            launch_spec_dropout(const_cast<uint8_t*>(drop(d)), B * per_sample, shard.sample_offset * per_sample, seed,
                                 step_state, k, d, st);
         }
     for (int i = 0; i + 1 < L; ++i) {
@@ -334,7 +365,7 @@ void TrainCall::run(int k) const {
         SpecTrainConv A{ux, l.Hi, l.Wi, l.Ci, up, udr, zu(i), l.Ho, l.Wo, l.Co, l.Co, 0, nullptr, 0,
                         params + l.w, (long long)l.Co * l.Ci, l.Ci, 1, params + l.b, B};
         launch_spec_train_conv(A, 1, st);
-        bn_forward(l, zu(i), su(i), level(d) + l.Co, 2 * l.Co, 0.f);
+        if (int rc = bn_forward(l, zu(i), su(i), level(d) + l.Co, 2 * l.Co, 0.f)) return rc;
     }
     const Layer& ml = net.mask;
     const uint8_t* mdrop = L > 1 ? drop(0) : nullptr;
@@ -355,10 +386,12 @@ void TrainCall::run(int k) const {
     }
 
     // ---- backward ----
+    // d loss / d output of the whole batch's mean: 1 / (global batch x elements per example x K)
     float* dlogit = at<float>(m->dlogit);
+    const int64_t GB = shard.global_batch;
     SpecMaskBwd M{X, mask, dlogit, H->n, H->T, raw_audio, out, targets + (int64_t)k * B * H->T,
                   at<float>(m->base.tmag) + k * bins,
-                  raw_audio ? (float)(1.0 / ((double)B * H->T * K)) : (float)(1.0 / ((double)bins * K))};
+                  raw_audio ? (float)(1.0 / ((double)GB * H->T * K)) : (float)(1.0 / ((double)(GB * H->n * kBins) * K))};
     launch_spec_mask_backward(M, B, st);
     {
         SpecChanSum S{};
@@ -374,7 +407,7 @@ void TrainCall::run(int k) const {
     for (int i = L - 2; i >= 0; --i) {
         const Layer& l = net.up[i];
         const int d = L - 2 - i;
-        bn_backward(l, zu(i), su(i), glevel(d) + l.Co, level(d) + l.Co, 2 * l.Co, 0.f);
+        if (int rc = bn_backward(l, zu(i), su(i), glevel(d) + l.Co, level(d) + l.Co, 2 * l.Co, 0.f)) return rc;
         const float* ux; int up; const uint8_t* udr; float* ug;
         up_in(i, &ux, &up, &udr, &ug);
         SpecWgrad G{ux, up, udr, l.Ci, zu(i), l.Co, l.Co, l.Hi, l.Wi, B, grads + l.w, (long long)l.Co * l.Ci, 1, l.Ci,
@@ -388,7 +421,7 @@ void TrainCall::run(int k) const {
     for (int d = L - 1; d >= 0; --d) {
         const Layer& l = net.down[d];
         const int pitch = level_pitch(l, d, L);
-        bn_backward(l, zd(d), sd(d), glevel(d), level(d), pitch, 0.2f);
+        if (int rc = bn_backward(l, zd(d), sd(d), glevel(d), level(d), pitch, 0.2f)) return rc;
         const float* xin = d == 0 ? logmag : level(d - 1);
         const int xin_pitch = d == 0 ? 1 : level_pitch(net.down[d - 1], d - 1, L);
         SpecWgrad G{zd(d), l.Co, nullptr, l.Co, xin, xin_pitch, l.Ci, l.Ho, l.Wo, B, grads + l.w, (long long)l.Ci * l.Co,
@@ -401,6 +434,7 @@ void TrainCall::run(int k) const {
             launch_spec_train_conv(D, 1, st);
         }
     }
+    return WUN_OK;
 }
 
 int check_train_call(const WunSpecHandle* h, int64_t batch, const void* ws, int64_t ws_bytes) {
@@ -591,9 +625,13 @@ double wun_spec_train_flops(const WunSpecHandle* h, int64_t batch) {
     return 3.0 * wun_spec_forward_flops(h, batch) - first;
 }
 
-int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
-                              int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
-                              void* workspace, int64_t workspace_bytes, void* stream) {
+}  // extern "C"
+
+namespace {
+
+int forward_backward(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
+                     int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss, void* workspace,
+                     int64_t workspace_bytes, void* stream, const WunSpecShard& shard) {
     if (!h || !params || !mix || !targets || !step_state || !grads || !loss) return fail(WUN_E_INVALID, "null argument");
     int rc = check_train_call(h, batch, workspace, workspace_bytes);
     if (rc != WUN_OK) return rc;
@@ -612,8 +650,11 @@ int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix,
         launch_spec_stft(Tg, K * B, st);
     }
     TrainCall call{h, params, grads, ws, &m, B, raw_audio_loss ? 1 : 0, (unsigned long long)seed, (long long*)step_state,
-                   targets, st};
-    for (int k = 0; k < K; ++k) call.run(k);
+                   targets, st, shard};
+    for (int k = 0; k < K; ++k) {
+        rc = call.run(k);
+        if (rc != WUN_OK) return rc;
+    }
     const int64_t per = raw_audio_loss ? (int64_t)B * h->T : (int64_t)B * h->n * kBins;
     launch_eval_loss(reinterpret_cast<float*>(ws + m.out), raw_audio_loss ? targets : reinterpret_cast<float*>(ws + m.base.tmag),
                      K, per, reinterpret_cast<double*>(ws + m.loss_state), loss, reinterpret_cast<double*>(ws + m.base.slots),
@@ -624,12 +665,61 @@ int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix,
     return WUN_OK;
 }
 
+}  // namespace
+
+extern "C" {
+
+int wun_spec_forward_backward(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
+                              int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
+                              void* workspace, int64_t workspace_bytes, void* stream) {
+    WunSpecShard one{};
+    one.rank = 0; one.world = 1; one.global_batch = batch; one.sample_offset = 0;
+    return forward_backward(h, params, mix, targets, batch, raw_audio_loss, seed, step_state, grads, loss, workspace,
+                            workspace_bytes, stream, one);
+}
+
+int wun_spec_forward_backward_dp(WunSpecHandle* h, float* params, const float* mix, const float* targets, int64_t batch,
+                                 int raw_audio_loss, uint64_t seed, int64_t* step_state, float* grads, double* loss,
+                                 void* workspace, int64_t workspace_bytes, void* stream, const WunSpecShard* shard) {
+    if (!h || !shard) return fail(WUN_E_INVALID, "null argument");
+    const WunSpecShard& s = *shard;
+    if (s.world < 1 || s.rank < 0 || s.rank >= s.world) return fail(WUN_E_INVALID, "shard: need 0 <= rank < world");
+    if (s.global_batch < batch || s.global_batch > 65535 || s.sample_offset < 0 || s.sample_offset + batch > s.global_batch)
+        return fail(WUN_E_INVALID, "shard: need 0 <= sample_offset and sample_offset + batch <= global_batch <= 65535");
+    if (s.world > 1 && !s.gather) return fail(WUN_E_INVALID, "shard: more than one rank needs a gather callback");
+    if (s.gather && (!s.gathered || s.gathered_bytes < (int64_t)s.world * 16 * widest_bn(h)))
+        return fail(WUN_E_INVALID, "shard: the gathered buffer needs world * 16 * num_initial_filters * 2^(num_layers-1) "
+                                   "bytes");
+    return forward_backward(h, params, mix, targets, batch, raw_audio_loss, seed, step_state, grads, loss, workspace,
+                            workspace_bytes, stream, s);
+}
+
 int wun_spec_debug_train_level(const WunSpecHandle* h, int64_t batch, int level, int64_t* offset_bytes, int64_t* elems) {
     if (!h || batch < 1 || level < 0 || level >= h->cfg.num_layers || !offset_bytes || !elems)
         return fail(WUN_E_INVALID, "bad argument");
     const Layer& l = h->nets[0].down[level];
     *offset_bytes = train_map(h, batch).base.level[level];
     *elems = batch * l.Ho * (int64_t)l.Wo * level_pitch(l, level, h->cfg.num_layers);
+    return WUN_OK;
+}
+
+int wun_spec_debug_train_buffer(const WunSpecHandle* h, int64_t batch, int what, int index, int64_t* offset_bytes,
+                                int64_t* elems) {
+    if (!h || batch < 1 || !offset_bytes || !elems || what < 0 || what > 2) return fail(WUN_E_INVALID, "bad argument");
+    const int L = h->cfg.num_layers;
+    const TrainMap m = train_map(h, batch);
+    const Net& net = h->nets[0];
+    if (what == 0) {
+        if (index < 0 || index >= L || m.drop[index] < 0) return fail(WUN_E_INVALID, "level has no dropout mask");
+        const Layer& l = net.down[index];
+        *offset_bytes = m.drop[index];
+        *elems = batch * l.Ho * (int64_t)l.Wo * level_pitch(l, index, L);
+        return WUN_OK;
+    }
+    const std::vector<int64_t>& at = what == 1 ? m.sdown : m.sup;
+    if (index < 0 || index >= (int)at.size()) return fail(WUN_E_INVALID, "no such layer");
+    *offset_bytes = at[index];
+    *elems = 2 * (what == 1 ? net.down[index] : net.up[index]).Co;
     return WUN_OK;
 }
 

@@ -25,8 +25,9 @@ SYMBOLS = [
     "wun_spec_param_count", "wun_spec_param_numel", "wun_spec_param_table", "wun_spec_workspace_bytes",
     "wun_spec_forward_flops", "wun_spec_launches_forward", "wun_spec_forward", "wun_spec_l1_batch_loss",
     "wun_spec_gather_windows", "wun_spec_scatter_windows",
-    "wun_spec_train_workspace_bytes", "wun_spec_train_flops", "wun_spec_forward_backward", "wun_spec_adam_step_device",
-    "wun_spec_feed_batch", "wun_spec_debug_train_level",
+    "wun_spec_train_workspace_bytes", "wun_spec_train_flops", "wun_spec_forward_backward", "wun_spec_forward_backward_dp",
+    "wun_spec_adam_step_device",
+    "wun_spec_feed_batch", "wun_spec_debug_train_level", "wun_spec_debug_train_buffer",
     "wun_flac_find_frames", "wun_flac_decode_frames",
 ]
 
@@ -50,6 +51,17 @@ class WunSpecConfig(ctypes.Structure):
 class WunSpecParamInfo(ctypes.Structure):
     _fields_ = [("name", ctypes.c_char * 64), ("ndim", ctypes.c_int32), ("shape", ctypes.c_int32 * 4),
                 ("offset", ctypes.c_int64), ("numel", ctypes.c_int64)]
+
+
+# int gather(void* ctx, const double* local, double* gathered, int64_t count, void* stream) (include/wun.h WunSpecGatherFn)
+SPEC_GATHER_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64,
+                                  ctypes.c_void_p)
+
+
+class WunSpecShard(ctypes.Structure):
+    _fields_ = [("rank", ctypes.c_int32), ("world", ctypes.c_int32), ("global_batch", ctypes.c_int64),
+                ("sample_offset", ctypes.c_int64), ("gathered", ctypes.c_void_p), ("gathered_bytes", ctypes.c_int64),
+                ("gather", SPEC_GATHER_FN), ("ctx", ctypes.c_void_p)]
 
 
 class WunFlacFrame(ctypes.Structure):
@@ -149,8 +161,10 @@ def _load():
         lib.wun_spec_train_flops.restype = ctypes.c_double
         lib.wun_spec_forward_backward.argtypes = [H, VP, VP, VP, I64, ctypes.c_int, ctypes.c_uint64, VP, VP, VP, VP, I64,
                                                   VP]
+        lib.wun_spec_forward_backward_dp.argtypes = lib.wun_spec_forward_backward.argtypes + [P(WunSpecShard)]
         lib.wun_spec_adam_step_device.argtypes = [H, VP, VP, VP, VP, VP, F, F, F, F, VP]
         lib.wun_spec_debug_train_level.argtypes = [H, I64, ctypes.c_int, P(I64), P(I64)]
+        lib.wun_spec_debug_train_buffer.argtypes = [H, I64, ctypes.c_int, ctypes.c_int, P(I64), P(I64)]
         lib.wun_spec_feed_batch.argtypes = [H, VP, I64, VP, VP, I64, I64, ctypes.c_int, ctypes.c_uint64, VP, VP, VP, VP, VP]
     return lib
 
@@ -712,6 +726,7 @@ class SpecEngine(object):
         self.param_numel = lib.wun_spec_param_numel(self._h)
         self._ws = {}
         self._train_ws = {}
+        self._gathered = {}
 
     def __del__(self):
         try:
@@ -793,10 +808,14 @@ class SpecEngine(object):
                                              batch_loss.data_ptr() if batch_loss is not None else None, ws.data_ptr(),
                                              ws.numel() * 4, Engine._stream(targets.device)))
 
-    def forward_backward(self, params, mix, targets, grads, loss, raw_audio_loss, seed, step_state):
+    def forward_backward(self, params, mix, targets, grads, loss, raw_audio_loss, seed, step_state, shard=None):
         """One training step's loss and gradients (wun_spec_forward_backward): mix [B, T, 1], targets [K, B, T, 1], grads
         float32 [param_numel], loss float64 [1], step_state int64 [1] (the dropout counter, advanced by one).  Updates the
-        moving statistics inside `params`."""
+        moving statistics inside `params`.
+        shard (optional, e.g. wun.parallel.BatchStatsGather): this call is one rank's shard of a data-parallel step
+        (wun_spec_forward_backward_dp).  It has rank, world, global_batch and sample_offset, and
+        gather(local, gathered, stream) that puts every rank's float64 CUDA tensor `local` [count] into `gathered`
+        [world * count] in rank order, only enqueueing work on the torch stream `stream`."""
         import torch
         B = int(mix.shape[0])
         assert mix.is_cuda and mix.dtype == torch.float32 and mix.is_contiguous(), "mix must be a contiguous float32 CUDA tensor"
@@ -809,14 +828,49 @@ class SpecEngine(object):
         key = (B, str(mix.device))
         ws = self._train_ws.get(key)        # kept while the engine lives: a captured CUDA graph bakes the pointer in
         if ws is None:
-            ws = torch.empty((self.train_workspace_bytes(B) + 3) // 4, dtype=torch.float32, device=mix.device)
+            ws = torch.empty((self.train_workspace_bytes(B) + 7) // 8 * 2, dtype=torch.float32, device=mix.device)
             self._train_ws[key] = ws
+        args = (self._h, params.data_ptr(), mix.data_ptr(), targets.data_ptr(), B, 1 if raw_audio_loss else 0,
+                int(seed) & (2 ** 64 - 1), step_state.data_ptr(), grads.data_ptr(), loss.data_ptr(), ws.data_ptr(),
+                ws.numel() * 4, Engine._stream(mix.device))
         with torch.cuda.device(mix.device):
-            check(lib.wun_spec_forward_backward(self._h, params.data_ptr(), mix.data_ptr(), targets.data_ptr(), B,
-                                                1 if raw_audio_loss else 0, int(seed) & (2 ** 64 - 1), step_state.data_ptr(),
-                                                grads.data_ptr(), loss.data_ptr(), ws.data_ptr(), ws.numel() * 4,
-                                                Engine._stream(mix.device)))
+            if shard is None:
+                check(lib.wun_spec_forward_backward(*args))
+                return loss
+            desc, errors, keep = self._shard_descriptor(shard, ws, mix.device)
+            rc = lib.wun_spec_forward_backward_dp(*(args + (ctypes.byref(desc),)))     # `keep` holds the callback
+            if errors:
+                raise errors[0]
+            check(rc)
         return loss
+
+    def _shard_descriptor(self, shard, ws, device):
+        """WunSpecShard for `shard`, with a gather callback that hands shard.gather torch views of the engine's buffers.
+        Returns (descriptor, the list that receives the callback's exception, the objects to keep alive for the call)."""
+        import torch
+        world = int(shard.world)
+        key = (world, str(device))
+        gathered = self._gathered.get(key)  # kept like the workspace: a captured graph bakes the pointer in
+        if gathered is None:
+            widest = self.cfg.num_initial_filters << (self.cfg.num_layers - 1)
+            gathered = torch.empty(world * 2 * widest, dtype=torch.float64, device=device)
+            self._gathered[key] = gathered
+        ws64 = ws.view(torch.float64)
+        errors = []
+
+        def gather(ctx, local, out, count, stream):
+            try:
+                lo, go = (local - ws64.data_ptr()) // 8, (out - gathered.data_ptr()) // 8
+                shard.gather(ws64[lo:lo + count], gathered[go:go + world * count], torch.cuda.current_stream(device))
+                return 0
+            except BaseException as e:       # an exception cannot cross the C frames: re-raised after the call
+                errors.append(e)
+                return 1
+
+        fn = SPEC_GATHER_FN(gather)
+        desc = WunSpecShard(int(shard.rank), world, int(shard.global_batch), int(shard.sample_offset), gathered.data_ptr(),
+                            gathered.numel() * 8, fn, None)
+        return desc, errors, (fn, gather)
 
     def debug_train_level(self, batch, level, device):
         """Tests: view of concatenation level `level` [B, H, W, C] in the training workspace - after forward_backward the
@@ -826,6 +880,27 @@ class SpecEngine(object):
         ws = self._train_ws[(int(batch), str(device))]
         H, W = self.stft_frames >> (level + 1), 512 >> (level + 1)
         return ws[off.value // 4:off.value // 4 + n.value].view(int(batch), H, W, -1)
+
+    def debug_train_keep(self, batch, level, device):
+        """Tests: the keep mask of dropped level `level` [B, H, W, C] uint8 in the training workspace (after forward_backward
+        the last source's)."""
+        import torch
+        off, n = self._debug_train_buffer(batch, 0, level)
+        ws = self._train_ws[(int(batch), str(device))]
+        H, W = self.stft_frames >> (level + 1), 512 >> (level + 1)
+        return ws.view(torch.uint8)[off:off + n].view(int(batch), H, W, -1)
+
+    def debug_train_stats(self, batch, layer, up, device):
+        """Tests: the batch statistics [C, 2] (mean, rstd) of down (or with `up`, up) layer `layer` in the training
+        workspace (after forward_backward the last source's)."""
+        off, n = self._debug_train_buffer(batch, 2 if up else 1, layer)
+        ws = self._train_ws[(int(batch), str(device))]
+        return ws[off // 4:off // 4 + n].view(-1, 2)
+
+    def _debug_train_buffer(self, batch, what, index):
+        off, n = ctypes.c_int64(), ctypes.c_int64()
+        check(lib.wun_spec_debug_train_buffer(self._h, int(batch), int(what), int(index), ctypes.byref(off), ctypes.byref(n)))
+        return off.value, n.value
 
     def adam_step_device(self, params, grads, m, v, state, lr, beta1=0.9, beta2=0.999, eps=1e-8):
         """Graph-safe Adam on the trainable variables: `state` = device float32[3] {beta1_power, beta2_power, step}."""

@@ -6,6 +6,9 @@ the gradient pre-scaled by 1/world (the loss is a mean over the batch, /root/ref
 all-reduce (sum) of the flat fp32 gradient buffer makes every replica apply the same Adam update.  Inference
 windows (/root/reference/Evaluate.py:125-139) are independent: contiguous ranges per rank, no collective.
 
+The spectrogram U-Net (U7 / U7a) has batch norm: its data-parallel step (sync_batch_norm) gathers every layer's
+per-channel sums from all ranks through BatchStatsGather, so that each rank normalises with the whole batch's statistics.
+
 Everything here works on CPU tensors with the gloo backend too (tests/test_parallel_cpu.py).
 """
 import torch
@@ -113,6 +116,35 @@ class BucketedAllReduce(object):
                 dist.all_reduce(view, op=dist.ReduceOp.SUM, group=self.group)
         self.done.record(self.comm)
         cur.wait_event(self.done)
+
+
+class BatchStatsGather(object):
+    """The shard of this rank in a data-parallel step of the spectrogram U-Net (wun.SpecEngine.forward_backward's `shard`):
+    examples [sample_offset, sample_offset + local_batch) of `global_batch` (shard_range), and the all-gather of the
+    batch-norm sums.  Under NCCL the gather is enqueued on the engine's stream, so a step stays capturable in a CUDA graph;
+    under another backend (gloo) it waits for the stream and goes through host memory."""
+
+    def __init__(self, global_batch, group=None):
+        import torch.distributed as dist
+        self.group = group
+        self.rank, self.world = dist.get_rank(group), dist.get_world_size(group)
+        self.global_batch = int(global_batch)
+        lo, hi = shard_range(self.global_batch, self.rank, self.world)
+        self.sample_offset, self.local_batch = lo, hi - lo
+        self.nccl = dist.get_backend(group) == "nccl"
+
+    def gather(self, local, gathered, stream):
+        """Every rank's float64 CUDA tensor `local` [count] into `gathered` [world * count], rank r's at r * count."""
+        import torch
+        import torch.distributed as dist
+        with torch.cuda.stream(stream):
+            if self.nccl:
+                dist.all_gather_into_tensor(gathered, local, group=self.group)
+                return
+            stream.synchronize()
+            parts = [torch.empty(local.numel(), dtype=local.dtype) for _ in range(self.world)]
+            dist.all_gather(parts, local.cpu(), group=self.group)
+            gathered.copy_(torch.cat(parts))
 
 
 def broadcast_parameters(flat_params, src=0, group=None):
