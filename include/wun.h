@@ -401,6 +401,27 @@ int wun_flac_decode_frames(const uint8_t* buf, int64_t nbytes, int32_t bps, int3
                            int32_t max_block, const int64_t* offsets, const int64_t* first_samples, int64_t nframes,
                            int32_t* out, int64_t total_samples, int32_t* status, void* stream);
 
+/* --- FLAC encoding (csrc/kernels_flac_encode.cu, DESIGN.md §4.11) --------------------------------
+ * The frames of a FLAC stream inside the streamable subset: fixed blocking at block_size (16..4608; the last frame shorter),
+ * LPC order <= 12 at rates <= 48 kHz (<= 32 above), 15-bit coefficients, shifts 0-15, Rice partition order <= 8, rate and
+ * sample size codes in every header (depths other than 8, 12, 16, 20 and 24 have no size code and take it from STREAMINFO,
+ * which leaves the subset).  Each frame's stereo mode, subframe types, predictors and Rice parameters are chosen by exact bit
+ * count.  4..24 bits per sample, 1..8 channels, any rate a frame header can express.  The same input gives the same bytes on
+ * every run.  wun.write_flac (wun/flac.py) adds the metadata. */
+#define WUN_FLAC_INT32 0       /* samples at full depth, within [-2^(bps-1), 2^(bps-1) - 1] */
+#define WUN_FLAC_FLOAT32 1     /* clamp(rint(x * 2^(bps-1)), -2^(bps-1), 2^(bps-1) - 1), ties to even, NaN -> 0 */
+/* Bytes of the workspace for n samples of `channels` channels (-1: arguments out of range).  Host only. */
+int64_t wun_flac_encode_workspace_bytes(int64_t n, int32_t channels, int32_t block_size);
+/* Bytes `out` needs: the sum of the frames' bounds (header, VERBATIM subframes, CRC-16), a multiple of 4.  Host only. */
+int64_t wun_flac_encode_capacity(int64_t n, int32_t channels, int32_t bps, int32_t block_size);
+/* Encode `samples` (DEVICE [n][channels] interleaved, int32 or float32 by sample_type) into the frame area at `out` (DEVICE,
+ * 4-byte aligned, out_capacity bytes; the bytes past the frames are zero).  frame_offsets (DEVICE int64, n_frames + 1):
+ * frame j occupies out[frame_offsets[j] .. frame_offsets[j + 1]); the last entry is the frame area's length, or -1 when an
+ * int32 sample lies outside the depth (then nothing is written).  workspace: DEVICE, 256-byte aligned. */
+int wun_flac_encode_frames(const void* samples, int32_t sample_type, int64_t n, int32_t channels, int32_t bps, int32_t rate,
+                           int32_t block_size, void* workspace, int64_t workspace_bytes, uint8_t* out, int64_t out_capacity,
+                           int64_t* frame_offsets, void* stream);
+
 /* --- diagnostics -------------------------------------------------------------------------------- */
 const char* wun_last_error(void);
 const char* wun_version(void);

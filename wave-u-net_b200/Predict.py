@@ -1,6 +1,7 @@
 """Prediction entry point (stand-in for /root/reference/Predict.py:1-17):
 
     python Predict.py with cfg.full_44KHz model_path=checkpoints/123/123-2000 input_path=song.wav [output_path=out]
+                      [output_format=flac [bit_depth=16|24]]
 
 model_path:  a TF-V2 checkpoint prefix (written by Training.py here or by the reference's Saver) or a round-1 .npz.
 input_path:
@@ -11,10 +12,16 @@ input_path:
          Evaluate.py:193).
   *.flac FLAC, 4 to 24 bits per sample, 1 to 8 channels, decoded on the GPU (wun.read_flac) and converted as the
          reference's ffmpeg path loads it: each sample shifted to 16 bits (left for fewer bits, arithmetically right for
-         more) and divided by 32768.  Then as for WAV; estimates are still written as float WAV.
+         more) and divided by 32768.  Then as for WAV.
   *.npy  a float array [n_frames, n_channels] already at model_config["expected_sr"]; estimates are written to
          <output_path or input_path>_<source>.npy.
 Other audio formats (mp3 and friends, Evaluate.py:172) are out of scope.
+
+output_format=wav (the default) writes the WAV / FLAC input's estimates as above.  output_format=flac writes them as
+<output_path or input_path>_<source>.flac instead, encoded on the GPU (wun.write_flac) at bit_depth bits (16, the default,
+or 24): each float sample x becomes clamp(rint(x * 2^(bit_depth-1))), so an estimate read back and divided by
+2^(bit_depth-1) is within 2^-bit_depth of the float one, except where it clipped at +-1.  bit_depth without
+output_format=flac is an error, as is output_format=flac with a .npy input.
 
 With references_path= and results_dir=<dir>, the predictions are also scored with BSS Eval v4 on the GPU
 (Evaluate.eval_track, the reference's museval.eval_mus_track at Evaluate.py:71) at the input's rate and written to
@@ -91,7 +98,35 @@ def load_references(references_path, rate):
         return {name: z[name] for name in z.files}
 
 
-def main(cfg, model_path, input_path, output_path=None, references_path=None, results_dir=None):
+def write_flac(path, audio, rate, bit_depth):
+    """`audio` [n_frames, n_channels] as a FLAC file of bit_depth bits, quantised and encoded on the GPU."""
+    import torch
+    import wun
+    wun.write_flac(torch.from_numpy(np.ascontiguousarray(audio, np.float32)).cuda(), rate, bit_depth, path)
+
+
+OUTPUT_FORMATS = ("wav", "flac")
+BIT_DEPTHS = (16, 24)
+
+
+def output_options(output_format=None, bit_depth=None):
+    """(format, bit depth or None) from the command line's output_format= and bit_depth=; ValueError for anything else."""
+    fmt = "wav" if output_format is None else str(output_format).lower()
+    if fmt not in OUTPUT_FORMATS:
+        raise ValueError("output_format=%s: must be one of %s" % (output_format, ", ".join(OUTPUT_FORMATS)))
+    if fmt != "flac":
+        if bit_depth is not None:
+            raise ValueError("bit_depth= is only meaningful with output_format=flac")
+        return fmt, None
+    depth = 16 if bit_depth is None else bit_depth
+    if isinstance(depth, bool) or not isinstance(depth, int) or depth not in BIT_DEPTHS:
+        raise ValueError("bit_depth=%s: must be 16 or 24" % (bit_depth,))
+    return fmt, depth
+
+
+def main(cfg, model_path, input_path, output_path=None, references_path=None, results_dir=None, output_format="wav",
+         bit_depth=None):
+    output_format, bit_depth = output_options(output_format, bit_depth)
     model_config = cfg["model_config"]
     base = output_path if output_path is not None else input_path
     track = os.path.splitext(os.path.basename(input_path))[0]
@@ -102,8 +137,13 @@ def main(cfg, model_path, input_path, output_path=None, references_path=None, re
         preds = Evaluate.predict(model_config, Evaluate.load_separator(model_config, model_path), mix, rate,
                                  references=refs, results_dir=results_dir, track_name=track)
         for name, audio in preds.items():
-            write_wav("%s_%s.wav" % (base, name), audio, rate)
+            if output_format == "flac":
+                write_flac("%s_%s.flac" % (base, name), audio, rate, bit_depth)
+            else:
+                write_wav("%s_%s.wav" % (base, name), audio, rate)
         return preds
+    if output_format != "wav":
+        raise ValueError("output_format=%s: .npy input writes .npy estimates" % output_format)
     mix = np.load(input_path)
     preds = Evaluate.produce_source_estimates(model_config, model_path, mix)
     for name, audio in preds.items():
@@ -126,6 +166,12 @@ if __name__ == "__main__":
     cfg, extras = Config.parse_command_line(sys.argv[1:])
     if "input_path" not in extras:
         raise SystemExit("Predict.py: input_path=<song.wav, song.flac or mix.npy> is required (the reference's default, an "
-                         "mp3 of audio_examples/, is not a format read here)\n" + __doc__)
+                         "mp3 of audio_examples/, is not a format read here); output_format=flac [bit_depth=16|24] writes "
+                         "FLAC estimates\n" + __doc__)
+    try:
+        output_options(extras.get("output_format"), extras.get("bit_depth"))
+    except ValueError as ex:
+        raise SystemExit("Predict.py: %s\n%s" % (ex, __doc__))
     main(cfg, extras.get("model_path", DEFAULT_MODEL_PATH), extras["input_path"], extras.get("output_path"),
-         extras.get("references_path"), extras.get("results_dir"))
+         extras.get("references_path"), extras.get("results_dir"), extras.get("output_format", "wav"),
+         extras.get("bit_depth"))

@@ -29,6 +29,7 @@ SYMBOLS = [
     "wun_spec_adam_step_device",
     "wun_spec_feed_batch", "wun_spec_debug_train_level", "wun_spec_debug_train_buffer",
     "wun_flac_find_frames", "wun_flac_decode_frames",
+    "wun_flac_encode_workspace_bytes", "wun_flac_encode_capacity", "wun_flac_encode_frames",
 ]
 
 
@@ -134,6 +135,13 @@ def _load():
         I32 = ctypes.c_int32
         lib.wun_flac_find_frames.argtypes = [VP, I64, I32, I32, I32, I32, VP, I64, VP, VP]
         lib.wun_flac_decode_frames.argtypes = [VP, I64, I32, I32, I32, I32, VP, VP, I64, VP, I64, VP, VP]
+    if hasattr(lib, "wun_flac_encode_frames"):  # likewise the FLAC encoder
+        I32 = ctypes.c_int32
+        lib.wun_flac_encode_workspace_bytes.argtypes = [I64, I32, I32]
+        lib.wun_flac_encode_workspace_bytes.restype = I64
+        lib.wun_flac_encode_capacity.argtypes = [I64, I32, I32, I32]
+        lib.wun_flac_encode_capacity.restype = I64
+        lib.wun_flac_encode_frames.argtypes = [VP, I32, I64, I32, I32, I32, I32, VP, I64, VP, I64, VP, VP]
     if hasattr(lib, "wun_snippet_batch"):   # likewise the validation-loss kernels
         lib.wun_snippet_batch.argtypes = [VP, I64, I64, I64, I64, I64, VP, I64, I64, VP, VP, VP, VP]
         lib.wun_eval_batch_loss.argtypes = [VP, VP, I64, I64, VP, VP, VP, I64, VP]
@@ -358,6 +366,58 @@ def read_flac(source, verify_md5=True, device="cuda"):
     if verify_md5 and info.md5 != bytes(16) and flac.md5_of(out, info.bps) != info.md5:
         raise ValueError("FLAC: the decoded samples do not match the stream's MD5")
     return info.rate, info.bps, out
+
+
+FLAC_BLOCK_SIZE = 4096
+
+
+def write_flac(samples, rate, bps, path=None, block_size=FLAC_BLOCK_SIZE):
+    """The bytes of a FLAC stream of `samples` encoded on the GPU (include/wun.h wun_flac_encode_frames, DESIGN.md §4.11),
+    written to `path` too when it is given.  `samples`: a CUDA tensor [n, channels] (or [n] for mono), int32 at full depth
+    or float32 (quantised as wun.flac.quantise: x * 2^(bps-1) rounded half to even and clipped, the inverse of reading
+    s / 2^(bps-1)).  4..24 bits per sample, 1..8 channels, any rate a frame header can express; fixed blocks of
+    `block_size` (16..4608) in FLAC's streamable subset.  The host adds STREAMINFO (with the MD5 of the integer samples,
+    as wun.read_flac checks it) and a VORBIS_COMMENT block; the frame area comes back in one device-to-host copy.  An int32
+    sample outside the depth raises ValueError."""
+    import numpy as np
+    import torch
+    from . import flac
+    assert samples.is_cuda and samples.dtype in (torch.int32, torch.float32), \
+        "samples must be an int32 or float32 CUDA tensor [n, channels]"
+    x = samples.reshape(-1, 1) if samples.dim() == 1 else samples
+    assert x.dim() == 2, "samples must be [n, channels]"
+    x = x.contiguous()
+    n, C = (int(v) for v in x.shape)
+    rate, bps, block_size = int(rate), int(bps), int(block_size)
+    ws_bytes = lib.wun_flac_encode_workspace_bytes(n, C, block_size)
+    capacity = lib.wun_flac_encode_capacity(n, C, bps, block_size)
+    if ws_bytes < 0 or capacity < 0 or not 4 <= bps <= 24:
+        raise ValueError("write_flac: need 4 <= bps <= 24, 1 to 8 channels and 16 <= block_size <= 4608 (got bps %d, "
+                         "%d channels, block_size %d)" % (bps, C, block_size))
+    if not (0 < rate < (1 << 20) and flac.header_rate_ok(rate)):
+        raise ValueError("write_flac: %d Hz cannot be written in a FLAC frame header" % rate)
+    dev = x.device
+    frames = (n + block_size - 1) // block_size
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    out = torch.empty(max(capacity, 4), dtype=torch.uint8, device=dev)
+    offsets = torch.empty(frames + 1, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        rc = lib.wun_flac_encode_frames(x.data_ptr(), 1 if x.dtype == torch.float32 else 0, n, C, bps, rate, block_size,
+                                        ws.data_ptr(), ws.numel(), out.data_ptr(), out.numel(), offsets.data_ptr(),
+                                        Engine._stream(dev))
+        if rc != WUN_OK:
+            raise WunError(rc, "wun_flac_encode_frames failed")
+        off = offsets.cpu().numpy()
+        if off[-1] < 0:
+            raise ValueError("write_flac: samples lie outside %d bits" % bps)
+        ints = x if x.dtype == torch.int32 else ws[:n * C * 4].view(torch.int32).view(n, C)
+        md5 = flac.md5_of(ints, bps)
+        area = out[:int(off[-1])].cpu().numpy().tobytes()
+    data = flac.assemble(area, off, block_size, rate, C, bps, n, md5)
+    if path is not None:
+        with open(path, "wb") as f:
+            f.write(data)
+    return data
 
 
 EVAL_LOSS_CTAS = 264        # include/wun.h WUN_EVAL_LOSS_CTAS

@@ -7,7 +7,12 @@ chain_frames(...)    keeps, out of the device's frame candidates, the frames tha
                         out; a broken chain raises ValueError naming the byte offset and the frame.
 md5_of(samples, bps) the STREAMINFO MD5: every sample as (bps + 7) // 8 little-endian bytes, channels interleaved.
 
-Pure host code; wun.read_flac runs the kernels between them.  Both O(metadata + frames).
+The host half of FLAC encoding (DESIGN.md §4.11):
+quantise(x, bps)     the rule the device applies to float input, restated in numpy for the tests.
+assemble(...)        `fLaC`, STREAMINFO (block and frame size bounds from the real frames, total samples, MD5) and a
+                        VORBIS_COMMENT block in front of the frame area wun.write_flac copied from the device.
+
+Pure host code; wun.read_flac and wun.write_flac run the kernels between them.  All O(metadata + frames).
 """
 import collections
 import hashlib
@@ -121,3 +126,37 @@ def to_float(samples, bps):
     x = np.asarray(samples, np.int32)
     x = x << (16 - bps) if bps <= 16 else x >> (bps - 16)
     return x.astype(np.float32) / np.float32(32768)
+
+
+VENDOR = b"wave-u-net_b200 GPU FLAC encoder"
+
+
+def quantise(x, bps):
+    """float samples -> int32 at `bps` bits: clamp(rint(x * 2^(bps-1)), -2^(bps-1), 2^(bps-1) - 1), ties to even, NaN -> 0
+    (include/wun.h WUN_FLAC_FLOAT32).  x * 2^(bps-1) is exact in float32, so s / 2^(bps-1) read back gives s again."""
+    x = np.asarray(x, np.float32)
+    with np.errstate(over="ignore", invalid="ignore"):                # +-inf clip like the device's saturation
+        v = np.rint(x * np.float32(1 << (bps - 1)))
+    v = np.clip(np.where(np.isnan(v), 0, v), -(1 << (bps - 1)), (1 << (bps - 1)) - 1)
+    return v.astype(np.int32)
+
+
+def header_rate_ok(rate):
+    """Whether a frame header can state `rate` (a table code, kHz in 8 bits, Hz or tens of Hz in 16 bits)."""
+    return rate in (8000, 16000, 22050, 24000, 32000, 44100, 48000, 88200, 96000, 176400, 192000) or \
+        (rate % 1000 == 0 and rate // 1000 <= 255) or 0 < rate <= 65535 or (rate % 10 == 0 and rate // 10 <= 65535)
+
+
+def _block(kind, body, last):
+    return bytes([(0x80 if last else 0) | kind]) + len(body).to_bytes(3, "big") + body
+
+
+def assemble(area, offsets, block_size, rate, channels, bps, total_samples, md5):
+    """The whole stream: `fLaC`, STREAMINFO, VORBIS_COMMENT (vendor string, no fields), then the frame area `area` (bytes)
+    whose frames start at offsets[:-1] (numpy int64, offsets[-1] == len(area))."""
+    sizes = np.diff(np.asarray(offsets, np.int64))
+    min_frame, max_frame = (int(sizes.min()), int(sizes.max())) if sizes.size else (0, 0)
+    info = (block_size.to_bytes(2, "big") * 2 + min_frame.to_bytes(3, "big") + max_frame.to_bytes(3, "big") +
+            ((rate << 44) | ((channels - 1) << 41) | ((bps - 1) << 36) | total_samples).to_bytes(8, "big") + md5)
+    comment = len(VENDOR).to_bytes(4, "little") + VENDOR + (0).to_bytes(4, "little")
+    return b"fLaC" + _block(0, info, False) + _block(4, comment, True) + bytes(area)
