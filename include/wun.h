@@ -190,6 +190,19 @@ int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, 
                  int64_t win, int64_t hop, double* metrics, double* filters, void* workspace, int64_t workspace_bytes,
                  void* stream);
 
+/* BSS Eval v3 as museval 0.2.0 evaluate(..., mode="v3") computes it: the decomposition of wun_bss_eval with the filters
+ * solved again for every frame from that frame's samples alone (G and D of the zero-extended slices), and only for frames
+ * that are not silent.  Inputs, metrics, argument checks and return codes as wun_bss_eval.
+ *   filters   optional DEVICE float64 [nwin][...]: frame t's C then Cj in wun_bss_eval's layout; NaN for silent frames
+ * The workspace holds the frames of one pass: wun_bss_eval_v3_workspace_bytes(..., frames_per_pass) bytes hold
+ * frames_per_pass of them (frames_per_pass >= 1; fewer when there are fewer frames).  wun_bss_eval_v3 fits as many frames per
+ * pass as workspace_bytes holds, at least one; the results are the same bits whatever that number is. */
+int64_t wun_bss_eval_v3_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop,
+                                        int64_t frames_per_pass);
+int wun_bss_eval_v3(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                    int64_t win, int64_t hop, double* metrics, double* filters, void* workspace, int64_t workspace_bytes,
+                    void* stream);
+
 /* --- resampling (no handle) ----------------------------------------------------------------------
  * librosa 0.6.2 resample(y, sr_in, sr_out) with res_type='kaiser_best', which the reference applies to every track before and
  * after separation (Evaluate.py:64,104, Utils.resample): resampy 0.2's resample_f bit for bit, then fix_length's zero

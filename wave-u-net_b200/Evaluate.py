@@ -11,7 +11,8 @@ is split over the ranks (no collective on the data path, results all-gathered at
 predict_track works on arrays already at model_config["expected_sr"]; predict() is the reference's predict() (Evaluate.py:
 60-71) on an array at any rate, resampling on the GPU with librosa's kaiser_best (wun.resample) on the way in and out.
 Scoring is here: evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS
-Eval v4 on the GPU (wun.bss_eval), and compute_mean_metrics is the reference's (Evaluate.py:195-232).
+Eval v4 on the GPU (wun.bss_eval), or with museval's mode="v3" (filters solved per frame) when asked for, and
+compute_mean_metrics is the reference's (Evaluate.py:195-232).
 produce_musdb_source_estimates runs them over the MUSDB18 WAV layout.  Audio decoding beyond WAV (Predict.py) and the musdb
 package are out of scope (SURVEY section 2).
 """
@@ -95,7 +96,7 @@ def _separate_on_device(model_config, separator, mix, batch_windows=16, device="
     return preds[:, :n_mix]
 
 
-def predict(model_config, separator, audio, rate, references=None, results_dir=None, track_name=None):
+def predict(model_config, separator, audio, rate, references=None, results_dir=None, track_name=None, mode="v4"):
     """The reference's predict() (Evaluate.py:60-71) on an array: `audio` float [n_frames, n_channels] at `rate` Hz.
     The mixture is downmixed or tiled to the model's channels, resampled to expected_sr with wun.resample (librosa's
     kaiser_best, Evaluate.py:104), separated, and every estimate is resampled back to `rate`, cut to n_frames and, for a
@@ -103,8 +104,8 @@ def predict(model_config, separator, audio, rate, references=None, results_dir=N
     upload to the download.  Returns OrderedDict name -> float32 [n_frames, n_channels].
 
     With `references` (name -> [n_frames, n_channels] at `rate`) the estimates are scored by eval_track at `rate` (the
-    reference's museval.eval_mus_track, :71), written to <results_dir>/<track_name>.json when results_dir is given, and the
-    per-target median SDR / ISR / SIR / SAR is printed."""
+    reference's museval.eval_mus_track, :71) with BSS Eval `mode` ("v4" or "v3"), written to <results_dir>/<track_name>.json
+    when results_dir is given, and the per-target median SDR / ISR / SIR / SAR is printed."""
     import torch
     import wun
     assert len(audio.shape) == 2
@@ -118,7 +119,7 @@ def predict(model_config, separator, audio, rate, references=None, results_dir=N
         result = np.tile(result, [1, 1, mix_channels])
     pred_audio = OrderedDict((name, result[k]) for k, name in enumerate(model_config["source_names"]))
     if references is not None:
-        scores = eval_track(references, pred_audio, rate, output_dir=results_dir, track_name=track_name)
+        scores = eval_track(references, pred_audio, rate, output_dir=results_dir, track_name=track_name, mode=mode)
         for target in scores["targets"]:
             print("%s ==> %s" % (target["name"], "  ".join(
                 "%s: %.3f" % (m, np.nanmedian([f["metrics"][m] for f in target["frames"]]))
@@ -145,11 +146,12 @@ def load_separator(model_config, load_model):
     return separator
 
 
-def produce_musdb_source_estimates(model_config, load_model, musdb_path, output_path, subsets=None):
+def produce_musdb_source_estimates(model_config, load_model, musdb_path, output_path, subsets=None, mode="v4"):
     """The reference's produce_musdb_source_estimates (Evaluate.py:147-159) over the MUSDB18 WAV layout: every track of
     `subsets` (both, as mus.run(subsets=None) does) is separated at its own rate with predict(), scored against its stems,
     and written as musdb and museval would: float32 WAV estimates in <output_path>/<subset>/<track>/<source>.wav and the BSS
-    Eval JSON in <output_path>/<subset>/<track>.json (Datasets.estimate_path / museval_json_dir).  The reference
+    Eval JSON (BSS Eval `mode`, "v4" or "v3") in <output_path>/<subset>/<track>.json (Datasets.estimate_path /
+    museval_json_dir).  The reference
     accompaniment is bass + drums + other, unclipped.  With torch.distributed every rank separates its share of the windows
     and rank 0 writes."""
     import Datasets
@@ -171,7 +173,7 @@ def produce_musdb_source_estimates(model_config, load_model, musdb_path, output_
             refs["accompaniment"] = acc
             results_dir = Datasets.museval_json_dir(output_path, subset) if rank == 0 else None
             preds = predict(model_config, separator, mix, rate, references=refs, results_dir=results_dir,
-                            track_name=track["name"])
+                            track_name=track["name"], mode=mode)
             if rank == 0:
                 for name, audio in preds.items():
                     path = Datasets.estimate_path(output_path, subset, track["name"], name)
@@ -187,13 +189,13 @@ def produce_source_estimates(model_config, load_model, mix_audio, separator=None
     return predict_track(model_config, separator, mix_audio)
 
 
-def _device_bss_eval(references, estimates, win, hop):
+def _device_bss_eval(references, estimates, win, hop, mode="v4"):
     """[nsrc, N, nchan] float arrays -> numpy float64 [4 (SDR, ISR, SIR, SAR), nsrc, nwin] from wun.bss_eval."""
     import torch
     import wun
     ref = torch.from_numpy(np.ascontiguousarray(references, dtype=np.float32)).cuda()
     est = torch.from_numpy(np.ascontiguousarray(estimates, dtype=np.float32)).cuda()
-    return torch.stack(wun.bss_eval(ref, est, win, hop)).cpu().numpy()
+    return torch.stack(wun.bss_eval(ref, est, win, hop, mode=mode)).cpu().numpy()
 
 
 def _pad_or_truncate(estimates, n):
@@ -202,23 +204,36 @@ def _pad_or_truncate(estimates, n):
     return np.pad(estimates, ((0, 0), (0, n - estimates.shape[1]), (0, 0)))
 
 
-def evaluate(references, estimates, win=44100, hop=44100):
-    """museval.evaluate(references, estimates, win, hop, mode="v4", padding=True): arrays [nsrc, n_samples, nchan];
-    estimates are cut or zero-extended to the references' length.  Returns SDR, ISR, SIR, SAR, each [nsrc, nwin]."""
+BSS_MODES = ("v4", "v3")
+
+
+def check_mode(mode):
+    if mode not in BSS_MODES:
+        raise ValueError("mode=%r: must be one of %s" % (mode, ", ".join(BSS_MODES)))
+
+
+def evaluate(references, estimates, win=44100, hop=44100, mode="v4"):
+    """museval.evaluate(references, estimates, win, hop, mode=mode, padding=True): arrays [nsrc, n_samples, nchan];
+    estimates are cut or zero-extended to the references' length.  mode "v4" solves the distortion filters once over the
+    track, "v3" again for every frame.  Returns SDR, ISR, SIR, SAR, each [nsrc, nwin]."""
+    check_mode(mode)
     references = np.asarray(references)
     estimates = _pad_or_truncate(np.asarray(estimates), references.shape[1])
-    sdr, isr, sir, sar = _device_bss_eval(references, estimates, int(win), int(hop))
+    args = (references, estimates, int(win), int(hop))         # v4 keeps the four-argument call
+    sdr, isr, sir, sar = _device_bss_eval(*args) if mode == "v4" else _device_bss_eval(*args, mode=mode)
     return sdr, isr, sir, sar
 
 
-def eval_track(references, estimates, rate, output_dir=None, track_name=None):
+def eval_track(references, estimates, rate, output_dir=None, track_name=None, mode="v4"):
     """museval.eval_mus_track with arrays: `references` and `estimates` map source names to [n_samples, nchan] arrays;
     the references' order plays the role of track.targets, and only names present in both are scored.  When vocals and
     accompaniment are both present, accompaniment leaves the list and the pair is scored as its own 2-source problem,
     reported last; the remaining targets (vocals included) are scored together if there are at least two of them, and
-    all but vocals are reported from that problem.  Frames are one second at `rate` (win = hop).  Returns
+    all but vocals are reported from that problem.  Frames are one second at `rate` (win = hop), scored with BSS Eval
+    `mode` (evaluate).  Returns
     {"targets": [...]} in museval's JSON layout (NaN for silent frames) and writes it to <output_dir>/<track_name>.json
     when output_dir is given."""
+    check_mode(mode)
     win = hop = int(rate)
     names = [n for n in references if n in estimates]
     has_acc = "vocals" in names and "accompaniment" in names
@@ -232,7 +247,7 @@ def eval_track(references, estimates, rate, output_dir=None, track_name=None):
     for group, report in scenarios:
         ref = np.stack([np.asarray(references[n]) for n in group])
         est = np.stack([_pad_or_truncate(np.asarray(estimates[n])[None], ref.shape[1])[0] for n in group])
-        sdr, isr, sir, sar = evaluate(ref, est, win, hop)
+        sdr, isr, sir, sar = evaluate(ref, est, win, hop, mode=mode)
         for k, name in enumerate(group):
             if name not in report:
                 continue

@@ -1,7 +1,7 @@
 """Prediction entry point (stand-in for /root/reference/Predict.py:1-17):
 
     python Predict.py with cfg.full_44KHz model_path=checkpoints/123/123-2000 input_path=song.wav [output_path=out]
-                      [output_format=flac [bit_depth=16|24]]
+                      [output_format=flac [bit_depth=16|24]] [references_path=refs results_dir=dir [bss_mode=v4|v3]]
 
 model_path:  a TF-V2 checkpoint prefix (written by Training.py here or by the reference's Saver) or a round-1 .npz.
 input_path:
@@ -25,7 +25,9 @@ output_format=flac is an error, as is output_format=flac with a .npy input.
 
 With references_path= and results_dir=<dir>, the predictions are also scored with BSS Eval v4 on the GPU
 (Evaluate.eval_track, the reference's museval.eval_mus_track at Evaluate.py:71) at the input's rate and written to
-<results_dir>/<input file name>.json, which Evaluate.compute_mean_metrics reads.  references_path is a directory of
+<results_dir>/<input file name>.json, which Evaluate.compute_mean_metrics reads.  bss_mode=v3 scores with museval's
+mode="v3" instead (distortion filters solved for every frame, as SiSEC 2016 / DSD100-era results were computed); the JSON
+layout is the same.  bss_mode without both references_path and results_dir is an error, as is any value but v4 or v3.  references_path is a directory of
 <source>.wav or <source>.flac stems at the input's rate, or a .npz with one [n_frames, n_channels] array per source name.  Mono-model
 estimates are tiled to the references' channel count (Evaluate.py:66-67).
 """
@@ -124,18 +126,32 @@ def output_options(output_format=None, bit_depth=None):
     return fmt, depth
 
 
+def scoring_options(references_path=None, results_dir=None, bss_mode=None):
+    """(score?, BSS Eval mode) from the command line's references_path=, results_dir= and bss_mode=; ValueError for a
+    mode other than v4 / v3, or for bss_mode without both references_path and results_dir."""
+    score = references_path is not None and results_dir is not None
+    if bss_mode is None:
+        return score, "v4"
+    if not score:
+        raise ValueError("bss_mode= is only meaningful with references_path= and results_dir=")
+    mode = str(bss_mode).lower()
+    if mode not in Evaluate.BSS_MODES:
+        raise ValueError("bss_mode=%s: must be one of %s" % (bss_mode, ", ".join(Evaluate.BSS_MODES)))
+    return score, mode
+
+
 def main(cfg, model_path, input_path, output_path=None, references_path=None, results_dir=None, output_format="wav",
-         bit_depth=None):
+         bit_depth=None, bss_mode=None):
     output_format, bit_depth = output_options(output_format, bit_depth)
+    score, mode = scoring_options(references_path, results_dir, bss_mode)
     model_config = cfg["model_config"]
     base = output_path if output_path is not None else input_path
     track = os.path.splitext(os.path.basename(input_path))[0]
-    score = references_path is not None and results_dir is not None
     if input_path.lower().endswith((".wav", ".flac")):
         rate, mix = read_audio(input_path)
         refs = load_references(references_path, rate) if score else None
         preds = Evaluate.predict(model_config, Evaluate.load_separator(model_config, model_path), mix, rate,
-                                 references=refs, results_dir=results_dir, track_name=track)
+                                 references=refs, results_dir=results_dir, track_name=track, mode=mode)
         for name, audio in preds.items():
             if output_format == "flac":
                 write_flac("%s_%s.flac" % (base, name), audio, rate, bit_depth)
@@ -153,7 +169,7 @@ def main(cfg, model_path, input_path, output_path=None, references_path=None, re
         nchan = next(iter(refs.values())).shape[1]
         est = {name: np.tile(audio, [1, nchan]) if audio.shape[1] == 1 and nchan > 1 else audio
                for name, audio in preds.items()}
-        Evaluate.eval_track(refs, est, model_config["expected_sr"], output_dir=results_dir, track_name=track)
+        Evaluate.eval_track(refs, est, model_config["expected_sr"], output_dir=results_dir, track_name=track, mode=mode)
     return preds
 
 
@@ -167,11 +183,12 @@ if __name__ == "__main__":
     if "input_path" not in extras:
         raise SystemExit("Predict.py: input_path=<song.wav, song.flac or mix.npy> is required (the reference's default, an "
                          "mp3 of audio_examples/, is not a format read here); output_format=flac [bit_depth=16|24] writes "
-                         "FLAC estimates\n" + __doc__)
+                         "FLAC estimates; references_path= results_dir= [bss_mode=v4|v3] scores them\n" + __doc__)
     try:
         output_options(extras.get("output_format"), extras.get("bit_depth"))
+        scoring_options(extras.get("references_path"), extras.get("results_dir"), extras.get("bss_mode"))
     except ValueError as ex:
         raise SystemExit("Predict.py: %s\n%s" % (ex, __doc__))
     main(cfg, extras.get("model_path", DEFAULT_MODEL_PATH), extras["input_path"], extras.get("output_path"),
          extras.get("references_path"), extras.get("results_dir"), extras.get("output_format", "wav"),
-         extras.get("bit_depth"))
+         extras.get("bit_depth"), extras.get("bss_mode"))

@@ -3,10 +3,15 @@
 // museval.eval_mus_track (Evaluate.py:71).  DESIGN.md §4.5 describes the stages; oracle/bsseval_oracle.py restates them
 // in numpy.
 //
+// BSS Eval v3 (mode="v3": the same decomposition with the filters solved again for every frame, from that frame's samples
+// only) runs the same stages over batches of frames (wun_bss_eval_v3, DESIGN.md §4.12).
+//
 // Every sum runs in a fixed order (per-CTA partial slots, then an ordered second pass; no float atomics), so a call
 // returns the same bits on every run.  fp32 inputs are widened to fp64 when staged: each product of two of them is exact.
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <algorithm>
 
 #include "../../include/wun.h"
 
@@ -24,20 +29,41 @@ constexpr int kEnergies = 7;
 
 __host__ __device__ constexpr int skew(int i) { return i + (i >> 4); }  // one pad double per 16: stride-8 reads hit distinct banks
 
+// The frames one launch covers.  v4 (list == nullptr): a single slot, the whole track.  v3: slot s of the pass is frame
+// list[1 + s0 + s] while s0 + s < list[0] (list holds the frames that are not silent, in order) and idle beyond, so that
+// silent frames cost no work although the host, which never synchronises, does not know how many there are.  Batched
+// kernels hold `per` systems per slot.
+struct Pass {
+    const int* list;
+    int64_t s0;
+    int per;
+};
+
+__device__ __forceinline__ int64_t pass_frame(const Pass& p, int64_t slot) {
+    if (!p.list) return 0;
+    return p.s0 + slot < p.list[0] ? p.list[1 + p.s0 + slot] : -1;
+}
+
 // ---- stage 1: lag correlations corr(x, y, tau) = sum_m x[m] y[m + tau], tau in [0, L) ----------------------------------------
 // Task t = a * 2nref + s pairs reference signal a = (k, c) with signal s: references 0..nref-1, then estimates.  G needs
 // every ordered reference pair (corr(a, b, -tau) = corr(b, a, tau)), D every (reference, estimate) pair.  CTA (seg, t) sums
 // its segment of samples; thread i owns lags 8i .. 8i+7 and slides a window of y through registers.
+// v3 (blockIdx.z: the pass's slot): the frame's slice [t*hop, t*hop + win) stands for the whole track, so a product that
+// reaches outside the frame is never formed - museval zero-extends each slice.
 __global__ void __launch_bounds__(kXcThreads) bss_xcorr_kernel(const float* __restrict__ ref, const float* __restrict__ est,
                                                                 int nsrc, int nchan, int64_t N, int64_t seg_len,
-                                                                double* __restrict__ slots) {
+                                                                double* __restrict__ slots, Pass pass, int64_t win,
+                                                                int64_t hop) {
+    const int64_t t = pass_frame(pass, blockIdx.z);
+    if (t < 0) return;
     __shared__ double xs[kXcChunk];
     __shared__ double ys[skew(kXcChunk + kL)];
     const int nref = nsrc * nchan, task = blockIdx.y, tid = threadIdx.x;
     const int a = task / (2 * nref), s = task % (2 * nref), b = s % nref;
-    const float* xp = ref + (int64_t)(a / nchan) * N * nchan + a % nchan;
-    const float* yp = (s < nref ? ref : est) + (int64_t)(b / nchan) * N * nchan + b % nchan;
-    const int64_t lo = (int64_t)blockIdx.x * seg_len, hi = min(N, lo + seg_len);
+    const int64_t f0 = pass.list ? t * hop : 0, len = pass.list ? win : N;
+    const float* xp = ref + ((int64_t)(a / nchan) * N + f0) * nchan + a % nchan;
+    const float* yp = (s < nref ? ref : est) + ((int64_t)(b / nchan) * N + f0) * nchan + b % nchan;
+    const int64_t lo = (int64_t)blockIdx.x * seg_len, hi = min(len, lo + seg_len);
     double acc[kR];
 #pragma unroll
     for (int i = 0; i < kR; ++i) acc[i] = 0.0;
@@ -49,7 +75,7 @@ __global__ void __launch_bounds__(kXcThreads) bss_xcorr_kernel(const float* __re
         }
         for (int i = tid; i < kXcChunk + kL; i += kXcThreads) {
             const int64_t m = m0 + i;
-            ys[skew(i)] = m < N ? (double)yp[m * nchan] : 0.0;
+            ys[skew(i)] = m < len ? (double)yp[m * nchan] : 0.0;
         }
         __syncthreads();
         double w[2 * kR];
@@ -68,15 +94,18 @@ __global__ void __launch_bounds__(kXcThreads) bss_xcorr_kernel(const float* __re
             for (int k = 0; k < kR; ++k) w[k] = w[kR + k];
         }
     }
-    double* out = slots + ((int64_t)blockIdx.x * gridDim.y + task) * kL + kR * tid;
+    double* out = slots + (((int64_t)blockIdx.z * gridDim.x + blockIdx.x) * gridDim.y + task) * kL + kR * tid;
 #pragma unroll
     for (int i = 0; i < kR; ++i) out[i] = acc[i];
 }
 
-// lags[t][tau] = sum over segments in order
-__global__ void bss_lag_reduce_kernel(const double* __restrict__ slots, int64_t nseg, int64_t nvals, double* __restrict__ lags) {
+// lags[t][tau] = sum over segments in order (blockIdx.y: the pass's slot)
+__global__ void bss_lag_reduce_kernel(const double* __restrict__ slots, int64_t nseg, int64_t nvals, double* __restrict__ lags,
+                                      Pass pass) {
     const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (v >= nvals) return;
+    if (v >= nvals || pass_frame(pass, blockIdx.y) < 0) return;
+    slots += (int64_t)blockIdx.y * nseg * nvals;
+    lags += (int64_t)blockIdx.y * nvals;
     double s = 0.0;
     for (int64_t g = 0; g < nseg; ++g) s += slots[g * nvals + v];
     lags[v] = s;
@@ -93,13 +122,17 @@ __device__ __forceinline__ double gram(const double* lags, int nref, int a, int 
 }
 
 // Lower triangle of G + eps I (z = 0, order nref*L) and of the diagonal blocks G[j,j] + eps I (z = 1 + j, order nchan*L).
-// The epsilon is museval's: numpy's float64 eps, added to the whole diagonal.
+// The epsilon is museval's: numpy's float64 eps, added to the whole diagonal.  blockIdx.z = slot * (1 + nsrc) + z.
 __global__ void bss_assemble_gram_kernel(const double* __restrict__ lags, int nsrc, int nchan, double* __restrict__ G,
-                                         double* __restrict__ Gjj) {
-    const int nref = nsrc * nchan, z = blockIdx.z;
+                                         double* __restrict__ Gjj, Pass pass) {
+    const int nref = nsrc * nchan, slot = blockIdx.z / (1 + nsrc), z = blockIdx.z % (1 + nsrc);
     const int n = (z == 0 ? nref : nchan) * kL, a0 = z == 0 ? 0 : (z - 1) * nchan;
     const int i = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || j > i) return;
+    if (i >= n || j > i || pass_frame(pass, slot) < 0) return;
+    const int64_t nbig = (int64_t)nref * kL, nsmall = (int64_t)nchan * kL;
+    lags += (int64_t)slot * 2 * nref * nref * kL;
+    G += slot * nbig * nbig;
+    Gjj += slot * nsrc * nsmall * nsmall;
     double* A = z == 0 ? G : Gjj + (int64_t)(z - 1) * n * n;
     double v = gram(lags, nref, a0 + i / kL, i % kL, a0 + j / kL, j % kL);
     if (i == j) v += 2.220446049250313e-16;
@@ -110,10 +143,13 @@ __global__ void bss_assemble_gram_kernel(const double* __restrict__ lags, int ns
 //   C  [j][e][(k, c, l)] = D_j[(k, c, l), e] = <S_l r_{k,c}, est_{j,e}>
 //   Cj [j][e][(c, l)]    = D_j[(j, c, l), e]   (source j's rows: the single-source system against G[j,j])
 __global__ void bss_assemble_rhs_kernel(const double* __restrict__ lags, int nsrc, int nchan, double* __restrict__ C,
-                                        double* __restrict__ Cj) {
+                                        double* __restrict__ Cj, Pass pass) {
     const int nref = nsrc * nchan, col = blockIdx.y, j = col / nchan, e = col % nchan;
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= nref * kL) return;
+    if (r >= nref * kL || pass_frame(pass, blockIdx.z) < 0) return;
+    lags += (int64_t)blockIdx.z * 2 * nref * nref * kL;
+    C += (int64_t)blockIdx.z * nref * nref * kL;
+    Cj += (int64_t)blockIdx.z * nref * nchan * kL;
     const int a = r / kL, l = r % kL;
     const double v = lag(lags, nref, a, nref + j * nchan + e, l);
     C[(int64_t)col * nref * kL + r] = v;
@@ -124,7 +160,8 @@ __global__ void bss_assemble_rhs_kernel(const double* __restrict__ lags, int nsr
 // After panel k0: L (unit diagonal implied) below the diagonal, D on it; the panel's columns of L are mirrored into the upper
 // triangle (A[p][i] = L[i][p], i beyond the panel's diagonal block) so that back substitution reads them coalesced.
 // Batch z: A + z * n * n.  n is a multiple of 64.
-__global__ void __launch_bounds__(256) bss_ldl_diag_kernel(double* __restrict__ A0, int n, int k0) {
+__global__ void __launch_bounds__(256) bss_ldl_diag_kernel(double* __restrict__ A0, int n, int k0, Pass pass) {
+    if (pass_frame(pass, blockIdx.x / pass.per) < 0) return;
     __shared__ double S[kPanel][kPanel + 1];
     double* A = A0 + (int64_t)blockIdx.x * n * n;
     const int tid = threadIdx.x;
@@ -150,7 +187,8 @@ __global__ void __launch_bounds__(256) bss_ldl_diag_kernel(double* __restrict__ 
 }
 
 // Rows below the diagonal block: l_i = (L11^{-1} a_i) / d, one row per thread.
-__global__ void __launch_bounds__(128) bss_ldl_panel_kernel(double* __restrict__ A0, int n, int k0) {
+__global__ void __launch_bounds__(128) bss_ldl_panel_kernel(double* __restrict__ A0, int n, int k0, Pass pass) {
+    if (pass_frame(pass, blockIdx.y / pass.per) < 0) return;
     extern __shared__ double sm[];
     double* Ld = sm;                          // [64][65]: L11 below, d on the diagonal
     double* R = sm + kPanel * (kPanel + 1);   // [64][129]: the CTA's rows, transposed
@@ -220,6 +258,60 @@ __global__ void __launch_bounds__(256) bss_ldl_update_kernel(double* __restrict_
         }
 }
 
+// D = A B + C on the FP64 tensor cores, one 8x8x4 step: a = A[g][q], b = B[q][g], c/d = C[g][2q + i] (g = lane / 4, q = lane % 4).
+__device__ __forceinline__ void dmma_8x8x4(double (&d)[2], double a, double b) {
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};\n"
+                 : "+d"(d[0]), "+d"(d[1])
+                 : "d"(a), "d"(b));
+}
+
+// The same trailing update as bss_ldl_update_kernel (v3's batches of frames, blockIdx.z = system), with the products on the
+// FP64 tensor cores: each warp owns a 16x32 part of the 64x64 tile as 2x4 accumulators of mma.m8n8k4, and the panel's
+// columns run in k order, four per MMA.  Row pitch 36 doubles (4 mod 16): a fragment load's 8 rows x 4 columns hit
+// distinct banks.
+__global__ void __launch_bounds__(256) bss_ldl_update_dmma_kernel(double* __restrict__ A0, int n, int k0, Pass pass) {
+    const int ti = blockIdx.y, tj = blockIdx.x;
+    if (tj > ti || pass_frame(pass, blockIdx.z / pass.per) < 0) return;
+    constexpr int kK = kPanel / 2, kPitch = kK + 4;
+    __shared__ double Li[kPanel][kPitch];
+    __shared__ double Lj[kPanel][kPitch];
+    double* A = A0 + (int64_t)blockIdx.z * n * n;
+    const int tid = threadIdx.x, lane = tid % 32, warp = tid / 32, g = lane / 4, q = lane % 4;
+    const int k1 = k0 + kPanel, i0 = k1 + ti * kPanel, j0 = k1 + tj * kPanel;
+    const int wr = (warp / 2) * 16, wc = (warp % 2) * 32;
+    double acc[2][4][2] = {};
+    for (int kh = 0; kh < kPanel; kh += kK) {
+        __syncthreads();
+        for (int idx = tid; idx < kPanel * kK; idx += 256) {
+            const int r = idx / kK, k = idx % kK, kk = k0 + kh + k;
+            Li[r][k] = A[(int64_t)(i0 + r) * n + kk];
+            Lj[r][k] = A[(int64_t)(j0 + r) * n + kk] * A[(int64_t)kk * n + kk];
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < kK; k += 4) {
+            double a[2], b[4];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) a[r] = Li[wr + 8 * r + g][k + q];
+#pragma unroll
+            for (int c = 0; c < 4; ++c) b[c] = Lj[wc + 8 * c + g][k + q];
+#pragma unroll
+            for (int r = 0; r < 2; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c) dmma_8x8x4(acc[r][c], a[r], b[c]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int i = i0 + wr + 8 * r + g, j = j0 + wc + 8 * c + 2 * q + h;
+                if (j <= i) A[(int64_t)i * n + j] -= acc[r][c][h];
+            }
+}
+
 __device__ __forceinline__ double warp_sum(double s) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
@@ -229,7 +321,9 @@ __device__ __forceinline__ double warp_sum(double s) {
 // L D L^T x = b for one right-hand side column per CTA (grid: columns x batch), solved in place.  Left-looking: each
 // panel's rows first subtract the finished part as warp dot products (coalesced along a row of L, or along the mirrored
 // row of L^T), then the 64x64 unit-triangular block is solved column by column.
-__global__ void __launch_bounds__(256) bss_ldl_solve_kernel(const double* __restrict__ A0, int n, double* __restrict__ B0) {
+__global__ void __launch_bounds__(256) bss_ldl_solve_kernel(const double* __restrict__ A0, int n, double* __restrict__ B0,
+                                                            Pass pass) {
+    if (pass_frame(pass, blockIdx.y / pass.per) < 0) return;
     extern __shared__ double y[];
     const double* A = A0 + (int64_t)blockIdx.y * n * n;
     double* b = B0 + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * n;
@@ -274,17 +368,21 @@ __global__ void __launch_bounds__(256) bss_ldl_solve_kernel(const double* __rest
 // and P_j = sum_c Cj_j * slice of r_{j,c}, over the frame's W = win + L - 1 samples (slices zero-extended, no context from
 // neighbouring frames).  Only the seven energies leave the CTA, as one ordered partial per tile.  Samples past W come out as
 // zero (every tap reads beyond the slice there) and add nothing.
-template <int NCH>
+// FRAMEWISE (v3): blockIdx.x / ntile is the pass's slot, which holds the frame's own filters; idle slots exit.
+template <int NCH, bool FRAMEWISE>
 __global__ void __launch_bounds__(kFrThreads) bss_frame_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est,
                                                                        const double* __restrict__ C, const double* __restrict__ Cj,
                                                                        int nsrc, int64_t N, int64_t win, int64_t hop, int ntile,
-                                                                       double* __restrict__ energies) {
+                                                                       double* __restrict__ energies, Pass pass) {
+    const int64_t t = FRAMEWISE ? pass_frame(pass, blockIdx.x / ntile) : blockIdx.x / ntile;
+    if (FRAMEWISE && t < 0) return;
+    const int64_t slot = FRAMEWISE ? blockIdx.x / ntile : 0;   // the frame's own filters
     __shared__ double xs[skew(kFrTile + kL)];
     __shared__ double h[NCH][kL], hj[NCH][kL];
     __shared__ double red[kEnergies][kFrThreads];
     const int nref = nsrc * NCH, tid = threadIdx.x, j = blockIdx.y;
     const int tile = blockIdx.x % ntile;
-    const int64_t t = blockIdx.x / ntile, f0 = t * hop, w0 = (int64_t)tile * kFrTile;
+    const int64_t f0 = t * hop, w0 = (int64_t)tile * kFrTile;
     double pa[NCH][kR], pj[NCH][kR];
 #pragma unroll
     for (int e = 0; e < NCH; ++e)
@@ -301,8 +399,8 @@ __global__ void __launch_bounds__(kFrThreads) bss_frame_energy_kernel(const floa
         }
         for (int u = tid; u < NCH * kL; u += kFrThreads) {
             const int e = u / kL, l = u % kL;
-            h[e][kL - 1 - l] = C[((int64_t)(j * NCH + e) * nref + a) * kL + l];
-            if (own) hj[e][kL - 1 - l] = Cj[((int64_t)(j * NCH + e) * NCH + a % NCH) * kL + l];
+            h[e][kL - 1 - l] = C[((slot * nref + j * NCH + e) * nref + a) * kL + l];
+            if (own) hj[e][kL - 1 - l] = Cj[((slot * nref + j * NCH + e) * NCH + a % NCH) * kL + l];
         }
         __syncthreads();
         double w[2 * kR];
@@ -365,13 +463,10 @@ __device__ __forceinline__ double safe_db(double num, double den) {
     return den == 0.0 ? __longlong_as_double(0x7ff0000000000000LL) : 10.0 * log10(num / den);
 }
 
-// One CTA per frame: museval's silence rule, then the four metrics of every target from its tiles' energies (in order).
-__global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __restrict__ ref, const float* __restrict__ est,
-                                                                int nsrc, int nchan, int64_t N, int64_t win, int64_t hop,
-                                                                int64_t nwin, int ntile, const double* __restrict__ energies,
-                                                                double* __restrict__ metrics) {
-    const int64_t t = blockIdx.x, f0 = t * hop;
-    // A frame is NaN for every target if some reference or some estimate has sum_c x[n][c] == 0 on every sample of it.
+// museval's _any_source_silent over references and estimates: frame t is NaN for every target if some reference or some
+// estimate has sum_c x[n][c] == 0 on every sample of it.  Called by every thread of the CTA.
+__device__ bool frame_silent(const float* __restrict__ ref, const float* __restrict__ est, int nsrc, int nchan, int64_t N,
+                             int64_t win, int64_t f0) {
     bool silent = false;
     for (int k = 0; k < 2 * nsrc; ++k) {
         const float* x = (k < nsrc ? ref : est) + (int64_t)(k % nsrc) * N * nchan;
@@ -383,6 +478,16 @@ __global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __r
         }
         silent |= !__syncthreads_or(nonzero);
     }
+    return silent;
+}
+
+// One CTA per frame: the silence rule, then the four metrics of every target from its tiles' energies (in order).
+__global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __restrict__ ref, const float* __restrict__ est,
+                                                                int nsrc, int nchan, int64_t N, int64_t win, int64_t hop,
+                                                                int64_t nwin, int ntile, const double* __restrict__ energies,
+                                                                double* __restrict__ metrics) {
+    const int64_t t = blockIdx.x, f0 = t * hop;
+    const bool silent = frame_silent(ref, est, nsrc, nchan, N, win, f0);
     const int j = threadIdx.x;
     if (j >= nsrc) return;
     double E[kEnergies] = {};
@@ -400,6 +505,37 @@ __global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __r
     metrics[m + o] = isr;
     metrics[2 * m + o] = sir;
     metrics[3 * m + o] = sar;
+}
+
+// ---- v3: the frames to solve ------------------------------------------------------------------------------------------------
+// One CTA per frame: silent[t] = the silence rule of bss_frame_metrics_kernel, which later turns the frame into NaN.
+__global__ void __launch_bounds__(256) bss_frame_silent_kernel(const float* __restrict__ ref, const float* __restrict__ est,
+                                                               int nsrc, int nchan, int64_t N, int64_t win, int64_t hop,
+                                                               int* __restrict__ silent) {
+    const bool s = frame_silent(ref, est, nsrc, nchan, N, win, (int64_t)blockIdx.x * hop);
+    if (threadIdx.x == 0) silent[blockIdx.x] = s;
+}
+
+// list[0] = the number of frames that are not silent, list[1..] those frames in order.  One thread: nwin is small.
+__global__ void bss_frame_list_kernel(const int* __restrict__ silent, int64_t nwin, int* __restrict__ list) {
+    int count = 0;
+    for (int64_t t = 0; t < nwin; ++t)
+        if (!silent[t]) list[1 + count++] = (int)t;
+    list[0] = count;
+}
+
+// filters[t] = (C, Cj) of frame t: the pass's slots copied to their frames (blockIdx.x: slot), or NaN for the silent
+// frames (silent != nullptr, blockIdx.x: frame), whose filters are never computed.
+__global__ void bss_frame_filters_kernel(const double* __restrict__ C, const double* __restrict__ Cj, int64_t csz, int64_t cjsz,
+                                         const int* __restrict__ silent, Pass pass, double* __restrict__ filters) {
+    const int64_t i = (int64_t)blockIdx.y * blockDim.x + threadIdx.x, b = blockIdx.x;
+    if (i >= csz + cjsz) return;
+    if (silent) {
+        if (silent[b]) filters[b * (csz + cjsz) + i] = __longlong_as_double(0x7ff8000000000000LL);
+        return;
+    }
+    const int64_t t = pass_frame(pass, b);
+    if (t >= 0) filters[t * (csz + cjsz) + i] = i < csz ? C[b * csz + i] : Cj[b * cjsz + i - csz];
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------------------
@@ -435,23 +571,27 @@ bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t ho
     return true;
 }
 
-// Blocked LDL^T of `batch` matrices of order n, then solve for ncol right-hand-side columns each.
-cudaError_t ldl_solve(double* A, int n, int batch, double* B, int ncol, cudaStream_t st) {
+// Blocked LDL^T of `batch` matrices of order n, then solve for ncol right-hand-side columns each.  v4 (pass.list == nullptr)
+// keeps its CUDA-core trailing update; v3's batches of frames take the tensor-core one.
+cudaError_t ldl_solve(double* A, int n, int batch, double* B, int ncol, Pass pass, cudaStream_t st) {
     const int panel_smem = (kPanel * (kPanel + 1) + kPanel * 129) * 8;
     cudaError_t e = cudaFuncSetAttribute(bss_ldl_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, panel_smem);
     if (e == cudaSuccess)
         e = cudaFuncSetAttribute(bss_ldl_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, n * 8);
     if (e != cudaSuccess) return e;
     for (int k0 = 0; k0 < n; k0 += kPanel) {
-        bss_ldl_diag_kernel<<<batch, 256, 0, st>>>(A, n, k0);
+        bss_ldl_diag_kernel<<<batch, 256, 0, st>>>(A, n, k0, pass);
         const int rest = n - k0 - kPanel;
         if (rest > 0) {
-            bss_ldl_panel_kernel<<<dim3((rest + 127) / 128, batch), 128, panel_smem, st>>>(A, n, k0);
+            bss_ldl_panel_kernel<<<dim3((rest + 127) / 128, batch), 128, panel_smem, st>>>(A, n, k0, pass);
             const int nt = rest / kPanel;
-            bss_ldl_update_kernel<<<dim3(nt, nt, batch), 256, 0, st>>>(A, n, k0);
+            if (pass.list)
+                bss_ldl_update_dmma_kernel<<<dim3(nt, nt, batch), 256, 0, st>>>(A, n, k0, pass);
+            else
+                bss_ldl_update_kernel<<<dim3(nt, nt, batch), 256, 0, st>>>(A, n, k0);
         }
     }
-    bss_ldl_solve_kernel<<<dim3(ncol, batch), 256, n * 8, st>>>(A, n, B);
+    bss_ldl_solve_kernel<<<dim3(ncol, batch), 256, n * 8, st>>>(A, n, B, pass);
     return cudaGetLastError();
 }
 
@@ -480,23 +620,25 @@ extern "C" int wun_bss_eval(const float* references, const float* estimates, int
            *Gjj = (double*)(ws + L.Gjj), *C = (double*)(ws + L.C), *Cj = (double*)(ws + L.Cj), *E = (double*)(ws + L.E);
     const int ns = (int)nsrc, nc = (int)nchan, nref = (int)L.nref;
 
+    const Pass whole{nullptr, 0, 1};
     bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)L.ntask), kXcThreads, 0, st>>>(references, estimates, ns, nc, nsampl,
-                                                                                        L.seg_len, slots);
+                                                                                        L.seg_len, slots, whole, win, hop);
     const int64_t nvals = L.ntask * kL;
-    bss_lag_reduce_kernel<<<(unsigned)((nvals + 255) / 256), 256, 0, st>>>(slots, L.nseg, nvals, lags);
-    bss_assemble_gram_kernel<<<dim3((unsigned)(L.n + 255) / 256, (unsigned)L.n, 1 + ns), 256, 0, st>>>(lags, ns, nc, G, Gjj);
-    bss_assemble_rhs_kernel<<<dim3((unsigned)(L.n + 255) / 256, nref), 256, 0, st>>>(lags, ns, nc, C, Cj);
+    bss_lag_reduce_kernel<<<(unsigned)((nvals + 255) / 256), 256, 0, st>>>(slots, L.nseg, nvals, lags, whole);
+    bss_assemble_gram_kernel<<<dim3((unsigned)(L.n + 255) / 256, (unsigned)L.n, 1 + ns), 256, 0, st>>>(lags, ns, nc, G, Gjj,
+                                                                                                       whole);
+    bss_assemble_rhs_kernel<<<dim3((unsigned)(L.n + 255) / 256, nref), 256, 0, st>>>(lags, ns, nc, C, Cj, whole);
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = ldl_solve(G, (int)L.n, 1, C, nref, st);
-    if (e == cudaSuccess) e = ldl_solve(Gjj, (int)L.m, ns, Cj, nc, st);
+    if (e == cudaSuccess) e = ldl_solve(G, (int)L.n, 1, C, nref, whole, st);
+    if (e == cudaSuccess) e = ldl_solve(Gjj, (int)L.m, ns, Cj, nc, whole, st);
     if (e == cudaSuccess && L.nwin > 0) {
         const dim3 grid((unsigned)(L.nwin * L.ntile), ns);
         if (nc == 1)
-            bss_frame_energy_kernel<1><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
-                                                                    (int)L.ntile, E);
+            bss_frame_energy_kernel<1, false><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win,
+                                                                           hop, (int)L.ntile, E, whole);
         else
-            bss_frame_energy_kernel<2><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
-                                                                    (int)L.ntile, E);
+            bss_frame_energy_kernel<2, false><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win,
+                                                                           hop, (int)L.ntile, E, whole);
         bss_frame_metrics_kernel<<<(unsigned)L.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, L.nwin,
                                                                    (int)L.ntile, E, metrics);
         e = cudaGetLastError();
@@ -504,6 +646,116 @@ extern "C" int wun_bss_eval(const float* references, const float* estimates, int
     if (e == cudaSuccess && filters) {
         e = cudaMemcpyAsync(filters, C, L.nref * L.n * 8, cudaMemcpyDeviceToDevice, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(filters + L.nref * L.n, Cj, L.nref * L.m * 8, cudaMemcpyDeviceToDevice, st);
+    }
+    return e == cudaSuccess ? WUN_OK : WUN_E_CUDA;
+}
+
+namespace {
+
+constexpr int kV3Segs = 16;            // sample segments of a frame's correlations (partial slots per lag)
+constexpr int64_t kV3MaxPass = 2048;   // frames per pass at most: keeps the assembly grid's z = slots * (1 + nsrc) in range
+
+// v3's workspace: the silence flags, the frame list and the energies of the whole call, then the per-frame arrays of one
+// pass of P frames.  Every per-frame array is a multiple of 4 KiB, so the total is fixed + P * per_frame.
+struct LayoutV3 {
+    Layout s;                          // shapes as v4 (nref, ntask, n, m, nwin, ntile); its offsets are not used
+    int64_t nseg, seg_len, P;
+    int64_t silent, list, E, slots, lags, G, Gjj, C, Cj;   // byte offsets into the workspace
+    int64_t fixed, per_frame, total;
+};
+
+bool make_layout_v3(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, int64_t frames_per_pass, LayoutV3* o) {
+    if (frames_per_pass < 1 || !make_layout(nsrc, nchan, N, win, hop, &o->s)) return false;
+    const Layout& S = o->s;
+    const int64_t nchunks = (win + kXcChunk - 1) / kXcChunk, per_seg = (nchunks + kV3Segs - 1) / kV3Segs;
+    o->nseg = (nchunks + per_seg - 1) / per_seg;
+    o->seg_len = per_seg * kXcChunk;
+    o->P = std::min(std::min(frames_per_pass, S.nwin), kV3MaxPass);
+    int64_t off = 0;
+    auto take = [&](int64_t bytes) { const int64_t at = off; off += (bytes + 255) / 256 * 256; return at; };
+    o->silent = take(S.nwin * 4);
+    o->list = take((1 + S.nwin) * 4);
+    o->E = take(S.nwin * nsrc * S.ntile * kEnergies * 8);
+    o->fixed = off;
+    const int64_t d_slots = o->nseg * S.ntask * kL, d_lags = S.ntask * kL, d_G = S.n * S.n, d_Gjj = nsrc * S.m * S.m,
+                  d_C = S.nref * S.n, d_Cj = S.nref * S.m;
+    o->per_frame = 8 * (d_slots + d_lags + d_G + d_Gjj + d_C + d_Cj);
+    o->slots = take(o->P * d_slots * 8);
+    o->lags = take(o->P * d_lags * 8);
+    o->G = take(o->P * d_G * 8);
+    o->Gjj = take(o->P * d_Gjj * 8);
+    o->C = take(o->P * d_C * 8);
+    o->Cj = take(o->P * d_Cj * 8);
+    o->total = off;
+    return true;
+}
+
+}  // namespace
+
+extern "C" int64_t wun_bss_eval_v3_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop,
+                                                   int64_t frames_per_pass) {
+    LayoutV3 L;
+    return make_layout_v3(nsrc, nchan, nsampl, win, hop, frames_per_pass, &L) ? L.total : WUN_E_INVALID;
+}
+
+extern "C" int wun_bss_eval_v3(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                               int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+    LayoutV3 L;
+    if (!make_layout_v3(nsrc, nchan, nsampl, win, hop, 1, &L)) return WUN_E_INVALID;
+    const Layout& S = L.s;
+    if (!references || !estimates || !workspace || (!metrics && S.nwin > 0)) return WUN_E_INVALID;
+    if (workspace_bytes < L.total || reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return WUN_E_INVALID;
+    if (S.nwin > 1) make_layout_v3(nsrc, nchan, nsampl, win, hop, (workspace_bytes - L.fixed) / L.per_frame, &L);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        return WUN_E_NOGPU;
+    }
+    if (S.nwin == 0) return WUN_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    int *silent = (int*)(ws + L.silent), *list = (int*)(ws + L.list);
+    double *slots = (double*)(ws + L.slots), *lags = (double*)(ws + L.lags), *G = (double*)(ws + L.G),
+           *Gjj = (double*)(ws + L.Gjj), *C = (double*)(ws + L.C), *Cj = (double*)(ws + L.Cj), *E = (double*)(ws + L.E);
+    const int ns = (int)nsrc, nc = (int)nchan, nref = (int)S.nref;
+    const int64_t csz = S.nref * S.n, cjsz = S.nref * S.m, nvals = S.ntask * kL;
+    const unsigned fblocks = (unsigned)((csz + cjsz + 255) / 256);
+
+    bss_frame_silent_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, silent);
+    bss_frame_list_kernel<<<1, 1, 0, st>>>(silent, S.nwin, list);
+    if (filters)
+        bss_frame_filters_kernel<<<dim3((unsigned)S.nwin, fblocks), 256, 0, st>>>(nullptr, nullptr, csz, cjsz, silent,
+                                                                                  Pass{nullptr, 0, 1}, filters);
+    cudaError_t e = cudaGetLastError();
+    for (int64_t s0 = 0; s0 < S.nwin && e == cudaSuccess; s0 += L.P) {
+        const unsigned np = (unsigned)std::min(L.P, S.nwin - s0);
+        const Pass pass{list, s0, 1}, per_source{list, s0, ns};
+        bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)S.ntask, np), kXcThreads, 0, st>>>(
+            references, estimates, ns, nc, nsampl, L.seg_len, slots, pass, win, hop);
+        bss_lag_reduce_kernel<<<dim3((unsigned)((nvals + 255) / 256), np), 256, 0, st>>>(slots, L.nseg, nvals, lags, pass);
+        bss_assemble_gram_kernel<<<dim3((unsigned)(S.n + 255) / 256, (unsigned)S.n, np * (1 + ns)), 256, 0, st>>>(
+            lags, ns, nc, G, Gjj, pass);
+        bss_assemble_rhs_kernel<<<dim3((unsigned)(S.n + 255) / 256, nref, np), 256, 0, st>>>(lags, ns, nc, C, Cj, pass);
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = ldl_solve(G, (int)S.n, (int)np, C, nref, pass, st);
+        if (e == cudaSuccess) e = ldl_solve(Gjj, (int)S.m, (int)np * ns, Cj, nc, per_source, st);
+        if (e != cudaSuccess) break;
+        const dim3 grid((unsigned)(np * S.ntile), ns);
+        if (nc == 1)
+            bss_frame_energy_kernel<1, true><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
+                                                                          (int)S.ntile, E, pass);
+        else
+            bss_frame_energy_kernel<2, true><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
+                                                                          (int)S.ntile, E, pass);
+        if (filters)
+            bss_frame_filters_kernel<<<dim3(np, fblocks), 256, 0, st>>>(C, Cj, csz, cjsz, nullptr, pass, filters);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        bss_frame_metrics_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, S.nwin,
+                                                                   (int)S.ntile, E, metrics);
+        e = cudaGetLastError();
     }
     return e == cudaSuccess ? WUN_OK : WUN_E_CUDA;
 }

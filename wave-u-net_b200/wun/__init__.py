@@ -19,7 +19,8 @@ SYMBOLS = [
     "wun_launches_forward_backward", "wun_forward", "wun_forward_backward", "wun_adam_step", "wun_adam_step_device", "wun_set_grad_buckets", "wun_stream_wait_grad_bucket",
     "wun_gather_windows", "wun_scatter_windows", "wun_feed_batch", "wun_last_error", "wun_version", "wun_describe",
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
-    "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_resample_frames", "wun_resample",
+    "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_bss_eval_v3_workspace_bytes", "wun_bss_eval_v3",
+    "wun_resample_frames", "wun_resample",
     "wun_snippet_batch", "wun_eval_batch_loss",
     "wun_spec_create", "wun_spec_destroy", "wun_spec_input_frames", "wun_spec_output_frames", "wun_spec_stft_frames",
     "wun_spec_param_count", "wun_spec_param_numel", "wun_spec_param_table", "wun_spec_workspace_bytes",
@@ -127,6 +128,10 @@ def _load():
         lib.wun_bss_eval_workspace_bytes.argtypes = [I64, I64, I64, I64, I64]
         lib.wun_bss_eval_workspace_bytes.restype = I64
         lib.wun_bss_eval.argtypes = [VP, VP, I64, I64, I64, I64, I64, VP, VP, VP, I64, VP]
+    if hasattr(lib, "wun_bss_eval_v3"):     # likewise, and builds from before v3 (WUN_LIB)
+        lib.wun_bss_eval_v3_workspace_bytes.argtypes = [I64, I64, I64, I64, I64, I64]
+        lib.wun_bss_eval_v3_workspace_bytes.restype = I64
+        lib.wun_bss_eval_v3.argtypes = lib.wun_bss_eval.argtypes
     if hasattr(lib, "wun_resample"):        # likewise the resampling kernel
         lib.wun_resample_frames.argtypes = [I64, I64, I64]
         lib.wun_resample_frames.restype = I64
@@ -200,41 +205,62 @@ def check(rc):
 
 
 BSS_FILTER_LEN = 512
+BSS_MODES = ("v4", "v3")
+BSS_V3_WORKSPACE_BYTES = 2 << 30        # 1-s frames at 44.1 kHz: 12 per pass at n = 4096 (4 stereo sources), 40 at n = 2048
 
 
-def bss_eval(references, estimates, win, hop, filters=False):
-    """BSS Eval v4 of `estimates` against `references` (include/wun.h wun_bss_eval): both contiguous float32 CUDA tensors
-    [nsrc, nsampl, nchan] on one device.  Returns float64 CUDA tensors (SDR, ISR, SIR, SAR), each [nsrc, nwin]; with
-    filters=True also (C [nsrc, nchan, nsrc, nchan, 512], Cj [nsrc, nchan, nchan, 512]): the filters for all sources and
-    for each source alone, indexed [target, estimate channel, (source,) reference channel, tap]."""
+def bss_eval(references, estimates, win, hop, filters=False, mode="v4", max_workspace_bytes=BSS_V3_WORKSPACE_BYTES):
+    """BSS Eval of `estimates` against `references` as museval.evaluate(..., mode=mode) computes it: both contiguous float32
+    CUDA tensors [nsrc, nsampl, nchan] on one device.  Returns float64 CUDA tensors (SDR, ISR, SIR, SAR), each [nsrc, nwin];
+    with filters=True also (C [nsrc, nchan, nsrc, nchan, 512], Cj [nsrc, nchan, nchan, 512]): the filters for all sources and
+    for each source alone, indexed [target, estimate channel, (source,) reference channel, tap].
+
+    mode="v4" (include/wun.h wun_bss_eval) solves the filters once over the whole track.  mode="v3" (wun_bss_eval_v3) solves
+    them for every frame from its own samples; the filters then have a leading [nwin] axis and are NaN for silent frames.
+    v3 processes frames in passes, as many per pass as fit in max_workspace_bytes (at least one); the results do not depend
+    on it."""
     import torch
+    if mode not in BSS_MODES:
+        raise ValueError("bss_eval: mode=%r, must be one of %s" % (mode, ", ".join(BSS_MODES)))
     for t in (references, estimates):
         assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 3, \
             "references / estimates must be contiguous float32 CUDA tensors [nsrc, nsampl, nchan]"
     assert estimates.shape == references.shape and estimates.device == references.device, "estimates must match references"
     nsrc, n, nchan = (int(s) for s in references.shape)
-    nbytes = lib.wun_bss_eval_workspace_bytes(nsrc, nchan, n, int(win), int(hop))
+    win, hop = int(win), int(hop)
+    nwin = (n - win) // hop + 1 if n >= win > 0 and hop > 0 else 0
+    if mode == "v4":
+        nbytes = lib.wun_bss_eval_workspace_bytes(nsrc, nchan, n, win, hop)
+    else:
+        nbytes = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, 1)
+        if nbytes >= 0 and nwin > 1:
+            per_frame = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, 2) - nbytes
+            fit = 1 + max(0, int(max_workspace_bytes) - nbytes) // per_frame
+            nbytes = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, min(fit, nwin))
     if nbytes < 0:
         raise WunError(WUN_E_INVALID, "bss_eval: need 1 <= nsrc <= 8, nchan 1 or 2, nsampl, win, hop >= 1 (got %d, %d, %d, %d, %d)"
                        % (nsrc, nchan, n, win, hop))
-    nwin = (n - win) // hop + 1 if n >= win else 0
     dev = references.device
     metrics = torch.empty((4, nsrc, nwin), dtype=torch.float64, device=dev)
+    fsz = nsrc * nchan * (nsrc * nchan + nchan) * BSS_FILTER_LEN
     filt = None
     if filters:
-        filt = torch.empty(nsrc * nchan * (nsrc * nchan + nchan) * BSS_FILTER_LEN, dtype=torch.float64, device=dev)
+        filt = torch.empty((nwin if mode == "v3" else 1) * fsz, dtype=torch.float64, device=dev)
     ws = torch.empty((nbytes + 255) // 256 * 32, dtype=torch.float64, device=dev)      # torch allocations are 256-B aligned
+    call = lib.wun_bss_eval if mode == "v4" else lib.wun_bss_eval_v3
     with torch.cuda.device(dev):
-        rc = lib.wun_bss_eval(references.data_ptr(), estimates.data_ptr(), nsrc, nchan, n, int(win), int(hop),
-                              metrics.data_ptr() if nwin else None, filt.data_ptr() if filt is not None else None,
-                              ws.data_ptr(), ws.numel() * 8, Engine._stream(dev))
+        rc = call(references.data_ptr(), estimates.data_ptr(), nsrc, nchan, n, win, hop,
+                  metrics.data_ptr() if nwin else None, filt.data_ptr() if filt is not None else None,
+                  ws.data_ptr(), ws.numel() * 8, Engine._stream(dev))
     if rc != WUN_OK:
-        raise WunError(rc, "wun_bss_eval failed")
+        raise WunError(rc, "%s failed" % ("wun_bss_eval" if mode == "v4" else "wun_bss_eval_v3"))
     out = tuple(metrics)
     if filters:
         nc = nsrc * nchan * nsrc * nchan * BSS_FILTER_LEN
-        out += (filt[:nc].view(nsrc, nchan, nsrc, nchan, BSS_FILTER_LEN),
-                filt[nc:].view(nsrc, nchan, nchan, BSS_FILTER_LEN))
+        f = filt.view(-1, fsz)
+        lead = (nwin,) if mode == "v3" else ()
+        out += (f[:, :nc].reshape(lead + (nsrc, nchan, nsrc, nchan, BSS_FILTER_LEN)),
+                f[:, nc:].reshape(lead + (nsrc, nchan, nchan, BSS_FILTER_LEN)))
     return out
 
 
