@@ -203,6 +203,31 @@ int wun_bss_eval_v3(const float* references, const float* estimates, int64_t nsr
                     int64_t win, int64_t hop, double* metrics, double* filters, void* workspace, int64_t workspace_bytes,
                     void* stream);
 
+/* museval 0.2.0 bss_eval(references, estimates, win, hop, compute_permutation, filters_len=512, framewise_filters,
+ * bsseval_sources_version) with its three switches as flags (the function behind museval.metrics' bss_eval_sources /
+ * bss_eval_images and their _framewise forms).  wun_bss_eval is flags 0, wun_bss_eval_v3 WUN_BSS_FRAMEWISE_FILTERS: the
+ * same bits and workspace sizes.
+ *   WUN_BSS_FRAMEWISE_FILTERS  the filters solved for every frame (v3); frames_per_pass as in wun_bss_eval_v3 (ignored
+ *                              without this flag)
+ *   WUN_BSS_PERMUTATION        every (reference jtrue, estimate jest) pair is scored; per frame the candidate of
+ *                              itertools.permutations(range(nsrc)) with the largest mean pair SIR is kept (the first on a
+ *                              tie, the identity for a silent frame)
+ *   WUN_BSS_SOURCES            the "sources" decomposition: SDR = |P_j|^2 / |est - P_j|^2, ISR NaN; SIR and SAR unchanged
+ *   metrics       DEVICE float64 [4][nsrc][nwin]; row j is estimate j (scored against reference perm[j][t])
+ *   perm          DEVICE int64 [nsrc][nwin], required with WUN_BSS_PERMUTATION (when nwin > 0), NULL without it
+ *   pair_metrics  optional DEVICE float64 [4][nsrc (jtrue)][nsrc (jest)][nwin] (WUN_BSS_PERMUTATION only, else NULL)
+ *   filters       optional, as in wun_bss_eval / wun_bss_eval_v3; with WUN_BSS_PERMUTATION the Cj part holds every pair,
+ *                 Cj[jtrue][jest][e][c][l]
+ * An unknown flag bit is WUN_E_INVALID; other checks and return codes as wun_bss_eval. */
+#define WUN_BSS_FRAMEWISE_FILTERS 1
+#define WUN_BSS_PERMUTATION       2
+#define WUN_BSS_SOURCES           4
+int64_t wun_bss_eval_ex_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop, int flags,
+                                        int64_t frames_per_pass);
+int wun_bss_eval_ex(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                    int64_t win, int64_t hop, int flags, double* metrics, int64_t* perm, double* pair_metrics,
+                    double* filters, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* --- resampling (no handle) ----------------------------------------------------------------------
  * librosa 0.6.2 resample(y, sr_in, sr_out) with res_type='kaiser_best', which the reference applies to every track before and
  * after separation (Evaluate.py:64,104, Utils.resample): resampy 0.2's resample_f bit for bit, then fix_length's zero

@@ -12,7 +12,9 @@ predict_track works on arrays already at model_config["expected_sr"]; predict() 
 60-71) on an array at any rate, resampling on the GPU with librosa's kaiser_best (wun.resample) on the way in and out.
 Scoring is here: evaluate() / eval_track() replace museval.evaluate / museval.eval_mus_track (Evaluate.py:71) with BSS
 Eval v4 on the GPU (wun.bss_eval), or with museval's mode="v3" (filters solved per frame) when asked for, and
-compute_mean_metrics is the reference's (Evaluate.py:195-232).
+compute_mean_metrics is the reference's (Evaluate.py:195-232).  bss_eval and bss_eval_sources / bss_eval_images (and their
+_framewise forms) are museval.metrics' functions of those names, with the permutation search and the "sources" decomposition,
+on the GPU as well; the MUSDB path above does not use them, since museval never permutes named targets.
 produce_musdb_source_estimates runs them over the MUSDB18 WAV layout.  Audio decoding beyond WAV (Predict.py) and the musdb
 package are out of scope (SURVEY section 2).
 """
@@ -262,6 +264,83 @@ def eval_track(references, estimates, rate, output_dir=None, track_name=None, mo
         with open(os.path.join(output_dir, "%s.json" % (track_name or "track")), "w") as f:
             json.dump(scores, f, indent=2, allow_nan=True)
     return scores
+
+
+def _device_bss_eval_ex(references, estimates, win, hop, compute_permutation, framewise_filters, sources_version):
+    """[nsrc, N, nchan] float arrays -> (numpy float64 [4 (SDR, ISR, SIR, SAR), nsrc, nwin], int64 popt [nsrc, nwin]) from
+    wun.bss_eval; popt is the identity without compute_permutation."""
+    import torch
+    import wun
+    ref = torch.from_numpy(np.ascontiguousarray(references, dtype=np.float32)).cuda()
+    est = torch.from_numpy(np.ascontiguousarray(estimates, dtype=np.float32)).cuda()
+    out = wun.bss_eval(ref, est, win, hop, mode="v3" if framewise_filters else "v4", permutation=compute_permutation,
+                       sources_version=sources_version)
+    metrics = torch.stack(out[:4]).cpu().numpy()
+    if compute_permutation:
+        return metrics, out[4].cpu().numpy()
+    return metrics, np.tile(np.arange(metrics.shape[1], dtype=np.int64)[:, None], (1, metrics.shape[2]))
+
+
+def _sources(x, what):
+    """[nsrc, nsampl] gets a channel axis: [nsrc, nsampl, 1]."""
+    x = np.asarray(x)
+    if x.ndim == 2:
+        x = x[:, :, None]
+    if x.ndim != 3:
+        raise ValueError("%s: expected [nsrc, nsampl] or [nsrc, nsampl, nchan], got shape %s" % (what, x.shape))
+    return x
+
+
+def bss_eval(reference_sources, estimated_sources, window=2 * 44100, hop=1.5 * 44100, compute_permutation=False,
+             filters_len=512, framewise_filters=False, bsseval_sources_version=False):
+    """museval.metrics.bss_eval on the GPU: arrays [nsrc, nsampl(, nchan)] of equal shape.  framewise_filters solves the
+    512-tap filters for every frame (mode="v3") instead of once over the signal (mode="v4"); compute_permutation scores every
+    (reference, estimate) pair and keeps, per frame, the permutation with the largest mean SIR; bsseval_sources_version
+    scores the "sources" decomposition (ISR is NaN).  Returns SDR, ISR, SIR, SAR, each [nsrc, nwin] with row j estimate j,
+    and popt [nsrc, nwin], the reference each estimate is scored against (the identity without compute_permutation)."""
+    if filters_len != 512:
+        raise ValueError("filters_len=%r: the GPU solves museval's 512-tap filters only" % (filters_len,))
+    ref, est = _sources(reference_sources, "reference_sources"), _sources(estimated_sources, "estimated_sources")
+    if ref.shape != est.shape:
+        raise ValueError("estimated_sources %s must have the shape of reference_sources %s" % (est.shape, ref.shape))
+    metrics, popt = _device_bss_eval_ex(ref, est, int(window), int(hop), bool(compute_permutation), bool(framewise_filters),
+                                        bool(bsseval_sources_version))
+    sdr, isr, sir, sar = metrics
+    return sdr, isr, sir, sar, popt
+
+
+def bss_eval_sources(reference_sources, estimated_sources, compute_permutation=True):
+    """museval.metrics.bss_eval_sources: the whole signal as one frame, filters over it, "sources" decomposition.
+    Returns SDR, SIR, SAR, perm, each [nsrc, 1]."""
+    n = np.shape(reference_sources)[1]
+    sdr, _, sir, sar, perm = bss_eval(reference_sources, estimated_sources, n, n, compute_permutation,
+                                      framewise_filters=True, bsseval_sources_version=True)
+    return sdr, sir, sar, perm
+
+
+def bss_eval_sources_framewise(reference_sources, estimated_sources, window=30 * 44100, hop=15 * 44100,
+                               compute_permutation=False):
+    """museval.metrics.bss_eval_sources_framewise: filters per frame, "sources" decomposition.  Returns SDR, SIR, SAR,
+    perm, each [nsrc, nwin]."""
+    sdr, _, sir, sar, perm = bss_eval(reference_sources, estimated_sources, window, hop, compute_permutation,
+                                      framewise_filters=True, bsseval_sources_version=True)
+    return sdr, sir, sar, perm
+
+
+def bss_eval_images(reference_sources, estimated_sources, compute_permutation=True):
+    """museval.metrics.bss_eval_images: the whole signal as one frame, filters over it, images decomposition.  Returns
+    SDR, ISR, SIR, SAR, perm, each [nsrc, 1]."""
+    n = np.shape(reference_sources)[1]
+    return bss_eval(reference_sources, estimated_sources, n, n, compute_permutation, framewise_filters=True,
+                    bsseval_sources_version=False)
+
+
+def bss_eval_images_framewise(reference_sources, estimated_sources, window=30 * 44100, hop=15 * 44100,
+                              compute_permutation=False):
+    """museval.metrics.bss_eval_images_framewise: filters per frame, images decomposition.  Returns SDR, ISR, SIR, SAR,
+    perm, each [nsrc, nwin]."""
+    return bss_eval(reference_sources, estimated_sources, window, hop, compute_permutation, framewise_filters=True,
+                    bsseval_sources_version=False)
 
 
 def compute_mean_metrics(json_folder, compute_averages=True, metric="SDR"):

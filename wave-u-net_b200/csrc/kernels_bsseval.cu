@@ -6,6 +6,10 @@
 // BSS Eval v3 (mode="v3": the same decomposition with the filters solved again for every frame, from that frame's samples
 // only) runs the same stages over batches of frames (wun_bss_eval_v3, DESIGN.md §4.12).
 //
+// museval's bss_eval switches (wun_bss_eval_ex, DESIGN.md §4.13): the permutation search scores every (reference,
+// estimate) pair and keeps, per frame, the pairing with the largest mean SIR; the "sources" decomposition changes SDR and
+// drops ISR.  wun_bss_eval and wun_bss_eval_v3 are that driver with flags 0 and WUN_BSS_FRAMEWISE_FILTERS.
+//
 // Every sum runs in a fixed order (per-CTA partial slots, then an ordered second pass; no float atomics), so a call
 // returns the same bits on every run.  fp32 inputs are widened to fp64 when staged: each product of two of them is exact.
 #include <cuda_runtime.h>
@@ -25,7 +29,6 @@ constexpr int kMaxSegs = 256;        // sample segments of the correlation (part
 constexpr int kPanel = 64;           // LDL^T panel width
 constexpr int kFrThreads = 128;
 constexpr int kFrTile = kFrThreads * kR;  // output samples per framewise CTA
-constexpr int kEnergies = 7;
 
 __host__ __device__ constexpr int skew(int i) { return i + (i >> 4); }  // one pad double per 16: stride-8 reads hit distinct banks
 
@@ -139,21 +142,23 @@ __global__ void bss_assemble_gram_kernel(const double* __restrict__ lags, int ns
     A[(int64_t)i * n + j] = v;
 }
 
-// Right-hand sides, one contiguous column per (target j, estimate channel e):
-//   C  [j][e][(k, c, l)] = D_j[(k, c, l), e] = <S_l r_{k,c}, est_{j,e}>
-//   Cj [j][e][(c, l)]    = D_j[(j, c, l), e]   (source j's rows: the single-source system against G[j,j])
-__global__ void bss_assemble_rhs_kernel(const double* __restrict__ lags, int nsrc, int nchan, double* __restrict__ C,
-                                        double* __restrict__ Cj, Pass pass) {
+// Right-hand sides, one contiguous column per (estimate j, estimate channel e):
+//   C  [j][e][(k, c, l)]      = D_j[(k, c, l), e] = <S_l r_{k,c}, est_{j,e}>
+//   Cj [jt][j'][e][(c, l)]    = D_j[(jt, c, l), e]   (reference jt's rows: the single-source system against G[jt,jt])
+// Without pairs (npair 1) only jt == j is kept, at j' = 0; with pairs (npair = nsrc) every jt, at j' = j.
+__global__ void bss_assemble_rhs_kernel(const double* __restrict__ lags, int nsrc, int nchan, int npair,
+                                        double* __restrict__ C, double* __restrict__ Cj, Pass pass) {
     const int nref = nsrc * nchan, col = blockIdx.y, j = col / nchan, e = col % nchan;
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= nref * kL || pass_frame(pass, blockIdx.z) < 0) return;
     lags += (int64_t)blockIdx.z * 2 * nref * nref * kL;
     C += (int64_t)blockIdx.z * nref * nref * kL;
-    Cj += (int64_t)blockIdx.z * nref * nchan * kL;
-    const int a = r / kL, l = r % kL;
+    Cj += (int64_t)blockIdx.z * nref * nchan * npair * kL;
+    const int a = r / kL, l = r % kL, jt = a / nchan;
     const double v = lag(lags, nref, a, nref + j * nchan + e, l);
     C[(int64_t)col * nref * kL + r] = v;
-    if (a / nchan == j) Cj[(int64_t)col * nchan * kL + (a % nchan) * kL + l] = v;
+    if (npair > 1 || jt == j)
+        Cj[(((int64_t)jt * npair + (npair > 1 ? j : 0)) * nchan + e) * nchan * kL + (a % nchan) * kL + l] = v;
 }
 
 // ---- stage 3: blocked LDL^T without pivoting, in place on the lower triangle ------------------------------------------------
@@ -364,16 +369,105 @@ __global__ void __launch_bounds__(256) bss_ldl_solve_kernel(const double* __rest
 }
 
 // ---- stage 4: framewise decomposition ---------------------------------------------------------------------------------------
-// CTA (tile, target j, frame t): output samples w = tile*1024 + 8*tid + i of P_all = sum_{k,c} C_j * frame slice of r_{k,c}
-// and P_j = sum_c Cj_j * slice of r_{j,c}, over the frame's W = win + L - 1 samples (slices zero-extended, no context from
-// neighbouring frames).  Only the seven energies leave the CTA, as one ordered partial per tile.  Samples past W come out as
-// zero (every tap reads beyond the slice there) and add nothing.
+// CTA (tile, estimate j, frame t): output samples w = tile*1024 + 8*tid + i of P_all = sum_{k,c} C_j * frame slice of r_{k,c}
+// and, for each scored reference jt, P_j = sum_c Cj_{jt,j} * slice of r_{jt,c}, over the frame's W = win + L - 1 samples
+// (slices zero-extended, no context from neighbouring frames).  Only the energies leave the CTA, as one ordered partial per
+// (pair, tile).  Samples past W come out as zero (every tap reads beyond the slice there) and add nothing.
+// Without pairs (npair 1) the one reference scored is jt = j.  With pairs (npair = nsrc) P_all is computed once and kept in
+// registers while each other reference's P_j is filtered from its own slices, staged again.
 // FRAMEWISE (v3): blockIdx.x / ntile is the pass's slot, which holds the frame's own filters; idle slots exit.
+constexpr int kEnergies = 8;   // the images version writes the first seven, the sources version all eight
+
+// xs[u] = slice[w0 - (L-1) + u] of signal xp (channel stride NCH), zero outside [0, win)
+template <int NCH>
+__device__ __forceinline__ void stage_slice(double* xs, const float* __restrict__ xp, int64_t f0, int64_t w0, int64_t win) {
+    __syncthreads();
+    for (int u = threadIdx.x; u < kFrTile + kL; u += kFrThreads) {
+        const int64_t v = w0 - (kL - 1) + u;
+        xs[skew(u)] = (v >= 0 && v < win) ? (double)xp[(f0 + v) * NCH] : 0.0;
+    }
+}
+
+// P[w] += sum_u h[u] xs[w - w0 + u] for this thread's 8 samples: into pa with the taps h (ALL), into pj with hj (own).
+template <int NCH, bool ALL>
+__device__ __forceinline__ void filter_slice(const double* xs, const double (*h)[kL], const double (*hj)[kL], bool own,
+                                             double (&pa)[NCH][kR], double (&pj)[NCH][kR]) {
+    const int tid = threadIdx.x;
+    double w[2 * kR];
+#pragma unroll
+    for (int k = 0; k < kR; ++k) w[k] = xs[skew(kR * tid + k)];
+    for (int ub = 0; ub < kL; ub += kR) {
+#pragma unroll
+        for (int k = 0; k < kR; ++k) w[kR + k] = xs[skew(ub + kR * tid + kR + k)];
+#pragma unroll
+        for (int st = 0; st < kR; ++st) {
+            if (ALL) {
+#pragma unroll
+                for (int e = 0; e < NCH; ++e) {
+                    const double he = h[e][ub + st];
+#pragma unroll
+                    for (int i = 0; i < kR; ++i) pa[e][i] = fma(he, w[st + i], pa[e][i]);
+                }
+            }
+            if (own) {
+#pragma unroll
+                for (int e = 0; e < NCH; ++e) {
+                    const double he = hj[e][ub + st];
+#pragma unroll
+                    for (int i = 0; i < kR; ++i) pj[e][i] = fma(he, w[st + i], pj[e][i]);
+                }
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < kR; ++k) w[k] = w[kR + k];
+    }
+}
+
+// The pair's energies (reference jt, estimate j) over the CTA, added in thread order into out[0 .. ne):
+// E0 |P_j|^2, E1 |est - r_jt|^2, E2 |r_jt|^2, E3 |P_j - r_jt|^2, E4 |P_all - P_j|^2, E5 |P_all|^2, E6 |est - P_all|^2,
+// E7 |est - P_j|^2.  The next use of `red` follows the barrier in stage_slice (or the kernel's end).
+template <int NCH>
+__device__ __forceinline__ void pair_energies(const float* __restrict__ ref, const float* __restrict__ est, int64_t N, int jt,
+                                              int j, int64_t f0, int64_t w0, int64_t win, const double (&pa)[NCH][kR],
+                                              const double (&pj)[NCH][kR], double (*red)[kFrThreads], int ne,
+                                              double* __restrict__ out) {
+    const int tid = threadIdx.x;
+    double en[kEnergies] = {};
+#pragma unroll
+    for (int i = 0; i < kR; ++i) {
+        const int64_t v = w0 + kR * tid + i;
+#pragma unroll
+        for (int e = 0; e < NCH; ++e) {
+            const int64_t off = (f0 + v) * NCH + e;
+            const double s = v < win ? (double)est[(int64_t)j * N * NCH + off] : 0.0;
+            const double r = v < win ? (double)ref[(int64_t)jt * N * NCH + off] : 0.0;
+            const double p = pj[e][i], q = pa[e][i];
+            en[0] += p * p;
+            en[1] += (s - r) * (s - r);
+            en[2] += r * r;
+            en[3] += (p - r) * (p - r);
+            en[4] += (q - p) * (q - p);
+            en[5] += q * q;
+            en[6] += (s - q) * (s - q);
+            en[7] += (s - p) * (s - p);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < kEnergies; ++k) red[k][tid] = en[k];
+    __syncthreads();
+    if (tid < ne) {
+        double s = 0.0;
+        for (int i = 0; i < kFrThreads; ++i) s += red[tid][i];
+        out[tid] = s;
+    }
+}
+
 template <int NCH, bool FRAMEWISE>
 __global__ void __launch_bounds__(kFrThreads) bss_frame_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est,
                                                                        const double* __restrict__ C, const double* __restrict__ Cj,
                                                                        int nsrc, int64_t N, int64_t win, int64_t hop, int ntile,
-                                                                       double* __restrict__ energies, Pass pass) {
+                                                                       int npair, int ne, double* __restrict__ energies,
+                                                                       Pass pass) {
     const int64_t t = FRAMEWISE ? pass_frame(pass, blockIdx.x / ntile) : blockIdx.x / ntile;
     if (FRAMEWISE && t < 0) return;
     const int64_t slot = FRAMEWISE ? blockIdx.x / ntile : 0;   // the frame's own filters
@@ -383,79 +477,44 @@ __global__ void __launch_bounds__(kFrThreads) bss_frame_energy_kernel(const floa
     const int nref = nsrc * NCH, tid = threadIdx.x, j = blockIdx.y;
     const int tile = blockIdx.x % ntile;
     const int64_t f0 = t * hop, w0 = (int64_t)tile * kFrTile;
+    const int jsel = npair > 1 ? j : 0;
+    const double* cj = Cj + slot * nsrc * npair * NCH * NCH * kL;   // + (jt * npair + jsel) * NCH * NCH * kL: [e][c][l] of (jt, j)
+    double* out = energies + (((int64_t)t * nsrc + j) * npair * ntile + tile) * ne;   // + (npair > 1 ? jt : 0) * ntile * ne
     double pa[NCH][kR], pj[NCH][kR];
 #pragma unroll
     for (int e = 0; e < NCH; ++e)
 #pragma unroll
         for (int i = 0; i < kR; ++i) pa[e][i] = pj[e][i] = 0.0;
+    // P_all from every reference, and the P_j of reference j from the same staged slices
     for (int a = 0; a < nref; ++a) {
         const bool own = a / NCH == j;
-        const float* xp = ref + (int64_t)(a / NCH) * N * NCH + a % NCH;
-        __syncthreads();
-        // xs[u] = slice[w0 - (L-1) + u]; taps reversed so that P[w] = sum_u h[u] xs[w - w0 + u]
-        for (int u = tid; u < kFrTile + kL; u += kFrThreads) {
-            const int64_t v = w0 - (kL - 1) + u;
-            xs[skew(u)] = (v >= 0 && v < win) ? (double)xp[(f0 + v) * NCH] : 0.0;
-        }
+        stage_slice<NCH>(xs, ref + (int64_t)(a / NCH) * N * NCH + a % NCH, f0, w0, win);
+        // taps reversed so that P[w] = sum_u h[u] xs[w - w0 + u]
         for (int u = tid; u < NCH * kL; u += kFrThreads) {
             const int e = u / kL, l = u % kL;
             h[e][kL - 1 - l] = C[((slot * nref + j * NCH + e) * nref + a) * kL + l];
-            if (own) hj[e][kL - 1 - l] = Cj[((slot * nref + j * NCH + e) * NCH + a % NCH) * kL + l];
+            if (own) hj[e][kL - 1 - l] = cj[((j * npair + jsel) * NCH * NCH + e * NCH + a % NCH) * kL + l];
         }
         __syncthreads();
-        double w[2 * kR];
+        filter_slice<NCH, true>(xs, h, hj, own, pa, pj);
+    }
+    pair_energies<NCH>(ref, est, N, j, j, f0, w0, win, pa, pj, red, ne, out + (npair > 1 ? j : 0) * ntile * ne);
+    for (int jt = 0; npair > 1 && jt < nsrc; ++jt) {
+        if (jt == j) continue;
 #pragma unroll
-        for (int k = 0; k < kR; ++k) w[k] = xs[skew(kR * tid + k)];
-        for (int ub = 0; ub < kL; ub += kR) {
+        for (int e = 0; e < NCH; ++e)
 #pragma unroll
-            for (int k = 0; k < kR; ++k) w[kR + k] = xs[skew(ub + kR * tid + kR + k)];
-#pragma unroll
-            for (int st = 0; st < kR; ++st) {
-#pragma unroll
-                for (int e = 0; e < NCH; ++e) {
-                    const double he = h[e][ub + st];
-#pragma unroll
-                    for (int i = 0; i < kR; ++i) pa[e][i] = fma(he, w[st + i], pa[e][i]);
-                }
-                if (own) {
-#pragma unroll
-                    for (int e = 0; e < NCH; ++e) {
-                        const double he = hj[e][ub + st];
-#pragma unroll
-                        for (int i = 0; i < kR; ++i) pj[e][i] = fma(he, w[st + i], pj[e][i]);
-                    }
-                }
+            for (int i = 0; i < kR; ++i) pj[e][i] = 0.0;
+        for (int c = 0; c < NCH; ++c) {
+            stage_slice<NCH>(xs, ref + (int64_t)jt * N * NCH + c, f0, w0, win);
+            for (int u = tid; u < NCH * kL; u += kFrThreads) {
+                const int e = u / kL, l = u % kL;
+                hj[e][kL - 1 - l] = cj[((jt * npair + j) * NCH * NCH + e * NCH + c) * kL + l];
             }
-#pragma unroll
-            for (int k = 0; k < kR; ++k) w[k] = w[kR + k];
+            __syncthreads();
+            filter_slice<NCH, false>(xs, h, hj, true, pa, pj);
         }
-    }
-    // E0 |P_j|^2, E1 |est - r_j|^2, E2 |r_j|^2, E3 |P_j - r_j|^2, E4 |P_all - P_j|^2, E5 |P_all|^2, E6 |est - P_all|^2
-    double en[kEnergies] = {};
-#pragma unroll
-    for (int i = 0; i < kR; ++i) {
-        const int64_t v = w0 + kR * tid + i;
-#pragma unroll
-        for (int e = 0; e < NCH; ++e) {
-            const int64_t off = ((int64_t)j * N + f0 + v) * NCH + e;
-            const double s = v < win ? (double)est[off] : 0.0, r = v < win ? (double)ref[off] : 0.0;
-            const double p = pj[e][i], q = pa[e][i];
-            en[0] += p * p;
-            en[1] += (s - r) * (s - r);
-            en[2] += r * r;
-            en[3] += (p - r) * (p - r);
-            en[4] += (q - p) * (q - p);
-            en[5] += q * q;
-            en[6] += (s - q) * (s - q);
-        }
-    }
-#pragma unroll
-    for (int k = 0; k < kEnergies; ++k) red[k][tid] = en[k];
-    __syncthreads();
-    if (tid < kEnergies) {
-        double s = 0.0;
-        for (int i = 0; i < kFrThreads; ++i) s += red[tid][i];
-        energies[(((int64_t)t * nsrc + j) * ntile + tile) * kEnergies + tid] = s;
+        pair_energies<NCH>(ref, est, N, jt, j, f0, w0, win, pa, pj, red, ne, out + jt * ntile * ne);
     }
 }
 
@@ -481,30 +540,105 @@ __device__ bool frame_silent(const float* __restrict__ ref, const float* __restr
     return silent;
 }
 
-// One CTA per frame: the silence rule, then the four metrics of every target from its tiles' energies (in order).
+// One CTA per frame: the silence rule, then the four metrics of every scored pair from its tiles' energies (in order).
+// Without pairs (npair 1): pair (j, j) into metrics [4][nsrc][nwin]; with pairs: every (jt, j) into [4][nsrc][nsrc][nwin].
 __global__ void __launch_bounds__(256) bss_frame_metrics_kernel(const float* __restrict__ ref, const float* __restrict__ est,
                                                                 int nsrc, int nchan, int64_t N, int64_t win, int64_t hop,
-                                                                int64_t nwin, int ntile, const double* __restrict__ energies,
+                                                                int64_t nwin, int ntile, int npair, bool sources,
+                                                                const double* __restrict__ energies,
                                                                 double* __restrict__ metrics) {
     const int64_t t = blockIdx.x, f0 = t * hop;
     const bool silent = frame_silent(ref, est, nsrc, nchan, N, win, f0);
-    const int j = threadIdx.x;
-    if (j >= nsrc) return;
+    const int p = threadIdx.x, ne = sources ? 8 : 7;
+    if (p >= nsrc * npair) return;
+    const int j = p / npair, js = p % npair, jt = npair > 1 ? js : j;   // estimate j scored against reference jt
     double E[kEnergies] = {};
     for (int tile = 0; tile < ntile; ++tile)
 #pragma unroll
-        for (int k = 0; k < kEnergies; ++k) E[k] += energies[(((int64_t)t * nsrc + j) * ntile + tile) * kEnergies + k];
+        for (int k = 0; k < kEnergies; ++k)
+            if (k < ne) E[k] += energies[((((int64_t)t * nsrc + j) * npair + js) * ntile + tile) * ne + k];
     const double nan = __longlong_as_double(0x7ff8000000000000LL);
-    // images decomposition: s_true = r_j, e_spat = P_j - r_j, e_interf = P_all - P_j, e_artif = est - P_all
-    const double sdr = silent ? nan : safe_db(E[2], E[1]);   // |s_true|^2 / |e_spat + e_interf + e_artif|^2
-    const double isr = silent ? nan : safe_db(E[2], E[3]);
+    double sdr, isr;
+    if (sources) {   // sources decomposition: s_filt = P_j
+        sdr = silent ? nan : safe_db(E[0], E[7]);   // |s_filt|^2 / |e_interf + e_artif|^2
+        isr = nan;
+    } else {         // images decomposition: s_true = r_j, e_spat = P_j - r_j, e_interf = P_all - P_j, e_artif = est - P_all
+        sdr = silent ? nan : safe_db(E[2], E[1]);   // |s_true|^2 / |e_spat + e_interf + e_artif|^2
+        isr = silent ? nan : safe_db(E[2], E[3]);
+    }
     const double sir = silent ? nan : safe_db(E[0], E[4]);
     const double sar = silent ? nan : safe_db(E[5], E[6]);
-    const int64_t o = (int64_t)j * nwin + t, m = (int64_t)nsrc * nwin;
+    const int64_t o = ((int64_t)jt * npair + (npair > 1 ? j : 0)) * nwin + t, m = (int64_t)nsrc * npair * nwin;
     metrics[o] = sdr;
     metrics[m + o] = isr;
     metrics[2 * m + o] = sir;
     metrics[3 * m + o] = sar;
+}
+
+// ---- permutation: choose, per frame, which reference each estimate is scored against ----------------------------------------
+// Candidate idx of itertools.permutations(range(nsrc)): lexicographic order, so idx's factorial-base digits pick the
+// remaining values in order.
+__device__ void nth_permutation(int idx, int nsrc, int* perm) {
+    int left[WUN_MAX_SOURCES];
+    int f = 1;
+    for (int k = 0; k < nsrc; ++k) left[k] = k;
+    for (int k = 2; k < nsrc; ++k) f *= k;   // (nsrc - 1)!
+    for (int pos = 0; pos < nsrc; ++pos) {
+        const int d = idx / f;
+        idx %= f;
+        perm[pos] = left[d];
+        for (int k = d; k < nsrc - 1 - pos; ++k) left[k] = left[k + 1];
+        if (pos < nsrc - 1) f /= nsrc - 1 - pos;
+    }
+}
+
+// numpy's argmax order: (a, ia) is taken over (b, ib) if it is the first NaN, or, with no NaN, the larger value or the
+// earlier candidate of equal ones.  ib < 0: nothing yet.  A total order, so any reduction tree picks the same candidate.
+__device__ __forceinline__ bool argmax_before(double a, int ia, double b, int ib) {
+    if (ia < 0) return false;
+    if (ib < 0) return true;
+    const bool an = isnan(a), bn = isnan(b);
+    if (an != bn) return an;
+    if (!an && a != b) return a > b;
+    return ia < ib;
+}
+
+// One CTA per frame: every candidate perm (estimate j paired with reference perm[j]) scored by its mean pair SIR, summed
+// over j in order and divided by nsrc; the first maximum wins.  Then perm[j][t] and metrics[.][j][t] = pair[.][perm[j]][j][t].
+__global__ void __launch_bounds__(256) bss_perm_select_kernel(const double* __restrict__ pair, int nsrc, int64_t nwin,
+                                                              double* __restrict__ metrics, int64_t* __restrict__ perm) {
+    __shared__ double bv[256];
+    __shared__ int bi[256];
+    const int64_t t = blockIdx.x;
+    const int tid = threadIdx.x;
+    const double* sir = pair + 2 * (int64_t)nsrc * nsrc * nwin;   // [jtrue][jest][nwin]
+    int ncand = 1;
+    for (int k = 2; k <= nsrc; ++k) ncand *= k;
+    double best = 0.0;
+    int besti = -1;
+    for (int i = tid; i < ncand; i += blockDim.x) {
+        int p[WUN_MAX_SOURCES];
+        nth_permutation(i, nsrc, p);
+        double s = sir[(int64_t)p[0] * nsrc * nwin + t];
+        for (int j = 1; j < nsrc; ++j) s += sir[((int64_t)p[j] * nsrc + j) * nwin + t];
+        const double mean = s / nsrc;
+        if (argmax_before(mean, i, best, besti)) { best = mean; besti = i; }
+    }
+    bv[tid] = best;
+    bi[tid] = besti;
+    __syncthreads();
+    for (int s = blockDim.x / 2; s > 0; s >>= 1) {
+        if (tid < s && argmax_before(bv[tid + s], bi[tid + s], bv[tid], bi[tid])) { bv[tid] = bv[tid + s]; bi[tid] = bi[tid + s]; }
+        __syncthreads();
+    }
+    if (tid < nsrc) {
+        int p[WUN_MAX_SOURCES];
+        nth_permutation(bi[0], nsrc, p);
+        const int j = tid, jt = p[j];
+        perm[j * nwin + t] = jt;
+        const int64_t m = (int64_t)nsrc * nwin, mp = (int64_t)nsrc * nsrc * nwin;
+        for (int k = 0; k < 4; ++k) metrics[k * m + j * nwin + t] = pair[k * mp + ((int64_t)jt * nsrc + j) * nwin + t];
+    }
 }
 
 // ---- v3: the frames to solve ------------------------------------------------------------------------------------------------
@@ -539,14 +673,18 @@ __global__ void bss_frame_filters_kernel(const double* __restrict__ C, const dou
 }
 
 // ---- host side --------------------------------------------------------------------------------------------------------------
+constexpr int kFlags = WUN_BSS_FRAMEWISE_FILTERS | WUN_BSS_PERMUTATION | WUN_BSS_SOURCES;
+
 struct Layout {
     int64_t nref, ntask, n, m, nseg, seg_len, nwin, ntile;
-    int64_t slots, lags, G, Gjj, C, Cj, E, total;   // byte offsets into the workspace
+    int npair, ne;       // references scored per estimate (nsrc with WUN_BSS_PERMUTATION, else 1); energies per pair
+    bool permute;
+    int64_t slots, lags, G, Gjj, C, Cj, E, PM, total;   // byte offsets into the workspace (v4)
 };
 
-bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, Layout* o) {
+bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, int flags, Layout* o) {
     if (nsrc < 1 || nsrc > WUN_MAX_SOURCES || (nchan != 1 && nchan != 2) || N < 1 || win < 1 || hop < 1) return false;
-    if (win > (int64_t)1 << 40 || hop > (int64_t)1 << 40 || N > (int64_t)1 << 40) return false;
+    if (win > (int64_t)1 << 40 || hop > (int64_t)1 << 40 || N > (int64_t)1 << 40 || (flags & ~kFlags)) return false;
     Layout& L = *o;
     L.nref = nsrc * nchan;
     L.ntask = 2 * L.nref * L.nref;
@@ -558,6 +696,9 @@ bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t ho
     L.nwin = N >= win ? (N - win) / hop + 1 : 0;   // floor((N - win + hop) / hop), at least 0
     L.ntile = (win + kL - 1 + kFrTile - 1) / kFrTile;
     if (L.nwin * L.ntile >= ((int64_t)1 << 31)) return false;
+    L.permute = flags & WUN_BSS_PERMUTATION;
+    L.npair = L.permute ? (int)nsrc : 1;
+    L.ne = flags & WUN_BSS_SOURCES ? 8 : 7;
     int64_t off = 0;
     auto take = [&](int64_t doubles) { const int64_t at = off; off += (doubles * 8 + 255) / 256 * 256; return at; };
     L.slots = take(L.nseg * L.ntask * kL);
@@ -565,8 +706,9 @@ bool make_layout(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t ho
     L.G = take(L.n * L.n);
     L.Gjj = take(nsrc * L.m * L.m);
     L.C = take(L.nref * L.n);
-    L.Cj = take(L.nref * L.m);
-    L.E = take(L.nwin * nsrc * L.ntile * kEnergies);
+    L.Cj = take(L.nref * L.m * L.npair);
+    L.E = take(L.nwin * nsrc * L.npair * L.ntile * L.ne);
+    L.PM = take(L.permute ? 4 * nsrc * nsrc * L.nwin : 0);
     L.total = off;
     return true;
 }
@@ -595,77 +737,64 @@ cudaError_t ldl_solve(double* A, int n, int batch, double* B, int ncol, Pass pas
     return cudaGetLastError();
 }
 
-}  // namespace
-
-extern "C" int64_t wun_bss_eval_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop) {
-    Layout L;
-    return make_layout(nsrc, nchan, nsampl, win, hop, &L) ? L.total : WUN_E_INVALID;
+void launch_energies(bool framewise, dim3 grid, cudaStream_t st, const float* ref, const float* est, const double* C,
+                     const double* Cj, int ns, int nc, int64_t N, int64_t win, int64_t hop, const Layout& S, double* E,
+                     Pass pass) {
+    const int ntile = (int)S.ntile;
+    if (nc == 1 && !framewise)
+        bss_frame_energy_kernel<1, false><<<grid, kFrThreads, 0, st>>>(ref, est, C, Cj, ns, N, win, hop, ntile, S.npair, S.ne, E, pass);
+    else if (nc == 1)
+        bss_frame_energy_kernel<1, true><<<grid, kFrThreads, 0, st>>>(ref, est, C, Cj, ns, N, win, hop, ntile, S.npair, S.ne, E, pass);
+    else if (!framewise)
+        bss_frame_energy_kernel<2, false><<<grid, kFrThreads, 0, st>>>(ref, est, C, Cj, ns, N, win, hop, ntile, S.npair, S.ne, E, pass);
+    else
+        bss_frame_energy_kernel<2, true><<<grid, kFrThreads, 0, st>>>(ref, est, C, Cj, ns, N, win, hop, ntile, S.npair, S.ne, E, pass);
 }
 
-extern "C" int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
-                            int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
-                            int64_t workspace_bytes, void* stream) {
-    Layout L;
-    if (!make_layout(nsrc, nchan, nsampl, win, hop, &L)) return WUN_E_INVALID;
-    if (!references || !estimates || !workspace || (!metrics && L.nwin > 0)) return WUN_E_INVALID;
-    if (workspace_bytes < L.total || reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return WUN_E_INVALID;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        return WUN_E_NOGPU;
-    }
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char* ws = static_cast<char*>(workspace);
+// v4: the filters once over the whole track, then the energies of every frame.
+cudaError_t energies_v4(const float* ref, const float* est, int ns, int nc, int64_t N, int64_t win, int64_t hop,
+                        const Layout& L, char* ws, double* filters, cudaStream_t st) {
     double *slots = (double*)(ws + L.slots), *lags = (double*)(ws + L.lags), *G = (double*)(ws + L.G),
            *Gjj = (double*)(ws + L.Gjj), *C = (double*)(ws + L.C), *Cj = (double*)(ws + L.Cj), *E = (double*)(ws + L.E);
-    const int ns = (int)nsrc, nc = (int)nchan, nref = (int)L.nref;
-
+    const int nref = (int)L.nref;
     const Pass whole{nullptr, 0, 1};
-    bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)L.ntask), kXcThreads, 0, st>>>(references, estimates, ns, nc, nsampl,
-                                                                                        L.seg_len, slots, whole, win, hop);
+    bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)L.ntask), kXcThreads, 0, st>>>(ref, est, ns, nc, N, L.seg_len, slots,
+                                                                                        whole, win, hop);
     const int64_t nvals = L.ntask * kL;
     bss_lag_reduce_kernel<<<(unsigned)((nvals + 255) / 256), 256, 0, st>>>(slots, L.nseg, nvals, lags, whole);
     bss_assemble_gram_kernel<<<dim3((unsigned)(L.n + 255) / 256, (unsigned)L.n, 1 + ns), 256, 0, st>>>(lags, ns, nc, G, Gjj,
                                                                                                        whole);
-    bss_assemble_rhs_kernel<<<dim3((unsigned)(L.n + 255) / 256, nref), 256, 0, st>>>(lags, ns, nc, C, Cj, whole);
+    bss_assemble_rhs_kernel<<<dim3((unsigned)(L.n + 255) / 256, nref), 256, 0, st>>>(lags, ns, nc, L.npair, C, Cj, whole);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = ldl_solve(G, (int)L.n, 1, C, nref, whole, st);
-    if (e == cudaSuccess) e = ldl_solve(Gjj, (int)L.m, ns, Cj, nc, whole, st);
+    if (e == cudaSuccess) e = ldl_solve(Gjj, (int)L.m, ns, Cj, nc * L.npair, whole, st);
     if (e == cudaSuccess && L.nwin > 0) {
-        const dim3 grid((unsigned)(L.nwin * L.ntile), ns);
-        if (nc == 1)
-            bss_frame_energy_kernel<1, false><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win,
-                                                                           hop, (int)L.ntile, E, whole);
-        else
-            bss_frame_energy_kernel<2, false><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win,
-                                                                           hop, (int)L.ntile, E, whole);
-        bss_frame_metrics_kernel<<<(unsigned)L.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, L.nwin,
-                                                                   (int)L.ntile, E, metrics);
+        launch_energies(false, dim3((unsigned)(L.nwin * L.ntile), ns), st, ref, est, C, Cj, ns, nc, N, win, hop, L, E, whole);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess && filters) {
         e = cudaMemcpyAsync(filters, C, L.nref * L.n * 8, cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(filters + L.nref * L.n, Cj, L.nref * L.m * 8, cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess)
+            e = cudaMemcpyAsync(filters + L.nref * L.n, Cj, L.nref * L.m * L.npair * 8, cudaMemcpyDeviceToDevice, st);
     }
-    return e == cudaSuccess ? WUN_OK : WUN_E_CUDA;
+    return e;
 }
-
-namespace {
 
 constexpr int kV3Segs = 16;            // sample segments of a frame's correlations (partial slots per lag)
 constexpr int64_t kV3MaxPass = 2048;   // frames per pass at most: keeps the assembly grid's z = slots * (1 + nsrc) in range
 
-// v3's workspace: the silence flags, the frame list and the energies of the whole call, then the per-frame arrays of one
-// pass of P frames.  Every per-frame array is a multiple of 4 KiB, so the total is fixed + P * per_frame.
+// v3's workspace: the silence flags, the frame list, the energies and pair metrics of the whole call, then the per-frame
+// arrays of one pass of P frames.  Every per-frame array is a multiple of 4 KiB, so the total is fixed + P * per_frame.
 struct LayoutV3 {
-    Layout s;                          // shapes as v4 (nref, ntask, n, m, nwin, ntile); its offsets are not used
+    Layout s;                          // shapes as v4 (nref, ntask, n, m, nwin, ntile, npair, ne); its offsets are not used
     int64_t nseg, seg_len, P;
-    int64_t silent, list, E, slots, lags, G, Gjj, C, Cj;   // byte offsets into the workspace
+    int64_t silent, list, E, PM, slots, lags, G, Gjj, C, Cj;   // byte offsets into the workspace
     int64_t fixed, per_frame, total;
 };
 
-bool make_layout_v3(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, int64_t frames_per_pass, LayoutV3* o) {
-    if (frames_per_pass < 1 || !make_layout(nsrc, nchan, N, win, hop, &o->s)) return false;
+bool make_layout_v3(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t hop, int flags, int64_t frames_per_pass,
+                    LayoutV3* o) {
+    if (frames_per_pass < 1 || !make_layout(nsrc, nchan, N, win, hop, flags, &o->s)) return false;
     const Layout& S = o->s;
     const int64_t nchunks = (win + kXcChunk - 1) / kXcChunk, per_seg = (nchunks + kV3Segs - 1) / kV3Segs;
     o->nseg = (nchunks + per_seg - 1) / per_seg;
@@ -675,10 +804,11 @@ bool make_layout_v3(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t
     auto take = [&](int64_t bytes) { const int64_t at = off; off += (bytes + 255) / 256 * 256; return at; };
     o->silent = take(S.nwin * 4);
     o->list = take((1 + S.nwin) * 4);
-    o->E = take(S.nwin * nsrc * S.ntile * kEnergies * 8);
+    o->E = take(S.nwin * nsrc * S.npair * S.ntile * S.ne * 8);
+    o->PM = take(S.permute ? 4 * nsrc * nsrc * S.nwin * 8 : 0);
     o->fixed = off;
     const int64_t d_slots = o->nseg * S.ntask * kL, d_lags = S.ntask * kL, d_G = S.n * S.n, d_Gjj = nsrc * S.m * S.m,
-                  d_C = S.nref * S.n, d_Cj = S.nref * S.m;
+                  d_C = S.nref * S.n, d_Cj = S.nref * S.m * S.npair;
     o->per_frame = 8 * (d_slots + d_lags + d_G + d_Gjj + d_C + d_Cj);
     o->slots = take(o->P * d_slots * 8);
     o->lags = take(o->P * d_lags * 8);
@@ -690,39 +820,18 @@ bool make_layout_v3(int64_t nsrc, int64_t nchan, int64_t N, int64_t win, int64_t
     return true;
 }
 
-}  // namespace
-
-extern "C" int64_t wun_bss_eval_v3_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop,
-                                                   int64_t frames_per_pass) {
-    LayoutV3 L;
-    return make_layout_v3(nsrc, nchan, nsampl, win, hop, frames_per_pass, &L) ? L.total : WUN_E_INVALID;
-}
-
-extern "C" int wun_bss_eval_v3(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
-                               int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
-                               int64_t workspace_bytes, void* stream) {
-    LayoutV3 L;
-    if (!make_layout_v3(nsrc, nchan, nsampl, win, hop, 1, &L)) return WUN_E_INVALID;
+// v3: the frames that are not silent, in passes of L.P; each pass solves its frames' filters and adds their energies.
+cudaError_t energies_v3(const float* ref, const float* est, int ns, int nc, int64_t N, int64_t win, int64_t hop,
+                        const LayoutV3& L, char* ws, double* filters, cudaStream_t st) {
     const Layout& S = L.s;
-    if (!references || !estimates || !workspace || (!metrics && S.nwin > 0)) return WUN_E_INVALID;
-    if (workspace_bytes < L.total || reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return WUN_E_INVALID;
-    if (S.nwin > 1) make_layout_v3(nsrc, nchan, nsampl, win, hop, (workspace_bytes - L.fixed) / L.per_frame, &L);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-        cudaGetLastError();
-        return WUN_E_NOGPU;
-    }
-    if (S.nwin == 0) return WUN_OK;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char* ws = static_cast<char*>(workspace);
     int *silent = (int*)(ws + L.silent), *list = (int*)(ws + L.list);
     double *slots = (double*)(ws + L.slots), *lags = (double*)(ws + L.lags), *G = (double*)(ws + L.G),
            *Gjj = (double*)(ws + L.Gjj), *C = (double*)(ws + L.C), *Cj = (double*)(ws + L.Cj), *E = (double*)(ws + L.E);
-    const int ns = (int)nsrc, nc = (int)nchan, nref = (int)S.nref;
-    const int64_t csz = S.nref * S.n, cjsz = S.nref * S.m, nvals = S.ntask * kL;
+    const int nref = (int)S.nref;
+    const int64_t csz = S.nref * S.n, cjsz = S.nref * S.m * S.npair, nvals = S.ntask * kL;
     const unsigned fblocks = (unsigned)((csz + cjsz + 255) / 256);
 
-    bss_frame_silent_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, silent);
+    bss_frame_silent_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(ref, est, ns, nc, N, win, hop, silent);
     bss_frame_list_kernel<<<1, 1, 0, st>>>(silent, S.nwin, list);
     if (filters)
         bss_frame_filters_kernel<<<dim3((unsigned)S.nwin, fblocks), 256, 0, st>>>(nullptr, nullptr, csz, cjsz, silent,
@@ -731,31 +840,91 @@ extern "C" int wun_bss_eval_v3(const float* references, const float* estimates, 
     for (int64_t s0 = 0; s0 < S.nwin && e == cudaSuccess; s0 += L.P) {
         const unsigned np = (unsigned)std::min(L.P, S.nwin - s0);
         const Pass pass{list, s0, 1}, per_source{list, s0, ns};
-        bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)S.ntask, np), kXcThreads, 0, st>>>(
-            references, estimates, ns, nc, nsampl, L.seg_len, slots, pass, win, hop);
+        bss_xcorr_kernel<<<dim3((unsigned)L.nseg, (unsigned)S.ntask, np), kXcThreads, 0, st>>>(ref, est, ns, nc, N, L.seg_len,
+                                                                                               slots, pass, win, hop);
         bss_lag_reduce_kernel<<<dim3((unsigned)((nvals + 255) / 256), np), 256, 0, st>>>(slots, L.nseg, nvals, lags, pass);
         bss_assemble_gram_kernel<<<dim3((unsigned)(S.n + 255) / 256, (unsigned)S.n, np * (1 + ns)), 256, 0, st>>>(
             lags, ns, nc, G, Gjj, pass);
-        bss_assemble_rhs_kernel<<<dim3((unsigned)(S.n + 255) / 256, nref, np), 256, 0, st>>>(lags, ns, nc, C, Cj, pass);
+        bss_assemble_rhs_kernel<<<dim3((unsigned)(S.n + 255) / 256, nref, np), 256, 0, st>>>(lags, ns, nc, S.npair, C, Cj,
+                                                                                             pass);
         e = cudaGetLastError();
         if (e == cudaSuccess) e = ldl_solve(G, (int)S.n, (int)np, C, nref, pass, st);
-        if (e == cudaSuccess) e = ldl_solve(Gjj, (int)S.m, (int)np * ns, Cj, nc, per_source, st);
+        if (e == cudaSuccess) e = ldl_solve(Gjj, (int)S.m, (int)np * ns, Cj, nc * S.npair, per_source, st);
         if (e != cudaSuccess) break;
-        const dim3 grid((unsigned)(np * S.ntile), ns);
-        if (nc == 1)
-            bss_frame_energy_kernel<1, true><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
-                                                                          (int)S.ntile, E, pass);
-        else
-            bss_frame_energy_kernel<2, true><<<grid, kFrThreads, 0, st>>>(references, estimates, C, Cj, ns, nsampl, win, hop,
-                                                                          (int)S.ntile, E, pass);
+        launch_energies(true, dim3((unsigned)(np * S.ntile), ns), st, ref, est, C, Cj, ns, nc, N, win, hop, S, E, pass);
         if (filters)
             bss_frame_filters_kernel<<<dim3(np, fblocks), 256, 0, st>>>(C, Cj, csz, cjsz, nullptr, pass, filters);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) {
+    return e;
+}
+
+}  // namespace
+
+extern "C" int64_t wun_bss_eval_ex_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop,
+                                                   int flags, int64_t frames_per_pass) {
+    LayoutV3 L;
+    if (flags & WUN_BSS_FRAMEWISE_FILTERS)
+        return make_layout_v3(nsrc, nchan, nsampl, win, hop, flags, frames_per_pass, &L) ? L.total : WUN_E_INVALID;
+    return make_layout(nsrc, nchan, nsampl, win, hop, flags, &L.s) ? L.s.total : WUN_E_INVALID;
+}
+
+extern "C" int wun_bss_eval_ex(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                               int64_t win, int64_t hop, int flags, double* metrics, int64_t* perm, double* pair_metrics,
+                               double* filters, void* workspace, int64_t workspace_bytes, void* stream) {
+    const bool framewise = flags & WUN_BSS_FRAMEWISE_FILTERS, permute = flags & WUN_BSS_PERMUTATION;
+    LayoutV3 L;
+    const Layout& S = L.s;
+    if (framewise ? !make_layout_v3(nsrc, nchan, nsampl, win, hop, flags, 1, &L)
+                  : !make_layout(nsrc, nchan, nsampl, win, hop, flags, &L.s))
+        return WUN_E_INVALID;
+    if (!references || !estimates || !workspace || (!metrics && S.nwin > 0)) return WUN_E_INVALID;
+    if (permute ? (!perm && S.nwin > 0) : (perm || pair_metrics)) return WUN_E_INVALID;
+    const int64_t need = framewise ? L.total : S.total;   // v3: one frame per pass at least
+    if (workspace_bytes < need || reinterpret_cast<uintptr_t>(workspace) % 256 != 0) return WUN_E_INVALID;
+    if (framewise && S.nwin > 1)
+        make_layout_v3(nsrc, nchan, nsampl, win, hop, flags, (workspace_bytes - L.fixed) / L.per_frame, &L);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+        cudaGetLastError();
+        return WUN_E_NOGPU;
+    }
+    if (framewise && S.nwin == 0) return WUN_OK;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    const int ns = (int)nsrc, nc = (int)nchan;
+    cudaError_t e = framewise ? energies_v3(references, estimates, ns, nc, nsampl, win, hop, L, ws, filters, st)
+                              : energies_v4(references, estimates, ns, nc, nsampl, win, hop, S, ws, filters, st);
+    if (e == cudaSuccess && S.nwin > 0) {
+        const double* E = (const double*)(ws + (framewise ? L.E : S.E));
+        double* pm = !permute ? metrics : pair_metrics ? pair_metrics : (double*)(ws + (framewise ? L.PM : S.PM));
         bss_frame_metrics_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(references, estimates, ns, nc, nsampl, win, hop, S.nwin,
-                                                                   (int)S.ntile, E, metrics);
+                                                                   (int)S.ntile, S.npair, flags & WUN_BSS_SOURCES, E, pm);
+        if (permute) bss_perm_select_kernel<<<(unsigned)S.nwin, 256, 0, st>>>(pm, ns, S.nwin, metrics, perm);
         e = cudaGetLastError();
     }
     return e == cudaSuccess ? WUN_OK : WUN_E_CUDA;
+}
+
+extern "C" int64_t wun_bss_eval_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop) {
+    return wun_bss_eval_ex_workspace_bytes(nsrc, nchan, nsampl, win, hop, 0, 1);
+}
+
+extern "C" int wun_bss_eval(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                            int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+    return wun_bss_eval_ex(references, estimates, nsrc, nchan, nsampl, win, hop, 0, metrics, nullptr, nullptr, filters,
+                           workspace, workspace_bytes, stream);
+}
+
+extern "C" int64_t wun_bss_eval_v3_workspace_bytes(int64_t nsrc, int64_t nchan, int64_t nsampl, int64_t win, int64_t hop,
+                                                   int64_t frames_per_pass) {
+    return wun_bss_eval_ex_workspace_bytes(nsrc, nchan, nsampl, win, hop, WUN_BSS_FRAMEWISE_FILTERS, frames_per_pass);
+}
+
+extern "C" int wun_bss_eval_v3(const float* references, const float* estimates, int64_t nsrc, int64_t nchan, int64_t nsampl,
+                               int64_t win, int64_t hop, double* metrics, double* filters, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+    return wun_bss_eval_ex(references, estimates, nsrc, nchan, nsampl, win, hop, WUN_BSS_FRAMEWISE_FILTERS, metrics, nullptr,
+                           nullptr, filters, workspace, workspace_bytes, stream);
 }

@@ -20,6 +20,7 @@ SYMBOLS = [
     "wun_gather_windows", "wun_scatter_windows", "wun_feed_batch", "wun_last_error", "wun_version", "wun_describe",
     "wun_layer_kernel", "wun_debug_tensor", "wun_debug_run_conv", "wun_debug_run_layer", "wun_crc32c", "wun_debug_plan", "wun_debug_launches",
     "wun_bss_eval_workspace_bytes", "wun_bss_eval", "wun_bss_eval_v3_workspace_bytes", "wun_bss_eval_v3",
+    "wun_bss_eval_ex_workspace_bytes", "wun_bss_eval_ex",
     "wun_resample_frames", "wun_resample",
     "wun_snippet_batch", "wun_eval_batch_loss",
     "wun_spec_create", "wun_spec_destroy", "wun_spec_input_frames", "wun_spec_output_frames", "wun_spec_stft_frames",
@@ -132,6 +133,10 @@ def _load():
         lib.wun_bss_eval_v3_workspace_bytes.argtypes = [I64, I64, I64, I64, I64, I64]
         lib.wun_bss_eval_v3_workspace_bytes.restype = I64
         lib.wun_bss_eval_v3.argtypes = lib.wun_bss_eval.argtypes
+    if hasattr(lib, "wun_bss_eval_ex"):     # likewise, and builds from before the permutation search (WUN_LIB)
+        lib.wun_bss_eval_ex_workspace_bytes.argtypes = [I64, I64, I64, I64, I64, ctypes.c_int, I64]
+        lib.wun_bss_eval_ex_workspace_bytes.restype = I64
+        lib.wun_bss_eval_ex.argtypes = [VP, VP, I64, I64, I64, I64, I64, ctypes.c_int, VP, VP, VP, VP, VP, I64, VP]
     if hasattr(lib, "wun_resample"):        # likewise the resampling kernel
         lib.wun_resample_frames.argtypes = [I64, I64, I64]
         lib.wun_resample_frames.restype = I64
@@ -207,9 +212,11 @@ def check(rc):
 BSS_FILTER_LEN = 512
 BSS_MODES = ("v4", "v3")
 BSS_V3_WORKSPACE_BYTES = 2 << 30        # 1-s frames at 44.1 kHz: 12 per pass at n = 4096 (4 stereo sources), 40 at n = 2048
+BSS_FRAMEWISE_FILTERS, BSS_PERMUTATION, BSS_SOURCES = 1, 2, 4       # include/wun.h WUN_BSS_*
 
 
-def bss_eval(references, estimates, win, hop, filters=False, mode="v4", max_workspace_bytes=BSS_V3_WORKSPACE_BYTES):
+def bss_eval(references, estimates, win, hop, filters=False, mode="v4", max_workspace_bytes=BSS_V3_WORKSPACE_BYTES,
+             permutation=False, sources_version=False, pair_metrics=False):
     """BSS Eval of `estimates` against `references` as museval.evaluate(..., mode=mode) computes it: both contiguous float32
     CUDA tensors [nsrc, nsampl, nchan] on one device.  Returns float64 CUDA tensors (SDR, ISR, SIR, SAR), each [nsrc, nwin];
     with filters=True also (C [nsrc, nchan, nsrc, nchan, 512], Cj [nsrc, nchan, nchan, 512]): the filters for all sources and
@@ -218,10 +225,19 @@ def bss_eval(references, estimates, win, hop, filters=False, mode="v4", max_work
     mode="v4" (include/wun.h wun_bss_eval) solves the filters once over the whole track.  mode="v3" (wun_bss_eval_v3) solves
     them for every frame from its own samples; the filters then have a leading [nwin] axis and are NaN for silent frames.
     v3 processes frames in passes, as many per pass as fit in max_workspace_bytes (at least one); the results do not depend
-    on it."""
+    on it.
+
+    museval's bss_eval switches (wun_bss_eval_ex): permutation=True scores every (reference, estimate) pair and keeps, per
+    frame, the pairing with the largest mean SIR; row j of the metrics is then estimate j, and `perm` (int64 CUDA [nsrc,
+    nwin], returned right after SAR) is the reference each estimate is scored against.  pair_metrics=True (with permutation)
+    also returns the metrics of every pair, float64 [4, nsrc (reference), nsrc (estimate), nwin], after perm; Cj then holds
+    every pair, [reference, estimate, estimate channel, reference channel, tap].  sources_version=True scores the "sources"
+    decomposition: SDR = |P_j|^2 / |est - P_j|^2 and ISR NaN; SIR and SAR as in the images version."""
     import torch
     if mode not in BSS_MODES:
         raise ValueError("bss_eval: mode=%r, must be one of %s" % (mode, ", ".join(BSS_MODES)))
+    if pair_metrics and not permutation:
+        raise ValueError("bss_eval: pair_metrics=True needs permutation=True")
     for t in (references, estimates):
         assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.dim() == 3, \
             "references / estimates must be contiguous float32 CUDA tensors [nsrc, nsampl, nchan]"
@@ -229,38 +245,43 @@ def bss_eval(references, estimates, win, hop, filters=False, mode="v4", max_work
     nsrc, n, nchan = (int(s) for s in references.shape)
     win, hop = int(win), int(hop)
     nwin = (n - win) // hop + 1 if n >= win > 0 and hop > 0 else 0
-    if mode == "v4":
-        nbytes = lib.wun_bss_eval_workspace_bytes(nsrc, nchan, n, win, hop)
-    else:
-        nbytes = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, 1)
-        if nbytes >= 0 and nwin > 1:
-            per_frame = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, 2) - nbytes
-            fit = 1 + max(0, int(max_workspace_bytes) - nbytes) // per_frame
-            nbytes = lib.wun_bss_eval_v3_workspace_bytes(nsrc, nchan, n, win, hop, min(fit, nwin))
+    flags = ((BSS_FRAMEWISE_FILTERS if mode == "v3" else 0) | (BSS_PERMUTATION if permutation else 0)
+             | (BSS_SOURCES if sources_version else 0))
+    nbytes = lib.wun_bss_eval_ex_workspace_bytes(nsrc, nchan, n, win, hop, flags, 1)
+    if mode == "v3" and nbytes >= 0 and nwin > 1:
+        per_frame = lib.wun_bss_eval_ex_workspace_bytes(nsrc, nchan, n, win, hop, flags, 2) - nbytes
+        fit = 1 + max(0, int(max_workspace_bytes) - nbytes) // per_frame
+        nbytes = lib.wun_bss_eval_ex_workspace_bytes(nsrc, nchan, n, win, hop, flags, min(fit, nwin))
     if nbytes < 0:
         raise WunError(WUN_E_INVALID, "bss_eval: need 1 <= nsrc <= 8, nchan 1 or 2, nsampl, win, hop >= 1 (got %d, %d, %d, %d, %d)"
                        % (nsrc, nchan, n, win, hop))
     dev = references.device
+    npair = nsrc if permutation else 1
     metrics = torch.empty((4, nsrc, nwin), dtype=torch.float64, device=dev)
-    fsz = nsrc * nchan * (nsrc * nchan + nchan) * BSS_FILTER_LEN
-    filt = None
-    if filters:
-        filt = torch.empty((nwin if mode == "v3" else 1) * fsz, dtype=torch.float64, device=dev)
+    perm = torch.empty((nsrc, nwin), dtype=torch.int64, device=dev) if permutation else None
+    pairs = torch.empty((4, nsrc, nsrc, nwin), dtype=torch.float64, device=dev) if pair_metrics else None
+    nc = nsrc * nchan * nsrc * nchan * BSS_FILTER_LEN
+    fsz = nc + nsrc * nchan * npair * nchan * BSS_FILTER_LEN
+    filt = torch.empty((nwin if mode == "v3" else 1) * fsz, dtype=torch.float64, device=dev) if filters else None
     ws = torch.empty((nbytes + 255) // 256 * 32, dtype=torch.float64, device=dev)      # torch allocations are 256-B aligned
-    call = lib.wun_bss_eval if mode == "v4" else lib.wun_bss_eval_v3
+    ptr = lambda t: t.data_ptr() if t is not None and nwin else None          # noqa: E731
     with torch.cuda.device(dev):
-        rc = call(references.data_ptr(), estimates.data_ptr(), nsrc, nchan, n, win, hop,
-                  metrics.data_ptr() if nwin else None, filt.data_ptr() if filt is not None else None,
-                  ws.data_ptr(), ws.numel() * 8, Engine._stream(dev))
+        rc = lib.wun_bss_eval_ex(references.data_ptr(), estimates.data_ptr(), nsrc, nchan, n, win, hop, flags, ptr(metrics),
+                                 ptr(perm), ptr(pairs), filt.data_ptr() if filt is not None else None, ws.data_ptr(),
+                                 ws.numel() * 8, Engine._stream(dev))
     if rc != WUN_OK:
-        raise WunError(rc, "%s failed" % ("wun_bss_eval" if mode == "v4" else "wun_bss_eval_v3"))
+        raise WunError(rc, "wun_bss_eval_ex (flags %d) failed" % flags)
     out = tuple(metrics)
+    if permutation:
+        out += (perm,)
+    if pair_metrics:
+        out += (pairs,)
     if filters:
-        nc = nsrc * nchan * nsrc * nchan * BSS_FILTER_LEN
         f = filt.view(-1, fsz)
         lead = (nwin,) if mode == "v3" else ()
+        cj = (nsrc, nsrc) if permutation else (nsrc,)
         out += (f[:, :nc].reshape(lead + (nsrc, nchan, nsrc, nchan, BSS_FILTER_LEN)),
-                f[:, nc:].reshape(lead + (nsrc, nchan, nchan, BSS_FILTER_LEN)))
+                f[:, nc:].reshape(lead + cj + (nchan, nchan, BSS_FILTER_LEN)))
     return out
 
 
